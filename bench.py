@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- atoms/sec of a full training step on synthetic radius-graph batches (BASELINE.json metric).
 
-    python bench.py --gpus 1 --steps 20 --warmup 5                     # engine arm, one B200, config C2 (QM9-shape PaiNN)
+    python bench.py --gpus 1 --steps 20 --warmup 5                     # engine arm, one GPU, config C2 (QM9-shape PaiNN)
     python bench.py --workload md17_egnn|oc20_mace|gfm_pnaeq|lj_egnn   # the other BASELINE.json configs (SURVEY 8d C3/C4/C5/C1)
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference --gpus 1 --steps 3 --warmup 1     # CPU arm (oracle on the host cores)
@@ -10,11 +10,18 @@ One "step" = neighbour build (radius graph, periodic for C1/C4, + CSR plans) -> 
 all-reduce -> fused AdamW on one batch.  Weak scaling: every rank owns ``--graphs`` graphs per step; ``value`` = atoms processed
 by all ranks / max-over-ranks device time.  Prints ONE JSON line on rank 0.
 
-Timing design (VERDICT r1 "weak" #1): every step is bracketed by its own CUDA event on every rank; the timed region runs
-``--regions`` (3) times and the MEDIAN region is the reported one (all regions are listed); per-step median / p90 / max and the
+Timing design (VERDICT r1 "weak" #1): every step is bracketed by its own CUDA event on every rank; the ``--steps`` timed steps
+are split into ``--regions`` (3) consecutive regions and the MEDIAN region's time per step is the reported one (all regions are
+listed); ``--e2e`` adds a second timed pass of ``--steps`` steps that also copies the inputs in and the loss out (without it
+the line's ``e2e`` field is null); per-step
+median / p90 / max and the
 slowest rank are printed; the clock sampler reads NVML in-process and is started BEFORE the warm-up, so nothing forks or
 initialises NVML inside a timed window; with N > 1 the NCCL all-reduce is captured INSIDE the step's CUDA graph, so a step is one
 replay with no host round-trip.
+
+``--dump-outputs DIR`` writes, after the timed steps, what the last timed step produced for its caller: ``loss.npy`` (the step's
+loss), ``grad.npy`` (the flat parameter gradient) and ``params.npy`` (the flat parameters after the AdamW update), float32.
+Inputs are seeded, so two builds run with the same arguments can be compared array for array.
 """
 import argparse
 import json
@@ -57,14 +64,17 @@ def parse():
     ap.add_argument("--workload", default="qm9_painn", choices=sorted(WL))
     ap.add_argument("--graphs", type=int, default=None, help="graphs per GPU per step (default: the workload's saturating batch)")
     ap.add_argument("--nbatches", type=int, default=4, help="distinct pre-generated batches cycled through")
-    ap.add_argument("--regions", type=int, default=3, help="how many times the timed region of --steps steps is run (median reported)")
+    ap.add_argument("--regions", type=int, default=3, help="consecutive regions the --steps timed steps are split into (median reported)")
+    ap.add_argument("--e2e", action="store_true", help="also time --steps steps that copy their inputs in and their loss out")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's loss / flat gradient / updated parameters as DIR/<name>.npy")
     ap.add_argument("--no-graph", action="store_true", help="eager launches instead of CUDA-graph replay")
     ap.add_argument("--no-capture-allreduce", action="store_true", help="keep the NCCL all-reduce outside the step graph (two replays per step)")
     ap.add_argument("--ref-graphs", type=int, default=None, help="graphs per step of the CPU arm / cpu_baseline sample")
     ap.add_argument("--skip-cpu-baseline", action="store_true")
     ap.add_argument("--skip-kernel-shares", action="store_true")
     ap.add_argument("--precision", default=None, choices=["bf16", "fp32"],
-                    help="bf16 = tensor-core (tcgen05, TF32-in/fp32-acc) Linears; fp32 = exact SIMT kernels; default: the config's")
+                    help="bf16 = tensor-core (wgmma, TF32-in/fp32-acc) Linears; fp32 = fp32-accurate kernels; default: the config's")
     a = ap.parse_args()
     w = WL[a.workload]
     a.graphs = a.graphs or w["graphs"]
@@ -77,8 +87,8 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 1451.0)), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1451.0, "fallback (B200_PROFILING.md)"
+        return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", 989.0)), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, 989.0, "H100 SXM data sheet (dense BF16), not measured"
 
 
 class ClockSampler:
@@ -453,37 +463,42 @@ def run_engine(args):
             loss_host.copy_(l.reshape(1), non_blocking=True)
             if args.nbatches > 1:
                 issue_copy(i + 1)
+        state["loss"] = l
 
-    K, R = args.steps, max(1, args.regions)
-    atoms_region = sum(n_atoms[i % args.nbatches] for i in range(K))           # atoms this rank processes in one region
+    K = max(1, args.steps)
+    R = max(1, min(args.regions, K))
+    region_steps = [K // R + (1 if r < K % R else 0) for r in range(R)]      # the K timed steps, split into R regions
+    atoms_timed = sum(n_atoms[i % args.nbatches] for i in range(K))          # atoms this rank processes in the K timed steps
 
     def timed(e2e, with_clocks):
-        """R regions of K steps; per-step CUDA events on every rank.  -> (per-rank [R, K] step ms, region ms [R])"""
+        """K steps in R consecutive regions; per-step CUDA events on every rank.  -> (per-rank [K] step ms, [R] region ms per step)"""
         for i in range(args.warmup):
             run_step(i, e2e)
         torch.cuda.synchronize()
-        per_step = torch.zeros(R, K, dtype=torch.float64)
+        per_step = torch.zeros(K, dtype=torch.float64)
         region_ms = torch.zeros(R, dtype=torch.float64)
-        for r in range(R):
-            state["prefetched"] = -1            # the first timed step issues (and waits for) its own copy
+        i0 = 0
+        for r, kr in enumerate(region_steps):
+            state["prefetched"] = -1            # the first timed step of a region issues (and waits for) its own copy
             if ws > 1:
                 dist.barrier()
             torch.cuda.synchronize()
-            evs = [torch.cuda.Event(enable_timing=True) for _ in range(K + 1)]
+            evs = [torch.cuda.Event(enable_timing=True) for _ in range(kr + 1)]
             if with_clocks and sampler:
                 sampler.mark_begin()
             evs[0].record()
-            for i in range(K):
-                run_step(i, e2e)
+            for i in range(kr):
+                run_step(i0 + i, e2e)
                 evs[i + 1].record()
             torch.cuda.synchronize()
             if with_clocks and sampler:
                 sampler.mark_end()
             if ws > 1:
                 dist.barrier()
-            for i in range(K):
-                per_step[r, i] = evs[i].elapsed_time(evs[i + 1])
-            region_ms[r] = evs[0].elapsed_time(evs[K])
+            for i in range(kr):
+                per_step[i0 + i] = evs[i].elapsed_time(evs[i + 1])
+            region_ms[r] = evs[0].elapsed_time(evs[kr]) / kr
+            i0 += kr
         return per_step, region_ms
 
     def reduce_timing(per_step, region_ms):
@@ -491,34 +506,38 @@ def run_engine(args):
         if ws > 1:
             allr = [torch.zeros(R, device=dev, dtype=torch.float64) for _ in range(ws)]
             dist.all_gather(allr, region_ms.to(dev))
-            alls = [torch.zeros(R, K, device=dev, dtype=torch.float64) for _ in range(ws)]
+            alls = [torch.zeros(K, device=dev, dtype=torch.float64) for _ in range(ws)]
             dist.all_gather(alls, per_step.to(dev))
-            allr, alls = torch.stack(allr).cpu(), torch.stack(alls).cpu()            # [ws, R], [ws, R, K]
-            an = torch.tensor([float(atoms_region)], device=dev, dtype=torch.float64)
+            allr, alls = torch.stack(allr).cpu(), torch.stack(alls).cpu()            # [ws, R], [ws, K]
+            an = torch.tensor([float(atoms_timed)], device=dev, dtype=torch.float64)
             dist.all_reduce(an)
             atoms_all = float(an)
         else:
-            allr, alls, atoms_all = region_ms[None], per_step[None], float(atoms_region)
+            allr, alls, atoms_all = region_ms[None], per_step[None], float(atoms_timed)
         reg = allr.max(dim=0).values                                                   # [R] max over ranks
         order = sorted(range(R), key=lambda r: float(reg[r]))
         med = order[len(order) // 2]
         steps_max = alls.max(dim=0).values.reshape(-1)                                 # per-step max over ranks, all regions
         srt = sorted(steps_max.tolist())
-        stats = {"regions_ms": [round(float(x), 4) for x in reg], "region_used": med,
+        stats = {"region_ms_per_step": [round(float(x), 4) for x in reg], "region_steps": region_steps, "region_used": med,
                  "step_ms_median": round(statistics.median(srt), 4), "step_ms_p90": round(srt[min(len(srt) - 1, int(0.9 * len(srt)))], 4),
                  "step_ms_max": round(srt[-1], 4), "slowest_rank": int(allr[:, med].argmax()),
                  "rank_region_ms": [round(float(x), 4) for x in allr[:, med]]}
-        return float(reg[med]) / K, atoms_all, stats
+        return float(reg[med]), atoms_all, stats
 
     ps, rg = timed(False, True)
     ms_dev, atoms_all, stats_dev = reduce_timing(ps, rg)
-    ps, rg = timed(True, False)
-    ms_e2e, _, stats_e2e = reduce_timing(ps, rg)
+    ms_e2e = stats_e2e = None
+    if args.e2e:
+        ps, rg = timed(True, False)
+        ms_e2e, _, stats_e2e = reduce_timing(ps, rg)
     torch.cuda.synchronize()
     ops.check_guard(dev)                                     # every captured neighbour build produced the promised edge count
     clocks = sampler.stop() if sampler else None
     value = atoms_all / K / (ms_dev * 1e-3)
-    e2e = atoms_all / K / (ms_e2e * 1e-3)
+    e2e = atoms_all / K / (ms_e2e * 1e-3) if ms_e2e else None
+    if args.dump_outputs and rank == 0:                      # before anything else runs a step and moves the parameters
+        dump_outputs(args.dump_outputs, {"loss": state["loss"], "grad": opt.flat_g, "params": opt.flat_p})
 
     roof, shares = None, None
     if rank == 0 and not args.skip_kernel_shares:
@@ -546,7 +565,7 @@ def run_engine(args):
                 "warmup": args.warmup, "ms_per_step": ms_dev, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "tf32" if args.precision == "bf16" else "f32", "data": "synthetic",
                 "config": {"workload": "%s (%s): %s" % (args.workload, wl["cfg"], wl["desc"]),
-                           "precision": "bf16 config -> fp32 parameters/activations, large-M Linears on tcgen05 kind::tf32 with fp32 "
+                           "precision": "bf16 config -> fp32 parameters/activations, large-M Linears on wgmma TF32 with fp32 "
                                         "accumulation (>= bf16 autocast of the reference)" if args.precision == "bf16" else "fp32",
                            "graphs_per_gpu": G, "atoms_per_gpu": n_atoms[0], "edges_per_gpu": n_edges[0],
                            "parallelism": "dp%d (graphs sharded by rank, one flat gradient all-reduce)" % ws,
@@ -557,24 +576,40 @@ def run_engine(args):
                            if use_graph else "eager",
                            "e2e_pipeline": "every step copies its inputs (%s) from pinned host memory (copy stream, issued one step "
                                            "ahead) and reads its loss back" % "/".join(host[0].keys()),
-                           "l2": "%d distinct batches cycled; per-step working set (activations + saved tensors) >> 126 MB L2" % args.nbatches,
-                           "timing": "%d regions of %d steps, median region reported; per-step CUDA events on every rank, max over ranks" % (R, K)},
+                           "l2": "%d distinct batches cycled; per-step working set (activations + saved tensors) >> 50 MB L2" % args.nbatches,
+                           "timing": "%d timed steps in %d regions, median region reported; per-step CUDA events on every rank, max over ranks"
+                                     % (K, R)},
                 "timing": stats_dev, "clocks": clocks, "gpu_launches": int(launches_per_step * K),
                 "e2e": {"value": e2e, "unit": "atoms/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": 4,
-                        "timing": stats_e2e},
+                        "timing": stats_e2e} if args.e2e else None,
                 "roofline": roof, "step_roofline": step_roof, "kernel_shares": shares, "cpu_baseline": cpu_base}
         print(json.dumps(line), flush=True)
     _shutdown(ws, dev, [graphs, g_opt])
 
 
+def dump_outputs(out_dir, arrays, limit=64 << 20):
+    """arrays {name: tensor} -> out_dir/<name>.npy (float32); a larger total is cut to a fixed, seeded sample of each array."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    host = {k: v.detach().float().reshape(-1).cpu().numpy() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in host.values())
+    for name, a in host.items():
+        if total > limit:
+            keep = max(1, int(a.size * limit / total))
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, keep, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def _shutdown(ws, dev, keep_alive):
-    """Leave without tearing NCCL down: destroying a process group whose collectives live inside captured CUDA graphs can block
-    forever at interpreter exit (observed: the 2-GPU run printed its line and then hung in teardown).  Every rank drains its GPU,
-    meets the others once, flushes and exits the process directly."""
+    """Drain the GPU and leave.  One process: a normal return, so the interpreter shuts down as usual (atexit handlers, library
+    destructors, profiler / CUPTI flushes).  N > 1: destroying a process group whose collectives live inside captured CUDA graphs
+    can block forever at interpreter exit (observed: the 2-GPU run printed its line and then hung in teardown), so every rank
+    meets the others once, flushes and exits the process directly; ``keep_alive`` holds the graphs until then."""
     torch.cuda.synchronize()
-    if ws > 1:
-        dist.barrier()
-        torch.cuda.synchronize()
+    if ws == 1:
+        return
+    dist.barrier()
+    torch.cuda.synchronize()
     sys.stdout.flush()
     sys.stderr.flush()
     os._exit(0)

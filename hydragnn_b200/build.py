@@ -1,5 +1,5 @@
-"""Builds hydragnn_b200/csrc/libhgb.so with nvcc for sm_100a (in-tree, so the .so travels to the
-GPU box with the gpurun snapshot).  No torch dependency: the library is a plain C-ABI shared object.
+"""Builds hydragnn_b200/csrc/libhgb.so with nvcc for sm_90a (H100), in-tree next to the sources, so the package
+imports from the repository without an install step.  No torch dependency: the library is a plain C-ABI shared object.
 """
 import hashlib
 import os
@@ -9,7 +9,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libhgb.so")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH_FLAGS + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -68,8 +69,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("libhgb.so build failed")
-    subprocess.check_call([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static",
-                                                                    "-Xcompiler", "-fPIC"])
+    subprocess.check_call([nvcc, "-shared", "-o", LIB] + objs + ARCH_FLAGS + ["-lcudart_static", "-Xcompiler", "-fPIC"])
     open(stamp_file, "w").write(stamp)
     return LIB
 

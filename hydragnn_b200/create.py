@@ -63,7 +63,7 @@ def create_model_config(config, verbosity=0, use_gpu=True):
 
 
 def set_precision(model, precision):
-    """'fp32': exact fp32 kernels everywhere.  'bf16': the large-M Linear layers run on the tcgen05 tensor-core
+    """'fp32': exact fp32 kernels everywhere.  'bf16': the large-M Linear layers run on the wgmma tensor-core
     kernels (TF32 products, fp32 accumulation; parameters and activations stay fp32 like the reference's
     autocast mode, hydragnn/train/train_validate_test.py:43-49)."""
     if precision not in ("fp32", "bf16"):

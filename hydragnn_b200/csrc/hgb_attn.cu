@@ -11,7 +11,7 @@
 #define ATT_TQ 128   // threads per block
 #define ATT_KS 4     // lanes that share one (row, head): each walks every 4th key of a tile; combined with shuffles.
 #define ATT_QPB (ATT_TQ / ATT_KS)   // rows per block.  (Sequences here are a few thousand atoms: one thread per row would
-                                    // leave most of the 148 SMs idle and serialise the whole key loop in one dependency chain.)
+                                    // leave most of the 132 SMs idle and serialise the whole key loop in one dependency chain.)
 
 // qkv [n, 3f]: row = [ q (f) | k (f) | v (f) ], head h owns columns h*D .. h*D+D-1 of each part
 template <int D>

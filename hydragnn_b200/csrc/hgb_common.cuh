@@ -1,4 +1,4 @@
-// Shared helpers for libhgb.so (sm_100a).  See include/hgb.h for the C-ABI.
+// Shared helpers for libhgb.so (sm_90a).  See include/hgb.h for the C-ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -28,7 +28,7 @@ void hgb_count_launch(int n = 1);
     hgb_count_launch();                                                          \
   } while (0)
 
-#define HGB_NUM_SMS 148
+#define HGB_NUM_SMS 132   // H100 SXM
 
 static inline int hgb_grid_for(int64_t work_items, int per_block, int max_blocks = HGB_NUM_SMS * 16) {
   int64_t b = (work_items + per_block - 1) / per_block;

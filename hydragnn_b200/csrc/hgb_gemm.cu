@@ -2,7 +2,7 @@
 // activation backward, column sums.
 //
 // These are the fp32 "any shape" kernels used by every Linear on the path (M = nodes/edges/graphs is
-// large, N and K are small: 1..192).  The bf16 tensor-core (tcgen05) path for the hot shapes lives in
+// large, N and K are small: 1..192).  The bf16 tensor-core (wgmma) path for the hot shapes lives in
 // hgb_tc_linear.cu; this file is the exact-fp32 path and the fallback for odd shapes.
 #include "hgb_common.cuh"
 

@@ -1,21 +1,24 @@
-// libhgb.so -- tensor-core (tcgen05 / TMEM / TMA) dense layers for the large-M, small-N/K GEMMs of the
-// node/edge MLPs.  sm_100a only.
+// libhgb.so -- tensor-core (wgmma / TMA / mbarrier) dense layers for the large-M, small-N/K GEMMs of the
+// node/edge MLPs.  sm_90a only.
 //
 // Why TF32: activations live in HBM as fp32 (parameters are fp32 in every reference precision mode,
-// hydragnn/train/train_validate_test.py:43-49).  kind::tf32 consumes fp32 bit patterns straight from shared
+// hydragnn/train/train_validate_test.py:43-49).  wgmma .tf32 consumes fp32 bit patterns straight from shared
 // memory, so the activation tiles go HBM -> smem by TMA with no conversion pass, and the result (10-bit mantissa
-// products, fp32 accumulation in TMEM) is strictly more accurate than the bf16 autocast the reference runs
+// products, fp32 accumulation in registers) is strictly more accurate than the bf16 autocast the reference runs
 // under precision="bf16".  These GEMMs are memory-bound (AI ~ 12-24 FLOP/B), so TF32's half-rate is irrelevant.
 //
-// Three kernels:
+// Kernels:
 //   tc_linear_kernel  : Y[M,NO] = act(A[M,KR] . B^T + bias)   B = W (NO x KR, forward) or W^T (dgrad)
-//                       persistent, warp-specialised: warp0 = TMA producer, warp1 = MMA issuer (+TMEM alloc),
-//                       warps 2-5 = epilogue (TMEM -> registers -> bias/act -> global).  The weight operand is
-//                       staged once per CTA; the A tiles stream through a 2-4 stage mbarrier ring; two TMEM
-//                       accumulators let the epilogue of tile i overlap the MMAs of tile i+1.
-//   tc_wgrad_kernel   : dW[NO,KO] (+ db[NO]) = dZ[M,NO]^T . X[M,KO]: both operands MN-major straight from the
-//                       row-major tensors, reduction over M split across CTAs, per-CTA partials + deterministic
-//                       final reduce.  The bias gradient rides along as 16 extra "ones" columns of the B operand.
+//                       persistent, warp-specialised: warp 0 = TMA producer, warps 1-3 = splitters (fp32-accurate mode),
+//                       warpgroups 1 and 2 = consumers.  The weight operand is staged once per CTA (K-major, 128-byte
+//                       swizzle); 64-row A tiles stream through mbarrier rings; the two consumer warpgroups take
+//                       alternate tiles (ping-pong), each from its OWN ring, so the epilogue of one overlaps the wgmma of
+//                       the other and every barrier is waited on phase by phase by the one warpgroup that consumes it.
+//   tc_wgrad_kernel   : dW[NO,KO] (+ db[NO]) = dZ[M,NO]^T . X[M,KO], reduction over M split across CTAs, per-CTA partials +
+//                       deterministic final reduce.  TF32 wgmma wants both operands K-major (M contiguous), the tensors are
+//                       row-major: the TMA lands row slabs and the consumer warpgroups transpose them into a K-major buffer
+//                       (splitting into TF32 hi / lo in fp32-accurate mode) while the previous buffer is on the tensor cores.
+//                       The bias gradient rides along as 16 extra "ones" rows of the B operand.
 #include <cuda.h>
 
 #include "hgb_common.cuh"
@@ -51,8 +54,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1) {
   asm volatile(
@@ -62,69 +64,61 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       : "memory");
 }
 
-// smem tile -> global through the TMA engine (hardware-coalesced, clips rows/cols outside the tensor)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tmap, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(smem_u32(smem_src)), "r"(c0),
-               "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_read_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// ---- wgmma (warpgroup MMA: 4 warps, A and B from shared memory, D in registers) ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// warpgroup register reallocation: the producer warpgroup hands registers to the accumulator-holding consumers
+template <int R>
+__device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 64 K registers
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* holder, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(holder)), "r"(cols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int N>
+__device__ __forceinline__ void fence_regs(float* r) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols));
-}
-// D[tmem] (+)= A[smem desc] . B[smem desc]   (issued by ONE thread)
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+// D[64 x 32] += A[64 x 8] . B[32 x 8]^T, tf32 in, fp32 accumulate.  Fragment: d[4i + 2h + e] = D(16 w + lane/4 + 8h, 8i + 2(lane%4) + e)
+__device__ __forceinline__ void wgmma_n32(float* d, uint64_t ad, uint64_t bd) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %18, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(ad), "l"(bd), "r"(1));
 }
-// arrive on an mbarrier when all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread t <- lane base+t)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
+// D[64 x 16] += A[64 x 8] . B[16 x 8]^T
+__device__ __forceinline__ void wgmma_n16(float* d, uint64_t ad, uint64_t bd) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
-      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %10, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(ad), "l"(bd), "r"(1));
 }
 
-// shared-memory matrix descriptor, SWIZZLE_128B, version 1 (cute/arch/mma_sm100_desc.hpp SmemDescriptor)
-// layout_type: 2 = SWIZZLE_128B (16-B atoms; K-major operands), 1 = SWIZZLE_128B_BASE32B (32-B atoms; what UMMA
-// needs for MN-major 32-bit operands, cute Layout_MN_SW128_32B_Atom)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type = 2) {
+// shared-memory matrix descriptor of a K-major operand in the 128-byte swizzle: rows of 32 fp32 (128 B), 8-row groups 1024 B
+// apart (SBO); the k-step of 8 tf32 inside the swizzle atom is a 32-byte advance of the start address.  The operand base must be
+// 1024-byte aligned (the swizzle phase is taken from the address bits).
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version (Blackwell)
-  d |= (uint64_t)layout_type << 61;
+  d |= (uint64_t)1 << 16;                 // leading byte offset: unused by swizzled K-major operands
+  d |= (uint64_t)(1024 >> 4) << 32;       // stride byte offset
+  d |= (uint64_t)1 << 62;                 // SWIZZLE_128B
   return d;
-}
-// instruction descriptor: D = f32, A = B = tf32 (cute/arch/mma_sm100_desc.hpp InstrDescriptor)
-__host__ __device__ constexpr uint32_t make_idesc(int m, int n, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-         ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
 }
 
 // byte offset of element (r, c) of a K-major SWIZZLE_128B operand stored as column blocks of 32 fp32:
@@ -132,6 +126,15 @@ __host__ __device__ constexpr uint32_t make_idesc(int m, int n, int a_mn_major, 
 __device__ __forceinline__ uint32_t kmajor_sw128_off(int r, int c, int rows) {
   const int cb = c >> 5, cc = (c & 31) >> 2, j = c & 3;
   return (uint32_t)cb * rows * 128 + (uint32_t)(r >> 3) * 1024 + (uint32_t)(r & 7) * 128 + (uint32_t)((cc ^ (r & 7)) << 4) + j * 4;
+}
+
+// round to TF32 (10 mantissa bits), nearest, ties away from zero -- what cvt.rna.tf32.f32 does, as two full-rate integer
+// instructions (the splitters run this on every operand element)
+__device__ __forceinline__ float tf32_rna(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
+
+__device__ __forceinline__ void split_f4(const float4 v, float4& h, float4& l) {
+  h.x = tf32_rna(v.x); h.y = tf32_rna(v.y); h.z = tf32_rna(v.z); h.w = tf32_rna(v.w);
+  l.x = tf32_rna(v.x - h.x); l.y = tf32_rna(v.y - h.y); l.z = tf32_rna(v.z - h.z); l.w = tf32_rna(v.w - h.w);
 }
 
 struct LinParams {
@@ -149,142 +152,132 @@ struct LinParams {
   const float* gsrc;    // optional [m, no] (row stride ldy): the result is multiplied by act'(gsrc), i.e. this GEMM is the dgrad of a
   int gact;             //   layer whose INPUT was act(.): gsrc = saved pre-activation (SiLU) or activation output (others)
   int z_deriv;          // forward with a SiLU and z != NULL: z receives silu'(pre-activation) instead of the pre-activation
-  int stages;
-  int tmem_cols;
+  int stages;           // in total: two rings (one per consumer warpgroup) of stages / 2 each
   int split;            // 1: fp32-accurate mode -- every operand is split into a TF32 hi / lo pair and each k-step runs the three
-                        //    products hi*hi + lo*hi + hi*lo (3xTF32); four extra warps (10..13) split the A stages in shared memory
+                        //    products lo*hi + hi*lo + hi*hi (3xTF32); warps 1..3 split the A stages in shared memory
 };
 
-// round to TF32 (10 mantissa bits), nearest, ties away from zero -- what cvt.rna.tf32.f32 does, as two full-rate integer
-// instructions (the splitter warps run this on every operand element)
-__device__ __forceinline__ float tf32_rna(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
+constexpr int TILE_M = 64;                       // rows per tile = one wgmma M
+constexpr uint32_t A_STAGE = TILE_M * 128;       // one pipeline stage = one [64 x 32 fp32] k-block (8 KB)
+constexpr int LIN_THREADS = 384;
 
-constexpr int TILE_M = 128;
+// the epilogue of two adjacent outputs (row, col), (row, col + 1)
+__device__ __forceinline__ void lin_epilogue2(const LinParams& p, const float* sbias, int row, int col, float v0, float v1) {
+  if (row >= p.m) return;
+  const int64_t o = (int64_t)row * p.ldy + col;
+  v0 += sbias[col];
+  v1 += sbias[col + 1];
+  if (p.z && !(p.z_deriv && p.act == HGB_ACT_SILU)) *reinterpret_cast<float2*>(p.z + o) = make_float2(v0, v1);
+  switch (p.act) {
+    case HGB_ACT_NONE: break;
+    case HGB_ACT_RELU: v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); break;
+    case HGB_ACT_SILU:
+      if (p.z && p.z_deriv) {   // z receives silu'(pre) = s + y (1 - s): the backward then needs one multiply per element
+        const float s0 = __fdividef(1.f, 1.f + __expf(-v0)), s1 = __fdividef(1.f, 1.f + __expf(-v1));
+        v0 *= s0;
+        v1 *= s1;
+        *reinterpret_cast<float2*>(p.z + o) = make_float2(fmaf(v0, 1.f - s0, s0), fmaf(v1, 1.f - s1, s1));
+      } else {
+        v0 = __fdividef(v0, 1.f + __expf(-v0));
+        v1 = __fdividef(v1, 1.f + __expf(-v1));
+      }
+      break;
+    case HGB_ACT_TANH: v0 = tanhf(v0); v1 = tanhf(v1); break;
+    default: v0 = hgb_act(v0, p.act, p.act_param); v1 = hgb_act(v1, p.act, p.act_param);
+  }
+  if (p.addend) {
+    const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + o));
+    v0 += a.x;
+    v1 += a.y;
+  }
+  if (p.gsrc) {
+    const float2 g = __ldg(reinterpret_cast<const float2*>(p.gsrc + o));
+    if (p.gact == HGB_ACT_DERIV) {          // gsrc already holds act'(.)
+      v0 *= g.x;
+      v1 *= g.y;
+    } else {
+      v0 *= hgb_act_grad(g.x, g.x, p.gact, p.act_param);
+      v1 *= hgb_act_grad(g.y, g.y, p.gact, p.act_param);
+    }
+  }
+  *reinterpret_cast<float2*>(p.y + o) = make_float2(v0, v1);
+}
 
-__global__ void __launch_bounds__(448, 1) tc_linear_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_y,
-                                                           const __grid_constant__ CUtensorMap tmap_z, const LinParams p) {
+template <int NC, bool SPLIT>   // NO = 32 * NC output columns; SPLIT: the fp32-accurate mode
+__global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_constant__ CUtensorMap tmap_a, const LinParams p) {
+  constexpr int NO = NC * 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int KB = p.kr >> 5;
-  const int NO = p.no;
-  const uint32_t b_bytes = (uint32_t)KB * NO * 128;
-  constexpr uint32_t a_stage = TILE_M * 128;   // one pipeline stage = one [128 x 32 fp32] k-block (16 KB)
-  const uint32_t b_pad = (b_bytes + 1023) & ~1023u;
+  const uint32_t b_pad = ((uint32_t)KB * NO * 128 + 1023) & ~1023u;
   uint8_t* sB = smem;
   uint8_t* sBlo = sB + b_pad;                                 // split mode only
-  uint8_t* sA = sB + (p.split ? 2 : 1) * (size_t)b_pad;
+  uint8_t* sA = sB + (SPLIT ? 2 : 1) * (size_t)b_pad;
   const int S = p.stages;
-  uint8_t* sAlo = sA + (size_t)S * a_stage;                   // split mode only
-  uint8_t* sOut = sA + (size_t)(p.split ? 2 : 1) * S * a_stage;   // 8 epilogue warps x 2 staging tiles x 4 KB (1024-aligned)
-  uint64_t* full = reinterpret_cast<uint64_t*>(sOut + 8 * 2 * 4096);
+  const int SR = S >> 1;                                      // stages per ring: stage (r * SR + slot) belongs to ring r
+  uint8_t* sAlo = sA + (size_t)S * A_STAGE;                   // split mode only
+  uint64_t* full = reinterpret_cast<uint64_t*>(sA + (size_t)(SPLIT ? 2 : 1) * S * A_STAGE);
   uint64_t* empty = full + S;
-  uint64_t* full2 = empty + S;                                // split mode: "stage s is split" (4 splitter warps arrive)
-  uint64_t* tfull = full2 + S;
-  uint64_t* tempty = tfull + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tempty + 2);
-  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_holder + 4) + 15) & ~(uintptr_t)15);   // [NO], 16-byte aligned
+  uint64_t* full2 = empty + S;                                // split mode: "stage s is split" (3 splitter warps arrive)
+  float* sbias = reinterpret_cast<float*>(full2 + S);         // [NO]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ntiles = (p.m + TILE_M - 1) / TILE_M;
   for (int i = threadIdx.x; i < NO; i += blockDim.x) sbias[i] = p.bias ? __ldg(p.bias + i) : 0.f;
-
-  // ---- one-time setup -------------------------------------------------------------------------------
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); mbar_init(full2 + s, 4); }
-    for (int a = 0; a < 2; ++a) { mbar_init(tfull + a, 1); mbar_init(tempty + a, 8); }
+    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 4); mbar_init(full2 + s, 3); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_holder, (uint32_t)p.tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  const uint32_t idesc = make_idesc(TILE_M, NO, 0, 0);
 
-  if (warp >= 10) {
-    // ===== splitter warps (split mode only; the launch has 320 threads otherwise): as soon as the TMA has landed stage s, rewrite it
-    // in place as the TF32 "hi" part and put the "lo" remainder at the same (swizzled) offsets of the twin buffer, then release the
-    // stage to the MMA warp.  Elementwise on 16 KB: 8 float4 per thread. =====
-    int s = 0;
-    uint32_t ph = 0;
-    const int tl = threadIdx.x - 320;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x)
-      for (int kb = 0; kb < KB; ++kb) {
-        mbar_wait(full + s, ph);
-        float4* pa = reinterpret_cast<float4*>(sA + (size_t)s * a_stage);
-        float4* pl = reinterpret_cast<float4*>(sAlo + (size_t)s * a_stage);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int idx = i * 128 + tl;
-          const float4 v = pa[idx];
-          float4 h, l;
-          h.x = tf32_rna(v.x); h.y = tf32_rna(v.y); h.z = tf32_rna(v.z); h.w = tf32_rna(v.w);
-          l.x = tf32_rna(v.x - h.x); l.y = tf32_rna(v.y - h.y); l.z = tf32_rna(v.z - h.z); l.w = tf32_rna(v.w - h.w);
-          pa[idx] = h;
-          pl[idx] = l;
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full2 + s);
-        if (++s == S) { s = 0; ph ^= 1; }
-      }
-  } else
-  if (warp == 0) {
-    // ===== TMA producer =====
+  if (warp < 4) {
+    regs_dec<PRODUCER_REGS>();
+    if (warp == 0) {
+    // ===== TMA producer: the A k-blocks of this CTA's tiles, in order; local tile li goes to ring li & 1 (its consumer's) =====
     if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      for (int t = blockIdx.x; t < ntiles; t += gridDim.x)
+      uint32_t li = 0;
+      for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++li)
         for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(empty + s, ph ^ 1);
-          mbar_expect_tx(full + s, a_stage);
-          tma_load_2d(sA + (size_t)s * a_stage, &tmap_a, full + s, kb * 32, t * TILE_M);
-          if (++s == S) { s = 0; ph ^= 1; }
+          const uint32_t n = (li >> 1) * KB + kb;             // item index within the ring
+          const int s = (li & 1) * SR + n % SR;
+          mbar_wait(empty + s, ((n / SR) & 1) ^ 1);
+          mbar_expect_tx(full + s, A_STAGE);
+          tma_load_2d(sA + (size_t)s * A_STAGE, &tmap_a, full + s, kb * 32, t * TILE_M);
         }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====  (waits until warps 2..9 have staged the weight operand; the TMA producer does not)
-    asm volatile("bar.sync 1, 288;" ::: "memory");
-    tc_fence_after();
-    if (lane == 0) {
-      int s = 0, acc = 0;
-      uint32_t ph = 0, aph = 0;
-      const uint32_t sA_addr = smem_u32(sA), sB_addr = smem_u32(sB);
-      for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-        mbar_wait(tempty + acc, aph ^ 1);
-        tc_fence_after();
-        const uint32_t d_addr = tmem_base + (uint32_t)acc * NO;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(p.split ? full2 + s : full + s, ph);
-          tc_fence_after();
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4) {
-            const uint64_t ad = make_desc(sA_addr + s * a_stage + k4 * 32, 16, 1024);
-            const uint64_t bd = make_desc(sB_addr + kb * NO * 128 + k4 * 32, 16, 1024);
-            if (p.split) {      // small terms first: lo*hi + hi*lo + hi*hi
-              const uint64_t adl = make_desc(smem_u32(sAlo) + s * a_stage + k4 * 32, 16, 1024);
-              const uint64_t bdl = make_desc(smem_u32(sBlo) + kb * NO * 128 + k4 * 32, 16, 1024);
-              umma_tf32(d_addr, adl, bd, idesc, (kb | k4) != 0);
-              umma_tf32(d_addr, ad, bdl, idesc, 1);
-              umma_tf32(d_addr, ad, bd, idesc, 1);
-            } else {
-              umma_tf32(d_addr, ad, bd, idesc, (kb | k4) != 0);
-            }
+    } else {
+    // ===== splitters (split mode only): as soon as the TMA has landed stage s, rewrite it in place as the TF32 "hi" part and put the
+    // "lo" remainder at the same (swizzled) offsets of the twin buffer, then release the stage to its consumer =====
+    if (SPLIT) {
+      const int tl = threadIdx.x - 32;
+      uint32_t li = 0;
+      for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++li)
+        for (int kb = 0; kb < KB; ++kb) {                     // every item of both rings, in the producer's order
+          const uint32_t n = (li >> 1) * KB + kb;
+          const int s = (li & 1) * SR + n % SR;
+          mbar_wait(full + s, (n / SR) & 1);
+          float4* pa = reinterpret_cast<float4*>(sA + (size_t)s * A_STAGE);
+          float4* pl = reinterpret_cast<float4*>(sAlo + (size_t)s * A_STAGE);
+          for (int idx = tl; idx < (int)(A_STAGE / 16); idx += 96) {
+            float4 h, l;
+            split_f4(pa[idx], h, l);
+            pa[idx] = h;
+            pl[idx] = l;
           }
-          umma_commit(empty + s);    // smem stage free once these MMAs have read it
-          if (++s == S) { s = 0; ph ^= 1; }
+          fence_proxy_async();
+          __syncwarp();
+          if (lane == 0) mbar_arrive(full2 + s);
         }
-        umma_commit(tfull + acc);    // accumulator ready for the epilogue
-        if (++acc == 2) { acc = 0; aph ^= 1; }
-      }
+    }
     }
   } else {
-    // ===== warps 2..9: first stage the weight operand into its K-major SWIZZLE_128B layout (generic-proxy stores made
-    // visible to the async proxy), release the MMA warp, then run the epilogue =====
+    regs_inc<CONSUMER_REGS>();
+    // ===== consumer warpgroups: stage the weight operand into its K-major SWIZZLE_128B layout (generic-proxy stores made visible to the
+    // async proxy), then run wgmma + epilogue on alternate tiles =====
     {
       const int total = NO * p.kr;
       constexpr int SU = 8;   // independent loads in flight per thread: the staging is latency-, not bandwidth-limited
-      for (int base = threadIdx.x - 64; base < total; base += 256 * SU) {
+      for (int base = threadIdx.x - 128; base < total; base += 256 * SU) {
         float val[SU];
         uint32_t off[SU];
 #pragma unroll
@@ -307,7 +300,7 @@ __global__ void __launch_bounds__(448, 1) tc_linear_kernel(const __grid_constant
 #pragma unroll
         for (int u = 0; u < SU; ++u)
           if (off[u] != 0xffffffffu) {
-            if (p.split) {
+            if (SPLIT) {
               const float hi = tf32_rna(val[u]);
               *reinterpret_cast<float*>(sB + off[u]) = hi;
               *reinterpret_cast<float*>(sBlo + off[u]) = tf32_rna(val[u] - hi);
@@ -318,118 +311,61 @@ __global__ void __launch_bounds__(448, 1) tc_linear_kernel(const __grid_constant
       }
       fence_proxy_async();
     }
-    asm volatile("bar.arrive 1, 288;" ::: "memory");
-    // ===== epilogue.  Warp w may only touch TMEM lanes 32*(w%4)..+31; the two warps that share a lane
-    // quarter split the 32-column chunks between them (even / odd chunk index). =====
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    int stile = 0;
-    int acc = 0;
-    uint32_t aph = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
-      mbar_wait(tfull + acc, aph);
-      tc_fence_after();
-      const int row = t * TILE_M + q * 32 + lane;
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)acc * NO;
-      uint8_t* stz = sOut + (size_t)(warp - 2) * 8192;          // this warp's staging tiles: [0] pre-activation, [1] output
-      uint8_t* sty = stz + 4096;                                //   (no pre-activation wanted: both hold outputs, alternately)
-      const int row0 = t * TILE_M + q * 32;
-      for (int c0 = half * 32; c0 < NO; c0 += 64) {
-        if (!p.z) { sty = stz + (stile & 1) * 4096; ++stile; }
-        float v[32];
-        tmem_ld32(taddr + c0, v);
-        {
-          const float4* bp = reinterpret_cast<const float4*>(sbias + c0);
+    named_bar_sync(1, 256);
+    const int cw = (warp - 4) >> 2;     // consumer warpgroup: takes local tiles cw, cw + 2, ... from ring cw, every item in order
+    const int wq = warp & 3;            // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of the tile
+    const uint32_t sA_addr = smem_u32(sA), sAlo_addr = smem_u32(sAlo), sB_addr = smem_u32(sB), sBlo_addr = smem_u32(sBlo);
+    float acc[NC][16];
+    int li = cw;
+    for (int t = blockIdx.x + cw * gridDim.x; t < ntiles; t += 2 * gridDim.x, li += 2) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 b4 = bp[j];
-            v[4 * j] += b4.x; v[4 * j + 1] += b4.y; v[4 * j + 2] += b4.z; v[4 * j + 3] += b4.w;
-          }
-        }
-        if (lane == 0) {                                      // the store that last read this tile has finished reading it
-          if (p.z) tma_store_wait_read(); else tma_store_wait_read_1();
-        }
-        __syncwarp();
-        if (p.z && !(p.z_deriv && p.act == HGB_ACT_SILU)) {
+      for (int c = 0; c < NC; ++c)
 #pragma unroll
-          for (int j = 0; j < 8; ++j)   // SWIZZLE_128B tile: 16-byte chunk j of row `lane` lives at chunk j ^ (lane & 7)
-            *reinterpret_cast<float4*>(stz + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        }
-        switch (p.act) {     // hoisted out of the element loop: one specialised, fully unrolled loop per activation
-          case HGB_ACT_NONE: break;
-          case HGB_ACT_RELU:
+        for (int j = 0; j < 16; ++j) acc[c][j] = 0.f;
+      const uint32_t n0 = (uint32_t)(li >> 1) * KB;             // first item of this tile within ring cw
+      for (int kb = 0; kb < KB; ++kb) {
+        const uint32_t n = n0 + kb;
+        const int s = cw * SR + n % SR;
+        mbar_wait(SPLIT ? full2 + s : full + s, (n / SR) & 1);
+        fence_regs<NC * 16>(&acc[0][0]);
+        wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-            break;
-          case HGB_ACT_SILU:
-            if (p.z && p.z_deriv) {   // z receives silu'(pre) = s + y (1 - s): the backward then needs one multiply per element
-              float d[32];
+        for (int k4 = 0; k4 < 4; ++k4) {
+          const uint64_t ad = make_desc(sA_addr + s * A_STAGE + k4 * 32);
+          const uint64_t adl = make_desc(sAlo_addr + s * A_STAGE + k4 * 32);
 #pragma unroll
-              for (int j = 0; j < 32; ++j) {
-                const float sg = __fdividef(1.f, 1.f + __expf(-v[j]));
-                v[j] *= sg;
-                d[j] = fmaf(v[j], 1.f - sg, sg);
-              }
-#pragma unroll
-              for (int j = 0; j < 8; ++j)
-                *reinterpret_cast<float4*>(stz + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]);
-            } else {
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = __fdividef(v[j], 1.f + __expf(-v[j]));
+          for (int c = 0; c < NC; ++c) {
+            const uint32_t boff = (uint32_t)kb * NO * 128 + c * 4096 + k4 * 32;
+            const uint64_t bd = make_desc(sB_addr + boff);
+            if (SPLIT) {        // small terms first: lo*hi + hi*lo + hi*hi
+              wgmma_n32(acc[c], adl, bd);
+              wgmma_n32(acc[c], ad, make_desc(sBlo_addr + boff));
             }
-            break;
-          case HGB_ACT_TANH:
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = tanhf(v[j]);
-            break;
-          default:
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = hgb_act(v[j], p.act, p.act_param);
-        }
-        if (p.addend && row < p.m) {
-          const float4* ap = reinterpret_cast<const float4*>(p.addend + (int64_t)row * p.ldy + c0);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 a4 = __ldg(ap + j);
-            v[4 * j] += a4.x; v[4 * j + 1] += a4.y; v[4 * j + 2] += a4.z; v[4 * j + 3] += a4.w;
+            wgmma_n32(acc[c], ad, bd);
           }
         }
-        if (p.gsrc && row < p.m) {
-          const float4* gp = reinterpret_cast<const float4*>(p.gsrc + (int64_t)row * p.ldy + c0);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 g4 = __ldg(gp + j);
-            if (p.gact == HGB_ACT_DERIV) {          // gsrc already holds act'(.)
-              v[4 * j] *= g4.x; v[4 * j + 1] *= g4.y; v[4 * j + 2] *= g4.z; v[4 * j + 3] *= g4.w;
-            } else {
-              v[4 * j] *= hgb_act_grad(g4.x, g4.x, p.gact, p.act_param);
-              v[4 * j + 1] *= hgb_act_grad(g4.y, g4.y, p.gact, p.act_param);
-              v[4 * j + 2] *= hgb_act_grad(g4.z, g4.z, p.gact, p.act_param);
-              v[4 * j + 3] *= hgb_act_grad(g4.w, g4.w, p.gact, p.act_param);
-            }
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<float4*>(sty + lane * 128 + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          if (p.z) tma_store_2d(&tmap_z, stz, c0, row0);
-          tma_store_2d(&tmap_y, sty, c0, row0);
-          tma_store_commit();
+        wgmma_commit();
+        fence_regs<NC * 16>(&acc[0][0]);
+        if (kb > 0) {                   // the MMAs of the previous k-block have read their stage: release it
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(empty + cw * SR + (n - 1) % SR);
         }
       }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty + acc);
-      if (++acc == 2) { acc = 0; aph ^= 1; }
+      wgmma_wait<0>();
+      fence_regs<NC * 16>(&acc[0][0]);
+      if (lane == 0) mbar_arrive(empty + cw * SR + (n0 + KB - 1) % SR);
+      // ===== epilogue straight from the accumulator registers =====
+      const int r0 = t * TILE_M + wq * 16 + (lane >> 2);
+#pragma unroll
+      for (int c = 0; c < NC; ++c)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int col = c * 32 + i * 8 + 2 * (lane & 3);
+          lin_epilogue2(p, sbias, r0, col, acc[c][4 * i], acc[c][4 * i + 1]);
+          lin_epilogue2(p, sbias, r0 + 8, col, acc[c][4 * i + 2], acc[c][4 * i + 3]);
+        }
     }
-    if (lane == 0) tma_store_wait_all();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -437,189 +373,188 @@ __global__ void __launch_bounds__(448, 1) tc_linear_kernel(const __grid_constant
 // ------------------------------------------------------------------------------------------------
 struct WgParams {
   int m, no, ko;
-  int chunks_per_cta;   // number of `rows`-row chunks each CTA reduces
-  int stages;
-  int tmem_cols;
-  int mblocks;          // ceil(no / 128)
-  int nmma;             // ko + 16 (ones columns for the bias gradient)
-  int rows;             // rows of dZ / X per pipeline stage (a multiple of 8: one MMA k-step = 8 rows): 32, or 16 when the stage is big
-  int split;            // 1: fp32-accurate mode -- both operands are split into TF32 hi / lo twins in shared memory (warps 2..5, before
-                        //    they turn into the epilogue) and every k-step runs hi*hi + lo*hi + hi*lo
-  int nhh;              // split mode: TMEM accumulators the hi*hi products rotate through (the two cross terms own one more).  The
-                        //    tensor core truncates when it adds into the accumulator, so short chains of large terms keep the sum accurate
+  int chunks_per_cta;   // number of 32-row chunks each CTA reduces
+  int stages;           // TMA ring of raw row slabs
+  int tbufs;            // K-major (transposed) operand buffers: 2 = transposition of chunk c+1 overlaps the MMAs of chunk c
+  int split;            // 1: fp32-accurate mode -- both operands are split into TF32 hi / lo twins and every k-step runs lo*hi + hi*lo + hi*hi
+  int flush;            // > 0: the register accumulators are added into the partial every `flush` chunks and restarted, so each chain
+                        //   of tensor-core additions stays short (the fp32-accurate mode)
   float* part;          // [gridDim.x, no, ko + 1]
 };
 
-__device__ __forceinline__ void split_f4(float4* hi_p, float4* lo_p) {
-  const float4 v = *hi_p;
-  float4 h, l;
-  h.x = tf32_rna(v.x); h.y = tf32_rna(v.y); h.z = tf32_rna(v.z); h.w = tf32_rna(v.w);
-  l.x = tf32_rna(v.x - h.x); l.y = tf32_rna(v.y - h.y); l.z = tf32_rna(v.z - h.z); l.w = tf32_rna(v.w - h.w);
-  *hi_p = h;
-  *lo_p = l;
-}
+constexpr int WG_ROWS = 32;                      // rows of dZ / X per chunk = one 128-byte K-major row of the transposed operands
+constexpr int WG_NA = 128;                       // rows of dW per CTA (two consumer warpgroups x 64)
+constexpr int WG_THREADS = 384;                  // 2 consumer warpgroups + 1 producer warpgroup (one warp issues the TMA)
 
-__global__ void __launch_bounds__(320, 1) tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz,
-                                                          const __grid_constant__ CUtensorMap tmap_x, const WgParams p) {
+template <int Q, bool SPLIT>    // KO = 32 * Q; SPLIT: the fp32-accurate mode
+__global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz,
+                                                                 const __grid_constant__ CUtensorMap tmap_x, const WgParams p) {
+  constexpr int KO = 32 * Q, NB = KO + 16;
+  constexpr uint32_t SLAB = WG_ROWS * 128;       // one [32 rows x 32 fp32] TMA box
+  constexpr uint32_t HI_BYTES = (uint32_t)(WG_NA + NB) * 128;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  const int R = p.rows;
-  const uint32_t CH = (uint32_t)R * 128;       // one [R x 32 fp32] slab
-  const int a_chunks = p.mblocks * 4;          // allocated MN slabs of the A operand (>= no/32; the tail is never read back)
-  const int b_chunks = (p.ko >> 5) + 1;        // + the ones slab
-  const uint32_t hi_bytes = (uint32_t)(a_chunks + b_chunks) * CH;
-  const uint32_t lo_bytes = p.split ? (uint32_t)(a_chunks + (p.ko >> 5)) * CH : 0u;   // lo twins (the ones slab has none: lo(1) = 0)
-  const uint32_t stage_bytes = hi_bytes + lo_bytes;
-  const int S = p.stages;
-  uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)S * stage_bytes);
+  const int n0 = blockIdx.y * WG_NA;
+  const int nrows = min(WG_NA, p.no - n0);
+  const int nsl = nrows >> 5;
+  const uint32_t raw_bytes = (uint32_t)(nsl + Q) * SLAB;
+  const uint32_t tb_bytes = HI_BYTES * (SPLIT ? 2 : 1);
+  const int S = p.stages, T = p.tbufs;
+  uint8_t* tbuf = smem;                                   // T x [A hi (128 rows) | B hi (NB rows) | A lo | B lo]
+  uint8_t* raw = smem + (size_t)T * tb_bytes;             // S x [nsl dZ slabs | Q X slabs], row-major as loaded
+  uint64_t* full = reinterpret_cast<uint64_t*>(raw + (size_t)S * raw_bytes);
   uint64_t* empty = full + S;
-  uint64_t* full2 = empty + S;                 // split mode: "stage s is split" (the four splitter warps arrive)
-  uint64_t* done = full2 + S;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(done + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  const int total_chunks = (p.m + R - 1) / R;
+  const int total_chunks = (p.m + WG_ROWS - 1) / WG_ROWS;
   const int c_beg = blockIdx.x * p.chunks_per_cta;
-  const int c_end = min(total_chunks, c_beg + p.chunks_per_cta);
-  const int nchunks = max(0, c_end - c_beg);
-  const int KS = R >> 3;                       // MMA k-steps per stage
+  const int nchunks = max(0, min(total_chunks, c_beg + p.chunks_per_cta) - c_beg);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 1); mbar_init(full2 + s, (blockDim.x >> 5) - 2); }
-    mbar_init(done, 1);
+    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 8); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_holder, (uint32_t)p.tmem_cols);
-  // ones slab of every stage (all elements equal, so the swizzle does not matter)
-  for (int s = 0; s < S; ++s) {
-    float* ones = reinterpret_cast<float*>(smem + (size_t)s * stage_bytes + (size_t)(a_chunks + b_chunks - 1) * CH);
-    for (int i = threadIdx.x; i < (int)(CH / 4); i += blockDim.x) ones[i] = 1.0f;
+  // transposed buffers: A rows >= nrows stay zero, B rows KO.. are the ones rows (lo twins: zero); everything else is rewritten per chunk
+  for (int i = threadIdx.x; i < (int)(T * tb_bytes / 4); i += blockDim.x) {
+    const uint32_t o = (uint32_t)i * 4 % tb_bytes;
+    const bool lo = o >= HI_BYTES;
+    const int row = (int)((lo ? o - HI_BYTES : o) / 128);
+    reinterpret_cast<float*>(tbuf)[i] = (!lo && row >= WG_NA + KO) ? 1.f : 0.f;
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  const uint32_t idesc = make_idesc(128, p.nmma, 1, 1);
-  const uint32_t idesc_ko = make_idesc(128, p.ko, 1, 1);     // hi(dZ) * lo(X): no ones columns
-  const uint32_t tx_bytes = (uint32_t)((p.no >> 5) + (p.ko >> 5)) * CH;
-  const int nused = min(p.nhh, nchunks * KS);                // hi*hi accumulators this CTA really wrote
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
+  if (warp >= 8) {
+    // ===== TMA producer: this CTA's dZ columns n0.. and all of X, 32 rows per chunk =====
+    regs_dec<PRODUCER_REGS>();
+    if (warp == 8 && lane == 0) {
       for (int c = 0; c < nchunks; ++c) {
-        mbar_wait(empty + s, ph ^ 1);
-        mbar_expect_tx(full + s, tx_bytes);
-        uint8_t* st = smem + (size_t)s * stage_bytes;
-        const int row0 = (c_beg + c) * R;
-        for (int j = 0; j < (p.no >> 5); ++j) tma_load_2d(st + (size_t)j * CH, &tmap_dz, full + s, j * 32, row0);
-        for (int j = 0; j < (p.ko >> 5); ++j) tma_load_2d(st + (size_t)(a_chunks + j) * CH, &tmap_x, full + s, j * 32, row0);
-        if (++s == S) { s = 0; ph ^= 1; }
+        const int s = c % S;
+        mbar_wait(empty + s, ((c / S) & 1) ^ 1);
+        mbar_expect_tx(full + s, raw_bytes);
+        uint8_t* st = raw + (size_t)s * raw_bytes;
+        const int row0 = (c_beg + c) * WG_ROWS;
+        for (int j = 0; j < nsl; ++j) tma_load_2d(st + (size_t)j * SLAB, &tmap_dz, full + s, n0 + j * 32, row0);
+        for (int j = 0; j < Q; ++j) tma_load_2d(st + (size_t)(nsl + j) * SLAB, &tmap_x, full + s, j * 32, row0);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int s = 0;
-      uint32_t ph = 0;
-      const uint32_t base = smem_u32(smem);
-      int it = 0;                                // running k-step of this CTA
-      for (int c = 0; c < nchunks; ++c) {
-        mbar_wait(p.split ? full2 + s : full + s, ph);
-        tc_fence_after();
-        const uint32_t st = base + s * stage_bytes;
-        for (int ks = 0; ks < KS; ++ks, ++it) {
-          const uint64_t bd = make_desc(st + a_chunks * CH + ks * 1024, CH, 512, 1);
-          if (!p.split) {
-            for (int mb = 0; mb < p.mblocks; ++mb) {
-              const uint64_t ad = make_desc(st + mb * 4 * CH + ks * 1024, CH, 512, 1);
-              umma_tf32(tmem_base + (uint32_t)mb * p.nmma, ad, bd, idesc, it != 0);
-            }
-          } else {
-            const uint64_t bdl = make_desc(st + hi_bytes + a_chunks * CH + ks * 1024, CH, 512, 1);
-            const int a = it % p.nhh;
-            for (int mb = 0; mb < p.mblocks; ++mb) {
-              const uint64_t ad = make_desc(st + mb * 4 * CH + ks * 1024, CH, 512, 1);
-              const uint64_t adl = make_desc(st + hi_bytes + mb * 4 * CH + ks * 1024, CH, 512, 1);
-              const uint32_t d_hh = tmem_base + (uint32_t)(a * p.mblocks + mb) * p.nmma;
-              const uint32_t d_x = tmem_base + (uint32_t)(p.nhh * p.mblocks + mb) * p.nmma;
-              umma_tf32(d_x, adl, bd, idesc, it != 0);          // lo(dZ) * hi(X | 1)
-              umma_tf32(d_x, ad, bdl, idesc_ko, 1);             // hi(dZ) * lo(X)
-              umma_tf32(d_hh, ad, bd, idesc, it >= p.nhh);      // hi * hi (first use of an accumulator overwrites it)
-            }
-          }
-        }
-        umma_commit(empty + s);
-        if (++s == S) { s = 0; ph ^= 1; }
-      }
-      umma_commit(done);
-    }
-  } else {
-    if (p.split) {
-      // splitter: rewrite the landed stage as TF32 hi (in place) + lo (same swizzled offsets of the twin region)
-      int s = 0;
-      uint32_t ph = 0;
-      const int tl = threadIdx.x - 64, nt = blockDim.x - 64;       // warps 2.. (the launch has 8 of them in split mode)
-      const int nA4 = (p.no >> 5) * (int)(CH / 16), nB4 = (p.ko >> 5) * (int)(CH / 16);
-      for (int c = 0; c < nchunks; ++c) {
-        mbar_wait(full + s, ph);
-        uint8_t* st = smem + (size_t)s * stage_bytes;
-        float4* ah = reinterpret_cast<float4*>(st);
-        float4* al = reinterpret_cast<float4*>(st + hi_bytes);
-        for (int i = tl; i < nA4; i += nt) split_f4(ah + i, al + i);
-        float4* bh = reinterpret_cast<float4*>(st + (size_t)a_chunks * CH);
-        float4* bl = reinterpret_cast<float4*>(st + hi_bytes + (size_t)a_chunks * CH);
-        for (int i = tl; i < nB4; i += nt) split_f4(bh + i, bl + i);
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full2 + s);
-        if (++s == S) { s = 0; ph ^= 1; }
-      }
-    }
-    // epilogue (warps 2..5, one per TMEM lane quarter): after the whole reduction, dump this CTA's partial
-    const int q = warp & 3;
-    if (warp < 6) {
-    mbar_wait(done, 0);
-    tc_fence_after();
-    float* part = p.part + (size_t)blockIdx.x * p.no * (p.ko + 1);
-    for (int mb = 0; mb < p.mblocks; ++mb) {
-      const int row = mb * 128 + q * 32 + lane;   // output row = weight row n
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)mb * p.nmma;
-      for (int c0 = 0; c0 < p.nmma; c0 += 32) {   // nmma = ko + 16: the last piece is read 32 wide and masked
-        float v[32];
-        tmem_ld32(taddr + c0, v);
-        if (p.split) {                            // sum of the accumulators, the two cross terms last (ordinary fp32 adds)
-          float t[32];
-          for (int a = 1; a < nused; ++a) {
-            tmem_ld32(taddr + (uint32_t)(a * p.mblocks) * p.nmma + c0, t);
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] += t[j];
-          }
-          tmem_ld32(taddr + (uint32_t)(p.nhh * p.mblocks) * p.nmma + c0, t);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += t[j];
-        }
-        if (row < p.no && nchunks > 0) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int col = c0 + j;
-            if (col <= p.ko) part[(size_t)row * (p.ko + 1) + col] = v[j];   // col == ko is the bias gradient
-          }
-        } else if (row < p.no) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int col = c0 + j;
-            if (col <= p.ko) part[(size_t)row * (p.ko + 1) + col] = 0.f;
-          }
-        }
-      }
-    }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
+
+  // ===== consumer warpgroups (threads 0..255): transpose, then wgmma; warpgroup wg owns dW rows n0 + 64 wg .. +63 =====
+  regs_inc<CONSUMER_REGS>();
+  const int wg = warp >> 2, wq = warp & 3;
+  const bool mma_on = wg * 64 < nrows;
+  const int rows_t = nsl * 32 + KO;                       // operand rows to transpose per chunk
+  float acc[Q][16], accb[8];
+#pragma unroll
+  for (int c = 0; c < Q; ++c)
+#pragma unroll
+    for (int j = 0; j < 16; ++j) acc[c][j] = 0.f;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) accb[j] = 0.f;
+  bool first = true;
+  float* part = p.part + (size_t)blockIdx.x * p.no * (p.ko + 1);
+
+  auto flush = [&]() {   // partial (+)= accumulators; accumulators restart at zero
+    if (mma_on) {
+      const int rb = n0 + wg * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = rb + 8 * h;
+        if (row < n0 + nrows) {
+          float* pr = part + (size_t)row * (KO + 1);
+#pragma unroll
+          for (int c = 0; c < Q; ++c)
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int col = c * 32 + i * 8 + 2 * (lane & 3) + e;
+                const float v = acc[c][4 * i + 2 * h + e];
+                pr[col] = first ? v : pr[col] + v;
+              }
+          if ((lane & 3) == 0) pr[KO] = first ? accb[2 * h] : pr[KO] + accb[2 * h];   // ones column KO: the bias gradient
+        }
+      }
+    }
+    first = false;
+#pragma unroll
+    for (int c = 0; c < Q; ++c)
+#pragma unroll
+      for (int j = 0; j < 16; ++j) acc[c][j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) accb[j] = 0.f;
+  };
+
+  for (int c = 0; c < nchunks; ++c) {
+    const int s = c % S;
+    uint8_t* tb = tbuf + (size_t)(c % T) * tb_bytes;
+    const uint8_t* st = raw + (size_t)s * raw_bytes;
+    mbar_wait(full + s, (c / S) & 1);
+    // transpose: operand row r (A: dZ column n0 + r; B: X column r - nrows) gets the 32 values of this chunk as one K-major 128-byte
+    // row; each item is 4 consecutive m of one row (four conflict-free column reads, one swizzled 16-byte store)
+    for (int it = threadIdx.x; it < rows_t * 8; it += 256) {
+      const int r = it % rows_t, m4 = it / rows_t;
+      const int slab = r < nrows ? r >> 5 : nsl + ((r - nrows) >> 5);
+      const float* src = reinterpret_cast<const float*>(st + (size_t)slab * SLAB) + (r & 31) + m4 * 4 * 32;
+      const float4 v = make_float4(src[0], src[32], src[64], src[96]);
+      const int orow = r < nrows ? r : WG_NA + (r - nrows);
+      const uint32_t off = (uint32_t)orow * 128 + ((m4 ^ (orow & 7)) << 4);
+      if (SPLIT) {
+        float4 h, l;
+        split_f4(v, h, l);
+        *reinterpret_cast<float4*>(tb + off) = h;
+        *reinterpret_cast<float4*>(tb + HI_BYTES + off) = l;
+      } else {
+        *reinterpret_cast<float4*>(tb + off) = v;
+      }
+    }
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty + s);               // the raw slabs are no longer needed
+    named_bar_sync(1, 256);                              // the transposed chunk is complete
+    if (mma_on) {
+      const uint32_t ta = smem_u32(tb);
+      fence_regs<Q * 16>(&acc[0][0]);
+      fence_regs<8>(accb);
+      wgmma_fence();
+#pragma unroll
+      for (int k4 = 0; k4 < 4; ++k4) {
+        const uint32_t aoff = (uint32_t)(wg * 64) * 128 + k4 * 32;
+        const uint64_t ad = make_desc(ta + aoff), adl = make_desc(ta + HI_BYTES + aoff);
+#pragma unroll
+        for (int j = 0; j < Q; ++j) {
+          const uint32_t boff = (uint32_t)WG_NA * 128 + (uint32_t)j * 4096 + k4 * 32;
+          const uint64_t bd = make_desc(ta + boff);
+          if (SPLIT) {                                   // small terms first: lo*hi + hi*lo + hi*hi
+            wgmma_n32(acc[j], adl, bd);
+            wgmma_n32(acc[j], ad, make_desc(ta + HI_BYTES + boff));
+          }
+          wgmma_n32(acc[j], ad, bd);
+        }
+        const uint64_t bones = make_desc(ta + (uint32_t)(WG_NA + KO) * 128 + k4 * 32);   // the 16 ones rows (lo(1) = 0: no hi*lo term)
+        if (SPLIT) wgmma_n16(accb, adl, bones);
+        wgmma_n16(accb, ad, bones);
+      }
+      wgmma_commit();
+      fence_regs<Q * 16>(&acc[0][0]);
+      fence_regs<8>(accb);
+    }
+    // the buffer transposed next must no longer be read by either warpgroup's MMAs
+    if (T == 2) wgmma_wait<1>(); else wgmma_wait<0>();
+    if (p.flush && (c + 1) % p.flush == 0 && c + 1 < nchunks) {
+      wgmma_wait<0>();
+      fence_regs<Q * 16>(&acc[0][0]);
+      fence_regs<8>(accb);
+      flush();
+    }
+    named_bar_sync(2, 256);
+  }
+  wgmma_wait<0>();
+  fence_regs<Q * 16>(&acc[0][0]);
+  fence_regs<8>(accb);
+  flush();                                                // (a CTA without chunks writes zeros)
 }
 
 // 32 outputs x 8 partial-walkers per block; fixed summation order
@@ -674,9 +609,8 @@ EncodeTiledFn get_encode() {
   return fn;
 }
 
-// 2-D fp32 row-major tensor [rows, cols] with row stride ld (elements); box = [box_rows x 32 cols], 128B swizzle
-int make_tmap(CUtensorMap* tm, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows,
-              CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+// 2-D fp32 row-major tensor [rows, cols] with row stride ld (elements); box = [box_rows x 32 cols]
+int make_tmap(CUtensorMap* tm, const float* base, int64_t rows, int64_t cols, int64_t ld, int box_rows, CUtensorMapSwizzle swz) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { hgb_set_error("tc: cuTensorMapEncodeTiled is not available from the driver"); return HGB_ECUDA; }
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -689,13 +623,37 @@ int make_tmap(CUtensorMap* tm, const float* base, int64_t rows, int64_t cols, in
   return HGB_OK;
 }
 
-int pow2_cols(int c) {
-  int p = 32;
-  while (p < c) p <<= 1;
-  return p;
+bool shape_ok(int kr, int no) { return kr >= 32 && kr <= 256 && kr % 32 == 0 && no >= 32 && no <= 256 && no % 32 == 0; }
+
+constexpr size_t SMEM_MAX = 227 * 1024;          // opt-in dynamic shared memory per block
+
+template <int NC, bool SPLIT>
+void launch_linear_t(int grid, size_t smem, cudaStream_t st, const CUtensorMap& tm, const LinParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaFuncSetAttribute(tc_linear_kernel<NC, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX);
+    attr_set = true;
+  }
+  tc_linear_kernel<NC, SPLIT><<<grid, LIN_THREADS, smem, st>>>(tm, p);
+}
+template <int NC>
+void launch_linear(int grid, size_t smem, cudaStream_t st, const CUtensorMap& tm, const LinParams& p) {
+  if (p.split) launch_linear_t<NC, true>(grid, smem, st, tm, p); else launch_linear_t<NC, false>(grid, smem, st, tm, p);
 }
 
-bool shape_ok(int kr, int no) { return kr >= 32 && kr <= 256 && kr % 32 == 0 && no >= 32 && no <= 256 && no % 32 == 0; }
+template <int Q, bool SPLIT>
+void launch_wgrad_t(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& tdz, const CUtensorMap& tx, const WgParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaFuncSetAttribute(tc_wgrad_kernel<Q, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX);
+    attr_set = true;
+  }
+  tc_wgrad_kernel<Q, SPLIT><<<grid, WG_THREADS, smem, st>>>(tdz, tx, p);
+}
+template <int Q>
+void launch_wgrad(dim3 grid, size_t smem, cudaStream_t st, const CUtensorMap& tdz, const CUtensorMap& tx, const WgParams& p) {
+  if (p.split) launch_wgrad_t<Q, true>(grid, smem, st, tdz, tx, p); else launch_wgrad_t<Q, false>(grid, smem, st, tdz, tx, p);
+}
 
 }  // namespace
 
@@ -711,12 +669,8 @@ static int tc_linear_piece(const float* a, int64_t lda, const float* w, int64_t 
   HGB_REQUIRE(a && w && y && m >= 128 && shape_ok(k_red, n_out), "tc_linear: unsupported shape m=%d n=%d k=%d", m, n_out, k_red);
   HGB_REQUIRE(lda % 4 == 0 && ldy % 4 == 0 && ((uintptr_t)a % 16 == 0) && ((uintptr_t)y % 16 == 0) && (!z || (uintptr_t)z % 16 == 0),
               "tc_linear: operands must be 16-byte aligned with a row stride that is a multiple of 4");
-  CUtensorMap tm, tmy, tmz;
-  int rc = make_tmap(&tm, a, m, k_red, lda, TILE_M);
-  if (rc) return rc;
-  rc = make_tmap(&tmy, y, m, n_out, ldy, 32);
-  if (rc) return rc;
-  rc = make_tmap(&tmz, z ? z : y, m, n_out, ldy, 32);
+  CUtensorMap tm;
+  int rc = make_tmap(&tm, a, m, k_red, lda, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   LinParams p;
   p.m = m; p.kr = k_red; p.no = n_out; p.w = w; p.ldw = ldw; p.trans_b = trans_b; p.bias = bias; p.act = act; p.act_param = act_param;
@@ -724,22 +678,27 @@ static int tc_linear_piece(const float* a, int64_t lda, const float* w, int64_t 
   const int KB = k_red / 32;
   const int dup = exact ? 2 : 1;                   // split mode keeps a hi and a lo copy of the weights and of every A stage
   const size_t b_bytes = ((size_t)KB * n_out * 128 + 1023) & ~(size_t)1023;
-  const size_t a_stage = (size_t)TILE_M * 128;
-  int stages = (int)((224 * 1024 - 2048 - 256 - 65536 - dup * b_bytes - (size_t)n_out * 4) / (dup * a_stage));
-  if (stages > 6) stages = 6;
-  HGB_REQUIRE(stages >= 2, "tc_linear: weight operand does not fit shared memory (n=%d k=%d)", n_out, k_red);
+  const size_t fixed = 1024 + dup * b_bytes + (size_t)n_out * 4 + 64;
+  int stages = fixed < SMEM_MAX ? (int)((SMEM_MAX - fixed) / (dup * A_STAGE + 3 * 8)) : 0;
+  if (stages > 8) stages = 8;
+  stages &= ~1;                                    // two equal rings, one per consumer warpgroup
+  HGB_REQUIRE(stages >= 4, "tc_linear: weight operand does not fit shared memory (n=%d k=%d)", n_out, k_red);
   p.stages = stages;
   p.split = exact ? 1 : 0;
-  p.tmem_cols = pow2_cols(2 * n_out);
-  const size_t smem = 1024 + dup * b_bytes + dup * stages * a_stage + 65536 + (3 * stages + 4) * 8 + 16 + (size_t)n_out * 4 + 48;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(tc_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    attr_set = true;
-  }
+  const size_t smem = fixed + (size_t)stages * (dup * A_STAGE + 3 * 8);
   const int ntiles = (m + TILE_M - 1) / TILE_M;
   const int grid = ntiles < HGB_NUM_SMS ? ntiles : HGB_NUM_SMS;
-  tc_linear_kernel<<<grid, exact ? 448 : 320, smem, (cudaStream_t)stream>>>(tm, tmy, tmz, p);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (n_out / 32) {
+    case 1: launch_linear<1>(grid, smem, st, tm, p); break;
+    case 2: launch_linear<2>(grid, smem, st, tm, p); break;
+    case 3: launch_linear<3>(grid, smem, st, tm, p); break;
+    case 4: launch_linear<4>(grid, smem, st, tm, p); break;
+    case 5: launch_linear<5>(grid, smem, st, tm, p); break;
+    case 6: launch_linear<6>(grid, smem, st, tm, p); break;
+    case 7: launch_linear<7>(grid, smem, st, tm, p); break;
+    default: launch_linear<8>(grid, smem, st, tm, p); break;
+  }
   HGB_LAUNCH_CHECK("tc_linear");
   return HGB_OK;
 }
@@ -752,9 +711,9 @@ extern "C" int hgb_tc_linear(const float* a, int64_t lda, const float* w, int64_
                              const float* gsrc, int32_t gact, int32_t exact, hgb_stream_t stream) {
   HGB_REQUIRE(a && w && y && hgb_tc_linear_supported(m, n_out, k_red), "tc_linear: unsupported shape m=%d n=%d k=%d", m, n_out, k_red);
   HGB_REQUIRE(k_red <= 256 || (act == HGB_ACT_NONE && !z && !gsrc), "tc_linear: reduction length %d > 256 needs a plain linear layer", k_red);
-  // piece sizes: the B piece (kc x nc fp32) stays resident in shared memory next to >= 2 A stages and the epilogue tiles
+  // piece sizes: the B piece (kc x nc fp32) stays resident in shared memory next to >= 2 A stages per consumer ring
   const int kc_max = k_red < 256 ? k_red : 256;
-  int nc_max = (int)(((exact ? 40 : 122) * 1024) / (4 * (size_t)kc_max) / 32) * 32;     // split mode: two weight copies + two copies per A stage
+  int nc_max = (int)(((exact ? 64 : 160) * 1024) / (4 * (size_t)kc_max) / 32) * 32;     // split mode: two weight copies + two copies per A stage
   if (nc_max > 256) nc_max = 256;
   for (int c0 = 0; c0 < n_out; c0 += nc_max) {
     const int nc = n_out - c0 < nc_max ? n_out - c0 : nc_max;
@@ -783,51 +742,51 @@ extern "C" int hgb_tc_wgrad(const float* dz, int64_t lddz, const float* x, int64
   HGB_REQUIRE(workspace_bytes >= hgb_tc_wgrad_workspace_bytes(n_out, k_out), "tc_wgrad: workspace too small");
   WgParams p;
   p.m = m; p.no = n_out; p.ko = k_out;
-  p.mblocks = (n_out + 127) / 128;
-  p.nmma = k_out + 16;
   p.split = exact ? 1 : 0;
-  p.nhh = 1;
-  if (exact) {                                   // (nhh + 1) accumulators + the 16 columns the epilogue's last 32-wide read runs over
-    HGB_REQUIRE(2 * p.mblocks * p.nmma + 16 <= 512, "tc_wgrad: exact mode needs two accumulators in TMEM (n=%d k=%d)", n_out, k_out);
-    p.nhh = (512 - 16) / (p.mblocks * p.nmma) - 1;
-    if (p.nhh > 4) p.nhh = 4;
+  // fp32-accurate mode: restart the register accumulators every 8 chunks (256 rows), so no chain of tensor-core additions grows long
+  p.flush = exact ? 8 : 0;
+  const int Q = k_out / 32;
+  const int nsl_max = (n_out < WG_NA ? n_out : WG_NA) / 32;
+  const size_t raw_bytes = (size_t)(nsl_max + Q) * WG_ROWS * 128;
+  const size_t tb_bytes = (size_t)(WG_NA + k_out + 16) * 128 * (exact ? 2 : 1);
+  const size_t budget = SMEM_MAX - 1024 - 256;
+  int tbufs = 2;
+  int stages = budget > 2 * tb_bytes ? (int)((budget - 2 * tb_bytes) / raw_bytes) : 0;
+  if (stages < 2) {
+    tbufs = 1;
+    stages = (int)((budget - tb_bytes) / raw_bytes);
   }
-  p.tmem_cols = pow2_cols((exact ? (p.nhh + 1) : 1) * p.mblocks * p.nmma + (exact ? 16 : 0));
-  HGB_REQUIRE(p.tmem_cols <= 512, "tc_wgrad: accumulator does not fit TMEM");
-  const int a_chunks = p.mblocks * 4, b_chunks = k_out / 32 + 1;
-  const int slabs = a_chunks + b_chunks + (exact ? a_chunks + k_out / 32 : 0);
-  // TF32: 64-row stages (measured best: 36 us vs 39 us with 32-row stages at the C2 shapes); exact: the stage also holds the lo
-  // twins, so 32 rows, or 16 when three 32-row stages do not fit
-  const size_t budget = exact ? 227 * 1024 - 1024 - 512 : 200 * 1024;
-  int rows = exact ? 32 : 64;
-  if (exact && budget / ((size_t)slabs * rows * 128) < 3) rows = 16;
-  const size_t stage_bytes = (size_t)slabs * rows * 128;
-  int stages = (int)(budget / stage_bytes);
-  if (stages > (exact ? 6 : 4)) stages = exact ? 6 : 4;
+  if (stages > 4) stages = 4;
   HGB_REQUIRE(stages >= 2, "tc_wgrad: stage does not fit shared memory");
-  p.rows = rows;
   p.stages = stages;
+  p.tbufs = tbufs;
   CUtensorMap tdz, tx;
-  int rc = make_tmap(&tdz, dz, m, n_out, lddz, rows, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+  int rc = make_tmap(&tdz, dz, m, n_out, lddz, WG_ROWS, CU_TENSOR_MAP_SWIZZLE_NONE);
   if (rc) return rc;
-  rc = make_tmap(&tx, x, m, k_out, ldx, rows, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B);
+  rc = make_tmap(&tx, x, m, k_out, ldx, WG_ROWS, CU_TENSOR_MAP_SWIZZLE_NONE);
   if (rc) return rc;
-  const int total_chunks = (m + rows - 1) / rows;
-  int grid = total_chunks < HGB_NUM_SMS ? total_chunks : HGB_NUM_SMS;
-  p.chunks_per_cta = (total_chunks + grid - 1) / grid;
-  grid = (total_chunks + p.chunks_per_cta - 1) / p.chunks_per_cta;
+  const int total_chunks = (m + WG_ROWS - 1) / WG_ROWS;
+  const int gy = (n_out + WG_NA - 1) / WG_NA;
+  const int max_x = HGB_NUM_SMS / gy;
+  int gx = total_chunks < max_x ? total_chunks : max_x;
+  p.chunks_per_cta = (total_chunks + gx - 1) / gx;
+  gx = (total_chunks + p.chunks_per_cta - 1) / p.chunks_per_cta;
   p.part = (float*)workspace;
-  const size_t smem = 1024 + stages * stage_bytes + (3 * stages + 1) * 8 + 16;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    attr_set = true;
-  }
+  const size_t smem = 1024 + tbufs * tb_bytes + stages * raw_bytes + 2 * stages * 8;
   cudaStream_t st = (cudaStream_t)stream;
-  tc_wgrad_kernel<<<grid, exact ? 320 : 192, smem, st>>>(tdz, tx, p);
+  const dim3 grid(gx, gy);
+  switch (Q) {
+    case 1: launch_wgrad<1>(grid, smem, st, tdz, tx, p); break;
+    case 2: launch_wgrad<2>(grid, smem, st, tdz, tx, p); break;
+    case 3: launch_wgrad<3>(grid, smem, st, tdz, tx, p); break;
+    case 4: launch_wgrad<4>(grid, smem, st, tdz, tx, p); break;
+    case 5: launch_wgrad<5>(grid, smem, st, tdz, tx, p); break;
+    case 6: launch_wgrad<6>(grid, smem, st, tdz, tx, p); break;
+    default: launch_wgrad<7>(grid, smem, st, tdz, tx, p); break;
+  }
   HGB_LAUNCH_CHECK("tc_wgrad");
   const int outs = n_out * (k_out + 1);
-  tc_wgrad_reduce_kernel<<<(outs + 31) / 32, dim3(32, 8), 0, st>>>(p.part, grid, n_out, k_out, dw, lddw, db, accumulate);
+  tc_wgrad_reduce_kernel<<<(outs + 31) / 32, dim3(32, 8), 0, st>>>(p.part, gx, n_out, k_out, dw, lddw, db, accumulate);
   HGB_LAUNCH_CHECK("tc_wgrad_reduce");
   return HGB_OK;
 }

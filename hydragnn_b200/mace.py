@@ -8,7 +8,7 @@ on a ``[(N (2l+1)), F_in]`` view, and the tensor product / scatter work on whole
 
 First-order path (ordinary training, inference, first-order forces): ``conv_tp`` + the receiver scatter and the
 correlation-2 symmetric contraction are the fused kernels of hgb_mace.cu (``ops.MaceTpScatterFn``,
-``ops.MaceSymContractFn``), the radial MLP and every equivariant Linear run on the tcgen05 / SIMT Linear kernels, the
+``ops.MaceSymContractFn``), the radial MLP and every equivariant Linear run on the wgmma / SIMT Linear kernels, the
 spherical harmonics and the radial basis are ATen elementwise glue on [E, 9]-sized tensors.  Any-order path (MLIP double
 backward), correlation 3 and channel counts that are not a multiple of 32: the per-path coupling and the contraction are
 composed from gathers / segment sums / MatMuls plus ATen einsum glue.

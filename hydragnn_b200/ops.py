@@ -208,8 +208,8 @@ def raw_gemm(a, b, ta, tb, out=None, beta_one=False):
     return out
 
 
-GEMM3 = os.environ.get("HGB_GEMM3", "0") == "1"      # 1: exact-fp32 GEMMs on the 4xTF32 mma.sync kernels (csrc/hgb_gemm3.cu); measured
-                                                     # slower than the SIMT tiles on B200 (legacy mma.sync issues 1 per ~10 clk per SMSP): off
+GEMM3 = os.environ.get("HGB_GEMM3", "0") == "1"      # 1: exact-fp32 GEMMs on the 4xTF32 mma.sync kernels (csrc/hgb_gemm3.cu); off by
+                                                     # default (four legacy-path MMAs per product)
 
 
 def gemm3_ok(a, b, out, m, n, k, ta, tb):
@@ -228,13 +228,13 @@ def raw_colsum(x2d):
     return out
 
 
-# ---- tensor-core (tcgen05 / TF32) dense layers: enabled per model by precision="bf16" -----------------
+# ---- tensor-core (wgmma / TF32) dense layers: enabled per model by precision="bf16" -----------------
 _TC = {"enabled": False}
 _DATA_ONLY = {"on": False}     # inside ``only_data_grads()``: the force pass of the MLIP loss
 
 
 class tensor_cores:
-    """Context manager: run the large-M Linear layers on the tcgen05 TF32 kernels (hgb_tc_*)."""
+    """Context manager: run the large-M Linear layers on the wgmma TF32 kernels (hgb_tc_*)."""
 
     def __init__(self, enabled=True):
         self.enabled, self.prev = bool(enabled), None
@@ -249,12 +249,12 @@ class tensor_cores:
         return False
 
 
-EXACT_TC = os.environ.get("HGB_EXACT_TC", "1") == "1"     # fp32 mode: large-M Linears on tcgen05 with the 3xTF32 split (fp32-accurate)
+EXACT_TC = os.environ.get("HGB_EXACT_TC", "1") == "1"     # fp32 mode: large-M Linears on wgmma with the 3xTF32 split (fp32-accurate)
 EXACT_WGRAD = os.environ.get("HGB_EXACT_WGRAD", "1") == "1"   # ... and their weight gradients (0: SIMT fp32 GEMM)
 
 
 def tc_wgrad_ok(m, n_out, k_out, *tensors):
-    """dW = dZ^T X on the tcgen05 kernel: always in TF32 mode, in fp32 mode when the split variant is enabled"""
+    """dW = dZ^T X on the wgmma kernel: always in TF32 mode, in fp32 mode when the split variant is enabled"""
     if not (_TC["enabled"] or (EXACT_TC and EXACT_WGRAD)):
         return False
     return k_out + 16 <= 256 and tc_ok(m, n_out, k_out, *tensors)
@@ -559,7 +559,7 @@ class SegmentSum(torch.autograd.Function):
 class MatMul(torch.autograd.Function):
     """``op(a) @ op(b)`` (2-D).  d/da and d/db are MatMuls again, so this is closed under autograd.  Under
     ``tensor_cores(True)`` (precision="bf16") the three shapes a training step produces -- x Wᵀ, g W and gᵀ x -- run on the
-    tcgen05 TF32 kernels; the flag travels with the node so that (double) backward passes outside the context keep it."""
+    wgmma TF32 kernels; the flag travels with the node so that (double) backward passes outside the context keep it."""
 
     @staticmethod
     def forward(ctx, a, b, ta, tb, b_is_weight=False):

@@ -570,7 +570,7 @@ class Base(nn.Module):
             raise RuntimeError("b200 engine kernels are fp32 (bf16 via autocast-style GEMMs); got " + str(x.dtype))
         higher = self._higher_order(data)
         if getattr(self, "precision", "fp32") == "bf16" and not ops._TC["enabled"]:
-            with ops.tensor_cores(True):       # large-M Linears on tcgen05 (TF32 in, fp32 accumulate)
+            with ops.tensor_cores(True):       # large-M Linears on wgmma (TF32 in, fp32 accumulate)
                 return self.forward(data)
         plan = self.plan_for(data)
         inv, equiv, conv_args = self._embedding(data, plan, higher)

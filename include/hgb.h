@@ -1,4 +1,4 @@
-/* hgb.h -- C-ABI of libhgb.so, the sm_100a hot-path library of hydragnn-b200.
+/* hgb.h -- C-ABI of libhgb.so, the sm_90a (H100) hot-path library of hydragnn-b200.
  *
  * The reference (ORNL/HydraGNN) is 100 % Python and has no FFI boundary of its own: every
  * GPU instruction on its hot path is issued by ATen or a third-party wheel (torch_scatter,
@@ -198,7 +198,7 @@ int hgb_linear_smallk_bwd(const float* dy, const float* y, const float* z, const
                           hgb_stream_t stream);
 int64_t hgb_linear_smallk_bwd_workspace_bytes(int32_t m, int32_t n, int32_t k);
 
-/* Tensor-core (tcgen05 kind::tf32, TMEM accumulators, TMA-fed) versions of the same dense layers for the
+/* Tensor-core (wgmma TF32, register accumulators, TMA-fed) versions of the same dense layers for the
  * large-M shapes of the node / edge MLPs: m >= 128, n_out and k_red multiples of 32 and <= 256.  Used under
  * precision="bf16" (TF32 products, fp32 accumulation: tighter than the bf16 autocast of the reference).
  * y[m,n_out] = act(a[m,k_red] . B^T + bias) with B(r,c) = w[r,c] (trans_b = 0: forward, w is [n_out,k_red])
@@ -210,17 +210,18 @@ int64_t hgb_linear_smallk_bwd_workspace_bytes(int32_t m, int32_t n, int32_t k);
  * activation-backward pass.  Forward calls with gsrc = NULL, gact = HGB_ACT_DERIV, act = SiLU and z != NULL store
  * silu'(pre-activation) in z instead of the pre-activation.  n_out, k_red up to 1024 are cut into <= 256 pieces.
  * exact != 0: fp32-accurate mode for the fp32 configs -- every operand is split in shared memory into a TF32 hi / lo
- * pair (four extra warps split each A stage as the TMA lands it) and each k-step issues hi*hi + lo*hi + hi*lo
+ * pair (three producer-side warps split each A stage as the TMA lands it) and each k-step issues hi*hi + lo*hi + hi*lo
  * ("3xTF32", error ~1e-6 relative against fp64, tests/test_gpu_round2.py).                                             */
 int hgb_tc_linear_supported(int32_t m, int32_t n_out, int32_t k_red);
 int hgb_tc_linear(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t trans_b, const float* bias,
                   int32_t m, int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z,
                   const float* addend, const float* gsrc, int32_t gact, int32_t exact, hgb_stream_t stream);
 /* dw[n_out,k_out] (row stride lddw) (+)= dz[m,n_out]^T . x[m,k_out] and db[n_out] (+)= column sums of dz
- * (db may be NULL) in one pass: both operands are consumed MN-major straight from the row-major tensors, the
- * bias gradient rides along as extra all-ones columns of the B operand.  Deterministic two-stage reduce.
- * exact = 1: fp32-accurate (both operands split into TF32 hi / lo twins in shared memory, three products per
- * k-step, the large products rotating through several TMEM accumulators); exact = 0: plain TF32.             */
+ * (db may be NULL) in one pass: row slabs of both operands arrive by TMA and are transposed to K-major in shared
+ * memory, the bias gradient rides along as extra all-ones rows of the B operand.  Deterministic two-stage reduce.
+ * exact = 1: fp32-accurate (both operands split into TF32 hi / lo twins during the transposition, three products per
+ * k-step, the register accumulators folded into the partial every 256 rows to keep the chains short); exact = 0:
+ * plain TF32.                                                                                                        */
 int hgb_tc_wgrad(const float* dz, int64_t lddz, const float* x, int64_t ldx, int32_t m, int32_t n_out,
                  int32_t k_out, float* dw, int64_t lddw, float* db, int32_t accumulate, int32_t exact,
                  void* workspace, int64_t workspace_bytes, hgb_stream_t stream);

@@ -1,4 +1,4 @@
-"""Round-2 diagnostics (run on the GPU box): (1) which EGNN parameter gradients differ between the fused path, the composed path
+"""Round-2 diagnostics (needs a GPU): (1) which EGNN parameter gradients differ between the fused path, the composed path
 and the fp64 oracle; (2) PNAEq+GPS gradient agreement with the tensor-core attention on / off; (3) attention kernel timings."""
 import os, sys, copy
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

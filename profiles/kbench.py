@@ -1,5 +1,5 @@
 """Isolated kernel timings (CUDA events, L2 flushed before every launch) on the bench shapes.
-usage: python profiles/kbench.py   (on the GPU box)"""
+usage: python profiles/kbench.py   (needs a GPU)"""
 import os, sys, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -539,11 +539,11 @@ def test_grouped_csr_build_equals_radix_sort_build():
     ops.check_guard(DEV)
 
 
-# ---- tcgen05 Linears in fp32 mode: the 3xTF32 split inside tc_linear (exact flag) -------------------------------------------
+# ---- tensor-core Linears in fp32 mode: the 3xTF32 split inside tc_linear (exact flag) -------------------------------------------
 @pytest.mark.parametrize("m,n,k", [(5000, 64, 64), (4097, 192, 128), (128, 32, 32), (30000, 64, 128), (2000, 448, 64), (700, 384, 128),
                                    (1500, 576, 192), (520, 768, 256), (9001, 128, 256)])
 def test_tc_linear_exact_mode_matches_fp64(m, n, k):
-    """fp32 mode routes the large-M Linears through the SAME tcgen05 kernel with every operand split into TF32 hi / lo pairs in
+    """fp32 mode routes the large-M Linears through the SAME wgmma kernel with every operand split into TF32 hi / lo pairs in
     shared memory (hi*hi + lo*hi + hi*lo per k-step): results within ~1e-6 of fp64, i.e. fp32-level -- the plain TF32 mode of the
     bf16 configs is ~1e-3."""
     g = torch.Generator().manual_seed(m + n)
@@ -647,9 +647,9 @@ def test_side_stream_weight_gradients_equal_single_stream(name, g, prec, deferre
 @pytest.mark.parametrize("m,n,k,shift", [(130, 64, 64, 0.0), (5000, 64, 64, 0.0), (200000, 64, 128, 0.0), (200000, 128, 128, 0.5),
                                          (60000, 192, 96, 0.5), (33000, 64, 224, 0.0), (9001, 384, 64, 0.5), (400000, 32, 32, 1.0)])
 def test_tc_wgrad_exact_mode_matches_fp64(m, n, k, shift):
-    """fp32 mode: dW = dZ^T X (+ db) on tcgen05 with both operands split into TF32 hi / lo twins in shared memory.  ``shift`` gives
+    """fp32 mode: dW = dZ^T X (+ db) on wgmma with both operands split into TF32 hi / lo twins in shared memory.  ``shift`` gives
     the operands a non-zero mean, so every product has the same sign on average and a truncating accumulator would drift -- the
-    kernel rotates the large products through several TMEM accumulators to keep the chains short.  fp32-level agreement with
+    kernel folds its register accumulators into the partial sum every 256 rows to keep the chains short.  fp32-level agreement with
     fp64 (the SIMT fp32 GEMM it replaces sits at the same level), bit-identical on repetition, pieces for wide outputs."""
     g = torch.Generator().manual_seed(m + n + k)
     dz, x = torch.randn(m, n, generator=g) + shift, torch.randn(m, k, generator=g) + shift

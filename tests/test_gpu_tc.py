@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 (TF32) dense-layer kernels against fp64 references.
+"""GPU parity tests of the wgmma (TF32) dense-layer kernels against fp64 references.
 Tolerance: TF32 truncates operands to 10 mantissa bits -> relative L2 error <= 2e-3 (well inside the 2e-2 the
 bf16 config allows, SURVEY 8d)."""
 import pytest
@@ -121,3 +121,29 @@ def test_mlip_double_backward_on_tensor_cores_close_to_fp32():
     num = sum(float((p - q).double().pow(2).sum()) for p, q in zip(out[1][1], out[0][1]))
     den = sum(float(q.double().pow(2).sum()) for q in out[0][1])
     assert (num / den) ** 0.5 < 3e-2
+
+
+@pytest.mark.parametrize("exact,k,n", [(False, 256, 160), (False, 256, 64), (True, 256, 64), (True, 224, 64), (True, 192, 96),
+                                       (True, 160, 64), (True, 128, 160)])
+def test_tc_linear_many_tiles_per_consumer(exact, k, n):
+    """Shapes whose tiles have more k-blocks than a consumer's stage ring holds, with m large enough that each of the two consumer
+    warpgroups of every CTA runs several tiles: the rings recycle their stages within a tile and across tiles.  fp64 agreement,
+    and bit-identical results when a weight-gradient kernel runs concurrently on a second stream (different timing, same result)."""
+    m = 70000
+    g = torch.Generator().manual_seed(k + n + int(exact))
+    x, w, b = torch.randn(m, k, generator=g), torch.randn(n, k, generator=g) * 0.2, torch.randn(n, generator=g)
+    xd, wd, bd = x.to(DEV), w.to(DEV), b.to(DEV)
+    ref_z = x.double() @ w.double().t() + b.double()
+    with ops.tensor_cores(not exact):                             # exact = the fp32-accurate split mode
+        y, z = ops.raw_tc_linear(xd, wd, False, bd, n, k, ops.ACT_CODES["silu"], 0.0, want_z=True)
+        dz, xo = torch.randn(m, 128, device=DEV), torch.randn(m, 128, device=DEV)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            ops.raw_tc_wgrad(dz, xo, want_bias=True)
+        y2, z2 = ops.raw_tc_linear(xd, wd, False, bd, n, k, ops.ACT_CODES["silu"], 0.0, want_z=True)
+        torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize()
+    tol = 2e-6 if exact else 2e-3
+    assert rel(z, ref_z) < tol and rel(y, torch.nn.functional.silu(ref_z)) < tol
+    assert torch.equal(y, y2) and torch.equal(z, z2)

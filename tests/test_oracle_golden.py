@@ -234,7 +234,11 @@ def test_node_heads_mlp_per_node_and_conv_match_reference_golden(golden_dir):
         m.train()
         d = _data(c["inputs"])
         pred = m(d)
-        torch.testing.assert_close(pred[0], c["pred"][0], **TOL)
+        # train-mode node outputs carry fp32 rounding that depends on the host CPU and its thread count: measured max |diff| against
+        # the golden 4.5e-6 .. 4.7e-6 on an 8-core Xeon with 1 / 3 / 8 / 32 threads, and on another host 3.4e-6 absolute / 2.2e-5
+        # relative (element (16, 0) of egnn_mlp_per_node), which the old rtol 1e-5 / atol 1e-6 rejected.  Tolerance of the
+        # train-mode predictions in test_gps_matches_reference_golden
+        torch.testing.assert_close(pred[0], c["pred"][0], rtol=1e-4, atol=1e-5)
         loss, _ = m.loss(pred, d.y, [torch.arange(d.y.shape[0])])
         torch.testing.assert_close(loss, c["loss"], **TOL)
         grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
