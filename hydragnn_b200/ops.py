@@ -273,6 +273,10 @@ def tc_ok(m, n_out, k_red, *tensors):
 
 def raw_tc_linear(a2, w, trans_b, bias, n_out, k_red, code=0, param=0.0, want_z=False, addend=None, gsrc=None, gact=0):
     m = a2.shape[0]
+    for t in (addend, gsrc):             # the epilogue reads them with y's row stride n_out
+        if t is not None and (tuple(t.shape) != (m, n_out) or not t.is_contiguous()):
+            raise RuntimeError("raw_tc_linear: addend / gsrc must be dense row-major [%d, %d] tensors, got shape %s stride %s"
+                               % (m, n_out, tuple(t.shape), t.stride()))
     y = torch.empty(m, n_out, dtype=a2.dtype, device=a2.device)
     z = torch.empty_like(y) if want_z else None
     _lib.call("hgb_tc_linear", _p(a2), a2.stride(0), _p(w), w.stride(0), int(trans_b), _p(bias), m, n_out, k_red, code, float(param),
@@ -491,6 +495,9 @@ def linear_bwd_dispatch(dz, x2, w, need_x=True, need_w=True, need_b=True, dx_add
     on the tensor-core path that happens in the dgrad epilogue."""
     m, n = dz.shape
     k = x2.shape[1]
+    # the tensor-core epilogue reads dx_addend / dx_gsrc with dx's row stride k and hgb_act_bwd reads dx_gsrc as a flat array:
+    # a column block of a wider tensor is copied to a dense [m, k] first
+    dx_addend, dx_gsrc = _dense_2d(dx_addend, m, k), _dense_2d(dx_gsrc, m, k)
 
     def through_act(dx):
         if dx is None or dx_gsrc is None:
@@ -516,6 +523,15 @@ def linear_bwd_dispatch(dz, x2, w, need_x=True, need_w=True, need_b=True, dx_add
             else:
                 dx = through_act(raw_gemm(dz, w, False, False))
     return dx, dw, db
+
+
+def _dense_2d(t, m, k):
+    """``t`` (a [m, k] tensor or None) as a dense row-major [m, k] tensor, copying only if it is strided."""
+    if t is None:
+        return None
+    if tuple(t.shape) != (m, k):
+        raise RuntimeError("expected a [%d, %d] tensor, got %s" % (m, k, tuple(t.shape)))
+    return _chk(t)
 
 
 def _row_major_2d(t):
