@@ -109,6 +109,59 @@ __device__ __forceinline__ void wgmma_n16(float* d, uint64_t ad, uint64_t bd) {
       : "l"(ad), "l"(bd), "r"(1));
 }
 
+// D[64 x 32 NC] += A[64 x 8] . B[32 NC x 8]^T: one instruction for every output column of a Linear piece, so A is read from shared
+// memory once per k-step.  Fragment: d[4i + 2h + e] = D(16 w + lane/4 + 8h, 8i + 2(lane%4) + e), i < 4 NC.
+template <int NC>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t ad, uint64_t bd);
+#define TC_R16_0 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define TC_R16_1 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define TC_R16_2 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define TC_R16_3 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define TC_R16_4 "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define TC_R16_5 "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define TC_R16_6 "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
+#define TC_R16_7 "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define TC_D16(o)                                                                                                                   \
+  "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7]),      \
+      "+f"(d[o + 8]), "+f"(d[o + 9]), "+f"(d[o + 10]), "+f"(d[o + 11]), "+f"(d[o + 12]), "+f"(d[o + 13]), "+f"(d[o + 14]),       \
+      "+f"(d[o + 15])
+// AD, BD, SC: the operand numbers of the two descriptors and of the scale-d flag, which follow the 16 NC accumulators
+#define TC_WGMMA(NC, SHAPE, AD, BD, SC, REGS, ...)                                                                                  \
+  template <>                                                                                                                       \
+  __device__ __forceinline__ void wgmma_tf32<NC>(float* d, uint64_t ad, uint64_t bd) {                                             \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " SC ", 0;\nwgmma.mma_async.sync.aligned." SHAPE ".f32.tf32.tf32 {" REGS     \
+                 "}, " AD ", " BD ", p, 1, 1;\n}"                                                                                  \
+                 : __VA_ARGS__                                                                                                      \
+                 : "l"(ad), "l"(bd), "r"(1));                                                                                       \
+  }
+TC_WGMMA(1, "m64n32k8", "%16", "%17", "%18", TC_R16_0, TC_D16(0))
+TC_WGMMA(2, "m64n64k8", "%32", "%33", "%34", TC_R16_0 ", " TC_R16_1, TC_D16(0), TC_D16(16))
+TC_WGMMA(3, "m64n96k8", "%48", "%49", "%50", TC_R16_0 ", " TC_R16_1 ", " TC_R16_2, TC_D16(0), TC_D16(16), TC_D16(32))
+TC_WGMMA(4, "m64n128k8", "%64", "%65", "%66", TC_R16_0 ", " TC_R16_1 ", " TC_R16_2 ", " TC_R16_3, TC_D16(0), TC_D16(16), TC_D16(32),
+         TC_D16(48))
+TC_WGMMA(5, "m64n160k8", "%80", "%81", "%82", TC_R16_0 ", " TC_R16_1 ", " TC_R16_2 ", " TC_R16_3 ", " TC_R16_4, TC_D16(0), TC_D16(16),
+         TC_D16(32), TC_D16(48), TC_D16(64))
+TC_WGMMA(6, "m64n192k8", "%96", "%97", "%98", TC_R16_0 ", " TC_R16_1 ", " TC_R16_2 ", " TC_R16_3 ", " TC_R16_4 ", " TC_R16_5, TC_D16(0),
+         TC_D16(16), TC_D16(32), TC_D16(48), TC_D16(64), TC_D16(80))
+TC_WGMMA(7, "m64n224k8", "%112", "%113", "%114", TC_R16_0 ", " TC_R16_1 ", " TC_R16_2 ", " TC_R16_3 ", " TC_R16_4 ", " TC_R16_5 ", " TC_R16_6,
+         TC_D16(0), TC_D16(16), TC_D16(32), TC_D16(48), TC_D16(64), TC_D16(80), TC_D16(96))
+TC_WGMMA(8, "m64n256k8", "%128", "%129", "%130", TC_R16_0 ", " TC_R16_1 ", " TC_R16_2 ", " TC_R16_3 ", " TC_R16_4 ", " TC_R16_5 ", " TC_R16_6
+         ", " TC_R16_7, TC_D16(0), TC_D16(16), TC_D16(32), TC_D16(48), TC_D16(64), TC_D16(80), TC_D16(96), TC_D16(112))
+#undef TC_WGMMA
+#undef TC_D16
+
+// TMA store of one box from shared memory, tracked by the issuing thread's bulk async-groups
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tmap, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(tmap), "r"(smem_u32(smem_src)),
+               "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the newest N bulk groups of this thread have finished reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
 // shared-memory matrix descriptor of a K-major operand in the 128-byte swizzle: rows of 32 fp32 (128 B), 8-row groups 1024 B
 // apart (SBO); the k-step of 8 tf32 inside the swizzle atom is a 32-byte advance of the start address.  The operand base must be
 // 1024-byte aligned (the swizzle phase is taken from the address bits).
@@ -155,56 +208,77 @@ struct LinParams {
   int stages;           // in total: two rings (one per consumer warpgroup) of stages / 2 each
   int split;            // 1: fp32-accurate mode -- every operand is split into a TF32 hi / lo pair and each k-step runs the three
                         //    products lo*hi + hi*lo + hi*hi (3xTF32); warps 1..3 split the A stages in shared memory
+  int slots;            // output staging buffers per consumer warpgroup (2 or 4), one [64 x 32] sub-tile each
 };
 
 constexpr int TILE_M = 64;                       // rows per tile = one wgmma M
 constexpr uint32_t A_STAGE = TILE_M * 128;       // one pipeline stage = one [64 x 32 fp32] k-block (8 KB)
+constexpr uint32_t SUB_BYTES = TILE_M * 128;     // one output staging buffer = one [64 x 32 fp32] TMA store box (8 KB)
 constexpr int LIN_THREADS = 384;
 
-// the epilogue of two adjacent outputs (row, col), (row, col + 1)
-__device__ __forceinline__ void lin_epilogue2(const LinParams& p, const float* sbias, int row, int col, float v0, float v1) {
-  if (row >= p.m) return;
-  const int64_t o = (int64_t)row * p.ldy + col;
-  v0 += sbias[col];
-  v1 += sbias[col + 1];
-  if (p.z && !(p.z_deriv && p.act == HGB_ACT_SILU)) *reinterpret_cast<float2*>(p.z + o) = make_float2(v0, v1);
-  switch (p.act) {
-    case HGB_ACT_NONE: break;
-    case HGB_ACT_RELU: v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); break;
-    case HGB_ACT_SILU:
-      if (p.z && p.z_deriv) {   // z receives silu'(pre) = s + y (1 - s): the backward then needs one multiply per element
-        const float s0 = __fdividef(1.f, 1.f + __expf(-v0)), s1 = __fdividef(1.f, 1.f + __expf(-v1));
-        v0 *= s0;
-        v1 *= s1;
-        *reinterpret_cast<float2*>(p.z + o) = make_float2(fmaf(v0, 1.f - s0, s0), fmaf(v1, 1.f - s1, s1));
-      } else {
-        v0 = __fdividef(v0, 1.f + __expf(-v0));
-        v1 = __fdividef(v1, 1.f + __expf(-v1));
-      }
-      break;
-    case HGB_ACT_TANH: v0 = tanhf(v0); v1 = tanhf(v1); break;
-    default: v0 = hgb_act(v0, p.act, p.act_param); v1 = hgb_act(v1, p.act, p.act_param);
+// epilogue kinds: the activation, picked once per sub-tile so that the element loop carries no dispatch
+enum { EPI_NONE, EPI_RELU, EPI_SILU, EPI_SILU_ZD, EPI_TANH, EPI_OTHER };
+
+// the epilogue of one output: v = accumulator + bias on entry; z receives what the z output stores
+template <int K>
+__device__ __forceinline__ float lin_epilogue1(const LinParams& p, float v, float& z, float a, float g) {
+  z = v;
+  if (K == EPI_RELU) v = fmaxf(v, 0.f);
+  if (K == EPI_SILU) v = __fdividef(v, 1.f + __expf(-v));
+  if (K == EPI_SILU_ZD) {     // z receives silu'(pre) = s + y (1 - s): the backward then needs one multiply per element
+    const float s = __fdividef(1.f, 1.f + __expf(-v));
+    v *= s;
+    z = fmaf(v, 1.f - s, s);
   }
-  if (p.addend) {
-    const float2 a = __ldg(reinterpret_cast<const float2*>(p.addend + o));
-    v0 += a.x;
-    v1 += a.y;
-  }
-  if (p.gsrc) {
-    const float2 g = __ldg(reinterpret_cast<const float2*>(p.gsrc + o));
-    if (p.gact == HGB_ACT_DERIV) {          // gsrc already holds act'(.)
-      v0 *= g.x;
-      v1 *= g.y;
-    } else {
-      v0 *= hgb_act_grad(g.x, g.x, p.gact, p.act_param);
-      v1 *= hgb_act_grad(g.y, g.y, p.gact, p.act_param);
-    }
-  }
-  *reinterpret_cast<float2*>(p.y + o) = make_float2(v0, v1);
+  if (K == EPI_TANH) v = tanhf(v);
+  if (K == EPI_OTHER) v = hgb_act(v, p.act, p.act_param);
+  if (p.addend) v += a;
+  if (p.gsrc) v *= p.gact == HGB_ACT_DERIV ? g : hgb_act_grad(g, g, p.gact, p.act_param);   // DERIV: gsrc already holds act'(.)
+  return v;
 }
 
+// Element loop over one [64 x 32] sub-tile of a warpgroup (tid 0..127): 4 float4 per thread, 8 threads per row.  ys holds the
+// accumulators in the TMA SWIZZLE_128B layout and receives y in place; zs receives z.  a / g: this thread's addend / gsrc values.
+template <int K>
+__device__ __forceinline__ void lin_epilogue_sub(const LinParams& p, const float* sb, uint8_t* ys, uint8_t* zs, int tid, const float4* a,
+                                                 const float4* g) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int idx = j * 128 + tid, r = idx >> 3, q = idx & 7;
+    const uint32_t off = (uint32_t)r * 128 + ((q ^ (r & 7)) << 4);
+    float4 v = *reinterpret_cast<float4*>(ys + off), z;
+    v.x = lin_epilogue1<K>(p, v.x + sb[4 * q], z.x, a[j].x, g[j].x);
+    v.y = lin_epilogue1<K>(p, v.y + sb[4 * q + 1], z.y, a[j].y, g[j].y);
+    v.z = lin_epilogue1<K>(p, v.z + sb[4 * q + 2], z.z, a[j].z, g[j].z);
+    v.w = lin_epilogue1<K>(p, v.w + sb[4 * q + 3], z.w, a[j].w, g[j].w);
+    *reinterpret_cast<float4*>(ys + off) = v;
+    if (zs) *reinterpret_cast<float4*>(zs + off) = z;
+  }
+}
+
+// this thread's addend / gsrc values of sub-tile c (columns 32 c ..) of the tile at row0, in lin_epilogue_sub's element order
+__device__ __forceinline__ void lin_load_operands(const LinParams& p, int row0, int c, int tid, float4* a, float4* g) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int idx = j * 128 + tid, row = row0 + (idx >> 3);
+    const int64_t o = (int64_t)row * p.ldy + c * 32 + (idx & 7) * 4;
+    const bool in = row < p.m;
+    if (p.addend) a[j] = in ? __ldg(reinterpret_cast<const float4*>(p.addend + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    if (p.gsrc) g[j] = in ? __ldg(reinterpret_cast<const float4*>(p.gsrc + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+}
+
+// Shared memory (bytes; B = KB * NO * 128 per weight copy, A stage = 8 KB, x2 in split mode; SMEM_MAX = 232,448):
+//   [B hi | B lo (split)] [2 warpgroups x slots x 8 KB output staging] [stages x A stage | A lo (split)] [3 x stages barriers] [bias]
+// The host piece rule keeps B <= 160 KB in TF32 mode and 2 x 64 KB in split mode.  Tightest TF32 case, k_red = 256 and a 160-column
+// piece: 1 KB alignment + 160 KB B + 32 KB staging (2 slots) + 0.7 KB bias / barriers leaves 33.7 KB = 4 A stages (2 per ring).
+// Tightest split case, 64 KB of weights per copy: 1 KB + 128 KB B + 32 KB staging leaves 66 KB = 4 A stages of 16 KB.  Four slots
+// per warpgroup (64 KB) are used when at least 4 stages still fit next to them: B <= 128 KB in TF32 mode, <= 48 KB per copy in split
+// mode (every C2 layer has B <= 48 KB).
 template <int NC, bool SPLIT>   // NO = 32 * NC output columns; SPLIT: the fp32-accurate mode
-__global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_constant__ CUtensorMap tmap_a, const LinParams p) {
+__global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_constant__ CUtensorMap tmap_a,
+                                                                   const __grid_constant__ CUtensorMap tmap_y,
+                                                                   const __grid_constant__ CUtensorMap tmap_z, const LinParams p) {
   constexpr int NO = NC * 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -212,7 +286,8 @@ __global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_
   const uint32_t b_pad = ((uint32_t)KB * NO * 128 + 1023) & ~1023u;
   uint8_t* sB = smem;
   uint8_t* sBlo = sB + b_pad;                                 // split mode only
-  uint8_t* sA = sB + (SPLIT ? 2 : 1) * (size_t)b_pad;
+  uint8_t* sOut = sB + (SPLIT ? 2 : 1) * (size_t)b_pad;       // [2][slots] staging buffers, 1024-byte aligned (TMA swizzle)
+  uint8_t* sA = sOut + (size_t)2 * p.slots * SUB_BYTES;
   const int S = p.stages;
   const int SR = S >> 1;                                      // stages per ring: stage (r * SR + slot) belongs to ring r
   uint8_t* sAlo = sA + (size_t)S * A_STAGE;                   // split mode only
@@ -314,57 +389,104 @@ __global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_
     named_bar_sync(1, 256);
     const int cw = (warp - 4) >> 2;     // consumer warpgroup: takes local tiles cw, cw + 2, ... from ring cw, every item in order
     const int wq = warp & 3;            // warp within the warpgroup: rows 16 wq .. 16 wq + 15 of the tile
+    const int tid = threadIdx.x & 127;  // thread within the warpgroup
     const uint32_t sA_addr = smem_u32(sA), sAlo_addr = smem_u32(sAlo), sB_addr = smem_u32(sB), sBlo_addr = smem_u32(sBlo);
-    float acc[NC][16];
+    // output staging: a sub-tile takes one buffer (y) or two (y, z); `ahead` = how many sub-tiles' TMA stores may still be reading
+    // their buffers when the next sub-tile is written
+    uint8_t* sOwn = sOut + (size_t)cw * p.slots * SUB_BYTES;
+    const int per_sub = p.z ? 2 : 1;
+    const int ahead = p.slots / per_sub - 1;            // 0, 1 or 3
+    const int kind = p.act == HGB_ACT_NONE ? EPI_NONE
+                     : p.act == HGB_ACT_RELU ? EPI_RELU
+                     : p.act == HGB_ACT_SILU ? (p.z && p.z_deriv ? EPI_SILU_ZD : EPI_SILU)
+                     : p.act == HGB_ACT_TANH ? EPI_TANH
+                                             : EPI_OTHER;
+    const bool operands = p.addend || p.gsrc;
+    float acc[NC * 16];
+    uint32_t sub = 0;                   // sub-tiles stored so far by this warpgroup
     int li = cw;
     for (int t = blockIdx.x + cw * gridDim.x; t < ntiles; t += 2 * gridDim.x, li += 2) {
+      const int row0 = t * TILE_M;
+      float4 opa[4], opg[4];
 #pragma unroll
-      for (int c = 0; c < NC; ++c)
+      for (int j = 0; j < 4; ++j) opa[j] = opg[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+      // the first sub-tile's addend / gsrc are in flight during the MMAs (at NC = 8 these 32 registers would spill: load after them)
+      constexpr bool early = NC < 8;
+      if (early && operands) lin_load_operands(p, row0, 0, tid, opa, opg);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) acc[c][j] = 0.f;
+      for (int j = 0; j < NC * 16; ++j) acc[j] = 0.f;
       const uint32_t n0 = (uint32_t)(li >> 1) * KB;             // first item of this tile within ring cw
       for (int kb = 0; kb < KB; ++kb) {
         const uint32_t n = n0 + kb;
         const int s = cw * SR + n % SR;
         mbar_wait(SPLIT ? full2 + s : full + s, (n / SR) & 1);
-        fence_regs<NC * 16>(&acc[0][0]);
+        fence_regs<NC * 16>(acc);
         wgmma_fence();
 #pragma unroll
         for (int k4 = 0; k4 < 4; ++k4) {
           const uint64_t ad = make_desc(sA_addr + s * A_STAGE + k4 * 32);
-          const uint64_t adl = make_desc(sAlo_addr + s * A_STAGE + k4 * 32);
-#pragma unroll
-          for (int c = 0; c < NC; ++c) {
-            const uint32_t boff = (uint32_t)kb * NO * 128 + c * 4096 + k4 * 32;
-            const uint64_t bd = make_desc(sB_addr + boff);
-            if (SPLIT) {        // small terms first: lo*hi + hi*lo + hi*hi
-              wgmma_n32(acc[c], adl, bd);
-              wgmma_n32(acc[c], ad, make_desc(sBlo_addr + boff));
-            }
-            wgmma_n32(acc[c], ad, bd);
+          const uint32_t boff = (uint32_t)kb * NO * 128 + k4 * 32;  // every output column: 8-row groups of B are 1024 B apart
+          const uint64_t bd = make_desc(sB_addr + boff);
+          if (SPLIT) {          // small terms first: lo*hi + hi*lo + hi*hi
+            wgmma_tf32<NC>(acc, make_desc(sAlo_addr + s * A_STAGE + k4 * 32), bd);
+            wgmma_tf32<NC>(acc, ad, make_desc(sBlo_addr + boff));
           }
+          wgmma_tf32<NC>(acc, ad, bd);
         }
         wgmma_commit();
-        fence_regs<NC * 16>(&acc[0][0]);
+        fence_regs<NC * 16>(acc);
         if (kb > 0) {                   // the MMAs of the previous k-block have read their stage: release it
           wgmma_wait<1>();
           if (lane == 0) mbar_arrive(empty + cw * SR + (n - 1) % SR);
         }
       }
       wgmma_wait<0>();
-      fence_regs<NC * 16>(&acc[0][0]);
+      fence_regs<NC * 16>(acc);
       if (lane == 0) mbar_arrive(empty + cw * SR + (n0 + KB - 1) % SR);
-      // ===== epilogue straight from the accumulator registers =====
-      const int r0 = t * TILE_M + wq * 16 + (lane >> 2);
-#pragma unroll
-      for (int c = 0; c < NC; ++c)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int col = c * 32 + i * 8 + 2 * (lane & 3);
-          lin_epilogue2(p, sbias, r0, col, acc[c][4 * i], acc[c][4 * i + 1]);
-          lin_epilogue2(p, sbias, r0 + 8, col, acc[c][4 * i + 2], acc[c][4 * i + 3]);
+      if (!early && operands) lin_load_operands(p, row0, 0, tid, opa, opg);
+      // ===== epilogue, one [64 x 32] sub-tile at a time: accumulators -> swizzled staging buffer -> element loop in place -> TMA
+      // store (rows >= m are clipped by the tensor map) =====
+#pragma unroll 1
+      for (int c = 0; c < NC; ++c, ++sub) {
+        uint8_t* ys = sOwn + (size_t)((sub % (p.slots / per_sub)) * per_sub) * SUB_BYTES;
+        uint8_t* zs = p.z ? ys + SUB_BYTES : nullptr;
+        if (tid == 0) {
+          if (ahead == 0) bulk_wait_read<0>(); else if (ahead == 1) bulk_wait_read<1>(); else bulk_wait_read<3>();
         }
+        named_bar_sync(2 + cw, 128);    // the buffers are free (and no thread still reads them)
+#pragma unroll
+        for (int cc = 0; cc < NC; ++cc)
+          if (cc == c) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int r = wq * 16 + (lane >> 2) + 8 * h, col = i * 8 + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(ys + kmajor_sw128_off(r, col, TILE_M)) =
+                    make_float2(acc[16 * cc + 4 * i + 2 * h], acc[16 * cc + 4 * i + 2 * h + 1]);
+              }
+          }
+        named_bar_sync(2 + cw, 128);
+        const float* sb = sbias + c * 32;
+        switch (kind) {
+          case EPI_NONE: lin_epilogue_sub<EPI_NONE>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_RELU: lin_epilogue_sub<EPI_RELU>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_SILU: lin_epilogue_sub<EPI_SILU>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_SILU_ZD: lin_epilogue_sub<EPI_SILU_ZD>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_TANH: lin_epilogue_sub<EPI_TANH>(p, sb, ys, zs, tid, opa, opg); break;
+          default: lin_epilogue_sub<EPI_OTHER>(p, sb, ys, zs, tid, opa, opg);
+        }
+        if (operands && c + 1 < NC) lin_load_operands(p, row0, c + 1, tid, opa, opg);
+        fence_proxy_async();            // the staged results are visible to the TMA
+        named_bar_sync(2 + cw, 128);
+        if (tid == 0) {
+          tma_store_2d(&tmap_y, ys, c * 32, row0);
+          if (zs) tma_store_2d(&tmap_z, zs, c * 32, row0);
+          bulk_commit();
+        }
+      }
     }
+    if (tid == 0) bulk_wait_all();      // the stores have completed before the CTA's shared memory goes away
   }
 }
 
@@ -628,16 +750,16 @@ bool shape_ok(int kr, int no) { return kr >= 32 && kr <= 256 && kr % 32 == 0 && 
 constexpr size_t SMEM_MAX = 227 * 1024;          // opt-in dynamic shared memory per block
 
 template <int NC, bool SPLIT>
-void launch_linear_t(int grid, size_t smem, cudaStream_t st, const CUtensorMap& tm, const LinParams& p) {
+void launch_linear_t(int grid, size_t smem, cudaStream_t st, const CUtensorMap* tm, const LinParams& p) {
   static bool attr_set = false;
   if (!attr_set) {
     cudaFuncSetAttribute(tc_linear_kernel<NC, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX);
     attr_set = true;
   }
-  tc_linear_kernel<NC, SPLIT><<<grid, LIN_THREADS, smem, st>>>(tm, p);
+  tc_linear_kernel<NC, SPLIT><<<grid, LIN_THREADS, smem, st>>>(tm[0], tm[1], tm[2], p);
 }
 template <int NC>
-void launch_linear(int grid, size_t smem, cudaStream_t st, const CUtensorMap& tm, const LinParams& p) {
+void launch_linear(int grid, size_t smem, cudaStream_t st, const CUtensorMap* tm, const LinParams& p) {  // tm: a, y, z
   if (p.split) launch_linear_t<NC, true>(grid, smem, st, tm, p); else launch_linear_t<NC, false>(grid, smem, st, tm, p);
 }
 
@@ -667,23 +789,34 @@ static int tc_linear_piece(const float* a, int64_t lda, const float* w, int64_t 
                            int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z, const float* addend,
                            const float* gsrc, int32_t gact, int64_t ldy, int32_t exact, hgb_stream_t stream) {
   HGB_REQUIRE(a && w && y && m >= 128 && shape_ok(k_red, n_out), "tc_linear: unsupported shape m=%d n=%d k=%d", m, n_out, k_red);
-  HGB_REQUIRE(lda % 4 == 0 && ldy % 4 == 0 && ((uintptr_t)a % 16 == 0) && ((uintptr_t)y % 16 == 0) && (!z || (uintptr_t)z % 16 == 0),
+  HGB_REQUIRE(lda % 4 == 0 && ldy % 4 == 0 && ((uintptr_t)a % 16 == 0) && ((uintptr_t)y % 16 == 0) && (!z || (uintptr_t)z % 16 == 0) &&
+                  (!addend || (uintptr_t)addend % 16 == 0) && (!gsrc || (uintptr_t)gsrc % 16 == 0),
               "tc_linear: operands must be 16-byte aligned with a row stride that is a multiple of 4");
-  CUtensorMap tm;
-  int rc = make_tmap(&tm, a, m, k_red, lda, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
+  CUtensorMap tm[3];                               // A loads; y and z stores: [64 x 32] boxes, rows >= m clipped
+  int rc = make_tmap(&tm[0], a, m, k_red, lda, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   LinParams p;
   p.m = m; p.kr = k_red; p.no = n_out; p.w = w; p.ldw = ldw; p.trans_b = trans_b; p.bias = bias; p.act = act; p.act_param = act_param;
   p.y = y; p.z = z; p.addend = addend; p.ldy = ldy; p.gsrc = gsrc; p.gact = gact; p.z_deriv = (!gsrc && gact == HGB_ACT_DERIV) ? 1 : 0;
+  rc = make_tmap(&tm[1], y, m, n_out, ldy, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
+  rc = make_tmap(&tm[2], z ? z : y, m, n_out, ldy, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
+  if (rc) return rc;
   const int KB = k_red / 32;
   const int dup = exact ? 2 : 1;                   // split mode keeps a hi and a lo copy of the weights and of every A stage
   const size_t b_bytes = ((size_t)KB * n_out * 128 + 1023) & ~(size_t)1023;
-  const size_t fixed = 1024 + dup * b_bytes + (size_t)n_out * 4 + 64;
-  int stages = fixed < SMEM_MAX ? (int)((SMEM_MAX - fixed) / (dup * A_STAGE + 3 * 8)) : 0;
-  if (stages > 8) stages = 8;
-  stages &= ~1;                                    // two equal rings, one per consumer warpgroup
+  int stages = 0, slots = 0;
+  size_t fixed = 0;
+  for (slots = 4; slots >= 2; slots -= 2) {        // four staging buffers per warpgroup where 4 A stages still fit, else two
+    fixed = 1024 + dup * b_bytes + (size_t)2 * slots * SUB_BYTES + (size_t)n_out * 4 + 64;
+    stages = fixed < SMEM_MAX ? (int)((SMEM_MAX - fixed) / (dup * A_STAGE + 3 * 8)) : 0;
+    if (stages > 8) stages = 8;
+    stages &= ~1;                                  // two equal rings, one per consumer warpgroup
+    if (stages >= 4) break;
+  }
   HGB_REQUIRE(stages >= 4, "tc_linear: weight operand does not fit shared memory (n=%d k=%d)", n_out, k_red);
   p.stages = stages;
+  p.slots = slots;
   p.split = exact ? 1 : 0;
   const size_t smem = fixed + (size_t)stages * (dup * A_STAGE + 3 * 8);
   const int ntiles = (m + TILE_M - 1) / TILE_M;

@@ -23,8 +23,40 @@ def timeit(fn, iters=10, warm=3):
     return sum(ts) / len(ts)
 
 
+def tc_linear_calls(n):
+    """The hgb_tc_linear calls of the C2 (qm9_painn) step at n nodes, each with its real epilogue operands.
+    GB/s: algorithmic bytes (bench._alg_bytes: 4 m (k_red + n_out (1 + z + addend + gsrc))) over device time."""
+    silu, tanh, deriv = ops.ACT_CODES["silu"], ops.ACT_CODES["tanh"], ops.ACT_DERIV
+    # name, m, k_red, n_out, trans_b, act, want_z, gact, addend, gsrc
+    calls = [("fwd 64->64 silu z=silu'", n, 64, 64, False, silu, True, deriv, False, False),
+             ("fwd 64->192", n, 64, 192, False, 0, False, 0, False, False),
+             ("fwd 64->128 (3N rows)", 3 * n, 64, 128, False, 0, False, 0, False, False),
+             ("fwd 128->64 silu z=silu'", n, 128, 64, False, silu, True, deriv, False, False),
+             ("fwd 64->128", n, 64, 128, False, 0, False, 0, False, False),
+             ("fwd 64->64 tanh", n, 64, 64, False, tanh, False, 0, False, False),
+             ("dgrad 64->64 gsrc=silu'", n, 64, 64, True, 0, False, deriv, False, True),
+             ("dgrad 64->192 gsrc=silu'", n, 192, 64, True, 0, False, deriv, False, True),
+             ("dgrad 128->64 gsrc=silu'", n, 64, 128, True, 0, False, deriv, False, True),
+             ("dgrad 64->64 gsrc=tanh", n, 64, 64, True, 0, False, tanh, False, True),
+             ("dgrad 64->128 (3N rows) +addend", 3 * n, 128, 64, True, 0, False, 0, True, False),
+             ("dgrad 64->128 plain", n, 128, 64, True, 0, False, 0, False, False)]
+    res = {}
+    for name, m, k, no, tb, act, want_z, gact, has_add, has_g in calls:
+        a = torch.randn(m, k, device=dev)
+        w = torch.randn(k, no, device=dev) if tb else torch.randn(no, k, device=dev)
+        bias = None if tb else torch.randn(no, device=dev)
+        add = torch.randn(m, no, device=dev) if has_add else None
+        g = torch.rand(m, no, device=dev) if has_g else None
+        t = timeit(lambda: ops.raw_tc_linear(a, w, tb, bias, no, k, act, 0.0, want_z, addend=add, gsrc=g, gact=gact))
+        nbytes = 4 * m * (k + no * (1 + int(want_z) + int(has_add) + int(has_g)))
+        res["tc_linear %s m=%d (ms | GB/s)" % (name, m)] = (round(t, 4), round(nbytes / t / 1e6, 1))
+    return res
+
+
 G = 16384
 b = make_samples("qm9_painn", G).to(dev); b._num_graphs = G
+if os.environ.get("KBENCH_ONLY") == "tc_linear":
+    print(json.dumps(tc_linear_calls(b.pos.shape[0]), indent=1)); sys.exit(0)
 b = hb.get_radius_graph(7.0, 5)(b)
 plan = Base.plan_for(b)
 n, e, f, r = plan.num_nodes, plan.num_edges, 64, 5
@@ -50,6 +82,7 @@ for (m, k, nn_) in [(n, 64, 64), (n, 64, 192), (3 * n, 64, 64), (n, 128, 64), (n
     x, w, bb = torch.randn(m, k, device=dev), torch.randn(nn_, k, device=dev), torch.randn(nn_, device=dev)
     t = timeit(lambda: ops.raw_tc_linear(x, w, False, bb, nn_, k))
     out["tc_linear m=%d k=%d n=%d (ms | GB/s)" % (m, k, nn_)] = (t, m * (k + nn_) * 4 / t / 1e6)
+out.update(tc_linear_calls(n))
 for (m, nn_, k) in [(n, 64, 64), (n, 192, 64), (3 * n, 64, 64)]:
     dz, x = torch.randn(m, nn_, device=dev), torch.randn(m, k, device=dev)
     t = timeit(lambda: ops.raw_tc_wgrad(dz, x))
