@@ -1045,8 +1045,9 @@ __global__ void painn_update_bwd_kernel(const float* __restrict__ gs_out, const 
       const int64_t o = i * 3 * f + k * f + c, op = (i * 3 + k) * ld + c;
       const float u = uv[op], w = vv[op];
       const float gvo = last ? 0.f : gv_out[o];
-      guv[op] = gvo * a_vv + g * a_sv * w;
-      gvv[op] = g * a_sv * u + gn_over * w;
+      // contracted explicitly (hgb_painn_tc.cu forms the same terms and must give the same bits)
+      guv[op] = fmaf(g * a_sv, w, gvo * a_vv);
+      gvv[op] = fmaf(g * a_sv, u, gn_over * w);
       if (gv) gv[o] = gvo;   // optional copy of the direct path v -> v_out (callers may pass gv_out itself as the dgrad addend)
     }
   }

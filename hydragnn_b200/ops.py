@@ -959,6 +959,72 @@ class PainnUpdateFn(torch.autograd.Function):
         return gs, gv.reshape(n, 3, f), gwuv[:f], gbuv[:f], gwuv[f:], gbuv[f:], gw1, gb1, gw2, gb2, None
 
 
+def painn_update_tc_ok(s, v):
+    """``PainnUpdateTcFn`` runs the block: TF32 mode, f = 64, as many rows as the tensor-core Linears take, dense 16-byte aligned
+    fp32 CUDA tensors."""
+    n, f = s.shape
+    return (_TC["enabled"] and f == 64 and tuple(v.shape) == (n, 3, f) and s.is_cuda and v.is_cuda
+            and s.dtype == torch.float32 and v.dtype == torch.float32 and s.is_contiguous() and v.is_contiguous()
+            and s.data_ptr() % 16 == 0 and v.data_ptr() % 16 == 0 and bool(_lib.query("hgb_tc_linear_supported", n, f, 2 * f)))
+
+
+def _aligned(t):
+    """dense and 16-byte aligned (a view at an odd offset is copied)"""
+    t = _chk(t)
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+class PainnUpdateTcFn(torch.autograd.Function):
+    """``PainnUpdateFn`` at f = 64 in TF32 mode without the [3n, 2f] U/V product in memory (csrc/hgb_painn_tc.cu): each step of the
+    block recomputes [uv | vv] from v on the tensor cores for its 64-node tiles and reduces over the three spatial rows in registers.
+    Forward: [|vv|, s] -> update_mlp (tc_linear) -> s_out (v_out).  Backward: ga -> the update_mlp backward -> [guv | gvv] and gv, the
+    U/V data gradient, in one kernel; the U/V weight gradient still reads [guv | gvv] on the side stream.  Same bits as
+    ``PainnUpdateFn``."""
+
+    @staticmethod
+    def forward(ctx, s, v, uw, ub, vw, vb, w1, b1, w2, b2, last):
+        n, f = s.shape
+        w1, b1, w2, b2 = [_chk(t) for t in (w1, b1, w2, b2)]
+        wuv, buv = torch.cat([uw, vw], dim=0).contiguous(), torch.cat([ub, vb], dim=0).contiguous()
+        mlp_in = torch.empty(n, 2 * f, dtype=s.dtype, device=s.device)
+        inner = torch.empty_like(s) if last else None       # a last layer's post and ga read it instead of recomputing [uv | vv]
+        _lib.call("hgb_painn_update_tc_fwd", _p(v), _p(s), _p(wuv), _p(buv), n, _p(mlp_in), _p(inner), _stream())
+        h, z1, deriv = linear_fwd_dispatch_ex(mlp_in, w1, b1, ACT_CODES["silu"], 0.0, want_z=True, z_deriv=True)
+        a, _ = linear_fwd_dispatch(h, w2, b2)
+        ctx.z1_code = ACT_DERIV if deriv else ACT_CODES["silu"]
+        s_out = torch.empty_like(s)
+        v_out = None if last else torch.empty_like(v)
+        _lib.call("hgb_painn_update_tc_post", _p(v), _p(s), _p(a), _p(inner), _p(wuv), _p(buv), n, int(last), _p(s_out), _p(v_out),
+                  _stream())
+        ctx.save_for_backward(v, mlp_in, z1, h, a, wuv, buv, w1, w2, inner)
+        ctx.last = bool(last)
+        ctx.leaves = ([uw, ub, vw, vb], [w1, b1], [w2, b2])
+        if last:
+            return s_out, s_out.new_zeros(0)
+        return s_out, v_out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gs_out, gv_out):
+        v, mlp_in, z1, h, a, wuv, buv, w1, w2, inner = ctx.saved_tensors
+        last = ctx.last
+        n, f = mlp_in.shape[0], v.shape[2]
+        gs_out = _aligned(gs_out)
+        gv_out = None if last else _aligned(gv_out)
+        ga = torch.empty_like(a)
+        _lib.call("hgb_painn_update_tc_bwd_a", _p(v), _p(gs_out), _p(gv_out), _p(inner), _p(wuv), _p(buv), n, int(last), _p(ga), _stream())
+        with tensor_cores(True):
+            gz1, gw2, gb2 = linear_bwd_dispatch(ga, h, w2, dx_gsrc=z1, dx_gact=ctx.z1_code, leaves=ctx.leaves[2])     # dgrad through the SiLU
+            g_mlp_in, gw1, gb1 = linear_bwd_dispatch(gz1, mlp_in, w1, leaves=ctx.leaves[1])
+        g_uv = torch.empty(3 * n, 2 * f, dtype=v.dtype, device=v.device)            # [guv | gvv]
+        gs, gv = torch.empty_like(gs_out), torch.empty_like(v)
+        _lib.call("hgb_painn_update_tc_bwd", _p(v), _p(gs_out), _p(gv_out), _p(g_mlp_in), _p(a), _p(mlp_in), _p(wuv), _p(buv), n, int(last),
+                  _p(g_uv), _p(gs), _p(gv), _stream())
+        with tensor_cores(True):
+            _, gwuv, gbuv = linear_bwd_dispatch(g_uv, v.reshape(3 * n, f), wuv, need_x=False, leaves=ctx.leaves[0])
+        return gs, gv, gwuv[:f], gbuv[:f], gwuv[f:], gbuv[f:], gw1, gb1, gw2, gb2, None
+
+
 SCALAR_UPDATE = os.environ.get("HGB_SCALAR", "1") == "1"   # PaiNN update block at node_size == 1 through the one-kernel path
 
 

@@ -302,7 +302,10 @@ class PainnUpdate(nn.Module):
                 return s + a_sv * inner + a_ss, None
             a_vv, a_sv, a_ss = torch.split(a, f, dim=1)
             return s + a_sv * inner + a_ss, v + a_vv.unsqueeze(1) * uv
-        fn = ops.PainnUpdateScalarFn if (f == 1 and ops.SCALAR_UPDATE) else ops.PainnUpdateFn   # width-1 layer (quirk Q4)
+        if f == 1 and ops.SCALAR_UPDATE:                        # width-1 layer (quirk Q4)
+            fn = ops.PainnUpdateScalarFn
+        else:
+            fn = ops.PainnUpdateTcFn if ops.painn_update_tc_ok(s, v) else ops.PainnUpdateFn
         s_out, v_out = fn.apply(s, v, self.update_U.weight, self.update_U.bias, self.update_V.weight,
                                                self.update_V.bias, self.update_mlp[0].weight, self.update_mlp[0].bias,
                                                self.update_mlp[2].weight, self.update_mlp[2].bias, self.last_layer)

@@ -311,6 +311,24 @@ int hgb_painn_update_bwd(const float* gs_out, const float* gv_out, const float* 
                          const float* a, const float* uv, const float* vv, int64_t ld, const float* mlp_in,
                          int32_t n, int32_t f, int32_t last, float* guv, float* gvv, float* gs,
                          float* gv, hgb_stream_t stream);
+/* The same block at f = 64 in TF32 mode on the tensor cores (hgb_painn_tc.cu), without the [3n, 2f] U/V product in
+ * memory: every call recomputes [uv | vv] = v [U; V]^T + [bu; bv] from v [n,3,64] per 64-node tile, with the same
+ * products and the same elementwise formulas as hgb_tc_linear + the calls above, so the results are the same bits.
+ * wuv [128,64] = [U; V], buv [128].  Every pointer 16-byte aligned, every tensor dense.
+ * fwd:   mlp_in [n,128] = [ |vv| , s ]; inner [n,64] = sum_d uv.vv (optional: NULL skips it)  (then a = mlp(mlp_in))
+ * post:  s_out, v_out (not last) as hgb_painn_update_post_fwd; last: elementwise from `inner` (v, wuv, buv unused)
+ * bwd_a: ga as hgb_painn_update_post_bwd_a; last: elementwise from `inner`  (then the update_mlp backward: g_mlp_in)
+ * bwd:   gs; g_uv [3n,128] = [guv | gvv] as hgb_painn_update_bwd (the operand of the U/V weight gradient); gv [n,3,64] =
+ *        g_uv [U; V] (+ gv_out when not last), the U/V data gradient computed in the same kernel.                   */
+int hgb_painn_update_tc_fwd(const float* v, const float* s, const float* wuv, const float* buv, int32_t n,
+                            float* mlp_in, float* inner, hgb_stream_t stream);
+int hgb_painn_update_tc_post(const float* v, const float* s, const float* a, const float* inner, const float* wuv,
+                             const float* buv, int32_t n, int32_t last, float* s_out, float* v_out, hgb_stream_t stream);
+int hgb_painn_update_tc_bwd_a(const float* v, const float* gs_out, const float* gv_out, const float* inner,
+                              const float* wuv, const float* buv, int32_t n, int32_t last, float* ga, hgb_stream_t stream);
+int hgb_painn_update_tc_bwd(const float* v, const float* gs_out, const float* gv_out, const float* g_mlp_in,
+                            const float* a, const float* mlp_in, const float* wuv, const float* buv, int32_t n,
+                            int32_t last, float* g_uv, float* gs, float* gv, hgb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * GPS global attention  (hydragnn/globalAtt/gps.py:126-133; ATen SDPA inside nn.MultiheadAttention)

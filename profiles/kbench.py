@@ -53,10 +53,47 @@ def tc_linear_calls(n):
     return res
 
 
+def painn_update_calls(n, f=64):
+    """The F = 64 PaiNN update block of the C2 step in TF32 mode, fused (PainnUpdateTcFn) and unfused (PainnUpdateFn), forward and
+    backward (weight gradients included, on one stream).  GB/s: algorithmic bytes, in units U = one [n, 64] fp32 tensor, counting
+    every tensor each kernel reads and writes (DESIGN.md section 4), over device time."""
+    from hydragnn_b200.stacks import PainnUpdate
+    # (forward, backward) bytes in U, by last.  Fused: fwd [|vv|, s] (+ inner) 7 | 6, MLP 4 + (3 | 4), post 5 | 11; bwd ga 4 | 10,
+    # dgrads 4 + 3 (5 + 3), [guv | gvv] + gv 18 | 22, weight gradients 15 | 16.  Unfused: fwd U/V 9, pre 6, MLP 4 + (3 | 4), post 10 | 17; bwd
+    # post_bwd_a 9 | 13, dgrads 4 + 3 (5 + 3), update_bwd 18 | 24, U/V dgrad 9 | 12, weight gradients 15 | 16.
+    units = {("fused", True): (19, 44), ("fused", False): (25, 56), ("unfused", True): (32, 58), ("unfused", False): (40, 72)}
+    U = n * f * 4
+    res = {}
+    overlap = ops.WGRAD_OVERLAP
+    ops.WGRAD_OVERLAP = False
+    try:
+        for last in (True, False):
+            upd = PainnUpdate(f, last).to(dev)
+            params = [upd.update_U.weight, upd.update_U.bias, upd.update_V.weight, upd.update_V.bias, upd.update_mlp[0].weight,
+                      upd.update_mlp[0].bias, upd.update_mlp[2].weight, upd.update_mlp[2].bias]
+            s = torch.randn(n, f, device=dev, requires_grad=True)
+            v = torch.randn(n, 3, f, device=dev, requires_grad=True)
+            for kind, fn in (("fused", ops.PainnUpdateTcFn), ("unfused", ops.PainnUpdateFn)):
+                with ops.tensor_cores(True):
+                    so, vo = fn.apply(s, v, *params, last)
+                    outs = (so,) if last else (so, vo)
+                    grads = tuple(torch.randn_like(o) for o in outs)
+                    t_f = timeit(lambda: fn.apply(s, v, *params, last))
+                    t_b = timeit(lambda: torch.autograd.grad(outs, [s, v] + params, grads, retain_graph=True))
+                uf, ub = units[(kind, last)]
+                res["painn_update %s last=%s fwd (ms | GB/s | U)" % (kind, last)] = (round(t_f, 4), round(uf * U / t_f / 1e6, 1), uf)
+                res["painn_update %s last=%s bwd (ms | GB/s | U)" % (kind, last)] = (round(t_b, 4), round(ub * U / t_b / 1e6, 1), ub)
+    finally:
+        ops.WGRAD_OVERLAP = overlap
+    return res
+
+
 G = 16384
 b = make_samples("qm9_painn", G).to(dev); b._num_graphs = G
 if os.environ.get("KBENCH_ONLY") == "tc_linear":
     print(json.dumps(tc_linear_calls(b.pos.shape[0]), indent=1)); sys.exit(0)
+if os.environ.get("KBENCH_ONLY") == "painn_update":
+    print(json.dumps(painn_update_calls(b.pos.shape[0]), indent=1)); sys.exit(0)
 b = hb.get_radius_graph(7.0, 5)(b)
 plan = Base.plan_for(b)
 n, e, f, r = plan.num_nodes, plan.num_edges, 64, 5
