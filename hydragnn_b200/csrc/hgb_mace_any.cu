@@ -17,6 +17,11 @@
 //       chan_rp  o[b, i, c]    = sum_p g[b, c, p] t[b, c, p, i]        ("reduce p")
 //     again mutually adjoint.  The U-matrix x weight products in front of them are plain MatMuls (closed already).
 //
+// (3) edge-attribute mixing of the 0e paths' weight blocks (edge_dim > 0):
+//       edge_mix    o[e, u]    = c * sum_v w[e, u, v] a[e, v]          a = [edge_attr, 1]
+//       edge_mix_t  o[e, u, v] = c * g[e, u] a[e, v]
+//     mutually adjoint and linear in w / g; the edge attributes are data.
+//
 // All are bandwidth-trivial elementwise-style SIMT kernels: one thread per output element (tp_y: one warp per edge).
 #include "hgb_common.cuh"
 
@@ -139,7 +144,47 @@ __global__ void chan_rp_kernel(const float* __restrict__ g, const float* __restr
   }
 }
 
+// edge-attribute mixing of a 0e path's [F, d+1] weight block; one thread per output element
+__global__ void edge_mix_kernel(const float* __restrict__ w, int64_t ld, const float* __restrict__ ea, int64_t e, int f, int d, float c,
+                                float* __restrict__ out) {
+  const int64_t total = e * f;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t ed = idx / f;
+    const int u = (int)(idx - ed * f);
+    const float* q = w + ed * ld + (int64_t)u * (d + 1);
+    float s = q[d];
+    for (int v = 0; v < d; ++v) s = fmaf(q[v], ea[ed * d + v], s);
+    out[idx] = c * s;
+  }
+}
+
+__global__ void edge_mix_t_kernel(const float* __restrict__ g, int64_t ld, const float* __restrict__ ea, int64_t e, int f, int d, float c,
+                                  float* __restrict__ out) {
+  const int64_t total = e * f * (d + 1);
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t eu = idx / (d + 1);
+    const int v = (int)(idx - eu * (d + 1));
+    const int64_t ed = eu / f;
+    const int u = (int)(eu - ed * f);
+    const float gv = c * g[ed * ld + u];
+    out[idx] = v < d ? gv * ea[ed * d + v] : gv;
+  }
+}
+
 }  // namespace
+
+extern "C" int hgb_mace_edge_mix(int32_t mode, const float* src, int64_t ld, const float* eattr, int64_t e, int32_t f, int32_t d, float c,
+                                 float* out, hgb_stream_t stream) {
+  HGB_REQUIRE((mode == 0 || mode == 1) && src && eattr && out && e >= 0 && f >= 1 && d >= 1 &&
+                  ld >= (mode == 0 ? (int64_t)f * (d + 1) : (int64_t)f),
+              "mace_edge_mix: bad arguments");
+  if (e == 0) return HGB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (mode == 0) edge_mix_kernel<<<hgb_grid_for(e * f, 256), 256, 0, st>>>(src, ld, eattr, e, f, d, c, out);
+  else edge_mix_t_kernel<<<hgb_grid_for(e * f * (d + 1), 256), 256, 0, st>>>(src, ld, eattr, e, f, d, c, out);
+  HGB_LAUNCH_CHECK("mace_edge_mix");
+  return HGB_OK;
+}
 
 #define HGB_TP_CHECK(name)                                                                                               \
   HGB_REQUIRE(e >= 0 && f >= 1 && ni >= 1 && nj >= 1 && nk >= 1 && ni <= 7 && nj <= 7 && nk <= 7 && cg && out, name ": bad arguments")

@@ -98,17 +98,23 @@ class RadialMLP(nn.Module):
 class Interaction(nn.Module):
     """RealAgnosticAttResidualInteractionBlock (blocks.py:297-402)."""
 
-    def __init__(self, channels, lmax_in, lmax_sh, lmax_hidden, num_radial, avg_num_neighbors):
+    def __init__(self, channels, lmax_in, lmax_sh, lmax_hidden, num_radial, avg_num_neighbors, edge_dim=0):
         super().__init__()
         f = channels
-        self.f, self.lmax_in, self.lmax_sh, self.avg = f, lmax_in, lmax_sh, avg_num_neighbors
+        self.f, self.lmax_in, self.lmax_sh, self.avg, self.edge_dim = f, lmax_in, lmax_sh, avg_num_neighbors, edge_dim
         feats = e3.hidden_irreps(f, lmax_in)
         target = e3.hidden_irreps(f, lmax_sh)
         hidden = e3.hidden_irreps(f, lmax_hidden)
         self.paths = e3.tp_paths(lmax_in, lmax_sh, lmax_sh)
+        # edge irreps (D+1)x0e + 1x1o + ... (MACEStack.py:198-203): a path whose edge irrep is 0e has a [F, D+1] weight block
+        # (u-major) in tpw, every other path F weights; _wcol[k] = first tpw column of path k
+        self._wcol, col = [], 0
+        for (_, l2, _) in self.paths:
+            self._wcol.append(col)
+            col += f * (edge_dim + 1 if l2 == 0 else 1)
         self.linear_up = E3Linear(feats, feats)
         self.linear_down = E3Linear(feats, [(f, 0, 1)])
-        self.conv_tp_weights = RadialMLP([num_radial + 2 * f] + 3 * [f] + [len(self.paths) * f])
+        self.conv_tp_weights = RadialMLP([num_radial + 2 * f] + 3 * [f] + [col])
         n_paths = [sum(1 for p in self.paths if p[2] == l) for l in range(lmax_sh + 1)]
         self.linear = E3Linear([(n_paths[l] * f, l, (-1) ** l) for l in range(lmax_sh + 1) if n_paths[l]], target)
         self.skip_linear = E3Linear(feats, hidden)
@@ -116,17 +122,18 @@ class Interaction(nn.Module):
         for k, (l1, l2, l3) in enumerate(self.paths):
             self.register_buffer("_cg%d" % k, (e3.w3j(l1, l2, l3) * math.sqrt(2 * l3 + 1)).float(), persistent=False)
 
-    def forward(self, xs, sh, radial, plan, higher=False):
-        f = self.f
+    def forward(self, xs, sh, radial, plan, higher=False, eattr=None):
+        f, d = self.f, self.edge_dim
         sc = self.skip_linear(xs, higher)
         up = self.linear_up(xs, higher)
         down = self.linear_down(xs, higher)[0].reshape(-1, f)
         gather = ops.GatherRows.apply
         tpw = self.conv_tp_weights.forward_split(radial, down, plan, higher)         # [E, n_paths * F]
         e = tpw.shape[0]
-        if not higher and ops.mace_tp_supported(self.lmax_in, self.lmax_sh, f):
-            # fused: coupling, path weights and the scatter over receivers in one kernel; mji [E, F (L+1)^2] never exists
-            packed = ops.MaceTpScatterFn.apply(torch.cat(up, dim=1), sh, tpw, plan, self.lmax_in, self.lmax_sh)
+        if not higher and ops.mace_tp_supported(self.lmax_in, self.lmax_sh, f, d):
+            # fused: coupling, path weights (mixed with the edge attributes) and the scatter over receivers in one kernel;
+            # mji [E, F (L+1)^2] never exists
+            packed = ops.MaceTpScatterFn.apply(torch.cat(up, dim=1), sh, tpw, plan, self.lmax_in, self.lmax_sh, eattr)
             n, msgs, off = up[0].shape[0], [], 0
             for l3 in range(self.lmax_sh + 1):
                 n_p = sum(1 for p in self.paths if p[2] == l3)
@@ -142,7 +149,13 @@ class Interaction(nn.Module):
         per_l = [[] for _ in range(self.lmax_sh + 1)]
         for k, (l1, l2, l3) in enumerate(self.paths):
             y = sh[:, l2 * l2:(l2 + 1) ** 2]
-            per_l[l3].append(ops.TpOut.apply(up_s[l1], y, tpw[:, k * f:(k + 1) * f], getattr(self, "_cg%d" % k)))   # [E, 2l3+1, F]
+            c0 = self._wcol[k]
+            if l2 == 0 and d:
+                # c = sqrt((2 l3 + 1) / (D + 1)): the 1/sqrt(D + 1) goes with the mixing, sqrt(2 l3 + 1) stays in _cg
+                w = ops.EdgeMix.apply(tpw[:, c0:c0 + f * (d + 1)], eattr, 1.0 / math.sqrt(d + 1))
+            else:
+                w = tpw[:, c0:c0 + f]
+            per_l[l3].append(ops.TpOut.apply(up_s[l1], y, w, getattr(self, "_cg%d" % k)))   # [E, 2l3+1, F]
         msgs = []
         for l3, parts in enumerate(per_l):
             if parts:
@@ -243,8 +256,8 @@ class MaceConv(nn.Module):
         super().__init__()
         self.module_1, self.module_2, self.module_3 = inter, prod, sizing
 
-    def forward(self, xs, sh, radial, plan, zcsr, higher=False):
-        msgs, sc = self.module_1(xs, sh, radial, plan, higher)
+    def forward(self, xs, sh, radial, plan, zcsr, higher=False, eattr=None):
+        msgs, sc = self.module_1(xs, sh, radial, plan, higher, eattr)
         return self.module_3(self.module_2(msgs, sc, zcsr, higher), higher)
 
 
@@ -343,7 +356,8 @@ class MultiheadDecoder(nn.Module):
 
 
 class MACEStack(nn.Module):
-    """hydragnn/models/MACEStack.py:70-498 (no GPS wrapping, no graph-attr conditioning, no edge_attr)."""
+    """hydragnn/models/MACEStack.py:70-498 (no GPS wrapping, no graph-attr conditioning).  With edge_dim = D > 0 every
+    convolution reads ``data.edge_attr`` [E, D] as D extra 0e edge irreps in front of the spherical harmonics."""
 
     def __init__(self, r_max, radial_type, distance_transform, num_bessel, edge_dim, max_ell, node_max_ell, avg_num_neighbors,
                  num_polynomial_cutoff, correlation, input_dim, hidden_dim, output_dim, output_type, config_heads,
@@ -352,13 +366,13 @@ class MACEStack(nn.Module):
         super().__init__()
         if global_attn_engine:
             raise ValueError("b200 engine: MACE inside GPS is not implemented")
-        if edge_dim:
-            raise ValueError("b200 engine: MACE with edge_attr is not implemented")
         if distance_transform in ("Agnesi", "Soft"):
             raise ValueError("b200 engine: MACE distance transforms need ase covalent radii and are not implemented")
         if max_ell > 3:
             raise ValueError("b200 engine: MACE max_ell <= 3")
         self.input_dim, self.hidden_dim, self.num_conv_layers, self.num_nodes = input_dim, hidden_dim, num_conv_layers, num_nodes
+        self.edge_dim = int(edge_dim or 0)
+        self.use_edge_attr = self.edge_dim > 0
         self.max_ell, self.node_max_ell, self.avg_num_neighbors = max_ell, node_max_ell, avg_num_neighbors
         self.head_dims, self.head_type = list(output_dim), list(output_type)
         self.num_heads, self.config_heads = len(self.head_dims), config_heads
@@ -433,7 +447,7 @@ class MACEStack(nn.Module):
     def _get_conv(self, lmax_in, last_layer):
         f = self.hidden_dim
         lmax_hidden = 0 if last_layer else self.node_max_ell
-        inter = Interaction(f, lmax_in, self.max_ell, lmax_hidden, self.num_bessel, self.avg_num_neighbors)
+        inter = Interaction(f, lmax_in, self.max_ell, lmax_hidden, self.num_bessel, self.avg_num_neighbors, self.edge_dim)
         prod = Product(f, self.max_ell, lmax_hidden, self.correlation[0])
         hid = e3.hidden_irreps(f, lmax_hidden)
         return MaceConv(inter, prod, E3Linear(hid, hid))
@@ -487,6 +501,7 @@ class MACEStack(nn.Module):
         gsum = ops.SegmentSum.apply(pos, ops.Csr(gcsr.idx, gcsr.rowptr, None, gcsr.n))
         pos = pos - ops.GatherRows.apply(gsum / cnt[:, None], gcsr)
         shifts = getattr(data, "edge_shifts", None)
+        eattr = self._edge_attr(data, plan.num_edges) if self.use_edge_attr else None
         if not higher and self.radial_type == "bessel" and EDGE_EMBED_KERNEL:
             # first-order path: geometry, spherical harmonics and Bessel x cutoff of every edge in ONE kernel (SURVEY K2)
             sh, radial = ops.MaceEdgeEmbedFn.apply(pos, shifts, plan, self.max_ell, self.num_bessel, self.radius, self.p_cut)
@@ -515,11 +530,23 @@ class MACEStack(nn.Module):
         onehot = torch.nn.functional.one_hot(z, NUM_ELEMENTS).to(pos.dtype)
         outputs = self.multihead_decoders[0](onehot, self._pool(onehot, gcsr, higher), batch, num_graphs, ds, higher)
         for conv, readout in zip(self.graph_convs, self.multihead_decoders[1:]):
-            xs = conv(xs, sh, radial, plan, zcsr, higher)
+            xs = conv(xs, sh, radial, plan, zcsr, higher, eattr)
             scalars = xs[0][:, 0, :]
             out = readout(scalars, self._pool(scalars, gcsr, higher), batch, num_graphs, ds, higher)
             outputs = [a + b for a, b in zip(outputs, out)]
         return outputs
+
+    def _edge_attr(self, data, num_edges):
+        """data.edge_attr as read by MACEStack.py:459-461.  Edge attributes are data, as every preprocessing produces them."""
+        ea = getattr(data, "edge_attr", None)
+        if ea is None:
+            raise ValueError("MACE with edge_dim=%d needs data.edge_attr [E, %d]" % (self.edge_dim, self.edge_dim))
+        if ea.dim() != 2 or tuple(ea.shape) != (num_edges, self.edge_dim) or ea.dtype != torch.float32:
+            raise ValueError("MACE edge_attr must be a float32 [E, edge_dim] = [%d, %d] tensor, got %s %s"
+                             % (num_edges, self.edge_dim, ea.dtype, tuple(ea.shape)))
+        if ea.requires_grad:
+            raise ValueError("MACE edge_attr must not require grad: edge attributes are data (detach them)")
+        return ea.contiguous()
 
     def _pool(self, x, gcsr, higher):
         if higher and self.graph_pooling != "max":

@@ -1408,32 +1408,39 @@ class EdgeLenBwdFn(torch.autograd.Function):
 # =====================================================================================================
 # MACE: fused tensor-product + scatter, symmetric contraction (first-order blocks)
 # =====================================================================================================
-def mace_tp_supported(lin, lsh, f):
-    return 0 <= lin <= 2 and 1 <= lsh <= 3 and lin <= lsh and f % 32 == 0
+MACE_TP_MAX_EDGE_DIM = 16       # MACE_TP_MAX_D of hgb_mace.cu: the largest edge_dim whose per-edge stage fits in shared memory
+
+
+def mace_tp_supported(lin, lsh, f, edge_dim=0):
+    return 0 <= lin <= 2 and 1 <= lsh <= 3 and lin <= lsh and f % 32 == 0 and 0 <= edge_dim <= MACE_TP_MAX_EDGE_DIM
 
 
 class MaceTpScatterFn(torch.autograd.Function):
-    """conv_tp + scatter-sum over receivers in one kernel (blocks.py:390-395).  up [N, S_in, F], sh [E, S_sh], tpw [E, P F];
-    returns the packed message buffer (per output degree l3 a [N, 2l3+1, n_paths(l3) F] block)."""
+    """conv_tp + scatter-sum over receivers in one kernel (blocks.py:390-395).  up [N, S_in, F], sh [E, S_sh], tpw [E, W];
+    returns the packed message buffer (per output degree l3 a [N, 2l3+1, n_paths(l3) F] block).  eattr: None (W = P F) or the
+    edge attributes [E, D]; then W = (P + D (lin + 1)) F, the 0e paths' [F, D+1] blocks in the reference's layout."""
 
     @staticmethod
-    def forward(ctx, up, sh, tpw, plan, lin, lsh):
+    def forward(ctx, up, sh, tpw, plan, lin, lsh, eattr=None):
         up, sh, tpw = _chk(up.contiguous()), _chk(sh.contiguous()), _chk(tpw.contiguous())
+        eattr = None if eattr is None else _chk(eattr.contiguous())
+        d = 0 if eattr is None else eattr.shape[1]
         n, f = up.shape[0], up.shape[2]
         nacc = _lib.query("hgb_mace_tp_num_acc", lin, lsh)
         out = torch.empty(nacc * n * f, dtype=up.dtype, device=up.device)
         csr = plan.by_col
         _lib.call("hgb_mace_tp_scatter_fwd", _p(up), _p(sh), _p(tpw), _p(csr.rowptr), _p(csr.perm), _p(plan.nbr("col")), n, f, lin, lsh,
-                  sh.shape[1], _p(out), _stream())
-        ctx.save_for_backward(up, sh, tpw)
+                  sh.shape[1], _p(eattr), d, _p(out), _stream())
+        ctx.save_for_backward(up, sh, tpw, eattr)
         ctx.plan, ctx.cfg = plan, (lin, lsh)
         return out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, g):
-        up, sh, tpw = ctx.saved_tensors
+        up, sh, tpw, eattr = ctx.saved_tensors
         plan, (lin, lsh) = ctx.plan, ctx.cfg
+        d = 0 if eattr is None else eattr.shape[1]
         n, s_in, f = up.shape
         e = tpw.shape[0]
         g = _chk(g.contiguous())
@@ -1442,9 +1449,9 @@ class MaceTpScatterFn(torch.autograd.Function):
         g_sh = torch.zeros_like(sh) if ctx.needs_input_grad[1] else None
         csr = plan.by_col
         _lib.call("hgb_mace_tp_scatter_bwd", _p(g), _p(up), _p(sh), _p(tpw), _p(csr.rowptr), _p(csr.perm), _p(plan.nbr("col")), n, f, lin,
-                  lsh, sh.shape[1], _p(g_tpw), _p(g_up_e), _p(g_sh), _stream())
+                  lsh, sh.shape[1], _p(eattr), d, _p(g_tpw), _p(g_up_e), _p(g_sh), _stream())
         g_up = raw_segment_sum(g_up_e, plan.by_row.rowptr, plan.by_row.perm, n).reshape(n, s_in, f) if ctx.needs_input_grad[0] else None
-        return g_up, g_sh, g_tpw, None, None, None
+        return g_up, g_sh, g_tpw, None, None, None, None
 
 
 def mace_sc_supported(lin, lout, correlation):
@@ -1540,6 +1547,50 @@ class TpW(torch.autograd.Function):
         gy = TpY.apply(a, g, gw, cg) if ctx.needs_input_grad[1] else None
         gg = TpOut.apply(a, y, gw, cg) if ctx.needs_input_grad[2] else None
         return ga, gy, gg, None
+
+
+def _edge_mix_call(mode, src, eattr, c, f):
+    """mode 0: src = w, rows [.., F (D+1) ..] of stride src.stride(0) -> [E, F];  mode 1: src = g [E, F] -> [E, F (D+1)]."""
+    if not src.is_cuda or src.dtype != torch.float32:
+        raise RuntimeError("mace_edge_mix: expected a float32 CUDA tensor, got %s on %s" % (src.dtype, src.device))
+    if src.stride(1) != 1:                       # rows may be strided (a column block of tpw); columns must be dense
+        src = src.contiguous()
+    e, d = eattr.shape
+    out = torch.empty(e, f if mode == 0 else f * (d + 1), dtype=src.dtype, device=src.device)
+    _lib.call("hgb_mace_edge_mix", mode, _p(src), src.stride(0), _p(eattr), e, f, d, float(c), _p(out), _stream())
+    return out
+
+
+class EdgeMix(torch.autograd.Function):
+    """o[e, u] = c sum_v w[e, u, v] a[e, v], a = [edge_attr, 1]: the per-edge weight of a 0e tensor-product path when the edge
+    irreps carry edge attributes (MACEStack.py:198-203).  w [E, F (D+1)] may be a column block of tpw.  Its adjoint is
+    EdgeMixT and vice versa, so every derivative order stays on hgb_mace_edge_mix.  eattr is data (no gradient)."""
+
+    @staticmethod
+    def forward(ctx, w, eattr, c):
+        ctx.save_for_backward(eattr)
+        ctx.c = c
+        return _edge_mix_call(0, w, eattr, c, w.shape[1] // (eattr.shape[1] + 1))
+
+    @staticmethod
+    def backward(ctx, g):
+        eattr, = ctx.saved_tensors
+        return EdgeMixT.apply(g, eattr, ctx.c), None, None
+
+
+class EdgeMixT(torch.autograd.Function):
+    """o[e, u, v] = c g[e, u] a[e, v] as [E, F (D+1)]."""
+
+    @staticmethod
+    def forward(ctx, g, eattr, c):
+        ctx.save_for_backward(eattr)
+        ctx.c = c
+        return _edge_mix_call(1, g, eattr, c, g.shape[1])
+
+    @staticmethod
+    def backward(ctx, go):
+        eattr, = ctx.saved_tensors
+        return EdgeMix.apply(go, eattr, ctx.c), None, None
 
 
 def _chan_call(mode, p0, p1, n, f, p, ni, out_shape):

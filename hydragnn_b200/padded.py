@@ -66,6 +66,11 @@ class PaddedGraphStep:
             raise ValueError("PaddedGraphStep: this model (global attention / node heads / branches) needs the eager train_step")
         self.model, self.opt, self.mlip, self.nb = model, opt, bool(compute_grad_energy), neighbour_build
         self.m = model.module
+        inner = getattr(self.m, "model", self.m)
+        reads_edge_attr = bool(getattr(inner, "use_edge_attr", False))
+        if neighbour_build and reads_edge_attr:
+            raise ValueError("PaddedGraphStep: neighbour_build makes edges without features, but this model reads edge_attr "
+                             "(edge_dim > 0); pass edge_index and edge_attr with every batch instead")
         self.dev = next(model.parameters()).device
         self.ws = dist.get_world_size() if dist.is_initialized() else 1
         self.capture_allreduce = capture_allreduce
@@ -73,7 +78,8 @@ class PaddedGraphStep:
         n, g = int(first_batch.pos.shape[0]), int(first_batch.num_graphs)
         e = 0 if neighbour_build else int(first_batch.edge_index.shape[1])
         self._widths = {k: (tuple(v.shape[1:]), v.dtype) for k, v in first_batch.items()
-                        if torch.is_tensor(v) and k in ("x", "pos", "y", "energy", "forces", "edge_shifts")}
+                        if torch.is_tensor(v) and (k in ("x", "pos", "y", "energy", "forces", "edge_shifts")
+                                                   or k == "edge_attr" and reads_edge_attr)}
         self._capture(node_cap or n, edge_cap or e, graph_cap or g)
         self.recaptures = 0
 
@@ -91,7 +97,7 @@ class PaddedGraphStep:
         hosts = [{}, {}]                                   # two pinned staging sets: the host fills one while the other's copy is in flight
         for key, (tail, dt) in self._widths.items():
             rows = {"x": self.n_cap, "pos": self.n_cap, "forces": self.n_cap, "y": self.g_cap, "energy": self.g_cap,
-                    "edge_shifts": self.e_cap}[key]
+                    "edge_shifts": self.e_cap, "edge_attr": self.e_cap}[key]
             if key == "edge_shifts" and self.nb:
                 continue
             for h in hosts:
@@ -139,7 +145,7 @@ class PaddedGraphStep:
             e_real = self.valid[2:3]
         _lib.call("hgb_pad_edges", _p(e_real), _p(self.valid[1:2]), self.n_cap, self.e_cap, _p(d.edge_index), _p(ops.guard_flag(self.dev)),
                   _stream())
-        for key in ("_hgb_plan", "_hgb_gcsr", "_hgb_col_sorted"):
+        for key in ("_hgb_plan", "_hgb_gcsr", "_hgb_col_sorted", "_hgb_zcsr"):     # MACE's element CSR follows x of each batch
             d.__dict__.pop(key, None)
         self.opt.zero_grad()
         if self.mlip:

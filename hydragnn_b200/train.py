@@ -267,7 +267,7 @@ class GraphedTrainStep:
     def _fwd_bwd(self):
         m = self.model.module
         d = self.data
-        for k in ("_hgb_plan", "_hgb_gcsr"):          # index plans are part of the step (ADVICE r1: stale CSR after refill)
+        for k in ("_hgb_plan", "_hgb_gcsr", "_hgb_zcsr"):   # index plans are part of the step (ADVICE r1: stale CSR after refill)
             d.__dict__.pop(k, None)
         self.opt.zero_grad()
         if self.mlip:

@@ -369,6 +369,13 @@ int hgb_mace_tp_path(int32_t mode, const float* p0, const float* p1, const float
 int hgb_mace_chan_contract(int32_t mode, const float* p0, const float* p1, int64_t n, int32_t f, int32_t p, int32_t ni,
                            float* out, hgb_stream_t stream);
 
+/* Edge-attribute mixing of a 0e tensor-product path (MACEStack.py:198-203, blocks.py:314-326), a = [eattr, 1] [E, d+1]:
+ *   mode 0: out [e, f]      = c * sum_v w[e, f*(d+1) + v] a[e, v]    (w: rows of stride ld >= f*(d+1), e.g. a column block of tpw)
+ *   mode 1: out [e, f*(d+1)] = c * g[e, f] a[e, f-major, v]            (g: rows of stride ld >= f)
+ * The two modes are each other's adjoint.  eattr [E, d] dense, d >= 1.                                                    */
+int hgb_mace_edge_mix(int32_t mode, const float* src, int64_t ld, const float* eattr, int64_t e, int32_t f, int32_t d, float c,
+                      float* out, hgb_stream_t stream);
+
 /* MACE edge embedding in one pass per edge (SURVEY K2): vec = pos[col] - pos[row] + shift -> real spherical harmonics
  * sh [e, (lmax+1)^2] (component normalisation, e3nn axis convention; MACEStack.py:455-466) and the Bessel basis times the
  * polynomial cutoff radial [e, num_bessel] (mace_utils/modules/radial.py:18-60,110-148; blocks.py:164-177).  lmax <= 3.
@@ -516,18 +523,21 @@ int hgb_pna_aggregate_bwd(const float* g_out, const float* m, const float* out, 
 int hgb_mace_tp_num_acc(int32_t lmax_in, int32_t lmax_sh);
 
 /* conv_tp (o3.TensorProduct "uvu", blocks.py:320-327,390) fused with scatter(..., receiver, "sum") (:393-395).
- * up [N,(lmax_in+1)^2,F], sh [E, sh_ld] (first (lmax_sh+1)^2 columns), tpw [E, n_paths*F]; (rowptr, perm, snd): CSR of the
- * receivers with the edge id and the sender of every slot.  out: packed, per output degree l3 a [N, 2l3+1, n_paths(l3)*F]
- * block starting at float offset N*F*acc_base(l3).                                                                      */
+ * up [N,(lmax_in+1)^2,F], sh [E, sh_ld] (first (lmax_sh+1)^2 columns), tpw [E, (n_paths + d*(lmax_in+1))*F]; (rowptr, perm,
+ * snd): CSR of the receivers with the edge id and the sender of every slot.  out: packed, per output degree l3 a
+ * [N, 2l3+1, n_paths(l3)*F] block starting at float offset N*F*acc_base(l3).
+ * Edge attributes (MACEStack.py:198-203): eattr [E, d], 0 <= d <= 16 (NULL when d = 0).  The lmax_in+1 paths whose edge
+ * irrep is 0e then read a [F, d+1] weight block of tpw (u-major, reference layout) mixed with [eattr, 1] / sqrt(d+1).       */
 int hgb_mace_tp_scatter_fwd(const float* up, const float* sh, const float* tpw, const int32_t* rowptr, const int32_t* perm,
-                            const int32_t* snd, int32_t n, int32_t f, int32_t lmax_in, int32_t lmax_sh, int32_t sh_ld, float* out,
-                            hgb_stream_t stream);
+                            const int32_t* snd, int32_t n, int32_t f, int32_t lmax_in, int32_t lmax_sh, int32_t sh_ld,
+                            const float* eattr, int32_t d, float* out, hgb_stream_t stream);
 
-/* backward: g_tpw [E, n_paths*F], g_up_edge [E,(lmax_in+1)^2,F] (per-edge sender gradients; reduce per sender with
+/* backward: g_tpw in tpw's layout, g_up_edge [E,(lmax_in+1)^2,F] (per-edge sender gradients; reduce per sender with
  * hgb_segment_sum), g_sh [E, sh_ld] or NULL (must be zero-filled by the caller when F/64 > 1).                          */
 int hgb_mace_tp_scatter_bwd(const float* g_out, const float* up, const float* sh, const float* tpw, const int32_t* rowptr,
                             const int32_t* perm, const int32_t* snd, int32_t n, int32_t f, int32_t lmax_in, int32_t lmax_sh,
-                            int32_t sh_ld, float* g_tpw, float* g_up_edge, float* g_sh, hgb_stream_t stream);
+                            int32_t sh_ld, const float* eattr, int32_t d, float* g_tpw, float* g_up_edge, float* g_sh,
+                            hgb_stream_t stream);
 
 /* SymmetricContraction with correlation 2 (symmetric_contraction.py:131-239): weight rows per output degree L are
  * [weights_max (P2(L)), weights.0 (P1(L))], concatenated over L: wall [118, KTOT, F]; z [N] element index (0-based);
