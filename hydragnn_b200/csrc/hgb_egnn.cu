@@ -510,12 +510,16 @@ extern "C" int hgb_egnn_edge_bwd_data(const float* g_out, const float* s, const 
                                       const int32_t* rowptr, const int32_t* perm, int32_t n, int32_t h, int32_t nodes_per_tile,
                                       float* g_p, int32_t ldp, float* gz1, float* gs, float* g_wd, float* g_b0, void* workspace,
                                       hgb_stream_t stream) {
-  if (n == 0) return HGB_OK;
   HGB_REQUIRE(hgb_egnn_edge_supported(h), "egnn_edge_bwd_data: hidden width must be 32 or 64 (got %d)", h);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n == 0) {                                          // no edges: the parameter sums are empty (as in hgb_egnn_edge_wgrad)
+    if (g_wd) cudaMemsetAsync(g_wd, 0, (size_t)h * 4, st);
+    if (g_b0) cudaMemsetAsync(g_b0, 0, (size_t)h * 4, st);
+    return HGB_OK;
+  }
   HGB_REQUIRE(g_out && s && wd && w1 && masks && rowptr && perm && g_p && gz1 && gs && nodes_per_tile >= 1 && nodes_per_tile <= NBMAX,
               "egnn_edge_bwd_data: bad arguments");
   HGB_REQUIRE((!g_wd && !g_b0) || (g_wd && g_b0 && workspace), "egnn_edge_bwd_data: g_wd and g_b0 come together and need the workspace");
-  cudaStream_t st = (cudaStream_t)stream;
   const int nb = nodes_per_tile, ntiles = (n + nb - 1) / nb, grid = egnn_grid(n, nb);
   float* partial = (g_wd || g_b0) ? (float*)workspace : nullptr;
   if (h == 64) {

@@ -432,7 +432,7 @@ int hgb_egnn_edge_fwd(const float* pq, const float* s, const float* wd, const fl
                       float* out, hgb_stream_t stream);
 /* gz1_e = mask1 * (W1^T (mask2 * g_out[row(e)])).  Writes g_p [n, h] (row stride ldp) = sum_{row} gz1,
  * gz1 [e, h] in EDGE order (the caller's by-col segment sum gives g_q), gs [e] = w_d . gz1_e and, when
- * g_wd / g_b0 are given (both or neither), g_wd = sum_e s_e gz1_e and g_b0 = sum_e gz1_e.
+ * g_wd / g_b0 are given (both or neither), g_wd = sum_e s_e gz1_e and g_b0 = sum_e gz1_e (zeros at n = 0).
  * workspace: hgb_egnn_edge_workspace_bytes.                                                            */
 int hgb_egnn_edge_bwd_data(const float* g_out, const float* s, const float* wd, const float* w1,
                            const uint64_t* masks, const int32_t* rowptr, const int32_t* perm, int32_t n,

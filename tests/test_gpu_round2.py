@@ -270,7 +270,9 @@ def _egnn_losses(em, gpu, mlip):
 def test_fused_egnn_block_equals_composed_path_and_oracle(name, g, k, mlip):
     """hgb_egnn_edge_{fwd,bwd_data,wgrad} (+ tangent mode in the double backward) against the round-1 composed path
     (gather / Linear / segment-sum closed primitives) and against the oracle: loss terms, and every parameter gradient of the
-    MLIP loss (second derivatives through the fused block).  k = 20 / 64 exercises multi-chunk node tiles."""
+    MLIP loss (second derivatives through the fused block).  k = 20 / 64 gives denser graphs, but the tile rule
+    (ops.egnn_nodes_per_tile: about 120 edges per tile) keeps every tile within one 128-edge chunk and every CTA on one tile
+    at these sizes; tests/test_gpu_egnn_edge.py covers the multi-chunk and multi-tile paths kernel by kernel."""
     w = dict(WORKLOADS[name], max_neighbours=k)
     cpu = make_samples(name, g)
     gpu = make_samples(name, g).to(DEV)
