@@ -7,7 +7,6 @@ in/out projections and the MLP are the engine's Linear kernels; BatchNorm stays 
 the north star); dropout is ATen RNG.
 """
 import math
-import os
 
 import torch
 from torch import nn
@@ -30,9 +29,6 @@ class PyGBatchNorm(nn.Module):
         return self.module(x)
 
 
-TC_ATTENTION = os.environ.get("HGB_TC_ATTENTION", "1") == "1"    # 0: the SIMT kernels of csrc/hgb_attn.cu for every head_dim
-
-
 class MhaFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, qkv, heads):
@@ -42,7 +38,7 @@ class MhaFn(torch.autograd.Function):
         out = torch.empty(n, f, dtype=qkv.dtype, device=qkv.device)
         lse = torch.empty(n, heads, dtype=qkv.dtype, device=qkv.device)
         # head_dim 8: tensor-core kernels (3xTF32 = fp32-level accuracy in fp32 mode, plain TF32 under precision="bf16")
-        ctx.tc = bool(TC_ATTENTION and _lib.query("hgb_mha_tc_supported", f, heads))
+        ctx.tc = bool(_lib.query("hgb_mha_tc_supported", f, heads))
         ctx.exact = 0 if ops._TC["enabled"] else 1
         if ctx.tc:
             _lib.call("hgb_mha_tc_fwd", _p(qkv), n, f, heads, ctx.exact, _p(out), _p(lse), _stream())

@@ -14,7 +14,6 @@ backward), correlation 3 and channel counts that are not a multiple of 32: the p
 composed from gathers / segment sums / MatMuls plus ATen einsum glue.
 """
 import math
-import os
 
 import torch
 from torch import nn
@@ -23,7 +22,6 @@ from . import e3, ops
 from .stacks import (_act_code, activation_function_selection, loss_function_selection, run_mlp)
 
 NUM_ELEMENTS = 118
-EDGE_EMBED_KERNEL = os.environ.get("HGB_MACE_EDGE_EMBED", "1") == "1"   # 0: spherical harmonics / radial basis as ATen glue
 
 
 def _lin(x, w_t, higher, act=None):
@@ -502,7 +500,7 @@ class MACEStack(nn.Module):
         pos = pos - ops.GatherRows.apply(gsum / cnt[:, None], gcsr)
         shifts = getattr(data, "edge_shifts", None)
         eattr = self._edge_attr(data, plan.num_edges) if self.use_edge_attr else None
-        if not higher and self.radial_type == "bessel" and EDGE_EMBED_KERNEL:
+        if not higher and self.radial_type == "bessel":
             # first-order path: geometry, spherical harmonics and Bessel x cutoff of every edge in ONE kernel (SURVEY K2)
             sh, radial = ops.MaceEdgeEmbedFn.apply(pos, shifts, plan, self.max_ell, self.num_bessel, self.radius, self.p_cut)
         else:

@@ -14,8 +14,6 @@ Two layers:
 
 Nothing here falls back to ATen/PyG scatter kernels; a missing library raises in ``_lib.lib()``.
 """
-import os
-
 import torch
 from torch.autograd.function import once_differentiable
 
@@ -94,7 +92,7 @@ class EdgePlan:
         ``graph_ptr`` [G+1] int32 as well, the by-source view is filled graph by graph without a sort."""
         ei = _chk(edge_index, torch.int64)
         self.num_nodes, self.num_edges = int(num_nodes), int(ei.shape[1])
-        if col_rowptr is not None and graph_ptr is not None and GROUPED_CSR:
+        if col_rowptr is not None and graph_ptr is not None:
             self.by_row = csr_build_grouped(ei[0], self.num_nodes, graph_ptr, col_rowptr, graph_ptr.numel() - 1)
         else:
             self.by_row = csr_build(ei[0], self.num_nodes)
@@ -194,30 +192,11 @@ def raw_gemm(a, b, ta, tb, out=None, beta_one=False):
     assert k == k2, "gemm inner dimensions differ"
     if out is None:
         out = torch.empty(m, n, dtype=a.dtype, device=a.device)
-    if gemm3_ok(a, b, out, m, n, k, ta, tb):
-        # fp32-accurate tensor-core path (4xTF32 split products, fp32 register accumulation): csrc/hgb_gemm3.cu
-        nbytes = _lib.query("hgb_gemm3_workspace_bytes", m, n, k, int(ta))
-        ws = _ws(nbytes, a.device) if nbytes else None
-        _lib.call("hgb_gemm3", _p(a), _p(b), _p(out), m, n, k, int(ta), int(tb), a.stride(0), b.stride(0), out.stride(0), int(beta_one),
-                  None, 0, 0.0, None, _p(ws), _stream())
-        return out
     nbytes = _lib.query("hgb_gemm_workspace_bytes", m, n, k, int(ta))
     ws = _ws(nbytes, a.device) if nbytes else None
     _lib.call("hgb_gemm", _p(a), _p(b), _p(out), m, n, k, int(ta), int(tb), a.stride(0), b.stride(0), out.stride(0),
               int(beta_one), _p(ws), nbytes, _stream())
     return out
-
-
-GEMM3 = os.environ.get("HGB_GEMM3", "0") == "1"      # 1: exact-fp32 GEMMs on the 4xTF32 mma.sync kernels (csrc/hgb_gemm3.cu); off by
-                                                     # default (four legacy-path MMAs per product)
-
-
-def gemm3_ok(a, b, out, m, n, k, ta, tb):
-    if not GEMM3 or a.dtype != torch.float32:
-        return False
-    if a.data_ptr() % 16 or out.data_ptr() % 16 or (ta and b.data_ptr() % 16):
-        return False
-    return bool(_lib.query("hgb_gemm3_supported", m, n, k, int(ta), int(tb), a.stride(0), b.stride(0), out.stride(0)))
 
 
 def raw_colsum(x2d):
@@ -228,13 +207,13 @@ def raw_colsum(x2d):
     return out
 
 
-# ---- tensor-core (wgmma / TF32) dense layers: enabled per model by precision="bf16" -----------------
+# ---- tensor-core (wgmma) dense layers: plain TF32 under precision="bf16", the fp32-accurate 3xTF32 split otherwise -----
 _TC = {"enabled": False}
 _DATA_ONLY = {"on": False}     # inside ``only_data_grads()``: the force pass of the MLIP loss
 
 
 class tensor_cores:
-    """Context manager: run the large-M Linear layers on the wgmma TF32 kernels (hgb_tc_*)."""
+    """Context manager: run the large-M Linear layers of the wgmma kernels (hgb_tc_*) in plain TF32, not the 3xTF32 split."""
 
     def __init__(self, enabled=True):
         self.enabled, self.prev = bool(enabled), None
@@ -249,20 +228,12 @@ class tensor_cores:
         return False
 
 
-EXACT_TC = os.environ.get("HGB_EXACT_TC", "1") == "1"     # fp32 mode: large-M Linears on wgmma with the 3xTF32 split (fp32-accurate)
-EXACT_WGRAD = os.environ.get("HGB_EXACT_WGRAD", "1") == "1"   # ... and their weight gradients (0: SIMT fp32 GEMM)
-
-
 def tc_wgrad_ok(m, n_out, k_out, *tensors):
-    """dW = dZ^T X on the wgmma kernel: always in TF32 mode, in fp32 mode when the split variant is enabled"""
-    if not (_TC["enabled"] or (EXACT_TC and EXACT_WGRAD)):
-        return False
+    """dW = dZ^T X on the wgmma kernel (TF32 mode, or the 3xTF32 split in fp32 mode)"""
     return k_out + 16 <= 256 and tc_ok(m, n_out, k_out, *tensors)
 
 
 def tc_ok(m, n_out, k_red, *tensors):
-    if not (_TC["enabled"] or EXACT_TC):
-        return False
     if not _lib.query("hgb_tc_linear_supported", m, n_out, k_red):
         return False
     for t in tensors:
@@ -328,8 +299,6 @@ def raw_smallk_bwd(dy, y, z, x2, w, code=0, param=0.0, need_x=True, need_w=True,
     return dx, dw, db
 
 
-GROUPED_CSR = os.environ.get("HGB_GROUPED_CSR", "1") == "1"   # sort-free by-source CSR for radius-graph edges
-COL_HINT = os.environ.get("HGB_COL_HINT", "1") == "1"   # reuse the radius graph's by-target offsets as the by_col CSR
 ACT_DERIV = 100   # HGB_ACT_DERIV: "the tensor already holds act'(.)"
 
 
@@ -362,7 +331,7 @@ def linear_fwd_dispatch_ex(x2, w, b, code=0, param=0.0, want_z=False, z_deriv=Fa
 # autograd from accumulating into them in place (it only does that to tensors nobody else holds).  Derived weights (scaled, sliced,
 # concatenated: MACE, PNAEq) are read by their own backward nodes right away -- those join immediately; so does everything outside
 # the context, where gradient hooks (torch DDP's reducer, user hooks) may read a gradient the moment it is accumulated.
-WGRAD_OVERLAP = os.environ.get("HGB_WGRAD_OVERLAP", "1") == "1"
+WGRAD_OVERLAP = True          # False: everything on the current stream (a profiler pass that attributes kernels to calls)
 _SIDE = {}
 
 
@@ -583,14 +552,14 @@ class MatMul(torch.autograd.Function):
         ctx.ta, ctx.tb, ctx.tc = ta, tb, _TC["enabled"]
         ctx.b_is_weight = bool(b_is_weight)
         a2, b2 = _row_major_2d(a), _row_major_2d(b)
-        if ctx.tc or EXACT_TC:      # precision "bf16": plain TF32; "fp32": the 3xTF32 split inside the same kernel (exact flag)
-            if not ta and tb and tc_ok(a2.shape[0], b2.shape[0], a2.shape[1], a2):             # [m,k] x [n,k]^T  (the small operand is staged
-                                                                                                 #  by plain loads: any row stride, e.g. a column slice)
-                return raw_tc_linear(a2, b2, False, None, b2.shape[0], a2.shape[1])[0]
-            if not ta and not tb and tc_ok(a2.shape[0], b2.shape[1], a2.shape[1], a2):         # [m,n] x [n,k]
-                return raw_tc_linear(a2, b2, True, None, b2.shape[1], a2.shape[1])[0]
-            if ta and not tb and tc_wgrad_ok(a2.shape[0], a2.shape[1], b2.shape[1], a2, b2):
-                return raw_tc_wgrad(a2, b2, want_bias=False)[0]                                    # [m,n]^T x [m,k]
+        # precision "bf16": plain TF32; "fp32": the 3xTF32 split inside the same kernel (exact flag)
+        if not ta and tb and tc_ok(a2.shape[0], b2.shape[0], a2.shape[1], a2):             # [m,k] x [n,k]^T  (the small operand is staged
+                                                                                             #  by plain loads: any row stride, e.g. a column slice)
+            return raw_tc_linear(a2, b2, False, None, b2.shape[0], a2.shape[1])[0]
+        if not ta and not tb and tc_ok(a2.shape[0], b2.shape[1], a2.shape[1], a2):         # [m,n] x [n,k]
+            return raw_tc_linear(a2, b2, True, None, b2.shape[1], a2.shape[1])[0]
+        if ta and not tb and tc_wgrad_ok(a2.shape[0], a2.shape[1], b2.shape[1], a2, b2):
+            return raw_tc_wgrad(a2, b2, want_bias=False)[0]                                    # [m,n]^T x [m,k]
         return raw_gemm(a2, b2, ta, tb)
 
     @staticmethod
@@ -763,7 +732,7 @@ class Mlp2ScalarFn(torch.autograd.Function):
 
 
 def mlp2(x, w1, b1, act1, p1, w2, b2, act2=None, p2=0.0):
-    if (SCALAR_UPDATE and act2 is None and b1 is not None and b2 is not None and x.dim() == 2 and x.shape[1] == 1
+    if (act2 is None and b1 is not None and b2 is not None and x.dim() == 2 and x.shape[1] == 1
             and w1.shape == (1, 1) and w2.shape[1] == 1 and w2.shape[0] <= 4):
         return Mlp2ScalarFn.apply(x, w1, b1, act1, p1, w2, b2)          # width-1 layer (quirk Q4)
     return Mlp2Fn.apply(x, w1, b1, act1, p1, w2, b2, act2, p2)
@@ -889,10 +858,6 @@ def raw_linear(x2, w, b, code=0, param=0.0, want_z=False):
     n = w.shape[0]
     y = torch.empty(m, n, dtype=x2.dtype, device=x2.device)
     z = torch.empty_like(y) if want_z else None
-    if gemm3_ok(x2, w, y, m, n, k, False, True):
-        _lib.call("hgb_gemm3", _p(x2), _p(w), _p(y), m, n, k, 0, 1, x2.stride(0), w.stride(0), n, 0, _p(b), code, float(param), _p(z), None,
-                  _stream())
-        return y, z
     _lib.call("hgb_linear_fwd", _p(x2), _p(w), _p(b), m, n, k, x2.stride(0), w.stride(0), code, float(param), _p(y), _p(z), _stream())
     return y, z
 
@@ -1023,9 +988,6 @@ class PainnUpdateTcFn(torch.autograd.Function):
         with tensor_cores(True):
             _, gwuv, gbuv = linear_bwd_dispatch(g_uv, v.reshape(3 * n, f), wuv, need_x=False, leaves=ctx.leaves[0])
         return gs, gv, gwuv[:f], gbuv[:f], gwuv[f:], gbuv[f:], gw1, gb1, gw2, gb2, None
-
-
-SCALAR_UPDATE = os.environ.get("HGB_SCALAR", "1") == "1"   # PaiNN update block at node_size == 1 through the one-kernel path
 
 
 class PainnUpdateScalarFn(torch.autograd.Function):
@@ -1202,9 +1164,6 @@ def grouped_mlp(seq_by_group, x, rowptr):
 # =====================================================================================================
 # fused EGNN edge block + closed edge-length primitives (any order of differentiation the MLIP loss needs)
 # =====================================================================================================
-FUSED_EGNN = os.environ.get("HGB_FUSED_EGNN", "1") == "1"     # 0: the round-1 composed path (gather / Linear / segment-sum)
-
-
 class only_data_grads:
     """Context manager for the FORCE pass of the MLIP loss (``torch.autograd.grad(E, pos, create_graph=True)``,
     hydragnn/models/create.py:718-724): fused blocks skip their parameter gradients there -- autograd would compute and drop

@@ -13,8 +13,6 @@ Every conv has two execution modes, selected per forward call:
   differentiated again -- hydragnn/models/create.py:718-724 with ``create_graph=True``): the same math
   composed from the closed primitives GatherRows / SegmentSum / MatMul, with ATen only for elementwise glue.
 """
-import os
-
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -95,7 +93,6 @@ class _Loss:
         return torch.sqrt(val) if self.sqrt else val
 
 
-PAD_MLP = os.environ.get("HGB_PAD_MLP", "1") == "1"
 PAD_MLP_MIN_ROWS = 32768      # below this the chain is launch-bound and the extra pad / slice kernels cost more than the GEMMs save
 
 
@@ -109,7 +106,7 @@ def _padded_chain(mods, x):
     zero-padded (tiny, differentiable ``F.pad``), the activations between the layers stay padded, the result is sliced once at the
     end.  Exact: the padded weight columns are zero, so whatever the activation makes of the padded columns meets a zero weight,
     and the gradient of the padding is dropped by ``F.pad``'s own backward.  Returns [(weight, bias)] per Linear, or None."""
-    if not (PAD_MLP and x.is_cuda and (ops._TC["enabled"] or ops.EXACT_TC)):
+    if not x.is_cuda:
         return None
     k0 = x.shape[-1]
     rows = x.numel() // max(k0, 1)
@@ -190,7 +187,7 @@ class E_GCL(nn.Module):
 
     def _fused_ok(self, x, edge_attr):
         hid = self.edge_mlp[2].weight.shape[0]
-        return (ops.FUSED_EGNN and not self.equivariant and edge_attr is None and x.is_cuda and ops.egnn_edge_supported(hid)
+        return (not self.equivariant and edge_attr is None and x.is_cuda and ops.egnn_edge_supported(hid)
                 and self.edge_mlp[2].weight.shape[1] == hid)
 
     def _forward_fused(self, x, coord, plan, edge_shifts, higher_order, cache):
@@ -302,7 +299,7 @@ class PainnUpdate(nn.Module):
                 return s + a_sv * inner + a_ss, None
             a_vv, a_sv, a_ss = torch.split(a, f, dim=1)
             return s + a_sv * inner + a_ss, v + a_vv.unsqueeze(1) * uv
-        if f == 1 and ops.SCALAR_UPDATE:                        # width-1 layer (quirk Q4)
+        if f == 1:                                              # width-1 layer (quirk Q4)
             fn = ops.PainnUpdateScalarFn
         else:
             fn = ops.PainnUpdateTcFn if ops.painn_update_tc_ok(s, v) else ops.PainnUpdateFn
@@ -539,7 +536,7 @@ class Base(nn.Module):
         ei = data.edge_index
         if plan is None or plan.num_edges != ei.shape[1] or plan.row.device != ei.device or plan._src is not ei:
             hint = data.__dict__.get("_hgb_col_sorted") if hasattr(data, "__dict__") else None     # (edge_index, rowptr[, graph_ptr])
-            ok = ops.COL_HINT and hint is not None and hint[0] is ei
+            ok = hint is not None and hint[0] is ei
             plan = ops.EdgePlan(ei, data.pos.shape[0] if data.pos is not None else data.x.shape[0],
                                 col_rowptr=hint[1] if ok else None, graph_ptr=hint[2] if (ok and len(hint) > 2) else None)
             plan._src = ei

@@ -12,8 +12,6 @@ hydragnn/utils/distributed/distributed.py:396-481, redesigned for one NVSwitch b
 * ``GraphedTrainStep`` captures forward + loss + backward + flatten + optimizer of a fixed-shape batch in a CUDA
   graph (all kernels are launched through ctypes on the capturing stream; nothing synchronises).
 """
-import os
-
 import torch
 import torch.distributed as dist
 
@@ -297,9 +295,6 @@ class GraphedTrainStep:
         return self.loss
 
 
-FAST_TRAIN = os.environ.get("HGB_FAST_TRAIN", "1") == "1"
-
-
 def _train_fast(loader, model, opt, compute_grad_energy, neighbour_build):
     """The epoch through ONE capacity-padded captured step (hydragnn_b200/padded.py): no per-step host synchronisation; the
     epoch sums stay on the device until the end."""
@@ -338,7 +333,7 @@ def train(loader, model, opt, verbosity=0, profiler=None, use_deepspeed=False, c
     dev = next(model.parameters()).device
     from . import padded
     if fast is None:
-        fast = FAST_TRAIN and dev.type == "cuda" and padded.supported(model) and isinstance(opt, FlatAdamW)
+        fast = dev.type == "cuda" and padded.supported(model) and isinstance(opt, FlatAdamW)
     if fast:
         model.train()
         train_error, tasks_error = _train_fast(loader, model, opt, compute_grad_energy, neighbour_build)

@@ -398,18 +398,6 @@ int hgb_grouped_linear(const float* x, int64_t ldx, const float* w, const float*
 int hgb_grouped_wgrad(const float* dy, const float* x, int64_t ldx, const int32_t* rowptr, int32_t groups, int32_t m, int32_t n,
                       int32_t k, float* dw, float* db, hgb_stream_t stream);
 
-/* fp32-ACCURATE tensor-core GEMMs for the exact-fp32 mode (nn.Linear forward / dgrad / wgrad of every stack under
- * precision "fp32", e.g. EGCLStack.py:245-263, PNAEqStack.py:326-476, Base.py heads): mma.sync m16n8k8 TF32 with every
- * product expanded into the four products of a hi/lo split and the long sums kept in fp32 registers (csrc/hgb_gemm3.cu).
- * Same operand convention as hgb_gemm; bias / act / z (pre-activation) only for trans_a == 0.
- * hgb_gemm3_supported tells which shapes take this path (large m or a long reduction; everything else stays on hgb_gemm). */
-int32_t hgb_gemm3_supported(int32_t m, int32_t n, int32_t k, int32_t trans_a, int32_t trans_b, int64_t lda,
-                            int64_t ldb, int64_t ldc);
-int64_t hgb_gemm3_workspace_bytes(int32_t m, int32_t n, int32_t k, int32_t trans_a);
-int hgb_gemm3(const float* a, const float* b, float* c, int32_t m, int32_t n, int32_t k, int32_t trans_a,
-              int32_t trans_b, int64_t lda, int64_t ldb, int64_t ldc, int32_t beta_one, const float* bias,
-              int32_t act, float act_param, float* z, void* workspace, hgb_stream_t stream);
-
 /* ------------------------------------------------------------------------------------------
  * Fused EGNN edge block (hydragnn/models/EGCLStack.py:245-258 edge_model, :256-263 the scatter of
  * node_model, :278-291 forward; unsorted_segment_sum :294-300).  The first Linear of edge_mlp is

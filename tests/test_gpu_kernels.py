@@ -417,10 +417,9 @@ def test_painn_update_vs_oracle(f, last):
 
 @pytest.mark.parametrize("last", [False, True])
 @pytest.mark.parametrize("n", [77, 100003])
-def test_painn_scalar_update_kernel_vs_oracle(last, n, monkeypatch):
+def test_painn_width_one_update_runs_one_kernel_and_matches_oracle(last, n):
     """node_size == 1 (first layer, quirk Q4): the one-kernel update block against the oracle, including the 13 parameter
     gradients that are reduced across blocks."""
-    monkeypatch.setattr(ops, "SCALAR_UPDATE", True)
     g = gen(900 + n)
     torch.manual_seed(3)
     upd_o = oracle.painn.PainnUpdate(1, last)

@@ -12,7 +12,7 @@ import torch
 pytestmark = pytest.mark.gpu
 
 import hydragnn_b200 as hb  # noqa: E402
-from hydragnn_b200 import ops, radius  # noqa: E402
+from hydragnn_b200 import ops, radius, stacks  # noqa: E402
 from hydragnn_b200.synthetic import ARCH, WORKLOADS, make_samples  # noqa: E402
 import oracle  # noqa: E402
 from oracle.workloads import add_edges_cpu, arch_for  # noqa: E402
@@ -267,7 +267,7 @@ def _egnn_losses(em, gpu, mlip):
 
 @pytest.mark.parametrize("name,g,k", [("md17_egnn", 24, 5), ("lj_egnn", 6, 5), ("md17_egnn", 5, 20), ("lj_egnn", 3, 64)])
 @pytest.mark.parametrize("mlip", [True, False])
-def test_fused_egnn_block_equals_composed_path_and_oracle(name, g, k, mlip):
+def test_fused_egnn_block_equals_composed_path_and_oracle(name, g, k, mlip, monkeypatch):
     """hgb_egnn_edge_{fwd,bwd_data,wgrad} (+ tangent mode in the double backward) against the round-1 composed path
     (gather / Linear / segment-sum closed primitives) and against the oracle: loss terms, and every parameter gradient of the
     MLIP loss (second derivatives through the fused block).  k = 20 / 64 gives denser graphs, but the tile rule
@@ -288,11 +288,9 @@ def test_fused_egnn_block_equals_composed_path_and_oracle(name, g, k, mlip):
     assert ops.egnn_edge_supported(kw["hidden_dim"])
     launches = hb._lib.launch_count()
     l1, t1, g1 = _egnn_losses(em, gpu, mlip)
-    ops.FUSED_EGNN = False
-    try:
+    with monkeypatch.context() as mp:
+        mp.setattr(stacks.E_GCL, "_fused_ok", lambda self, x, edge_attr: False)
         l0, t0, g0 = _egnn_losses(em, gpu, mlip)
-    finally:
-        ops.FUSED_EGNN = True
     torch.testing.assert_close(l1, l0, rtol=2e-5, atol=1e-7)
     for a, b in zip(t1, t0):
         torch.testing.assert_close(a, b, rtol=2e-5, atol=1e-7)
@@ -343,7 +341,7 @@ def test_edge_len_primitives_double_backward_matches_autograd():
 # ---- tensor-core attention, head_dim 8 (row a9) ---------------------------------------------------------------------------
 @pytest.mark.parametrize("n,f,heads", [(1, 8, 1), (65, 16, 2), (300, 64, 8), (1000, 64, 8), (4099, 64, 8)])
 @pytest.mark.parametrize("mode", ["exact", "tf32"])
-def test_tensor_core_attention_matches_fp64_reference(n, f, heads, mode):
+def test_tensor_core_attention_matches_fp64_reference(n, f, heads, mode, monkeypatch):
     """hgb_mha_tc_{fwd,bwd}: 3xTF32 ("exact") within the fp32 parity tolerance, plain TF32 within the bf16-config tolerance;
     the SIMT kernels are the second witness."""
     from hydragnn_b200 import gps
@@ -362,13 +360,12 @@ def test_tensor_core_attention_matches_fp64_reference(n, f, heads, mode):
     tol_o, tol_g = (2e-6, 1e-5) if mode == "exact" else (2e-3, 5e-3)
     assert rel_l2(out.detach(), ref.detach()) < tol_o
     assert rel_l2(ge, gr) < tol_g
-    gps.TC_ATTENTION = False
-    try:
+    query = hb._lib.query
+    with monkeypatch.context() as mp:                            # the library reports no tensor-core attention: SIMT kernels
+        mp.setattr(hb._lib, "query", lambda name, *args: 0 if name == "hgb_mha_tc_supported" else query(name, *args))
         qs = qkv.to(DEV).requires_grad_(True)
         outs = gps.MhaFn.apply(qs, heads)
         gs, = torch.autograd.grad(outs, qs, go.to(DEV))
-    finally:
-        gps.TC_ATTENTION = True
     assert rel_l2(out.detach(), outs.detach()) < 10 * tol_o and rel_l2(ge, gs) < 10 * tol_g
 
 
@@ -419,15 +416,12 @@ def test_train_fast_path_equals_eager_on_variable_batches(name, mlip, build):
     assert o1._hgb_fast.recaptures >= 1
 
 
-# ---- fp32-accurate tensor-core GEMMs (4xTF32) used by the exact-fp32 mode ---------------------------------------------------
+# ---- SIMT fp32 GEMMs: the shapes the tensor-core Linear and weight gradient do not take ---------------------------------------
 @pytest.mark.parametrize("m,n,k", [(5000, 64, 64), (4097, 200, 128), (20000, 24, 8), (513, 64, 16), (3000, 192, 64)])
-def test_gemm3_rows_forms_match_fp64(m, n, k, monkeypatch):
+def test_simt_rows_forms_match_fp64(m, n, k):
     g = torch.Generator().manual_seed(m + n + k)
     x, w, b = torch.randn(m, k, generator=g), torch.randn(n, k, generator=g) * 0.3, torch.randn(n, generator=g)
     xd, wd, bd = x.to(DEV), w.to(DEV), b.to(DEV)
-    monkeypatch.setattr(ops, "GEMM3", True)
-    assert ops.gemm3_ok(xd, wd, torch.empty(m, n, device=DEV), m, n, k, False, True)
-    before = hb._lib.launch_count()
     y, z = ops.raw_linear(xd, wd, bd, ops.ACT_CODES["silu"], 0.0, want_z=True)          # x W^T + b, SiLU, pre-activation kept
     zr = x.double() @ w.double().t() + b.double()
     assert rel_l2(z, zr) < 5e-7 and rel_l2(y, torch.nn.functional.silu(zr)) < 5e-7
@@ -442,21 +436,11 @@ def test_gemm3_rows_forms_match_fp64(m, n, k, monkeypatch):
 
 
 @pytest.mark.parametrize("r,mo,no", [(50000, 64, 64), (4099, 192, 64), (100000, 64, 128), (9000, 16, 8)])
-def test_gemm3_weight_gradient_form_matches_fp64(r, mo, no):
+def test_simt_weight_gradient_form_matches_fp64(r, mo, no):
     g = torch.Generator().manual_seed(r + mo)
     dz, x = torch.randn(r, mo, generator=g), torch.randn(r, no, generator=g)
-    ops.GEMM3 = True
-    assert ops.gemm3_ok(dz.to(DEV), x.to(DEV), torch.empty(mo, no, device=DEV), mo, no, r, True, False)
     dw = ops.raw_gemm(dz.to(DEV), x.to(DEV), True, False)
-    ref = dz.double().t() @ x.double()
-    assert rel_l2(dw, ref) < 5e-7
-    # the SIMT kernel is the second witness
-    ops.GEMM3 = False
-    try:
-        dw2 = ops.raw_gemm(dz.to(DEV), x.to(DEV), True, False)
-    finally:
-        ops.GEMM3 = False
-    assert rel_l2(dw2, ref) < 5e-6
+    assert rel_l2(dw, dz.double().t() @ x.double()) < 5e-6
 
 
 def test_pna_aggregate_kernel_hand_computed_cases():
@@ -544,14 +528,14 @@ def test_grouped_csr_build_equals_radix_sort_build():
 # ---- tensor-core Linears in fp32 mode: the 3xTF32 split inside tc_linear (exact flag) -------------------------------------------
 @pytest.mark.parametrize("m,n,k", [(5000, 64, 64), (4097, 192, 128), (128, 32, 32), (30000, 64, 128), (2000, 448, 64), (700, 384, 128),
                                    (1500, 576, 192), (520, 768, 256), (9001, 128, 256)])
-def test_tc_linear_exact_mode_matches_fp64(m, n, k):
+def test_fp32_linear_runs_tc_exact_mode_and_matches_fp64(m, n, k):
     """fp32 mode routes the large-M Linears through the SAME wgmma kernel with every operand split into TF32 hi / lo pairs in
     shared memory (hi*hi + lo*hi + hi*lo per k-step): results within ~1e-6 of fp64, i.e. fp32-level -- the plain TF32 mode of the
     bf16 configs is ~1e-3."""
     g = torch.Generator().manual_seed(m + n)
     x, w, b = torch.randn(m, k, generator=g), torch.randn(n, k, generator=g) * 0.3, torch.randn(n, generator=g)
     xd, wd, bd = x.to(DEV), w.to(DEV), b.to(DEV)
-    assert ops.EXACT_TC and not ops._TC["enabled"] and ops.tc_ok(m, n, k, xd)
+    assert not ops._TC["enabled"] and ops.tc_ok(m, n, k, xd)
     hb._lib.trace_begin()
     y, z, _ = ops.linear_fwd_dispatch_ex(xd, wd, bd, ops.ACT_CODES["silu"], 0.0, want_z=True)
     calls = [c for c in hb._lib.trace_end() if c[0] == "hgb_tc_linear"]
@@ -684,11 +668,10 @@ def test_tc_wgrad_exact_mode_matches_fp64(m, n, k, shift):
 
 # ---- head MLPs with the reference's odd widths on the tensor-core Linear (stacks._padded_chain) --------------------------------------
 @pytest.mark.parametrize("name,g", [("md17_egnn", 256), ("lj_egnn", 256), ("qm9_painn", 4500)])
-def test_zero_padded_head_mlps_equal_the_unpadded_chain(name, g, monkeypatch):
+def test_zero_padded_head_mlps_equal_the_chain_below_the_row_threshold(name, g, monkeypatch):
     """Widths 60 / 20 / 1 (node heads) and 5 (shared graph layers) are rounded up to multiples of 32 with zero-padded weights so the
     chain runs on hgb_tc_linear; outputs, loss, forces and every parameter gradient (through the MLIP double backward) equal the
     unpadded SIMT chain to fp32 rounding, and the padded path really is the tensor-core one."""
-    from hydragnn_b200 import stacks
     cpu = add_edges_cpu(make_samples(name, g), name)
     gpu = _gpu_batch(cpu, name, g)
     kw = arch_for(name, cpu)
@@ -696,10 +679,8 @@ def test_zero_padded_head_mlps_equal_the_unpadded_chain(name, g, monkeypatch):
     hi = [h.to(DEV) for h in hb.get_head_indices(em, gpu)]
     mlip = bool(kw.get("enable_interatomic_potential"))
 
-    monkeypatch.setattr(stacks, "PAD_MLP_MIN_ROWS", 1024)          # the production threshold is 32768 rows
-
-    def run(pad):
-        monkeypatch.setattr(stacks, "PAD_MLP", pad)
+    def run(min_rows):
+        monkeypatch.setattr(stacks, "PAD_MLP_MIN_ROWS", min_rows)
         em.zero_grad(set_to_none=True)
         hb._lib.trace_begin()
         if mlip:
@@ -713,8 +694,8 @@ def test_zero_padded_head_mlps_equal_the_unpadded_chain(name, g, monkeypatch):
         calls = hb._lib.trace_end()
         return [p.detach().clone() for p in pred], loss.detach().clone(), {k: p.grad.clone() for k, p in em.named_parameters()}, calls
 
-    p0, l0, g0, c0 = run(False)
-    p1, l1, g1, c1 = run(True)
+    p0, l0, g0, c0 = run(gpu.pos.shape[0] + 1)                  # more rows than any head sees: the unpadded chain
+    p1, l1, g1, c1 = run(1024)                                     # the production threshold is 32768 rows
     n_gemm = lambda cs: sum(1 for c in cs if c[0] == "hgb_gemm")            # noqa: E731
     n_tc = lambda cs: sum(1 for c in cs if c[0] in ("hgb_tc_linear", "hgb_tc_wgrad"))   # noqa: E731
     assert n_tc(c1) > n_tc(c0) and n_gemm(c1) < n_gemm(c0)

@@ -1,7 +1,7 @@
 """GPU parity tests of the wgmma (TF32) dense-layer kernels against fp64 references.
 Tolerance: TF32 truncates operands to 10 mantissa bits -> relative L2 error <= 2e-3 (well inside the 2e-2 the
 bf16 config allows, SURVEY 8d).  The fp32-accurate 3xTF32 mode ("exact", the default of the fp32 configs) is fp32-level:
-<= 2e-6 for a Linear (tests/test_gpu_round2.py::test_tc_linear_exact_mode_matches_fp64)."""
+<= 2e-6 for a Linear (tests/test_gpu_round2.py::test_fp32_linear_runs_tc_exact_mode_and_matches_fp64)."""
 import pytest
 import torch
 
