@@ -13,7 +13,7 @@ from torch import nn
 from . import ops
 from .stacks import EGCLStack, PAINNStack
 
-SUPPORTED = ("EGNN", "PAINN", "PNAEq", "MACE")
+SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAEq", "MACE")
 
 
 def get_device(use_gpu=True):
@@ -99,6 +99,10 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
         model = EGCLStack(edge_dim, max_neighbours=max_neighbours, **common)
     elif mpnn_type == "PAINN":
         model = PAINNStack(edge_dim, num_radial, radius, **common)
+    elif mpnn_type == "PNA":
+        assert pna_deg is not None, "PNA requires degree input."
+        from .pna import PNAStack
+        model = PNAStack(pna_deg, edge_dim, **common)
     elif mpnn_type == "PNAEq":
         assert pna_deg is not None, "PNAEq requires degree input."
         from .pnaeq import PNAEqStack

@@ -209,6 +209,34 @@ extern "C" int hgb_segment_argminmax(const float* m, const int32_t* rowptr, cons
 // of the first minimum / maximum (-1 for an empty segment) for the backward.  std = sqrt(clamp(E[x^2] - E[x]^2, 1e-5)),
 // reported as 0 where it equals sqrt(1e-5) (PyG masks the clamped entries).
 #define PNA_EPS 1e-5f
+
+// The four aggregators of one (segment, channel), fed one value per edge in CSR order.  Shared by pna_aggregate_fwd (messages
+// read from memory) and pna_conv_fwd (messages formed on the fly), so both apply the same tie and std rules.
+struct PnaAcc {
+  float s1 = 0.f, s2 = 0.f, vmin = 0.f, vmax = 0.f;
+  int imin = -1, imax = -1;
+
+  __device__ __forceinline__ void push(float v, int e) {
+    s1 += v;
+    s2 = fmaf(v, v, s2);
+    if (imin < 0 || v < vmin) { vmin = v; imin = e; }
+    if (imax < 0 || v > vmax) { vmax = v; imax = e; }
+  }
+
+  // o: the channel's column in an [.., 4c] output row; inv = 1 / max(segment length, 1)
+  __device__ __forceinline__ void store(float inv, float* o, int c, int32_t* arg_min, int32_t* arg_max) const {
+    const float mean = s1 * inv;
+    float sd = sqrtf(fmaxf(s2 * inv - mean * mean, PNA_EPS));
+    if (sd <= sqrtf(PNA_EPS)) sd = 0.f;
+    o[0] = mean;
+    o[c] = vmin;
+    o[2 * c] = vmax;
+    o[3 * c] = sd;
+    *arg_min = imin;
+    *arg_max = imax;
+  }
+};
+
 __global__ void pna_aggregate_fwd_kernel(const float* __restrict__ m, const int32_t* __restrict__ rowptr,
                                          const int32_t* __restrict__ perm, int n, int c, int lanes, float* __restrict__ out,
                                          int32_t* __restrict__ amin, int32_t* __restrict__ amax) {
@@ -218,26 +246,12 @@ __global__ void pna_aggregate_fwd_kernel(const float* __restrict__ m, const int3
     const int lo = rowptr[row], hi = rowptr[row + 1];
     const float inv = 1.f / (float)max(hi - lo, 1);
     for (int ch = sub; ch < c; ch += lanes) {
-      float s1 = 0.f, s2 = 0.f, vmin = 0.f, vmax = 0.f;
-      int imin = -1, imax = -1;
+      PnaAcc acc;
       for (int p = lo; p < hi; ++p) {
         const int e = perm ? perm[p] : p;
-        const float v = __ldg(m + (int64_t)e * c + ch);
-        s1 += v;
-        s2 = fmaf(v, v, s2);
-        if (imin < 0 || v < vmin) { vmin = v; imin = e; }
-        if (imax < 0 || v > vmax) { vmax = v; imax = e; }
+        acc.push(__ldg(m + (int64_t)e * c + ch), e);
       }
-      const float mean = s1 * inv;
-      float sd = sqrtf(fmaxf(s2 * inv - mean * mean, PNA_EPS));
-      if (sd <= sqrtf(PNA_EPS)) sd = 0.f;
-      float* o = out + (int64_t)row * 4 * c;
-      o[ch] = mean;
-      o[c + ch] = vmin;
-      o[2 * c + ch] = vmax;
-      o[3 * c + ch] = sd;
-      amin[(int64_t)row * c + ch] = imin;
-      amax[(int64_t)row * c + ch] = imax;
+      acc.store(inv, out + (int64_t)row * 4 * c + ch, c, amin + (int64_t)row * c + ch, amax + (int64_t)row * c + ch);
     }
   }
 }
@@ -280,5 +294,287 @@ extern "C" int hgb_pna_aggregate_bwd(const float* g_out, const float* m, const f
   HGB_REQUIRE(m, "pna_aggregate_bwd: null messages");
   pna_aggregate_bwd_kernel<<<hgb_grid_for(e * c, 256), 256, 0, (cudaStream_t)stream>>>(g_out, m, out, idx, rowptr, argmin, argmax, e * c, c, g_m);
   HGB_LAUNCH_CHECK("pna_aggregate_bwd");
+  return HGB_OK;
+}
+
+// ---- PNAConv message + aggregation in one pass (torch_geometric 2.6.1 PNAConv with towers = pre_layers = post_layers = 1,
+// hydragnn/models/PNAStack.py:42-53).  The pre_nn Linear is affine in its blocks, so for the edge e = (j -> i)
+//   h_e = P[i] + Q[j] + M a_e + c,   [P | Q] = x [W_a; W_b]^T (one per-node Linear), M = W_c W_enc [f, d], c = W_c b_enc + b_pre,
+// and h_e is formed in registers and reduced straight into [mean | min | max | std]: no [E, f] tensor is written.
+//
+// Thread mapping: a group of `lanes` threads (a power of two <= 256) owns one target node; every thread owns a FIXED set of
+// VEC consecutive channels (blockIdx.y selects the channel tile when f needs more than 256 * VEC), so M's rows for those
+// channels stay in registers and the backward's parameter sums accumulate per thread across every node the thread visits.
+#define PNA_MAX_D 16
+#define PNA_BLOCK 256
+#define PNA_BWD_MAX_BLOCKS (HGB_NUM_SMS * 4)
+
+template <int VEC, int MAXD>
+struct PnaChan {
+  float m[MAXD > 0 ? MAXD : 1][VEC];   // M[ch, k] of the thread's channels
+  float c[VEC];
+
+  __device__ __forceinline__ void load(const float* __restrict__ mt, const float* __restrict__ cvec, int d, int f, int ch0) {
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) c[j] = cvec ? __ldg(cvec + ch0 + j) : 0.f;
+#pragma unroll
+    for (int k = 0; k < MAXD; ++k)
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) m[k][j] = k < d ? __ldg(mt + (int64_t)k * f + ch0 + j) : 0.f;
+  }
+};
+
+template <int VEC>
+__device__ __forceinline__ void pna_load(const float* __restrict__ p, float (&v)[VEC]) {
+  if constexpr (VEC == 4) {
+    const float4 t = __ldg(reinterpret_cast<const float4*>(p));
+    v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+  } else {
+    v[0] = __ldg(p);
+  }
+}
+
+// h_e for the thread's channels: base = P[i] + c (per node), then + Q[src] + sum_k M[., k] a_e[k].  The forward and the
+// backward both call this, so the backward sees the forward's h_e bit for bit (its argmin / argmax / std mask agree).
+template <int VEC, int MAXD>
+__device__ __forceinline__ void pna_message(const PnaChan<VEC, MAXD>& ch, const float (&base)[VEC], const float* __restrict__ q_row,
+                                            const float* __restrict__ a_row, int d, float (&h)[VEC]) {
+  pna_load<VEC>(q_row, h);
+#pragma unroll
+  for (int j = 0; j < VEC; ++j) h[j] += base[j];
+  if (MAXD > 0 && d > 0) {
+#pragma unroll
+    for (int k = 0; k < MAXD; ++k) {
+      if (k < d) {
+        const float a = __ldg(a_row + k);
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) h[j] = fmaf(ch.m[k][j], a, h[j]);
+      }
+    }
+  }
+}
+
+template <int VEC, int MAXD>
+__global__ void __launch_bounds__(PNA_BLOCK, 1) pna_conv_fwd_kernel(
+    const float* __restrict__ pq, const int32_t* __restrict__ rowptr, const int32_t* __restrict__ perm,
+    const int32_t* __restrict__ src, const float* __restrict__ eattr, int d, const float* __restrict__ mt,
+    const float* __restrict__ cvec, int n, int f, int lanes, float* __restrict__ out, int32_t* __restrict__ amin,
+    int32_t* __restrict__ amax) {
+  const int gpb = blockDim.x / lanes;
+  const int ch0 = (blockIdx.y * lanes + threadIdx.x % lanes) * VEC;
+  if (ch0 >= f) return;                                  // no block-wide synchronisation below
+  PnaChan<VEC, MAXD> chan;
+  chan.load(mt, cvec, d, f, ch0);
+  for (int row = blockIdx.x * gpb + threadIdx.x / lanes; row < n; row += gridDim.x * gpb) {
+    const int lo = rowptr[row], hi = rowptr[row + 1];
+    const float inv = 1.f / (float)max(hi - lo, 1);
+    float base[VEC];
+    pna_load<VEC>(pq + (int64_t)row * 2 * f + ch0, base);
+#pragma unroll
+    for (int j = 0; j < VEC; ++j) base[j] += chan.c[j];
+    PnaAcc acc[VEC];
+    for (int p = lo; p < hi; ++p) {
+      const int e = perm ? perm[p] : p;
+      float h[VEC];
+      pna_message<VEC, MAXD>(chan, base, pq + (int64_t)src[p] * 2 * f + f + ch0, eattr + (int64_t)e * d, d, h);
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) acc[j].push(h[j], e);
+    }
+#pragma unroll
+    for (int j = 0; j < VEC; ++j)
+      acc[j].store(inv, out + (int64_t)row * 4 * f + ch0 + j, f, amin + (int64_t)row * f + ch0 + j, amax + (int64_t)row * f + ch0 + j);
+  }
+}
+
+// g_h_e = g_mean / deg + [e = amin] g_min + [e = amax] g_max + g_std (h_e - mean) / (deg std)   (std term 0 where std was masked),
+// the same rule as pna_aggregate_bwd_kernel.  g_p[i] = sum over i's segment; g_h written once per edge (Q was gathered by the
+// source, so g_Q is a segment sum over the by-source CSR).  part [gridDim.x, 1 + d, f]: per-CTA sum_e g_h_e and sum_e g_h_e a_e^T.
+template <int VEC, int MAXD>
+__global__ void __launch_bounds__(PNA_BLOCK, 1) pna_conv_bwd_kernel(
+    const float* __restrict__ g_out, const float* __restrict__ pq, const int32_t* __restrict__ rowptr,
+    const int32_t* __restrict__ perm, const int32_t* __restrict__ src, const float* __restrict__ eattr, int d,
+    const float* __restrict__ mt, const float* __restrict__ cvec, const float* __restrict__ agg,
+    const int32_t* __restrict__ amin, const int32_t* __restrict__ amax, int n, int f, int lanes, float* __restrict__ g_p,
+    int ldgp, float* __restrict__ g_h, float* __restrict__ part) {
+  __shared__ float red[PNA_BLOCK * VEC];
+  const int gpb = blockDim.x / lanes;
+  const int sub = threadIdx.x % lanes;
+  const int ch0 = (blockIdx.y * lanes + sub) * VEC;
+  const bool active = ch0 < f;
+  PnaChan<VEC, MAXD> chan;
+  float gc[VEC], gm[MAXD > 0 ? MAXD : 1][VEC];
+#pragma unroll
+  for (int j = 0; j < VEC; ++j) {
+    gc[j] = 0.f;
+#pragma unroll
+    for (int k = 0; k < MAXD; ++k) gm[k][j] = 0.f;
+  }
+  if (active) {
+    chan.load(mt, cvec, d, f, ch0);
+    for (int row = blockIdx.x * gpb + threadIdx.x / lanes; row < n; row += gridDim.x * gpb) {
+      const int lo = rowptr[row], hi = rowptr[row + 1];
+      const float inv = 1.f / (float)max(hi - lo, 1);
+      const float* g = g_out + (int64_t)row * 4 * f + ch0;
+      const float* o = agg + (int64_t)row * 4 * f + ch0;
+      float base[VEC], gmean[VEC], gmin[VEC], gmax[VEC], kstd[VEC], mean[VEC], gp[VEC];
+      int imin[VEC], imax[VEC];
+      pna_load<VEC>(pq + (int64_t)row * 2 * f + ch0, base);
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) {
+        base[j] += chan.c[j];
+        gmean[j] = g[j] * inv;
+        gmin[j] = g[f + j];
+        gmax[j] = g[2 * f + j];
+        mean[j] = o[j];
+        const float sd = o[3 * f + j];
+        kstd[j] = sd > 0.f ? g[3 * f + j] * inv / sd : 0.f;
+        imin[j] = amin[(int64_t)row * f + ch0 + j];
+        imax[j] = amax[(int64_t)row * f + ch0 + j];
+        gp[j] = 0.f;
+      }
+      for (int p = lo; p < hi; ++p) {
+        const int e = perm ? perm[p] : p;
+        const float* a_row = eattr + (int64_t)e * d;
+        float h[VEC];
+        pna_message<VEC, MAXD>(chan, base, pq + (int64_t)src[p] * 2 * f + f + ch0, a_row, d, h);
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) {
+          float acc = gmean[j];
+          if (imin[j] == e) acc += gmin[j];
+          if (imax[j] == e) acc += gmax[j];
+          if (kstd[j] != 0.f) acc = fmaf(kstd[j], h[j] - mean[j], acc);
+          h[j] = acc;                                      // h now holds g_h_e
+          gp[j] += acc;
+          gc[j] += acc;
+        }
+        if (MAXD > 0 && d > 0) {
+#pragma unroll
+          for (int k = 0; k < MAXD; ++k) {
+            if (k < d) {
+              const float a = __ldg(a_row + k);
+#pragma unroll
+              for (int j = 0; j < VEC; ++j) gm[k][j] = fmaf(h[j], a, gm[k][j]);
+            }
+          }
+        }
+        float* gh = g_h + (int64_t)e * f + ch0;
+        if constexpr (VEC == 4) *reinterpret_cast<float4*>(gh) = make_float4(h[0], h[1], h[2], h[3]);
+        else gh[0] = h[0];
+      }
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) g_p[(int64_t)row * ldgp + ch0 + j] = gp[j];
+    }
+  }
+  // fixed-order reduction over the CTA's node groups, one parameter row (c, then M[:, k]) at a time
+#pragma unroll
+  for (int k = 0; k <= MAXD; ++k) {
+    if (k <= d) {
+#pragma unroll
+      for (int j = 0; j < VEC; ++j) red[threadIdx.x * VEC + j] = k == 0 ? gc[j] : gm[k > 0 ? k - 1 : 0][j];
+      __syncthreads();
+      if (threadIdx.x < lanes && active) {
+#pragma unroll
+        for (int j = 0; j < VEC; ++j) {
+          float s = 0.f;
+          for (int grp = 0; grp < gpb; ++grp) s += red[(grp * lanes + sub) * VEC + j];
+          part[((int64_t)blockIdx.x * (d + 1) + k) * f + ch0 + j] = s;
+        }
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// out[r] = sum over the CTAs in index order (fp64) of part[b, r]
+__global__ void pna_conv_reduce_kernel(const float* __restrict__ part, int nblk, int rows, float* __restrict__ out) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < rows; r += gridDim.x * blockDim.x) {
+    double s = 0.0;
+    for (int b = 0; b < nblk; ++b) s += (double)part[(int64_t)b * rows + r];
+    out[r] = (float)s;
+  }
+}
+
+namespace {
+struct PnaLaunch {
+  bool v4;
+  int lanes, gpb;
+  dim3 grid;
+};
+
+PnaLaunch pna_launch(const float* pq, int32_t n, int32_t f, int max_blocks, const void* extra_aligned = nullptr) {
+  PnaLaunch L;
+  L.v4 = (f % 4 == 0) && ((uintptr_t)pq % 16 == 0) && ((uintptr_t)extra_aligned % 16 == 0);
+  const int cv = L.v4 ? f / 4 : f;
+  L.lanes = 1;
+  while (L.lanes < cv && L.lanes < PNA_BLOCK) L.lanes <<= 1;
+  L.gpb = PNA_BLOCK / L.lanes;
+  L.grid = dim3(hgb_grid_for(n, L.gpb, max_blocks), (cv + L.lanes - 1) / L.lanes);
+  return L;
+}
+}  // namespace
+
+// instantiations by vector width and edge-attribute capacity (0, 4 or 16): the registers holding M and the backward's
+// g_M accumulators are sized by the capacity, so narrow or absent edge attributes do not pay for d = 16
+#define PNA_DISPATCH(LAUNCH)                           \
+  do {                                                 \
+    if (L.v4) {                                        \
+      if (d == 0) LAUNCH(4, 0);                        \
+      else if (d <= 4) LAUNCH(4, 4);                   \
+      else LAUNCH(4, 16);                              \
+    } else {                                           \
+      if (d == 0) LAUNCH(1, 0);                        \
+      else if (d <= 4) LAUNCH(1, 4);                   \
+      else LAUNCH(1, 16);                              \
+    }                                                  \
+  } while (0)
+
+extern "C" int64_t hgb_pna_conv_workspace_bytes(int32_t f, int32_t d) {
+  if (f <= 0 || d < 0 || d > PNA_MAX_D) return -1;
+  return (int64_t)PNA_BWD_MAX_BLOCKS * (d + 1) * f * (int64_t)sizeof(float);
+}
+
+extern "C" int hgb_pna_conv_fwd(const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                                const float* eattr, int32_t d, const float* mt, const float* cvec, int32_t n, int32_t f,
+                                float* out, int32_t* argmin, int32_t* argmax, hgb_stream_t stream) {
+  HGB_REQUIRE(n >= 0 && f > 0 && d >= 0 && d <= PNA_MAX_D, "pna_conv_fwd: bad sizes (n %d, f %d, d %d; d <= %d)", n, f, d, PNA_MAX_D);
+  HGB_REQUIRE(pq && rowptr && src && out && argmin && argmax, "pna_conv_fwd: null argument");
+  HGB_REQUIRE(d == 0 || (eattr && mt), "pna_conv_fwd: d > 0 needs edge attributes and M");
+  if (n == 0) return HGB_OK;
+  const PnaLaunch L = pna_launch(pq, n, f, HGB_NUM_SMS * 16);
+#define PNA_FWD(V, D)                                                                                                        \
+  pna_conv_fwd_kernel<V, D><<<L.grid, PNA_BLOCK, 0, (cudaStream_t)stream>>>(pq, rowptr, perm, src, eattr, d, mt, cvec, n, f, \
+                                                                           L.lanes, out, argmin, argmax)
+  PNA_DISPATCH(PNA_FWD);
+#undef PNA_FWD
+  HGB_LAUNCH_CHECK("pna_conv_fwd");
+  return HGB_OK;
+}
+
+extern "C" int hgb_pna_conv_bwd(const float* g_out, const float* pq, const int32_t* rowptr, const int32_t* perm,
+                                const int32_t* src, const float* eattr, int32_t d, const float* mt, const float* cvec,
+                                const float* out, const int32_t* argmin, const int32_t* argmax, int32_t n, int32_t f,
+                                float* g_p, int32_t ldgp, float* g_h, float* g_cm, void* workspace, hgb_stream_t stream) {
+  HGB_REQUIRE(n >= 0 && f > 0 && d >= 0 && d <= PNA_MAX_D && ldgp >= f,
+              "pna_conv_bwd: bad sizes (n %d, f %d, d %d, ldgp %d)", n, f, d, ldgp);
+  HGB_REQUIRE(g_out && pq && rowptr && src && out && argmin && argmax && g_p && g_h && g_cm && workspace,
+              "pna_conv_bwd: null argument");
+  HGB_REQUIRE(d == 0 || (eattr && mt), "pna_conv_bwd: d > 0 needs edge attributes and M");
+  if (n == 0) {
+    cudaMemsetAsync(g_cm, 0, sizeof(float) * (size_t)(d + 1) * f, (cudaStream_t)stream);
+    HGB_LAUNCH_CHECK("pna_conv_bwd");
+    return HGB_OK;
+  }
+  // the float4 path also stores g_h with float4 writes, so g_h must be 16-byte aligned as well
+  const PnaLaunch L = pna_launch(pq, n, f, PNA_BWD_MAX_BLOCKS, g_h);
+  float* part = static_cast<float*>(workspace);
+#define PNA_BWD(V, D)                                                                                                         \
+  pna_conv_bwd_kernel<V, D><<<L.grid, PNA_BLOCK, 0, (cudaStream_t)stream>>>(g_out, pq, rowptr, perm, src, eattr, d, mt, cvec, \
+                                                                           out, argmin, argmax, n, f, L.lanes, g_p, ldgp, g_h, part)
+  PNA_DISPATCH(PNA_BWD);
+#undef PNA_BWD
+  HGB_LAUNCH_CHECK("pna_conv_bwd");
+  const int rows = (d + 1) * f;
+  pna_conv_reduce_kernel<<<hgb_grid_for(rows, 256), 256, 0, (cudaStream_t)stream>>>(part, (int)L.grid.x, rows, g_cm);
+  HGB_LAUNCH_CHECK("pna_conv_reduce");
   return HGB_OK;
 }

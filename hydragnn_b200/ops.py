@@ -1097,6 +1097,69 @@ class PnaAggregateFn(torch.autograd.Function):
         return gm, None
 
 
+PNA_CONV_MAX_EDGE_DIM = 16
+
+
+def raw_pna_conv_fwd(pq, eattr, mt, cvec, plan):
+    """-> (agg [n, 4f], argmin, argmax [n, f] int32): hgb_pna_conv_fwd over the by-target CSR of ``plan``."""
+    n, f = pq.shape[0], pq.shape[1] // 2
+    d = 0 if eattr is None else eattr.shape[1]
+    col = plan.by_col
+    agg = torch.empty(n, 4 * f, dtype=pq.dtype, device=pq.device)
+    amin = torch.empty(n, f, dtype=torch.int32, device=pq.device)
+    amax = torch.empty_like(amin)
+    _lib.call("hgb_pna_conv_fwd", _p(pq), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col")), _p(eattr), d, _p(mt), _p(cvec), n, f,
+              _p(agg), _p(amin), _p(amax), _stream())
+    return agg, amin, amax
+
+
+def raw_pna_conv_bwd(g_agg, pq, eattr, mt, cvec, agg, amin, amax, plan):
+    """-> (g_pq [n, 2f], g_h [e, f], g_cm [1 + d, f] = [g_c ; g_M^T])."""
+    n, f = pq.shape[0], pq.shape[1] // 2
+    d = 0 if eattr is None else eattr.shape[1]
+    dev = pq.device
+    g_pq = torch.empty(n, 2 * f, dtype=pq.dtype, device=dev)
+    g_h = torch.empty(plan.num_edges, f, dtype=pq.dtype, device=dev)
+    g_cm = torch.empty(1 + d, f, dtype=pq.dtype, device=dev)
+    ws = _ws(_lib.query("hgb_pna_conv_workspace_bytes", f, d), dev)
+    col = plan.by_col
+    _lib.call("hgb_pna_conv_bwd", _p(g_agg), _p(pq), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col")), _p(eattr), d, _p(mt), _p(cvec),
+              _p(agg), _p(amin), _p(amax), n, f, _p(g_pq), 2 * f, _p(g_h), _p(g_cm), _p(ws), _stream())
+    # g_Q: Q was gathered by the source of every edge, so its gradient is the by-source segment sum of g_h
+    row = plan.by_row
+    _lib.call("hgb_segment_sum_strided", _p(g_h), _p(row.rowptr), _p(row.perm), n, f, _p(g_pq[:, f:]), 2 * f, _stream())
+    return g_pq, g_h, g_cm
+
+
+class PnaConvFn(torch.autograd.Function):
+    """agg = [mean | min | max | std] over the targets i = edge_index[1] of h_e = P[i] + Q[j] + M a_e + c, with
+    [P | Q] = ``pq`` [n, 2f], M = ``mt``ᵀ [f, d] and c = ``cvec`` [f] -- PNAConv's pre_nn Linear and its four aggregators
+    (torch_geometric 2.6.1 PNAConv.message / DegreeScalerAggregation) in one kernel; the [E, f] messages never reach memory.
+    ``eattr`` [e, d] with d <= 16, or None."""
+
+    @staticmethod
+    def forward(ctx, pq, eattr, mt, cvec, plan):
+        pq, cvec = _chk(pq), _chk(cvec)
+        eattr = _chk(eattr) if eattr is not None else None
+        mt = _chk(mt) if eattr is not None else None
+        agg, amin, amax = raw_pna_conv_fwd(pq, eattr, mt, cvec, plan)
+        ctx.save_for_backward(pq, eattr, mt, cvec, agg, amin, amax)
+        ctx.plan = plan
+        return agg
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_agg):
+        pq, eattr, mt, cvec, agg, amin, amax = ctx.saved_tensors
+        g_pq, g_h, g_cm = raw_pna_conv_bwd(_chk(g_agg.contiguous()), pq, eattr, mt, cvec, agg, amin, amax, ctx.plan)
+        g_eattr = g_mt = None
+        if eattr is not None:
+            g_mt = g_cm[1:]
+            if ctx.needs_input_grad[1]:
+                g_eattr = raw_gemm(g_h, mt, False, True)                           # [e, f] x [d, f]^T
+        return g_pq, g_eattr, g_mt, g_cm[0], None
+
+
 # =====================================================================================================
 # grouped dense layers (multi-branch decoding)
 # =====================================================================================================

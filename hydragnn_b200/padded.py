@@ -16,7 +16,8 @@ one graph.  A batch larger than a capacity re-captures with grown capacities (ho
 (edge count of an on-device neighbour build, checked by ``check()`` / at the end of ``train``).
 
 Supported: EGNN / PaiNN / MACE / PNAEq stacks without BatchNorm-carrying wrappers (GPS mixes every atom of the mini-batch:
-filler atoms would leak into real ones), heads all of graph type, or the MLIP wrapper (energy + forces).
+filler atoms would leak into real ones) or BatchNorm feature layers (PNA: the same leak through the batch statistics), heads
+all of graph type, or the MLIP wrapper (energy + forces).
 """
 import torch
 import torch.distributed as dist
@@ -51,7 +52,10 @@ def supported(model):
     inner = getattr(m, "model", m)
     if getattr(inner, "use_global_attn", False) or getattr(inner, "global_attn_engine", None):
         return False
-    if getattr(m, "model", None) is not None:                # MLIP wrapper: one head
+    # BatchNorm feature layers (PNA) take batch statistics over every row: the filler atoms of a padded batch would enter them
+    if any(isinstance(f, torch.nn.BatchNorm1d) for layer in getattr(inner, "feature_layers", ()) for f in layer.modules()):
+        return False
+    if getattr(m, "model", None) is not None:               # MLIP wrapper: one head
         return True
     return all(t == "graph" for t in inner.head_type) and getattr(inner, "num_branches", 1) == 1
 

@@ -110,6 +110,18 @@ class DegreeScalerAggregation(nn.Module):
         return torch.cat(res, dim=-1)
 
 
+def post_linear_scaled(post, x, agg4, aggr_module, csr):
+    """``post([x | s_1 A | ... | s_k A])`` for the post Linear of a PNA layer, A = ``agg4`` [N, 4 F_in] = [mean | min | max | std]
+    and s_k the per-node degree scalers of ``aggr_module`` over ``csr``.  The scalers are per-node factors, so
+        post([x | s_1 A | ... | s_k A]) = x W_x^T + b + sum_k s_k (A W_k^T):
+    the (4k + 1) F_in-wide input is never built."""
+    fin, fout = x.shape[1], post.weight.shape[0]
+    ns = len(aggr_module.scaler)
+    wk = post.weight[:, fin:].reshape(fout, ns, 4 * fin).permute(1, 0, 2).reshape(ns * fout, 4 * fin)
+    bk = ops.linear_act(agg4, wk, None).reshape(-1, ns, fout)                        # [N, k, F_out]
+    return ops.linear_act(x, post.weight[:, :fin], post.bias) + (bk * aggr_module.scaler_factors(csr)[:, :, None]).sum(dim=1)
+
+
 class PainnMessage(nn.Module):
     def __init__(self, node_size, x_aggregators, x_scalers, deg, edge_dim, num_radial):
         super().__init__()
@@ -143,14 +155,9 @@ class PainnMessage(nn.Module):
         m_v = GatherRows.apply(v, dst) * g_v.unsqueeze(1) + g_e.unsqueeze(1) * vec.unsqueeze(-1)
         am = self.aggr_module
         if not higher_order and am.aggr == ["mean", "min", "max", "std"]:
-            # fused: the four aggregators in one pass; the degree scalers are per-node factors, so
-            #   post_nn([x | s_1 A | ... | s_5 A]) = x W_x^T + b + sum_k s_k (A W_k^T):  the 20F-wide tensor is never built
+            # fused: the four aggregators in one pass; the degree scalers are folded into post_nn (the 20F-wide tensor is never built)
             agg4 = ops.PnaAggregateFn.apply(m_s.contiguous(), src)                   # [N, 4F]
-            post = self.post_nns[0][0]
-            ns = len(am.scaler)
-            wk = post.weight[:, F:].reshape(F, ns, 4 * F).permute(1, 0, 2).reshape(ns * F, 4 * F)
-            bk = ops.linear_act(agg4, wk, None).reshape(-1, ns, F)                    # [N, 5, F]
-            dx = ops.linear_act(x, post.weight[:, :F], post.bias) + (bk * am.scaler_factors(src)[:, :, None]).sum(dim=1)
+            dx = post_linear_scaled(self.post_nns[0][0], x, agg4, am, src)
         else:
             agg = am(m_s, src)                                        # :396-400
             dx = run_mlp(self.post_nns[0], torch.cat([x, agg], dim=-1), higher_order)

@@ -26,6 +26,10 @@ WORKLOADS = {
                       pbc_box=True, two_heads=True),
     # the same with exactly 80 atoms per cell (unit tests)
     "oc20_mace_80": dict(n=80, rho=0.05, species=list(range(1, 84)), radius=6.0, max_neighbours=128, pbc_box=True, two_heads=True),
+    # PNA on examples/eam (NiNb EAM): periodic 32-atom metal cells at a metallic number density, r = 3 A
+    "eam_pna": dict(n=32, rho=0.085, species=[28, 41], radius=3.0, max_neighbours=20, pbc_box=True),
+    # PNA on examples/ogb (ogb_gap): molecule-sized graphs of 9 to 30 atoms, k = 20
+    "ogb_pna": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
 }
 
 ARCH = {
@@ -66,6 +70,17 @@ ARCH = {
 }
 
 
+# PNA (PNAStack.py) at the widths of examples/eam/NiNb_EAM_*.json and examples/ogb/ogb_gap.json; pna_deg is filled in from the
+# batch (in-degree histogram) by the caller, eam_pna reads the edge length as a 1-wide edge attribute
+ARCH["eam_pna"] = dict(mpnn_type="PNA", input_dim=1, hidden_dim=50, num_conv_layers=10, edge_dim=1, radius=3.0, max_neighbours=20,
+                       output_dim=[1], output_type=["node"], task_weights=[1.0],
+                       output_heads={"node": {"num_headlayers": 2, "dim_headlayers": [50, 25], "type": "mlp"}},
+                       activation_function="relu", loss_function_type="mse", graph_pooling="mean")
+ARCH["ogb_pna"] = dict(mpnn_type="PNA", input_dim=1, hidden_dim=55, num_conv_layers=6, radius=5.0, max_neighbours=20,
+                       output_dim=[1], output_type=["graph"], task_weights=[1.0],
+                       output_heads={"graph": {"num_sharedlayers": 1, "dim_sharedlayers": 55, "num_headlayers": 2,
+                                               "dim_headlayers": [55, 55]}},
+                       activation_function="relu", loss_function_type="mse", graph_pooling="mean")
 ARCH["oc20_mace_80"] = ARCH["oc20_mace"]
 ARCH["gfm_pnaeq_mini"] = dict(ARCH["gfm_pnaeq"], output_dim=[1], output_type=["graph"], task_weights=[1.0], loss_function_type="mse",
                               output_heads={"graph": ARCH["gfm_pnaeq"]["output_heads"]["graph"]})

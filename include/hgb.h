@@ -503,6 +503,24 @@ int hgb_pna_aggregate_fwd(const float* m, const int32_t* rowptr, const int32_t* 
 int hgb_pna_aggregate_bwd(const float* g_out, const float* m, const float* out, const int32_t* idx, const int32_t* rowptr,
                           const int32_t* argmin, const int32_t* argmax, int64_t e, int32_t c, float* g_m, hgb_stream_t stream);
 
+/* PNAConv message + aggregation fused (hydragnn/models/PNAStack.py:42-53; torch_geometric 2.6.1 PNAConv with towers = 1,
+ * pre_layers = post_layers = 1, aggregators mean, min, max, std).  (rowptr, perm): CSR of the targets edge_index[1];
+ * src [slot] = source node of every CSR slot.  pq [n, 2f] = [P | Q] = x [W_a; W_b]^T; eattr [e, d] with 0 <= d <= 16 (NULL
+ * when d = 0); mt [d, f] = (W_c W_enc)^T; cvec [f] = W_c b_enc + b_pre (NULL: zero).  For every edge of the segment of i,
+ * h = P[i] + Q[src] + M a_e + c is formed in registers: out [n, 4f] and argmin / argmax [n, f] are exactly those of
+ * hgb_pna_aggregate_fwd on the [e, f] messages h, which are never written.  Deterministic: no atomics.
+ * Backward: g_p [n, f] (row stride ldgp) = per-target sum of g_h; g_h [e, f] in edge order (g_Q = hgb_segment_sum of it over
+ * the CSR of the sources); g_cm [1 + d, f] = [sum_e g_h_e ; (sum_e g_h_e a_e^T)^T] from per-CTA partials reduced in fixed
+ * order.  workspace: hgb_pna_conv_workspace_bytes(f, d) bytes (-1: d out of range).                                        */
+int64_t hgb_pna_conv_workspace_bytes(int32_t f, int32_t d);
+int hgb_pna_conv_fwd(const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src, const float* eattr,
+                     int32_t d, const float* mt, const float* cvec, int32_t n, int32_t f, float* out, int32_t* argmin,
+                     int32_t* argmax, hgb_stream_t stream);
+int hgb_pna_conv_bwd(const float* g_out, const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                     const float* eattr, int32_t d, const float* mt, const float* cvec, const float* out, const int32_t* argmin,
+                     const int32_t* argmax, int32_t n, int32_t f, float* g_p, int32_t ldgp, float* g_h, float* g_cm,
+                     void* workspace, hgb_stream_t stream);
+
 /* ---- MACE (hydragnn/utils/model/mace_utils/modules/blocks.py:369-402, symmetric_contraction.py:92-242) ------------------
  * Features are channel-last: [N, spherical index, F].  lmax_in <= 2, 1 <= lmax_sh <= 3, lmax_in <= lmax_sh, F % 32 == 0.
  * Path order / coupling constants = tp_out_irreps_with_instructions (irreps_tools.py:15-44) with e3nn's real Wigner 3j.   */
