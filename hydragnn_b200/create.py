@@ -13,7 +13,7 @@ from torch import nn
 from . import ops
 from .stacks import EGCLStack, PAINNStack
 
-SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAEq", "MACE")
+SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAEq", "MACE", "SchNet")
 
 
 def get_device(use_gpu=True):
@@ -50,6 +50,7 @@ def create_model_config(config, verbosity=0, use_gpu=True):
         task_weights=arch["task_weights"], num_conv_layers=arch["num_conv_layers"],
         freeze_conv=g("freeze_conv_layers", False), initial_bias=g("initial_bias"), num_nodes=g("num_nodes"),
         max_neighbours=g("max_neighbours"), edge_dim=g("edge_dim"), pna_deg=g("pna_deg"), num_radial=g("num_radial"),
+        num_gaussians=g("num_gaussians"), num_filters=g("num_filters"),
         radial_type=g("radial_type"), distance_transform=g("distance_transform"), radius=g("radius"),
         equivariance=g("equivariance"), correlation=g("correlation"), max_ell=g("max_ell"), node_max_ell=g("node_max_ell"),
         avg_num_neighbors=g("avg_num_neighbors"), conv_checkpointing=training.get("conv_checkpointing", False),
@@ -120,6 +121,12 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
                           activation_function, loss_function_type, loss_weights=task_weights, freeze_conv=freeze_conv,
                           initial_bias=initial_bias, num_conv_layers=num_conv_layers, num_nodes=num_nodes,
                           graph_pooling=graph_pooling, global_attn_engine=global_attn_engine)
+    elif mpnn_type == "SchNet":
+        assert num_gaussians is not None, "SchNet requires num_guassians input."
+        assert num_filters is not None, "SchNet requires num_filters input."
+        assert radius is not None, "SchNet requires radius input."
+        from .schnet import SCFStack
+        model = SCFStack(num_filters, edge_dim, num_gaussians, radius, max_neighbours=max_neighbours, **common)
     else:
         raise ValueError("Unknown mpnn_type: {0}".format(mpnn_type))
     if enable_interatomic_potential:

@@ -1160,6 +1160,66 @@ class PnaConvFn(torch.autograd.Function):
         return g_pq, g_eattr, g_mt, g_cm[0], None
 
 
+def cfconv_supported(g, nf, d):
+    """Shapes ``CfConvFn`` takes: 1 <= num_gaussians <= 64, 1 <= num_filters <= 128, raw edge input width <= 16."""
+    return bool(_lib.query("hgb_cfconv_supported", int(g), int(nf), int(d)))
+
+
+class CfConvFn(torch.autograd.Function):
+    """SchNet's CFConv message and sum over the targets i = edge_index[1] (hgb_cfconv_fwd): out_i = sum_e xl[j] * W_e with the
+    filter W_e = (ssp([rbf(d_e) | r_e] A + b1) W2^T + b2) * C(d_e) formed per edge on chip, d_e = |pos[i] - pos[j]|.
+    ``a1t`` [G + d, nf] = [W1[:, :G]^T ; Mt], ``r`` [e, d] or None, ``mu`` the Gaussian centres.  With ``want_we`` the
+    filter W_e [e, nf] is returned as a second output (the equivariant coordinate MLP reads it), else None."""
+
+    @staticmethod
+    def forward(ctx, xl, pos, r, a1t, b1, w2, b2, mu, coeff, cutoff, plan, want_we):
+        xl, pos, a1t, b1, w2, b2, mu = (_chk(t) for t in (xl, pos, a1t, b1, w2, b2, mu))
+        r = _chk(r) if r is not None else None
+        n, nf = xl.shape
+        g, d, e = mu.numel(), (0 if r is None else r.shape[1]), plan.num_edges
+        out = torch.empty(n, nf, dtype=xl.dtype, device=xl.device)
+        w_e = torch.empty(e, nf, dtype=xl.dtype, device=xl.device) if want_we else None
+        col = plan.by_col
+        _lib.call("hgb_cfconv_fwd", _p(xl), _p(pos), _p(plan.row), _p(col.rowptr), _p(col.perm), _p(r), d, _p(mu), float(coeff),
+                  float(cutoff), _p(a1t), _p(b1), _p(w2), _p(b2), n, e, g, nf, _p(out), _p(w_e), _stream())
+        ctx.save_for_backward(xl, pos, r, a1t, b1, w2, b2, mu)
+        ctx.coeff, ctx.cutoff, ctx.plan = float(coeff), float(cutoff), plan
+        if w_e is not None:
+            return out, w_e
+        return out, None
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out, g_we):
+        xl, pos, r, a1t, b1, w2, b2, mu = ctx.saved_tensors
+        plan = ctx.plan
+        n, nf = xl.shape
+        g, d, e = mu.numel(), (0 if r is None else r.shape[1]), plan.num_edges
+        dev = xl.device
+        need_xl, need_pos, need_r = ctx.needs_input_grad[0], ctx.needs_input_grad[1], r is not None and ctx.needs_input_grad[2]
+        g_xle = torch.empty(e, nf, dtype=xl.dtype, device=dev) if need_xl else None
+        g_dist = torch.empty(e, dtype=xl.dtype, device=dev) if need_pos else None
+        g_r = torch.empty(e, d, dtype=xl.dtype, device=dev) if need_r else None
+        need_params = any(ctx.needs_input_grad[3:7])
+        g_params = torch.empty((g + d) * nf + nf + nf * nf + nf, dtype=xl.dtype, device=dev) if need_params else None
+        ws = _ws(_lib.query("hgb_cfconv_workspace_bytes", g, nf, d), dev) if need_params else None
+        g_out = _chk(g_out.contiguous())
+        g_we = _chk(g_we.contiguous()) if g_we is not None else None
+        _lib.call("hgb_cfconv_bwd", _p(g_out), _p(g_we), _p(xl), _p(pos), _p(plan.row), _p(plan.col), _p(r), d, _p(mu), ctx.coeff,
+                  ctx.cutoff, _p(a1t), _p(b1), _p(w2), _p(b2), n, e, g, nf, _p(g_xle), _p(g_dist), _p(g_r), _p(g_params), _p(ws),
+                  _stream())
+        g_xl = raw_segment_sum(g_xle, plan.by_row.rowptr, plan.by_row.perm, n) if need_xl else None     # xl was gathered by source
+        g_pos = _raw_edge_len_bwd(g_dist, pos, None, plan) if need_pos else None
+        if not need_params:
+            return g_xl, g_pos, g_r, None, None, None, None, None, None, None, None, None
+        k = (g + d) * nf
+        g_a1t = g_params[:k].view(g + d, nf)
+        g_b1 = g_params[k:k + nf]
+        g_w2 = g_params[k + nf:k + nf + nf * nf].view(nf, nf)
+        g_b2 = g_params[k + nf + nf * nf:]
+        return g_xl, g_pos, g_r, g_a1t, g_b1, g_w2, g_b2, None, None, None, None, None
+
+
 # =====================================================================================================
 # grouped dense layers (multi-branch decoding)
 # =====================================================================================================

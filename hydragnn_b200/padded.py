@@ -52,6 +52,9 @@ def supported(model):
     inner = getattr(m, "model", m)
     if getattr(inner, "use_global_attn", False) or getattr(inner, "global_attn_engine", None):
         return False
+    # SchNet builds its radius graphs in the layers (or, with edge attributes, was not checked against the padded step): eager
+    if str(inner) == "SCFStack":
+        return False
     # BatchNorm feature layers (PNA) take batch statistics over every row: the filler atoms of a padded batch would enter them
     if any(isinstance(f, torch.nn.BatchNorm1d) for layer in getattr(inner, "feature_layers", ()) for f in layer.modules()):
         return False

@@ -546,6 +546,10 @@ class Base(nn.Module):
                 pass
         return plan
 
+    def _edge_plan(self, data):
+        """The plan of ``data.edge_index`` the convolutions share; a stack that builds its graphs in the layers returns None."""
+        return self.plan_for(data)
+
     def _gps_embed(self, data, higher):
         """Node / edge embeddings used when global attention is on (Base.py:477-491): returns (x, edge_attr)."""
         lin = (lambda m, t: ops.linear_any_order(t, m.weight, None)) if higher else (lambda m, t: ops.linear_act(t, m.weight, None))
@@ -572,7 +576,7 @@ class Base(nn.Module):
         if getattr(self, "precision", "fp32") == "bf16" and not ops._TC["enabled"]:
             with ops.tensor_cores(True):       # large-M Linears on wgmma (TF32 in, fp32 accumulate)
                 return self.forward(data)
-        plan = self.plan_for(data)
+        plan = self._edge_plan(data)
         inv, equiv, conv_args = self._embedding(data, plan, higher)
         for conv, feat in zip(self.graph_convs, self.feature_layers):
             inv, equiv = conv(inv_node_feat=inv, equiv_node_feat=equiv, plan=plan, higher_order=higher, **conv_args)

@@ -30,6 +30,12 @@ WORKLOADS = {
     "eam_pna": dict(n=32, rho=0.085, species=[28, 41], radius=3.0, max_neighbours=20, pbc_box=True),
     # PNA on examples/ogb (ogb_gap): molecule-sized graphs of 9 to 30 atoms, k = 20
     "ogb_pna": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    # SchNet on examples/qm9 and examples/md17 (GPS: the positional encodings pe, rel_pe = |pe[row] - pe[col]| once the edges
+    # exist, see add_rel_pe), and without GPS at the CI widths, building its radius graphs in the layers
+    "qm9_schnet": dict(n=9, rho=0.10, species=[1, 6, 7, 8, 9], radius=7.0, max_neighbours=5, pe_dim=2),
+    "md17_schnet": dict(n=21, rho=0.08, species=[6] * 9 + [1] * 8 + [8] * 4, radius=7.0, max_neighbours=5, fixed_species=True,
+                        pe_dim=6),
+    "ci_schnet": dict(n=9, rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
 }
 
 ARCH = {
@@ -81,6 +87,20 @@ ARCH["ogb_pna"] = dict(mpnn_type="PNA", input_dim=1, hidden_dim=55, num_conv_lay
                        output_heads={"graph": {"num_sharedlayers": 1, "dim_sharedlayers": 55, "num_headlayers": 2,
                                                "dim_headlayers": [55, 55]}},
                        activation_function="relu", loss_function_type="mse", graph_pooling="mean")
+# SchNet (SCFStack.py): examples/qm9/qm9.json exactly, examples/md17/md17.json (6 layers, pe_dim 6), and the in-layer branch at
+# the widths of tests/inputs/ci.json (num_filters 126, num_gaussians 50) with hidden 64 and three layers
+ARCH["qm9_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_conv_layers=2, num_gaussians=10, num_filters=8,
+                          radius=7.0, max_neighbours=5, global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=8,
+                          pe_dim=2, output_dim=[1], output_type=["graph"], task_weights=[1.0],
+                          output_heads={"graph": {"num_sharedlayers": 2, "dim_sharedlayers": 5, "num_headlayers": 2,
+                                                  "dim_headlayers": [50, 25]}},
+                          activation_function="relu", loss_function_type="mse", graph_pooling="mean")
+ARCH["md17_schnet"] = dict(ARCH["qm9_schnet"], num_conv_layers=6, pe_dim=6)
+ARCH["ci_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_conv_layers=3, num_gaussians=50, num_filters=126,
+                         radius=5.0, max_neighbours=20, output_dim=[1], output_type=["graph"], task_weights=[1.0],
+                         output_heads={"graph": {"num_sharedlayers": 2, "dim_sharedlayers": 4, "num_headlayers": 2,
+                                                 "dim_headlayers": [10, 10]}},
+                         activation_function="relu", loss_function_type="mse", graph_pooling="mean")
 ARCH["oc20_mace_80"] = ARCH["oc20_mace"]
 ARCH["gfm_pnaeq_mini"] = dict(ARCH["gfm_pnaeq"], output_dim=[1], output_type=["graph"], task_weights=[1.0], loss_function_type="mse",
                               output_heads={"graph": ARCH["gfm_pnaeq"]["output_heads"]["graph"]})
@@ -188,3 +208,10 @@ def make_samples(name, num_graphs, seed=1234, with_edges=None):
         out.cell = (torch.eye(3) * L)[None].expand(num_graphs, 3, 3).contiguous()
         out.pbc = torch.ones(num_graphs, 3, dtype=torch.bool)
     return out
+
+
+def add_rel_pe(batch):
+    """rel_pe = |pe[row] - pe[col]| on the batch's edges (hydragnn/preprocess/serialized_dataset_loader.py:186-189)."""
+    row, col = batch.edge_index
+    batch.rel_pe = (batch.pe[row] - batch.pe[col]).abs().contiguous()
+    return batch

@@ -521,6 +521,27 @@ int hgb_pna_conv_bwd(const float* g_out, const float* pq, const int32_t* rowptr,
                      const int32_t* argmax, int32_t n, int32_t f, float* g_p, int32_t ldgp, float* g_h, float* g_cm,
                      void* workspace, hgb_stream_t stream);
 
+/* SchNet continuous-filter convolution fused (hydragnn/models/SCFStack.py:267-301, CFConv.forward / message with aggr "add",
+ * filter network of get_conv :97-103, PyG GaussianSmearing / ShiftedSoftplus).  For the edge e = (row[e] -> col[e]):
+ * d_e = |pos[col] - pos[row]|, a_e = [exp(coeff (d_e - mu_k)^2), k < g | r_e] with r [e, d] (NULL when d = 0),
+ * W_e = (ssp(a_e^T a1t + b1) w2^T + b2) * 0.5 (cos(pi d_e / cutoff) + 1), ssp(x) = softplus(x, threshold 20) - log 2, and
+ * out [n, nf] = sum over the CSR (rowptr, perm) of the targets of xl[row[e]] * W_e.  a1t [g + d, nf] = [W1[:, :g]^T ; Mt];
+ * w2 [nf, nf], b1 / b2 [nf], mu [g].  w_e [e, nf] (NULL: not written) receives W_e in edge order.  1 <= g <= 64,
+ * 1 <= nf <= 128, 0 <= d <= 16 (hgb_cfconv_supported).  Backward (g_out [n, nf], g_we [e, nf] or NULL): g_xle [e, nf] =
+ * g_out[col] * W_e in edge order (the host sums it over the sources), g_dist [e] = dL/dd_e and g_r [e, d] (each NULL: not
+ * computed), g_params = [g_a1t [g + d, nf] | g_b1 [nf] | g_w2 [nf, nf] | g_b2 [nf]] (NULL: not computed) from per-CTA
+ * partials reduced in fixed order in fp64.  Deterministic: no atomics.  workspace: hgb_cfconv_workspace_bytes(g, nf, d) bytes (-1: unsupported).      */
+int hgb_cfconv_supported(int32_t g, int32_t nf, int32_t d);
+int64_t hgb_cfconv_workspace_bytes(int32_t g, int32_t nf, int32_t d);
+int hgb_cfconv_fwd(const float* xl, const float* pos, const int32_t* row, const int32_t* rowptr, const int32_t* perm,
+                   const float* r, int32_t d, const float* mu, float coeff, float cutoff, const float* a1t, const float* b1,
+                   const float* w2, const float* b2, int32_t n, int64_t e, int32_t g, int32_t nf, float* out, float* w_e,
+                   hgb_stream_t stream);
+int hgb_cfconv_bwd(const float* g_out, const float* g_we, const float* xl, const float* pos, const int32_t* row,
+                   const int32_t* col, const float* r, int32_t d, const float* mu, float coeff, float cutoff, const float* a1t,
+                   const float* b1, const float* w2, const float* b2, int32_t n, int64_t e, int32_t g, int32_t nf, float* g_xle,
+                   float* g_dist, float* g_r, float* g_params, void* workspace, hgb_stream_t stream);
+
 /* ---- MACE (hydragnn/utils/model/mace_utils/modules/blocks.py:369-402, symmetric_contraction.py:92-242) ------------------
  * Features are channel-last: [N, spherical index, F].  lmax_in <= 2, 1 <= lmax_sh <= 3, lmax_in <= lmax_sh, F % 32 == 0.
  * Path order / coupling constants = tp_out_irreps_with_instructions (irreps_tools.py:15-44) with e3nn's real Wigner 3j.   */
