@@ -11,7 +11,7 @@ import torch
 from torch import nn
 
 from . import ops
-from .stacks import EGCLStack, PAINNStack
+from .stacks import EGCLStack, PAINNStack, cached, graph_sum
 
 SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAEq", "MACE", "SchNet")
 
@@ -117,10 +117,7 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
         assert node_max_ell >= 1, "MACE requires node_max_ell >= 1."
         from .mace import MACEStack
         model = MACEStack(radius, radial_type, distance_transform, num_radial, edge_dim, max_ell, node_max_ell, avg_num_neighbors,
-                          envelope_exponent, correlation, input_dim, hidden_dim, output_dim, output_type, heads,
-                          activation_function, loss_function_type, loss_weights=task_weights, freeze_conv=freeze_conv,
-                          initial_bias=initial_bias, num_conv_layers=num_conv_layers, num_nodes=num_nodes,
-                          graph_pooling=graph_pooling, global_attn_engine=global_attn_engine)
+                          envelope_exponent, correlation, **common)
     elif mpnn_type == "SchNet":
         assert num_gaussians is not None, "SchNet requires num_guassians input."
         assert num_filters is not None, "SchNet requires num_filters input."
@@ -159,9 +156,9 @@ class EnhancedModelWrapper(nn.Module):
             "data.pos does not have grad, so force predictions cannot be computed. Check that data.pos has grad set to true before prediction."
         assert self.num_heads == 1, "Force predictions require exactly one head."
         lf = self.loss_function
+        gcsr = self.graph_index(data)[2]
         if self.head_type[0] == "node":
-            gcsr = data._hgb_gcsr
-            graph_energy_pred = ops.SegmentSum.apply(pred[0], ops.Csr(gcsr.idx, gcsr.rowptr, None, gcsr.n)).squeeze().float()
+            graph_energy_pred = graph_sum(pred[0], gcsr).squeeze().float()
         elif self.head_type[0] == "graph":
             if getattr(self.model, "graph_pooling", "mean") not in ["add"]:
                 raise ValueError("Graph head force loss requires sum pooling (graph_pooling='add').")
@@ -169,11 +166,10 @@ class EnhancedModelWrapper(nn.Module):
         else:
             raise ValueError("Force predictions are only supported for node or graph energy heads.")
         graph_energy_true = data.energy.squeeze().float()
-        valid = data.__dict__.get("_hgb_valid") if hasattr(data, "__dict__") else None
+        valid = cached(data, "_hgb_valid")
         if valid is not None:
             # capacity-padded batch (hydragnn_b200/padded.py): means run over the real graphs / atoms only; the counts live
             # on the device, nothing is read back
-            gcsr = data._hgb_gcsr
             gmask = (torch.arange(gcsr.n, device=valid.device) < valid[0]).to(graph_energy_pred.dtype)
             nmask = (torch.arange(data.pos.shape[0], device=valid.device) < valid[1]).to(graph_energy_pred.dtype)
             gcount = valid[0].to(graph_energy_pred.dtype).clamp(min=1)
@@ -190,7 +186,6 @@ class EnhancedModelWrapper(nn.Module):
         tot_loss = 0
         if ew > 0:
             tot_loss = tot_loss + tasks_loss[0] * ew
-        gcsr = data._hgb_gcsr
         natoms = (gcsr.rowptr[1:] - gcsr.rowptr[:-1]).to(graph_energy_pred.dtype)
         peratom = energy_loss(graph_energy_pred / natoms, graph_energy_true / natoms)
         tasks_loss.append(peratom)

@@ -19,7 +19,8 @@ import torch
 from torch import nn
 
 from . import e3, ops
-from .stacks import (_act_code, activation_function_selection, loss_function_selection, run_mlp)
+from .stacks import (ELEMENT_CSR, Base, cached, decode_branches, graph_head_mlp, graph_shared_mlp, graph_sum, remember,
+                     run_mlp)
 
 NUM_ELEMENTS = 118
 
@@ -294,26 +295,13 @@ class MultiheadDecoder(nn.Module):
         self.heads_NN = nn.ModuleList()
         if nonlinear and "graph" in config_heads:
             for br in config_heads["graph"]:
-                a = br["architecture"]
-                dim = a["dim_sharedlayers"]
-                layers = [nn.Linear(in_scalars, dim), act]
-                for _ in range(a["num_sharedlayers"] - 1):
-                    layers += [nn.Linear(dim, dim), act]
-                self.graph_shared[br["type"]] = nn.Sequential(*layers)
+                self.graph_shared[br["type"]] = graph_shared_mlp(in_scalars, br["architecture"], act)
         for ih in range(len(head_dims)):
             head = nn.ModuleDict({})
             if head_type[ih] == "graph":
                 for br in config_heads["graph"]:
-                    a = br["architecture"]
-                    if nonlinear:
-                        dims = a["dim_headlayers"]
-                        layers = [nn.Linear(a["dim_sharedlayers"], dims[0]), act]
-                        for k in range(a["num_headlayers"] - 1):
-                            layers += [nn.Linear(dims[k], dims[k + 1]), act]
-                        layers.append(nn.Linear(dims[-1], head_dims[ih]))
-                    else:
-                        layers = [nn.Linear(in_scalars, head_dims[ih])]
-                    head[br["type"]] = nn.Sequential(*layers)
+                    head[br["type"]] = (graph_head_mlp(br["architecture"], head_dims[ih], act) if nonlinear
+                                        else nn.Sequential(nn.Linear(in_scalars, head_dims[ih])))
             elif head_type[ih] == "node":
                 for br in config_heads["node"]:
                     a = br["architecture"]
@@ -331,66 +319,33 @@ class MultiheadDecoder(nn.Module):
         ids = None if dataset_name is None else dataset_name[:, 0]
         outs = []
         for hd, head, kind in zip(self.head_dims, self.heads_NN, self.head_type):
-            if kind == "graph":
-                if len(head) == 1:
-                    z = run_mlp(self.graph_shared["branch-0"], pooled, higher) if self.nonlinear else pooled
-                    out = run_mlp(head["branch-0"], z, higher)[:, :hd]
-                else:
-                    out = pooled.new_zeros(num_graphs, hd)
-                    for b in ids.unique():
-                        m, key = ids == b, "branch-%d" % int(b)
-                        z = run_mlp(self.graph_shared[key], pooled[m], higher) if self.nonlinear else pooled[m]
-                        out[m] = run_mlp(head[key], z, higher)[:, :hd]
+            if len(head) > 1:
+                outs.append(decode_branches(kind, head, self.graph_shared, ids, scalars, pooled, batch, hd, num_graphs, higher))
+            elif kind == "graph":
+                z = run_mlp(self.graph_shared["branch-0"], pooled, higher) if self.nonlinear else pooled
+                outs.append(run_mlp(head["branch-0"], z, higher)[:, :hd])
             else:
-                if len(head) == 1:
-                    out = head["branch-0"](scalars, higher)[:, :hd]
-                else:
-                    out = scalars.new_zeros(scalars.shape[0], hd)
-                    for b in ids.unique():
-                        m = (ids == b)[batch]
-                        out[m] = head["branch-%d" % int(b)](scalars[m], higher)[:, :hd]
-            outs.append(out)
+                outs.append(head["branch-0"](scalars, higher)[:, :hd])
         return outs
 
 
-class MACEStack(nn.Module):
+class MACEStack(Base):
     """hydragnn/models/MACEStack.py:70-498 (no GPS wrapping, no graph-attr conditioning).  With edge_dim = D > 0 every
     convolution reads ``data.edge_attr`` [E, D] as D extra 0e edge irreps in front of the spherical harmonics."""
 
     def __init__(self, r_max, radial_type, distance_transform, num_bessel, edge_dim, max_ell, node_max_ell, avg_num_neighbors,
-                 num_polynomial_cutoff, correlation, input_dim, hidden_dim, output_dim, output_type, config_heads,
-                 activation_function_type, loss_function_type, loss_weights=None, freeze_conv=False, initial_bias=None,
-                 num_conv_layers=2, num_nodes=None, graph_pooling="mean", global_attn_engine=None):
-        super().__init__()
-        if global_attn_engine:
+                 num_polynomial_cutoff, correlation, *args, **kwargs):
+        # refused before Base.__init__, which would build the GPS embeddings first
+        if kwargs.get("global_attn_engine"):
             raise ValueError("b200 engine: MACE inside GPS is not implemented")
         if distance_transform in ("Agnesi", "Soft"):
             raise ValueError("b200 engine: MACE distance transforms need ase covalent radii and are not implemented")
         if max_ell > 3:
             raise ValueError("b200 engine: MACE max_ell <= 3")
-        self.input_dim, self.hidden_dim, self.num_conv_layers, self.num_nodes = input_dim, hidden_dim, num_conv_layers, num_nodes
+        # ---- prior to inheritance (:111-150): Base.__init__ calls _init_conv, which reads these
+        num_conv_layers = kwargs["num_conv_layers"]
         self.edge_dim = int(edge_dim or 0)
-        self.use_edge_attr = self.edge_dim > 0
         self.max_ell, self.node_max_ell, self.avg_num_neighbors = max_ell, node_max_ell, avg_num_neighbors
-        self.head_dims, self.head_type = list(output_dim), list(output_type)
-        self.num_heads, self.config_heads = len(self.head_dims), config_heads
-        self.activation_function = activation_function_selection(activation_function_type)
-        self.var_output = 0
-        if loss_function_type == "GaussianNLLLoss":
-            raise ValueError("GaussianNLLLoss is not supported by the b200 engine")
-        self.loss_function_type, self.loss_function = loss_function_type, loss_function_selection(loss_function_type)
-        self.ilossweights_hyperp, self.ilossweights_nll = 1, 0
-        loss_weights = list(loss_weights if loss_weights is not None else [1.0] * self.num_heads)
-        if len(loss_weights) != self.num_heads:
-            raise ValueError("Inconsistent number of loss weights and tasks: " + str(len(loss_weights)) + " VS " + str(self.num_heads))
-        tot = sum(abs(w) for w in loss_weights)
-        self.loss_weights = [w / tot for w in loss_weights]
-        mode = graph_pooling.lower()
-        mode = "add" if mode == "sum" else mode
-        if mode not in ("mean", "add", "max"):
-            raise ValueError("Unsupported graph_pooling: " + graph_pooling)
-        self.graph_pooling = mode
-        self.freeze_conv, self.initial_bias, self.force_higher_order = freeze_conv, initial_bias, False
         p_cut = 5 if num_polynomial_cutoff is None else num_polynomial_cutoff
         if correlation is None:
             self.correlation = [2] * num_conv_layers
@@ -404,21 +359,8 @@ class MACEStack(nn.Module):
         if self.radial_type not in ("bessel", "gaussian", "chebyshev"):
             raise ValueError("unknown radial_type " + str(radial_type))
         self.num_bessel, self.radius, self.p_cut = num_bessel, float(r_max), float(p_cut)
-        # ---- decoders and convolutions interleaved, as MACEStack._init_conv creates them (:190-275)
-        self.graph_convs, self.multihead_decoders = nn.ModuleList(), nn.ModuleList()
-        f = hidden_dim
-        last = num_conv_layers == 1
-        self.multihead_decoders.append(self._decoder(last, NUM_ELEMENTS))
-        self.graph_convs.append(self._get_conv(0, last))
-        self.multihead_decoders.append(self._decoder(last, f))
-        for i in range(num_conv_layers - 1):
-            last = i == num_conv_layers - 2
-            self.graph_convs.append(self._get_conv(node_max_ell, last))
-            self.multihead_decoders.append(self._decoder(last, f))
-        if freeze_conv:
-            for p in self.graph_convs.parameters():
-                p.requires_grad = False
-        # ---- post-inheritance part of MACEStack.__init__ (:154-187)
+        super().__init__(*args, **kwargs)
+        # ---- post inheritance (:154-187)
         self.register_buffer("atomic_numbers", torch.arange(1, NUM_ELEMENTS + 1, dtype=torch.int64))
         self.register_buffer("r_max", torch.tensor(float(r_max)))
         self.register_buffer("num_interactions", torch.tensor(num_conv_layers, dtype=torch.int64))
@@ -436,7 +378,18 @@ class MACEStack(nn.Module):
         self.radial_embedding.cutoff_fn.register_buffer("p", torch.tensor(float(p_cut)))
         self.radial_embedding.cutoff_fn.register_buffer("r_max", torch.tensor(float(r_max)))
         self.node_embedding = nn.Module()
-        self.node_embedding.linear = E3Linear([(NUM_ELEMENTS, 0, 1)], [(f, 0, 1)])
+        self.node_embedding.linear = E3Linear([(NUM_ELEMENTS, 0, 1)], [(self.hidden_dim, 0, 1)])
+
+    def _init_conv(self):
+        """Decoders and convolutions interleaved, in the order MACEStack._init_conv creates them (:190-275)."""
+        self.multihead_decoders = nn.ModuleList([self._decoder(self.num_conv_layers == 1, NUM_ELEMENTS)])
+        for i in range(self.num_conv_layers):
+            last = i == self.num_conv_layers - 1
+            self.graph_convs.append(self._get_conv(self.node_max_ell if i else 0, last))
+            self.multihead_decoders.append(self._decoder(last, self.hidden_dim))
+
+    def _multihead(self):
+        """Nothing (:500): every decoder is one of ``multihead_decoders``."""
 
     def _decoder(self, nonlinear, in_scalars):
         return MultiheadDecoder(nonlinear, in_scalars, self.config_heads, self.head_dims, self.head_type, self.activation_function,
@@ -466,38 +419,15 @@ class MACEStack(nn.Module):
             radial = torch.special.chebyshev_polynomial_t(d.repeat(1, self.num_bessel), bf.n.repeat(len(d), 1))
         return radial * cutoff
 
-    def _higher_order(self, data):
-        pos = data.pos
-        return bool(self.force_higher_order or (self.training and torch.is_grad_enabled() and pos is not None and pos.requires_grad))
-
-    def forward(self, data):
-        from .stacks import Base
-        if data.x.dtype != torch.float32:
-            raise RuntimeError("b200 engine kernels are fp32 (bf16 via autocast-style GEMMs); got " + str(data.x.dtype))
+    def _forward(self, data, higher):
+        """MACEStack.forward (:375-421): a readout before the convolutions and after each, outputs summed."""
         assert data.pos is not None, "MACE requires node positions (data.pos) to be set."
-        higher = self._higher_order(data)
-        if getattr(self, "precision", "fp32") == "bf16" and not ops._TC["enabled"]:
-            with ops.tensor_cores(True):
-                return self.forward(data)
-        plan = Base.plan_for(data)
-        pos, batch = data.pos, data.batch
-        n = pos.shape[0]
-        if batch is None:
-            batch = torch.zeros(n, dtype=torch.long, device=pos.device)
-        num_graphs = data.__dict__.get("_num_graphs") if hasattr(data, "__dict__") else None
-        if num_graphs is None:
-            num_graphs = int(batch.max()) + 1
-        gcsr = data.__dict__.get("_hgb_gcsr") if hasattr(data, "__dict__") else None
-        if gcsr is None or gcsr.n != num_graphs or gcsr.idx.numel() != n:
-            gcsr = ops.graph_ptr_from_batch(batch, num_graphs)
-            try:
-                data._hgb_gcsr = gcsr
-            except Exception:
-                pass
+        plan = self.plan_for(data)
+        batch, num_graphs, gcsr = self.graph_index(data)
+        pos, n = data.pos, data.pos.shape[0]
         # centre every graph (MACEStack.py:438-443); deterministic segmented mean + gather back
         cnt = (gcsr.rowptr[1:] - gcsr.rowptr[:-1]).clamp(min=1).to(pos.dtype)
-        gsum = ops.SegmentSum.apply(pos, ops.Csr(gcsr.idx, gcsr.rowptr, None, gcsr.n))
-        pos = pos - ops.GatherRows.apply(gsum / cnt[:, None], gcsr)
+        pos = pos - ops.GatherRows.apply(graph_sum(pos, gcsr) / cnt[:, None], gcsr)
         shifts = getattr(data, "edge_shifts", None)
         eattr = self._edge_attr(data, plan.num_edges) if self.use_edge_attr else None
         if not higher and self.radial_type == "bessel":
@@ -514,23 +444,19 @@ class MACEStack(nn.Module):
         z = data.x.squeeze()
         assert z.dim() == 1, "MACE only supports raw atomic numbers as node_attributes."
         z = (z.clamp(min=1, max=NUM_ELEMENTS) - 1).long()
-        zcsr = data.__dict__.get("_hgb_zcsr") if hasattr(data, "__dict__") else None
+        zcsr = cached(data, ELEMENT_CSR)
         if zcsr is None or zcsr.idx.numel() != n:
-            zcsr = ops.csr_build(z, NUM_ELEMENTS)
-            try:
-                data._hgb_zcsr = zcsr
-            except Exception:
-                pass
+            zcsr = remember(data, ELEMENT_CSR, ops.csr_build(z, NUM_ELEMENTS))
         emb = self.node_embedding.linear
         table = emb.weight.reshape(NUM_ELEMENTS, self.hidden_dim) * emb.alpha[0]      # one-hot @ W == row gather
         xs = [ops.GatherRows.apply(table, zcsr)[:, None, :]]
         ds = getattr(data, "dataset_name", None)
         onehot = torch.nn.functional.one_hot(z, NUM_ELEMENTS).to(pos.dtype)
-        outputs = self.multihead_decoders[0](onehot, self._pool(onehot, gcsr, higher), batch, num_graphs, ds, higher)
+        outputs = self.multihead_decoders[0](onehot, self.pool(onehot, gcsr, higher), batch, num_graphs, ds, higher)
         for conv, readout in zip(self.graph_convs, self.multihead_decoders[1:]):
             xs = conv(xs, sh, radial, plan, zcsr, higher, eattr)
             scalars = xs[0][:, 0, :]
-            out = readout(scalars, self._pool(scalars, gcsr, higher), batch, num_graphs, ds, higher)
+            out = readout(scalars, self.pool(scalars, gcsr, higher), batch, num_graphs, ds, higher)
             outputs = [a + b for a, b in zip(outputs, out)]
         return outputs
 
@@ -545,25 +471,6 @@ class MACEStack(nn.Module):
         if ea.requires_grad:
             raise ValueError("MACE edge_attr must not require grad: edge attributes are data (detach them)")
         return ea.contiguous()
-
-    def _pool(self, x, gcsr, higher):
-        if higher and self.graph_pooling != "max":
-            out = ops.SegmentSum.apply(x, ops.Csr(gcsr.idx, gcsr.rowptr, None, gcsr.n))
-            if self.graph_pooling == "mean":
-                out = out / (gcsr.rowptr[1:] - gcsr.rowptr[:-1]).clamp(min=1).to(x.dtype)[:, None]
-            return out
-        return ops.PoolFn.apply(x.contiguous(), gcsr, self.graph_pooling)
-
-    def loss(self, pred, value, head_index):
-        """``loss_hpweighted`` (hydragnn/models/Base.py:879-906)."""
-        tot_loss, tasks_loss = 0, []
-        for ihead in range(self.num_heads):
-            head_pre = pred[ihead]
-            head_val = value[head_index[ihead]].reshape(head_pre.shape)
-            li = self.loss_function(head_pre, head_val)
-            tot_loss = tot_loss + li * self.loss_weights[ihead]
-            tasks_loss.append(li)
-        return tot_loss, tasks_loss
 
     def __str__(self):
         return "MACEStack"

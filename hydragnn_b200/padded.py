@@ -25,6 +25,7 @@ import torch.distributed as dist
 from . import _lib, ops, radius
 from .data import Batch
 from .ops import _p, _stream
+from .stacks import forget_plans
 
 
 def _round_up(x, m):
@@ -152,8 +153,7 @@ class PaddedGraphStep:
             e_real = self.valid[2:3]
         _lib.call("hgb_pad_edges", _p(e_real), _p(self.valid[1:2]), self.n_cap, self.e_cap, _p(d.edge_index), _p(ops.guard_flag(self.dev)),
                   _stream())
-        for key in ("_hgb_plan", "_hgb_gcsr", "_hgb_col_sorted", "_hgb_zcsr"):     # MACE's element CSR follows x of each batch
-            d.__dict__.pop(key, None)
+        forget_plans(d)                     # index plans are part of the step: every batch brings new edges and elements
         self.opt.zero_grad()
         if self.mlip:
             d.pos.requires_grad_(True)

@@ -129,6 +129,36 @@ def _padded_chain(mods, x):
     return out
 
 
+# Per-batch index plans, cached on the batch object: the CSR views of edge_index (ops.EdgePlan), the graph offsets, MACE's
+# element CSR, and the (edge_index, rowptr, graph_ptr) hint a radius build leaves.  A step that copies a new batch into the same
+# tensors must forget them (``forget_plans``).
+PLAN_KEYS = EDGE_PLAN, GRAPH_CSR, ELEMENT_CSR, COL_SORTED = ("_hgb_plan", "_hgb_gcsr", "_hgb_zcsr", "_hgb_col_sorted")
+
+
+def cached(data, key):
+    """The value cached on ``data`` under ``key``, or None."""
+    return data.__dict__.get(key) if hasattr(data, "__dict__") else None
+
+
+def remember(data, key, value):
+    """Cache ``value`` on ``data`` under ``key`` when the object takes attributes; returns ``value``."""
+    try:
+        setattr(data, key, value)
+    except Exception:
+        pass
+    return value
+
+
+def forget_plans(data):
+    for key in PLAN_KEYS:
+        data.__dict__.pop(key, None)
+
+
+def graph_sum(x, gcsr):
+    """Sum of the rows of ``x`` over the atoms of every graph: [G, ...].  Atoms are sorted by graph, so no permutation."""
+    return SegmentSum.apply(x, ops.Csr(gcsr.idx, gcsr.rowptr, None, gcsr.n))
+
+
 def run_mlp(seq, x, higher_order=False):
     """Execute an ``nn.Sequential`` of Linear / activation modules on the engine: every Linear (with the
     activation that follows it) is one fused kernel; in any-order mode it is MatMul + ATen glue."""
@@ -367,6 +397,42 @@ class MLPNode(nn.Module):
         return torch.stack([run_mlp(self.mlp[i], xs[:, i, :].contiguous(), higher_order) for i in range(k)], dim=1).reshape(x.shape[0], -1)
 
 
+def graph_shared_mlp(in_dim, arch, act):
+    """Shared layers of one graph-head branch (Base.py:600-610): ``num_sharedlayers`` Linear + act, ``dim_sharedlayers`` wide."""
+    dim = arch["dim_sharedlayers"]
+    layers = [nn.Linear(in_dim, dim), act]
+    for _ in range(arch["num_sharedlayers"] - 1):
+        layers += [nn.Linear(dim, dim), act]
+    return nn.Sequential(*layers)
+
+
+def graph_head_mlp(arch, out_dim, act):
+    """Head layers of one graph-head branch (Base.py:619-640), reading the output of ``graph_shared_mlp``."""
+    hid = list(arch["dim_headlayers"])
+    layers = [nn.Linear(arch["dim_sharedlayers"], hid[0]), act]
+    for j in range(arch["num_headlayers"] - 1):
+        layers += [nn.Linear(hid[j], hid[j + 1]), act]
+    layers.append(nn.Linear(hid[-1], out_dim))
+    return nn.Sequential(*layers)
+
+
+def decode_branches(kind, head, graph_shared, ids, x, x_graph, batch, hd, num_graphs, higher_order):
+    """One head over several dataset branches (Base.py:770-780, 816-840): the graphs (or their atoms) of branch b go through
+    ``head["branch-b"]``, graph heads after ``graph_shared["branch-b"]`` when the decoder has shared layers."""
+    if kind == "graph":
+        out = x_graph.new_zeros(num_graphs, hd)
+        for b in ids.unique():
+            msk, key = ids == b, "branch-%d" % int(b)
+            z = run_mlp(graph_shared[key], x_graph[msk], higher_order) if key in graph_shared else x_graph[msk]
+            out[msk] = run_mlp(head[key], z, higher_order)[:, :hd]
+    else:
+        out = x.new_zeros(x.shape[0], hd)
+        for b in ids.unique():
+            msk = (ids == b)[batch]
+            out[msk] = head["branch-%d" % int(b)](x[msk], higher_order)[:, :hd]
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # Base: encoder loop + pooling + multi-head decoder
 # ------------------------------------------------------------------------------------------------
@@ -458,11 +524,7 @@ class Base(nn.Module):
         if "graph" in self.config_heads:
             self.num_branches = len(self.config_heads["graph"])
             for br in self.config_heads["graph"]:
-                a = br["architecture"]
-                layers = [nn.Linear(self.hidden_dim, a["dim_sharedlayers"]), act]
-                for _ in range(a["num_sharedlayers"] - 1):
-                    layers += [nn.Linear(a["dim_sharedlayers"], a["dim_sharedlayers"]), act]
-                self.graph_shared[br["type"]] = nn.Sequential(*layers)
+                self.graph_shared[br["type"]] = graph_shared_mlp(self.hidden_dim, br["architecture"], act)
         if "node" in self.config_heads:
             self._init_node_conv()
         inode = 0
@@ -470,13 +532,7 @@ class Base(nn.Module):
             head = nn.ModuleDict()
             if self.head_type[ih] == "graph":
                 for br in self.config_heads["graph"]:
-                    a = br["architecture"]
-                    hid = list(a["dim_headlayers"])
-                    layers = [nn.Linear(a["dim_sharedlayers"], hid[0]), act]
-                    for j in range(a["num_headlayers"] - 1):
-                        layers += [nn.Linear(hid[j], hid[j + 1]), act]
-                    layers.append(nn.Linear(hid[-1], self.head_dims[ih]))
-                    head[br["type"]] = nn.Sequential(*layers)
+                    head[br["type"]] = graph_head_mlp(br["architecture"], self.head_dims[ih], act)
             elif self.head_type[ih] == "node":
                 for br in self.config_heads["node"]:
                     a = br["architecture"]
@@ -532,19 +588,30 @@ class Base(nn.Module):
     # -- per-batch preparation -----------------------------------------------------------------------
     @staticmethod
     def plan_for(data):
-        plan = data.__dict__.get("_hgb_plan") if hasattr(data, "__dict__") else None
+        plan = cached(data, EDGE_PLAN)
         ei = data.edge_index
         if plan is None or plan.num_edges != ei.shape[1] or plan.row.device != ei.device or plan._src is not ei:
-            hint = data.__dict__.get("_hgb_col_sorted") if hasattr(data, "__dict__") else None     # (edge_index, rowptr[, graph_ptr])
+            hint = cached(data, COL_SORTED)                                   # (edge_index, rowptr[, graph_ptr])
             ok = hint is not None and hint[0] is ei
             plan = ops.EdgePlan(ei, data.pos.shape[0] if data.pos is not None else data.x.shape[0],
                                 col_rowptr=hint[1] if ok else None, graph_ptr=hint[2] if (ok and len(hint) > 2) else None)
             plan._src = ei
-            try:
-                data._hgb_plan = plan
-            except Exception:
-                pass
+            remember(data, EDGE_PLAN, plan)
         return plan
+
+    @staticmethod
+    def graph_index(data):
+        """(batch, num_graphs, gcsr): the graph of every atom, the number of graphs and the graph offsets as a CSR."""
+        batch = data.batch
+        if batch is None:
+            batch = torch.zeros(data.x.shape[0], dtype=torch.long, device=data.x.device)
+        num_graphs = cached(data, "_num_graphs")
+        if num_graphs is None:
+            num_graphs = int(batch.max()) + 1
+        gcsr = cached(data, GRAPH_CSR)
+        if gcsr is None or gcsr.n != num_graphs or gcsr.idx.numel() != batch.numel():
+            gcsr = remember(data, GRAPH_CSR, ops.graph_ptr_from_batch(batch, num_graphs))
+        return batch, num_graphs, gcsr
 
     def _edge_plan(self, data):
         """The plan of ``data.edge_index`` the convolutions share; a stack that builds its graphs in the layers returns None."""
@@ -569,32 +636,22 @@ class Base(nn.Module):
                     (self.training and torch.is_grad_enabled() and pos is not None and pos.requires_grad))
 
     def forward(self, data):
-        x = data.x
-        if x.dtype != torch.float32:
-            raise RuntimeError("b200 engine kernels are fp32 (bf16 via autocast-style GEMMs); got " + str(x.dtype))
-        higher = self._higher_order(data)
+        if data.x.dtype != torch.float32:
+            raise RuntimeError("b200 engine kernels are fp32 (bf16 via autocast-style GEMMs); got " + str(data.x.dtype))
         if getattr(self, "precision", "fp32") == "bf16" and not ops._TC["enabled"]:
             with ops.tensor_cores(True):       # large-M Linears on wgmma (TF32 in, fp32 accumulate)
-                return self.forward(data)
+                return self._forward(data, self._higher_order(data))
+        return self._forward(data, self._higher_order(data))
+
+    def _forward(self, data, higher):
+        """Encoder loop, pooling and heads (Base.py:697-846); ``higher``: any-order differentiable path."""
         plan = self._edge_plan(data)
         inv, equiv, conv_args = self._embedding(data, plan, higher)
         for conv, feat in zip(self.graph_convs, self.feature_layers):
             inv, equiv = conv(inv_node_feat=inv, equiv_node_feat=equiv, plan=plan, higher_order=higher, **conv_args)
             inv = self.activation_function(feat(inv))                        # Base.py:726
         x = inv
-        batch = data.batch
-        if batch is None:
-            batch = torch.zeros(x.shape[0], dtype=torch.long, device=x.device)
-        num_graphs = data.__dict__.get("_num_graphs") if hasattr(data, "__dict__") else None
-        if num_graphs is None:
-            num_graphs = int(batch.max()) + 1
-        gcsr = data.__dict__.get("_hgb_gcsr") if hasattr(data, "__dict__") else None
-        if gcsr is None or gcsr.n != num_graphs or gcsr.idx.numel() != batch.numel():
-            gcsr = ops.graph_ptr_from_batch(batch, num_graphs)
-            try:
-                data._hgb_gcsr = gcsr
-            except Exception:
-                pass
+        batch, num_graphs, gcsr = self.graph_index(data)
         x_graph = self.pool(x, gcsr, higher)                                  # Base.py:733-738
         ds = getattr(data, "dataset_name", None)
         outputs = []
@@ -615,20 +672,8 @@ class Base(nn.Module):
                 continue
             ids = ds[:, 0]                                                   # Base.py:770-780, 816-840
             out = None if higher else self._grouped_decode(kind, head, ids, x, x_graph, batch, hd, num_graphs)
-            if out is not None:
-                outputs.append(out)
-                continue
-            if kind == "graph":
-                out = x.new_zeros(num_graphs, hd)
-                for b in ids.unique():
-                    msk = ids == b
-                    key = "branch-%d" % int(b)
-                    out[msk] = run_mlp(head[key], run_mlp(self.graph_shared[key], x_graph[msk], higher), higher)[:, :hd]
-            else:
-                out = x.new_zeros(x.shape[0], hd)
-                for b in ids.unique():
-                    msk = (ids == b)[batch]
-                    out[msk] = head["branch-%d" % int(b)](x[msk], higher)[:, :hd]
+            if out is None:
+                out = decode_branches(kind, head, self.graph_shared, ids, x, x_graph, batch, hd, num_graphs, higher)
             outputs.append(out)
         return outputs
 
@@ -657,7 +702,7 @@ class Base(nn.Module):
 
     def pool(self, x, gcsr, higher_order=False):
         if higher_order and self.graph_pooling != "max":
-            out = SegmentSum.apply(x, ops.Csr(gcsr.idx, gcsr.rowptr, None, gcsr.n))
+            out = graph_sum(x, gcsr)
             if self.graph_pooling == "mean":
                 cnt = (gcsr.rowptr[1:] - gcsr.rowptr[:-1]).clamp(min=1).to(x.dtype)
                 out = out / cnt[:, None]

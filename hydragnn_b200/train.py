@@ -16,6 +16,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops
+from .stacks import forget_plans
 
 PRECISION_MAP = {"bf16": torch.float32, "fp32": torch.float32}     # parameters stay fp32 (reference :43-49)
 
@@ -265,8 +266,7 @@ class GraphedTrainStep:
     def _fwd_bwd(self):
         m = self.model.module
         d = self.data
-        for k in ("_hgb_plan", "_hgb_gcsr", "_hgb_zcsr"):   # index plans are part of the step (ADVICE r1: stale CSR after refill)
-            d.__dict__.pop(k, None)
+        forget_plans(d)                     # index plans are part of the step: a refill may bring new edges and elements
         self.opt.zero_grad()
         if self.mlip:
             d.pos.requires_grad_(True)
