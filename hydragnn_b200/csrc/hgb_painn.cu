@@ -191,21 +191,36 @@ __device__ __forceinline__ void pm_cp_async16(void* smem, const void* g) {
 __device__ __forceinline__ void pm_cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void pm_cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-template <bool HAS_EF, int RT, int FT>
+__device__ __forceinline__ float pm_lds_f1(uint32_t addr) {
+  float r;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(addr));
+  return r;
+}
+
+// Affine v (AV, FT = 64 only): the layer's v is v[n, k, c] = fmaf(v_in[n, k], v_w[c], v_b[c]) -- PaiNN's first-layer
+// vec_embed_out, Linear(1, F) of a [N, 3, 1] tensor, with exactly the rounding of linear_smallk_fwd_vec4_kernel<1>.  Only
+// v_in ([tn, 3] floats per tile) is staged; every v value is formed in registers, so the [N, 3, F] v never leaves the chip.
+// A tile start must be 16-byte aligned in v_in (tn % 4 == 0); the last tile's 4..12-byte tail is stored by the issuing thread.
+#define AV_TILE_BYTES(tn) ((((uint32_t)(tn) * 12u) + 15u) & ~15u)
+
+template <bool HAS_EF, int RT, int FT, bool AV>
 __global__ void __launch_bounds__(TWPB * 32, 2)
 painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __restrict__ s, const float* __restrict__ v,
+                               const float* __restrict__ v_in, const float* __restrict__ v_w, const float* __restrict__ v_b,
                                const int32_t* __restrict__ rowptr, const float* __restrict__ rec, const float* __restrict__ wf,
                                const float* __restrict__ bf, const float* __restrict__ efilt, int n, int f_rt, int r, int tn,
                                float* __restrict__ s_out, float* __restrict__ v_out) {
+  static_assert(!AV || FT == 64, "affine v: one 64-channel block");
   extern __shared__ __align__(128) uint8_t pm_smem[];
   const int f = FT ? FT : f_rt;   // FT = 64: strides become immediates
   const int f3 = 3 * f;
   const uint32_t tile_bytes = (uint32_t)tn * f3 * 4;
-  // buffer b: phi tile at pm_smem + 2 b tile_bytes, v tile right behind it (pointer arithmetic, not an indexed array:
-  // a dynamically indexed pointer array would live in local memory)
-  auto sphi = [&](int b) { return reinterpret_cast<float*>(pm_smem + (size_t)(2 * b) * tile_bytes); };
-  auto sv = [&](int b) { return reinterpret_cast<float*>(pm_smem + (size_t)(2 * b + 1) * tile_bytes); };
-  uint64_t* full = reinterpret_cast<uint64_t*>(pm_smem + 4 * (size_t)tile_bytes);
+  const uint32_t vt_bytes = AV ? AV_TILE_BYTES(tn) : tile_bytes;
+  // buffer b: phi tile at pm_smem + b (tile_bytes + vt_bytes), v (or v_in) tile right behind it (pointer arithmetic, not an
+  // indexed array: a dynamically indexed pointer array would live in local memory)
+  auto sphi = [&](int b) { return reinterpret_cast<float*>(pm_smem + (size_t)b * (tile_bytes + vt_bytes)); };
+  auto sv = [&](int b) { return reinterpret_cast<float*>(pm_smem + (size_t)b * (tile_bytes + vt_bytes) + tile_bytes); };
+  uint64_t* full = reinterpret_cast<uint64_t*>(pm_smem + 2 * ((size_t)tile_bytes + vt_bytes));
   uint64_t* empty = full + 2;
   // per warp: 2 x (8 edge records [32 float4] + the node's s row slice [16 float4])
   float4* scr = reinterpret_cast<float4*>(full + 4) + (threadIdx.x >> 5) * 96;
@@ -223,6 +238,14 @@ painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __res
   auto issue = [&](int t, int buf) {   // one thread: two bulk copies for tile t
     const int n0 = t * tn;
     const uint32_t bytes = (uint32_t)(min(n, n0 + tn) - n0) * f3 * 4;
+    if (AV) {
+      const uint32_t vb = (uint32_t)(min(n, n0 + tn) - n0) * 12u, vbulk = vb & ~15u;
+      for (uint32_t q = vbulk / 4; q < vb / 4; ++q) sv(buf)[q] = __ldg(v_in + (int64_t)n0 * 3 + q);   // released by the arrive below
+      pm_mbar_expect_tx(full + buf, bytes + vbulk);
+      pm_bulk_g2s(sphi(buf), phi + (int64_t)n0 * f3, bytes, full + buf);
+      if (vbulk) pm_bulk_g2s(sv(buf), v_in + (int64_t)n0 * 3, vbulk, full + buf);
+      return;
+    }
     pm_mbar_expect_tx(full + buf, 2 * bytes);
     pm_bulk_g2s(sphi(buf), phi + (int64_t)n0 * f3, bytes, full + buf);
     pm_bulk_g2s(sv(buf), v + (int64_t)n0 * f3, bytes, full + buf);
@@ -269,6 +292,8 @@ painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __res
     const uint32_t tphi_u = pm_smem_u32(sphi(buf)), tv_u = pm_smem_u32(sv(buf));
     for (int cb = 0; cb < ncb; ++cb) {
       const int cc = cb * 64 + lane * 2;
+      float aw[2] = {0.f, 0.f}, ab[2] = {0.f, 0.f};   // AV: this lane's two channels of v_w / v_b
+      if (AV) { aw[0] = __ldg(v_w + cc); aw[1] = __ldg(v_w + cc + 1); ab[0] = __ldg(v_b + cc); ab[1] = __ldg(v_b + cc + 1); }
       float wr[3][2][RT + 1];
 #pragma unroll
       for (int a = 0; a < 3; ++a)
@@ -309,14 +334,28 @@ painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __res
             const uint32_t off = (uint32_t)((j - n0) * f3 + cc) * 4u;
 #pragma unroll
             for (int a = 0; a < 3; ++a) {
-              const float2 x2 = pm_lds_f2(tphi_u + off + a * f * 4), y2 = pm_lds_f2(tv_u + off + a * f * 4);
-              pv[a][0] = x2.x; pv[a][1] = x2.y; vv[a][0] = y2.x; vv[a][1] = y2.y;
+              const float2 x2 = pm_lds_f2(tphi_u + off + a * f * 4);
+              pv[a][0] = x2.x; pv[a][1] = x2.y;
+              if (AV) {
+                const float x0 = pm_lds_f1(tv_u + (uint32_t)((j - n0) * 3 + a) * 4u);
+                vv[a][0] = fmaf(x0, aw[0], ab[0]); vv[a][1] = fmaf(x0, aw[1], ab[1]);
+              } else {
+                const float2 y2 = pm_lds_f2(tv_u + off + a * f * 4);
+                vv[a][0] = y2.x; vv[a][1] = y2.y;
+              }
             }
           } else {
             const float* ph = phi + (int64_t)j * f3 + cc;
-            const float* vj = v + (int64_t)j * f3 + cc;
 #pragma unroll
-            for (int a = 0; a < 3; ++a) { ChanVec<2>::ld(ph + a * f, pv[a]); ChanVec<2>::ld(vj + a * f, vv[a]); }
+            for (int a = 0; a < 3; ++a) {
+              ChanVec<2>::ld(ph + a * f, pv[a]);
+              if (AV) {
+                const float x0 = __ldg(v_in + (int64_t)j * 3 + a);
+                vv[a][0] = fmaf(x0, aw[0], ab[0]); vv[a][1] = fmaf(x0, aw[1], ab[1]);
+              } else {
+                ChanVec<2>::ld(v + (int64_t)j * f3 + a * f + cc, vv[a]);
+              }
+            }
           }
           float ef[3][2];
           if (HAS_EF) {
@@ -345,7 +384,13 @@ painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __res
         ChanVec<2>::st(s_out + (int64_t)i * f + cc, so);
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
-          const float2 own = *reinterpret_cast<const float2*>(tv + (size_t)(i - n0) * f3 + k * f + cc);
+          float2 own;
+          if (AV) {
+            const float x0 = tv[(i - n0) * 3 + k];
+            own = make_float2(fmaf(x0, aw[0], ab[0]), fmaf(x0, aw[1], ab[1]));
+          } else {
+            own = *reinterpret_cast<const float2*>(tv + (size_t)(i - n0) * f3 + k * f + cc);
+          }
           tmp[0] = own.x + av[k][0]; tmp[1] = own.y + av[k][1];
           ChanVec<2>::st(v_out + (int64_t)i * f3 + k * f + cc, tmp);
         }
@@ -361,33 +406,42 @@ painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __res
 static int painn_group(int f) { int g = 32; if (f < 32) { g = 1; while (g < f) g <<= 1; } return g; }
 static int painn_cpl(int f) { return (f >= 64 && f % 2 == 0) ? 2 : 1; }
 
-extern "C" int hgb_painn_message_fwd(const float* phi, const float* s, const float* v, const int32_t* rowptr,
-                                     const int32_t* perm, const int32_t* nbr, const float* epack, const float* rec, const float* wf,
-                                     const float* bf, const float* efilt, int32_t n, int32_t f, int32_t r, float* s_out, float* v_out,
-                                     hgb_stream_t stream) {
+extern "C" int hgb_painn_message_affine_v_supported(int32_t n, int32_t f) { return (f == 64 && n >= 256) ? 1 : 0; }
+
+extern "C" int hgb_painn_message_fwd(const float* phi, const float* s, const float* v, const float* v_in, const float* v_w,
+                                     const float* v_b, const int32_t* rowptr, const int32_t* perm, const int32_t* nbr,
+                                     const float* epack, const float* rec, const float* wf, const float* bf, const float* efilt,
+                                     int32_t n, int32_t f, int32_t r, float* s_out, float* v_out, hgb_stream_t stream) {
   HGB_REQUIRE(n >= 0 && f > 0 && r > 0 && r <= RMAX, "painn_message_fwd: need 0 < num_radial <= %d (got %d)", RMAX, r);
-  HGB_REQUIRE(phi && s && v && rowptr && nbr && epack && wf && bf && s_out && v_out, "painn_message_fwd: null pointer");
+  const bool av = v_in != nullptr;
+  HGB_REQUIRE(phi && s && (av ? (v_w && v_b && !v) : v != nullptr) && rowptr && nbr && epack && wf && bf && s_out && v_out,
+              "painn_message_fwd: null pointer (or both v and v_in)");
+  HGB_REQUIRE(!av || (hgb_painn_message_affine_v_supported(n, f) && rec &&
+                      (((uintptr_t)phi | (uintptr_t)s | (uintptr_t)rec | (uintptr_t)v_in) % 16 == 0)),
+              "painn_message_fwd: affine v needs f = 64, n >= 256, edge records and 16-byte aligned rows (n=%d f=%d)", n, f);
   if (n == 0) return HGB_OK;
   cudaStream_t st = (cudaStream_t)stream;
   if (rec && f % 64 == 0 && f <= 256 && n >= 256 && (((uintptr_t)phi | (uintptr_t)v | (uintptr_t)s | (uintptr_t)rec) % 16 == 0)) {
-    // tiled path: two double-buffered [tn x 3f] fp32 tiles
-    int tn = (int)((110 * 1024 - TWPB * 1536 - 64) / ((size_t)4 * 3 * f * 4));   // two blocks per SM
-    tn = (tn / TWPB) * TWPB;                                   // whole nodes per warp
-    if (tn > 3 * TWPB) tn = 3 * TWPB;
-    if (tn < TWPB) tn = TWPB;
-    const size_t smem = (size_t)4 * tn * 3 * f * 4 + 64 + TWPB * 1536;
+    // tiled path: two double-buffered [tn x 3f] fp32 tiles of phi and of v (affine v: of phi and of the [tn x 3] v_in)
+    const size_t fixed = TWPB * 1536 + 64, row = av ? (size_t)2 * 3 * f * 4 + 2 * 12 : (size_t)4 * 3 * f * 4;
+    const int step = av ? 2 * TWPB : TWPB;                     // whole nodes per warp; affine v: tile starts 16-byte aligned in v_in
+    int tn = (int)((110 * 1024 - fixed) / row);                // two blocks per SM
+    tn = (tn / step) * step;
+    if (tn < step) tn = step;
+    const size_t smem = av ? (size_t)2 * tn * 3 * f * 4 + 2 * AV_TILE_BYTES(tn) + fixed : (size_t)4 * tn * 3 * f * 4 + fixed;
     static bool attr_done = false;
     if (!attr_done) {
-#define SETA(E, R) cudaFuncSetAttribute(painn_message_fwd_tiled_kernel<E, R, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
-                   cudaFuncSetAttribute(painn_message_fwd_tiled_kernel<E, R, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
+#define SETA(E, R) cudaFuncSetAttribute(painn_message_fwd_tiled_kernel<E, R, 64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
+                   cudaFuncSetAttribute(painn_message_fwd_tiled_kernel<E, R, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
+                   cudaFuncSetAttribute(painn_message_fwd_tiled_kernel<E, R, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
       SETA(false, 5); SETA(false, 8); SETA(true, 5); SETA(true, 8);
 #undef SETA
       attr_done = true;
     }
     const int ntiles = (n + tn - 1) / tn;
     const int g1 = ntiles < 2 * HGB_NUM_SMS ? ntiles : 2 * HGB_NUM_SMS;
-#define LAUNCH_F(E, R, F) painn_message_fwd_tiled_kernel<E, R, F><<<g1, TWPB * 32, smem, st>>>(phi, s, v, rowptr, rec, wf, bf, efilt, n, f, r, tn, s_out, v_out)
-#define LAUNCH_T(E, R) do { if (f == 64) LAUNCH_F(E, R, 64); else LAUNCH_F(E, R, 0); } while (0)
+#define LAUNCH_F(E, R, F, A) painn_message_fwd_tiled_kernel<E, R, F, A><<<g1, TWPB * 32, smem, st>>>(phi, s, v, v_in, v_w, v_b, rowptr, rec, wf, bf, efilt, n, f, r, tn, s_out, v_out)
+#define LAUNCH_T(E, R) do { if (av) LAUNCH_F(E, R, 64, true); else if (f == 64) LAUNCH_F(E, R, 64, false); else LAUNCH_F(E, R, 0, false); } while (0)
     if (efilt) { if (r <= 5) LAUNCH_T(true, 5); else LAUNCH_T(true, 8); }
     else { if (r <= 5) LAUNCH_T(false, 5); else LAUNCH_T(false, 8); }
 #undef LAUNCH_T
@@ -578,13 +632,18 @@ painn_message_bwd_kernel(const float* __restrict__ gs_out, const float* __restri
 // ---- tiled backward (F % 64 == 0): the incoming gradients gs_out / gv_out of a tile of consecutive nodes are staged in
 // shared memory (bulk async copies, double buffered); the warp that owns source node j gathers the gradient rows of the
 // nodes it sent messages to from shared memory.  rec is the by-col CSR record array (neighbour = aggregating node).
-template <bool HAS_EF, bool NEED_EDGE, int RT, int FT>
+// Affine v (AV): the node's own v row is formed from v_in as in the forward (only v_in[j], 12 bytes, is staged instead of
+// the 768-byte v row).  gv is still stored: its reduction to the gradients of v_in, v_w and v_b stays with
+// hgb_linear_smallk_bwd, whose summation order the weight and bias gradients must keep to give the bits of the composed path.
+template <bool HAS_EF, bool NEED_EDGE, int RT, int FT, bool AV>
 __global__ void __launch_bounds__(WPB * 32, 2)
 painn_message_bwd_tiled_kernel(const float* __restrict__ gs_out, const float* __restrict__ gv_out, const float* __restrict__ phi,
-                               const float* __restrict__ v, const int32_t* __restrict__ rowptr, const float* __restrict__ rec,
+                               const float* __restrict__ v, const float* __restrict__ v_in, const float* __restrict__ v_w,
+                               const float* __restrict__ v_b, const int32_t* __restrict__ rowptr, const float* __restrict__ rec,
                                const float* __restrict__ wf, const float* __restrict__ bf, const float* __restrict__ efilt, int n,
                                int f_rt, int r, int tn, float* __restrict__ gphi, float* __restrict__ gv, float* __restrict__ part,
                                float* __restrict__ g_epack, float* __restrict__ g_efilt, int multi_cb) {
+  static_assert(!AV || FT == 64, "affine v: one 64-channel block");
   extern __shared__ __align__(128) uint8_t pm_smem[];
   const int f = FT ? FT : f_rt;
   const int f3 = 3 * f;
@@ -631,12 +690,16 @@ painn_message_bwd_tiled_kernel(const float* __restrict__ gs_out, const float* __
   auto stage = [&](int jn, int lo_n, int hi_n, float4* dst) {
     if (lane < 4 * min(8, hi_n - lo_n)) pm_cp_async16(dst + lane, rec4 + (int64_t)lo_n * 4 + lane);
     const float* pj = phi + (int64_t)jn * f3 + cb * 64;
-    const float* vjp = v + (int64_t)jn * f3 + cb * 64;
     pm_cp_async16(dst + 32 + lane, pj + (lane >> 4) * f + (lane & 15) * 4);
-    pm_cp_async16(dst + 80 + lane, vjp + (lane >> 4) * f + (lane & 15) * 4);
-    if (lane < 16) {
-      pm_cp_async16(dst + 64 + lane, pj + 2 * f + lane * 4);
-      pm_cp_async16(dst + 112 + lane, vjp + 2 * f + lane * 4);
+    if (lane < 16) pm_cp_async16(dst + 64 + lane, pj + 2 * f + lane * 4);
+    if (AV) {
+      if (lane < 3)
+        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(pm_smem_u32(reinterpret_cast<float*>(dst + 80) + lane)),
+                     "l"(v_in + (int64_t)jn * 3 + lane) : "memory");
+    } else {
+      const float* vjp = v + (int64_t)jn * f3 + cb * 64;
+      pm_cp_async16(dst + 80 + lane, vjp + (lane >> 4) * f + (lane & 15) * 4);
+      if (lane < 16) pm_cp_async16(dst + 112 + lane, vjp + 2 * f + lane * 4);
     }
   };
   // the warp's node sequence: n0 + warp, + WPB, ... inside a tile, then the same in the block's next tile
@@ -683,11 +746,19 @@ painn_message_bwd_tiled_kernel(const float* __restrict__ gs_out, const float* __
       }
       pm_cp_async_commit();
       float ph[3][2], vj[3][2], aphi[3][2], agv[3][2];
+      const float* x0 = reinterpret_cast<const float*>(cur + 80);   // AV: v_in[j]
+      float2 aw = make_float2(0.f, 0.f), ab = aw;   // scalar loads: parameters may be 4-byte aligned views of a flat buffer
+      if (AV) { aw = make_float2(__ldg(v_w + cc), __ldg(v_w + cc + 1)); ab = make_float2(__ldg(v_b + cc), __ldg(v_b + cc + 1)); }
 #pragma unroll
       for (int a = 0; a < 3; ++a) {
         const float2 p2 = *(reinterpret_cast<const float2*>(cur + 32 + a * 16) + lane);
-        const float2 v2 = *(reinterpret_cast<const float2*>(cur + 80 + a * 16) + lane);
-        ph[a][0] = p2.x; ph[a][1] = p2.y; vj[a][0] = v2.x; vj[a][1] = v2.y;
+        ph[a][0] = p2.x; ph[a][1] = p2.y;
+        if (AV) {
+          vj[a][0] = fmaf(x0[a], aw.x, ab.x); vj[a][1] = fmaf(x0[a], aw.y, ab.y);
+        } else {
+          const float2 v2 = *(reinterpret_cast<const float2*>(cur + 80 + a * 16) + lane);
+          vj[a][0] = v2.x; vj[a][1] = v2.y;
+        }
         aphi[a][0] = aphi[a][1] = 0.f; agv[a][0] = agv[a][1] = 0.f;
       }
       for (int p = lo; p < hi; ++p) {
@@ -857,14 +928,19 @@ extern "C" int64_t hgb_painn_message_bwd_workspace_bytes(int32_t n, int32_t f, i
   return (int64_t)painn_bwd_grid(n, f) * 3 * f * (r + 1) * 4;
 }
 
-extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, const float* phi, const float* v,
-                                     const int32_t* rowptr_src, const int32_t* perm_src, const int32_t* nbr_agg, const float* epack,
-                                     const float* rec, const float* wf, const float* bf, const float* efilt, int32_t n, int32_t f, int32_t r,
-                                     float* gphi, float* gv, float* gwf, float* gbf, float* g_epack, float* g_efilt, void* workspace,
-                                     int64_t workspace_bytes, hgb_stream_t stream) {
+extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, const float* phi, const float* v, const float* v_in,
+                                     const float* v_w, const float* v_b, const int32_t* rowptr_src, const int32_t* perm_src,
+                                     const int32_t* nbr_agg, const float* epack, const float* rec, const float* wf, const float* bf,
+                                     const float* efilt, int32_t n, int32_t f, int32_t r, float* gphi, float* gv, float* gwf, float* gbf,
+                                     float* g_epack, float* g_efilt, void* workspace, int64_t workspace_bytes, hgb_stream_t stream) {
   HGB_REQUIRE(n >= 0 && f > 0 && r > 0 && r <= RMAX, "painn_message_bwd: need 0 < num_radial <= %d (got %d)", RMAX, r);
-  HGB_REQUIRE(gs_out && gv_out && phi && v && rowptr_src && nbr_agg && epack && wf && bf && gphi && gv && gwf && gbf && workspace,
-              "painn_message_bwd: null pointer");
+  const bool av = v_in != nullptr;
+  HGB_REQUIRE(gs_out && gv_out && phi && (av ? (v_w && v_b && !v) : v != nullptr) && rowptr_src && nbr_agg && epack && wf && bf &&
+              gphi && gv && gwf && gbf && workspace,
+              "painn_message_bwd: null pointer (or both v and v_in)");
+  HGB_REQUIRE(!av || (hgb_painn_message_affine_v_supported(n, f) && rec &&
+                      (((uintptr_t)gs_out | (uintptr_t)gv_out | (uintptr_t)phi | (uintptr_t)rec) % 16 == 0)),
+              "painn_message_bwd: affine v needs f = 64, n >= 256, edge records and 16-byte aligned rows (n=%d f=%d)", n, f);
   const bool need_edge = g_epack != nullptr;
   HGB_REQUIRE((efilt != nullptr) == (g_efilt != nullptr), "painn_message_bwd: g_efilt iff efilt");
   HGB_REQUIRE(workspace_bytes >= hgb_painn_message_bwd_workspace_bytes(n, f, r), "painn_message_bwd: workspace too small");
@@ -886,8 +962,9 @@ extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, c
     const size_t smem = (size_t)2 * tn * 4 * f * 4 + fixed;
     static bool attr_done = false;
     if (!attr_done) {
-#define SETA(E, G, R) cudaFuncSetAttribute(painn_message_bwd_tiled_kernel<E, G, R, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
-                      cudaFuncSetAttribute(painn_message_bwd_tiled_kernel<E, G, R, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
+#define SETA(E, G, R) cudaFuncSetAttribute(painn_message_bwd_tiled_kernel<E, G, R, 64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
+                      cudaFuncSetAttribute(painn_message_bwd_tiled_kernel<E, G, R, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024); \
+                      cudaFuncSetAttribute(painn_message_bwd_tiled_kernel<E, G, R, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024)
       SETA(false, false, 5); SETA(false, true, 5); SETA(true, false, 5); SETA(true, true, 5);
       SETA(false, false, 8); SETA(false, true, 8); SETA(true, false, 8); SETA(true, true, 8);
 #undef SETA
@@ -899,8 +976,8 @@ extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, c
     if (gx > 2 * HGB_NUM_SMS) gx = 2 * HGB_NUM_SMS;
     const int ncb2 = f / 64;
     dim3 grid2(gx, ncb2);
-#define LAUNCH_F(E, G, R, F) painn_message_bwd_tiled_kernel<E, G, R, F><<<grid2, WPB * 32, smem, st>>>(gs_out, gv_out, phi, v, rowptr_src, rec, wf, bf, efilt, n, f, r, tn, gphi, gv, part, g_epack, g_efilt, ncb2 > 1)
-#define LAUNCH_T(E, G, R) do { if (f == 64) LAUNCH_F(E, G, R, 64); else LAUNCH_F(E, G, R, 0); } while (0)
+#define LAUNCH_F(E, G, R, F, A) painn_message_bwd_tiled_kernel<E, G, R, F, A><<<grid2, WPB * 32, smem, st>>>(gs_out, gv_out, phi, v, v_in, v_w, v_b, rowptr_src, rec, wf, bf, efilt, n, f, r, tn, gphi, gv, part, g_epack, g_efilt, ncb2 > 1)
+#define LAUNCH_T(E, G, R) do { if (av) LAUNCH_F(E, G, R, 64, true); else if (f == 64) LAUNCH_F(E, G, R, 64, false); else LAUNCH_F(E, G, R, 0, false); } while (0)
 #define LAUNCH_TR(E, G) do { if (r <= 5) LAUNCH_T(E, G, 5); else LAUNCH_T(E, G, 8); } while (0)
     if (efilt) { if (need_edge) LAUNCH_TR(true, true); else LAUNCH_TR(true, false); }
     else { if (need_edge) LAUNCH_TR(false, true); else LAUNCH_TR(false, false); }

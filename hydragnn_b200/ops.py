@@ -14,6 +14,8 @@ Two layers:
 
 Nothing here falls back to ATen/PyG scatter kernels; a missing library raises in ``_lib.lib()``.
 """
+from typing import NamedTuple
+
 import torch
 from torch.autograd.function import once_differentiable
 
@@ -797,32 +799,62 @@ class PainnEdgeEmbedFn(torch.autograd.Function):
         return g_unit, g_len, None, None
 
 
+class AffineV(NamedTuple):
+    """The layer input v[n, k, c] = v0[n, k, 0] * weight[c, 0] + bias[c] (a Linear(1, F) of a [N, 3, 1] tensor: PaiNN's first
+    vec_embed_out), kept unevaluated so that the message kernels can form it on chip."""
+    v0: torch.Tensor
+    weight: torch.Tensor
+    bias: torch.Tensor
+
+    def materialize(self, higher_order=False):
+        return linear_any_order(self.v0, self.weight, self.bias) if higher_order else linear_act(self.v0, self.weight, self.bias)
+
+
+def painn_affine_v_ok(v, s, rec_row):
+    """True when the tiled message kernels can take ``v`` as its AffineV record."""
+    n, f = s.shape
+    return (isinstance(v, AffineV) and rec_row is not None and s.is_cuda and v.v0.is_contiguous() and v.v0.data_ptr() % 16 == 0
+            and bool(_lib.query("hgb_painn_message_affine_v_supported", n, f)))
+
+
 class PainnMessageFn(torch.autograd.Function):
-    """Fused PaiNN message (hydragnn/models/PAINNStack.py:239-270): returns (s + ds, v + dv)."""
+    """Fused PaiNN message (hydragnn/models/PAINNStack.py:239-270): returns (s + ds, v + dv).  The input v is either a
+    [n, 3, f] tensor (``v0 = vw = vb = None``) or, with ``v = None``, the affine v0 [n, 3, 1], vw [f, 1], vb [f] of an
+    ``AffineV`` (``painn_affine_v_ok``)."""
 
     @staticmethod
-    def forward(ctx, phi, s, v, epack, wf, bf, efilt, plan, rec_row=None):
+    def forward(ctx, phi, s, v, epack, wf, bf, efilt, plan, rec_row=None, v0=None, vw=None, vb=None):
         n, f = s.shape
         r = wf.shape[1]
-        phi, s, v = _chk(phi), _chk(s), _chk(v)
-        s_out, v_out = torch.empty_like(s), torch.empty_like(v)
+        phi, s = _chk(phi), _chk(s)
+        av = v0 is not None
+        if av:
+            v, v0, vw, vb = None, _chk(v0), _chk(vw), _chk(vb)
+            v_out = torch.empty(n, 3, f, dtype=s.dtype, device=s.device)
+        else:
+            v = _chk(v)
+            v_out = torch.empty_like(v)
+        s_out = torch.empty_like(s)
         agg = plan.by_row     # messages are summed into edge[:,0] = edge_index[0]
-        _lib.call("hgb_painn_message_fwd", _p(phi), _p(s), _p(v), _p(agg.rowptr), _p(agg.perm), _p(plan.nbr("row")), _p(epack),
-                  _p(rec_row), _p(_chk(wf)), _p(_chk(bf)), _p(_chk(efilt)), n, f, r, _p(s_out), _p(v_out), _stream())
-        ctx.save_for_backward(phi, v, epack, wf, bf, efilt)
+        _lib.call("hgb_painn_message_fwd", _p(phi), _p(s), _p(v), _p(v0), _p(vw), _p(vb), _p(agg.rowptr), _p(agg.perm),
+                  _p(plan.nbr("row")), _p(epack), _p(rec_row), _p(_chk(wf)), _p(_chk(bf)), _p(_chk(efilt)), n, f, r, _p(s_out),
+                  _p(v_out), _stream())
+        ctx.save_for_backward(phi, v, epack, wf, bf, efilt, v0, vw, vb)
         ctx.plan, ctx.use_rec = plan, rec_row is not None
         return s_out, v_out
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gs_out, gv_out):
-        phi, v, epack, wf, bf, efilt = ctx.saved_tensors
+        phi, v, epack, wf, bf, efilt, v0, vw, vb = ctx.saved_tensors
         plan = ctx.plan
         n, f = gs_out.shape
         r = wf.shape[1]
         gs_out, gv_out = _chk(gs_out), _chk(gv_out)
         need_edge = ctx.needs_input_grad[3]
-        gphi, gv = torch.empty_like(phi), torch.empty_like(v)
+        av = v0 is not None
+        gphi = torch.empty_like(phi)
+        gv = torch.empty(n, 3, f, dtype=phi.dtype, device=phi.device)
         gwf, gbf = torch.empty_like(wf), torch.empty_like(bf)
         cpl = 2 if (f >= 64 and f % 2 == 0) else 1          # mirrors painn_cpl / painn_group in csrc/hgb_painn.cu
         multi = f > 32 * cpl                                # several channel blocks accumulate into g_epack
@@ -839,10 +871,15 @@ class PainnMessageFn(torch.autograd.Function):
                 cache.clear()
                 cache[key] = painn_edge_records(epack, plan, "col")
             rec_col = cache[key]
-        _lib.call("hgb_painn_message_bwd", _p(gs_out), _p(gv_out), _p(phi), _p(v), _p(src.rowptr), _p(src.perm), _p(plan.nbr("col")),
-                  _p(epack), _p(rec_col), _p(wf), _p(bf), _p(efilt), n, f, r, _p(gphi), _p(gv), _p(gwf), _p(gbf), _p(g_epack), _p(g_ef),
-                  _p(ws), nbytes, _stream())
-        return gphi, gs_out, gv, g_epack, gwf, gbf, g_ef, None, None
+        _lib.call("hgb_painn_message_bwd", _p(gs_out), _p(gv_out), _p(phi), _p(v), _p(v0), _p(vw), _p(vb), _p(src.rowptr),
+                  _p(src.perm), _p(plan.nbr("col")), _p(epack), _p(rec_col), _p(wf), _p(bf), _p(efilt), n, f, r, _p(gphi), _p(gv),
+                  _p(gwf), _p(gbf), _p(g_epack), _p(g_ef), _p(ws), nbytes, _stream())
+        if not av:
+            return gphi, gs_out, gv, g_epack, gwf, gbf, g_ef, None, None, None, None, None
+        # v = Linear(1, f)(v0): the same small-k backward LinearAct runs on a stored v, so all three gradients keep its bits
+        g_v0, g_vw, g_vb = raw_smallk_bwd(gv.reshape(3 * n, f), None, None, v0.reshape(3 * n, 1), vw, 0, 0.0,
+                                          ctx.needs_input_grad[9], ctx.needs_input_grad[10], ctx.needs_input_grad[11])
+        return gphi, gs_out, None, g_epack, gwf, gbf, g_ef, None, None, (g_v0.reshape(v0.shape) if g_v0 is not None else None), g_vw, g_vb
 
 
 def painn_edge_records(epack, plan, which):

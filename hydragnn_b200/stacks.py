@@ -287,6 +287,8 @@ class PainnMessage(nn.Module):
     def forward(self, s, v, plan, geom, edge_attr=None, higher_order=False):
         f = self.node_size
         if higher_order:
+            if isinstance(v, ops.AffineV):
+                v = v.materialize(True)
             diff, dist = geom["unit"], geom["len"]
             n = torch.arange(1, self.num_radial + 1, device=dist.device)
             rbf = torch.sin(dist * n * torch.pi / self.cutoff) / dist
@@ -304,8 +306,12 @@ class PainnMessage(nn.Module):
         efilt = run_mlp(self.edge_filter, edge_attr) if edge_attr is not None else None
         if "rec_row" not in geom and self.node_size % 64 == 0:      # built once per batch, reused by every layer
             geom["rec_row"] = ops.painn_edge_records(geom["epack"], plan, "row")
-        return ops.PainnMessageFn.apply(phi, s, v, geom["epack"], self.filter_layer.weight, self.filter_layer.bias, efilt, plan,
-                                        geom.get("rec_row"))
+        args = (phi, s, v, geom["epack"], self.filter_layer.weight, self.filter_layer.bias, efilt, plan, geom.get("rec_row"))
+        if isinstance(v, ops.AffineV):
+            if ops.painn_affine_v_ok(v, s, geom.get("rec_row")):     # v = vec_embed_out(v0) is formed inside the message kernels
+                return ops.PainnMessageFn.apply(*args[:2], None, *args[3:], *v)
+            args = args[:2] + (v.materialize(),) + args[3:]
+        return ops.PainnMessageFn.apply(*args)
 
 
 class PainnUpdate(nn.Module):
@@ -367,8 +373,12 @@ class PainnConv(nn.Module):
         if self.last:
             return s, v          # PAINNStack.py:124-147: v passes through unchanged in the last layer
         lin = self.module_3
-        v_new = ops.linear_any_order(v_new, lin.weight, lin.bias) if higher_order else ops.linear_act(v_new, lin.weight, lin.bias)
-        return s, v_new
+        if higher_order:
+            return s, ops.linear_any_order(v_new, lin.weight, lin.bias)
+        if lin.in_features == 1 and isinstance(self.module_0, PainnMessage):
+            # reference quirk Q4: the first layer runs at width 1; the next layer's PainnMessage forms v itself
+            return s, ops.AffineV(v_new, lin.weight, lin.bias)
+        return s, ops.linear_act(v_new, lin.weight, lin.bias)
 
 
 class MLPNode(nn.Module):

@@ -266,11 +266,16 @@ int hgb_painn_edge_embed_bwd(const float* unit, const float* len, const float* g
  *   s_out[i] = s[i] + sum m_s;  v_out[i,k] = v[i,k] + sum (v[nbr,k] * g_v + g_e * dir[e,k])
  * Replaces filter GEMM + 2 gathers + 2 index_add_ (PAINNStack.py:239-270); nothing per-edge is written, no
  * atomics, summation in ascending edge id.  Algorithmic bytes: E*(6F*4 + 8 + 48) + N*(8F*4 + 4).
- * phi [n,3f], s [n,f], v [n,3,f], wf [3f,r], bf [3f], efilt [e,3f] or NULL.                                 */
-int hgb_painn_message_fwd(const float* phi, const float* s, const float* v, const int32_t* rowptr,
-                          const int32_t* perm, const int32_t* nbr, const float* epack, const float* rec,
-                          const float* wf, const float* bf, const float* efilt, int32_t n, int32_t f, int32_t r,
-                          float* s_out, float* v_out, hgb_stream_t stream);
+ * phi [n,3f], s [n,f], v [n,3,f], wf [3f,r], bf [3f], efilt [e,3f] or NULL.
+ * Affine v: with v = NULL and v_in [n,3], v_w [f], v_b [f] set, v[i,k,c] = fmaf(v_in[i,k], v_w[c], v_b[c]) (a
+ * Linear(1, f) of a [n,3,1] tensor, PaiNN's first vec_embed_out) is formed on chip and never stored; only when
+ * hgb_painn_message_affine_v_supported(n, f), `rec` is given and phi, s, rec, v_in are 16-byte aligned.       */
+int hgb_painn_message_fwd(const float* phi, const float* s, const float* v, const float* v_in, const float* v_w,
+                          const float* v_b, const int32_t* rowptr, const int32_t* perm, const int32_t* nbr,
+                          const float* epack, const float* rec, const float* wf, const float* bf, const float* efilt,
+                          int32_t n, int32_t f, int32_t r, float* s_out, float* v_out, hgb_stream_t stream);
+/* 1 when the tiled message kernels take the affine-v form: f == 64 and n >= 256.                              */
+int hgb_painn_message_affine_v_supported(int32_t n, int32_t f);
 /* CSR-ordered 64-byte edge records rec [e,16] = { epack[perm[p]] (12), nbr[p] (int bits), perm[p] (int bits), 0, 0 }:
  * a node's records are contiguous and carry the gather index.  When `rec` is passed to hgb_painn_message_fwd and
  * f % 64 == 0, the shared-memory-tiled kernel is used: the phi / v rows of 32 consecutive nodes are staged with
@@ -281,12 +286,15 @@ int hgb_painn_edge_records(const float* epack, const int32_t* perm, const int32_
  * nbr_agg [e] = edge[:,0] of every slot of that CSR.  gs_out [n,f], gv_out [n,3,f] are the incoming gradients.
  * Outputs: gphi [n,3f]; gv [n,3,f] (= gv_out + gathered part; gs_in == gs_out is the caller's); gwf [3f,r],
  * gbf [3f] (via workspace partials); optional g_epack [e,12] (zero-initialised by the caller when f > 64) and
- * g_efilt [e,3f] (iff efilt).  `rec` (optional): by-col CSR edge records -> shared-memory-tiled kernel.       */
-int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, const float* phi, const float* v,
-                          const int32_t* rowptr_src, const int32_t* perm_src, const int32_t* nbr_agg,
-                          const float* epack, const float* rec, const float* wf, const float* bf, const float* efilt, int32_t n,
-                          int32_t f, int32_t r, float* gphi, float* gv, float* gwf, float* gbf, float* g_epack,
-                          float* g_efilt, void* workspace, int64_t workspace_bytes, hgb_stream_t stream);
+ * g_efilt [e,3f] (iff efilt).  `rec` (optional): by-col CSR edge records -> shared-memory-tiled kernel.
+ * Affine v (v = NULL, v_in / v_w / v_b as in the forward): v is formed on chip, gv is written as usual; the caller
+ * reduces gv to the gradients of v_in, v_w, v_b with hgb_linear_smallk_bwd, as for a stored Linear(1, f) output.  */
+int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, const float* phi, const float* v, const float* v_in,
+                          const float* v_w, const float* v_b, const int32_t* rowptr_src, const int32_t* perm_src,
+                          const int32_t* nbr_agg, const float* epack, const float* rec, const float* wf, const float* bf,
+                          const float* efilt, int32_t n, int32_t f, int32_t r, float* gphi, float* gv, float* gwf,
+                          float* gbf, float* g_epack, float* g_efilt, void* workspace, int64_t workspace_bytes,
+                          hgb_stream_t stream);
 int64_t hgb_painn_message_bwd_workspace_bytes(int32_t n, int32_t f, int32_t r);
 
 /* Update block glue (PAINNStack.py:298-328).  uv, vv are update_U(v), update_V(v) as [3n, f] matrices with row
