@@ -13,7 +13,7 @@ from torch import nn
 from . import ops
 from .stacks import EGCLStack, PAINNStack, cached, graph_sum
 
-SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAEq", "MACE", "SchNet")
+SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet")
 
 
 def get_device(use_gpu=True):
@@ -50,7 +50,7 @@ def create_model_config(config, verbosity=0, use_gpu=True):
         task_weights=arch["task_weights"], num_conv_layers=arch["num_conv_layers"],
         freeze_conv=g("freeze_conv_layers", False), initial_bias=g("initial_bias"), num_nodes=g("num_nodes"),
         max_neighbours=g("max_neighbours"), edge_dim=g("edge_dim"), pna_deg=g("pna_deg"), num_radial=g("num_radial"),
-        num_gaussians=g("num_gaussians"), num_filters=g("num_filters"),
+        num_gaussians=g("num_gaussians"), num_filters=g("num_filters"), envelope_exponent=g("envelope_exponent"),
         radial_type=g("radial_type"), distance_transform=g("distance_transform"), radius=g("radius"),
         equivariance=g("equivariance"), correlation=g("correlation"), max_ell=g("max_ell"), node_max_ell=g("node_max_ell"),
         avg_num_neighbors=g("avg_num_neighbors"), conv_checkpointing=training.get("conv_checkpointing", False),
@@ -104,6 +104,13 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
         assert pna_deg is not None, "PNA requires degree input."
         from .pna import PNAStack
         model = PNAStack(pna_deg, edge_dim, **common)
+    elif mpnn_type == "PNAPlus":
+        assert pna_deg is not None, "PNAPlus requires degree input."
+        assert envelope_exponent is not None, "PNAPlus requires envelope_exponent input."
+        assert num_radial is not None, "PNAPlus requires num_radial input."
+        assert radius is not None, "PNAPlus requires radius input."
+        from .pnaplus import PNAPlusStack
+        model = PNAPlusStack(pna_deg, edge_dim, envelope_exponent, num_radial, radius, **common)
     elif mpnn_type == "PNAEq":
         assert pna_deg is not None, "PNAEq requires degree input."
         from .pnaeq import PNAEqStack

@@ -578,3 +578,414 @@ extern "C" int hgb_pna_conv_bwd(const float* g_out, const float* pq, const int32
   HGB_LAUNCH_CHECK("pna_conv_reduce");
   return HGB_OK;
 }
+
+// ---- PNAPlus: PNAConv with a Bessel-gated message (hydragnn/models/PNAPlusStack.py:144-279, torch_geometric 2.6.1
+// BesselBasisLayer / Envelope), message and four-way aggregation in one pass.  For the edge e = (j -> i) with length d_e:
+//   x = d_e / radius,  rbf_k = env(x) sin(freq_k x)  (0 for x >= 1),  u_e = relu(W_r rbf + b_r),
+//   h_e = P[i] + Q[j] + M_r u_e + M_a a_e + c,  m_e = h_e * (W_l rbf),
+// reduced straight into [mean | min | max | std] by the PnaAcc of pna_conv_fwd.  Only d_e [E] is read per edge: the [E, R]
+// basis, the [E, F] embedding u and the message are formed on chip.
+//
+// Thread mapping: one warp owns one target node, lane l the channels l and l + 32 (F <= 64).  The per-edge F x F product
+// M_r u_e is SIMT: u_e goes through a per-warp shared row, M_r sits in shared memory with an odd row stride, so both the
+// row-wise read of the forward and the column-wise read of the backward are free of bank conflicts.
+#define PNAP_MAX_F 64
+#define PNAP_MAX_R 16
+#define PNAP_MAX_D 16
+#define PNAP_BWD_MAX_BLOCKS (HGB_NUM_SMS * 2)
+
+static __host__ __device__ __forceinline__ int pnap_stride(int f) { return f | 1; }
+
+// parameters staged in shared memory once per CTA: mr [f][s] (s odd), wr / wl [r][f], ma [d][f], br, cv [f], fr [r]
+struct PnapParams {
+  float *mr, *wr, *wl, *ma, *br, *cv, *fr, *end;
+
+  static __host__ __device__ int64_t floats(int f, int r, int d) { return (int64_t)f * pnap_stride(f) + 2 * r * f + d * f + 2 * f + r; }
+
+  __device__ void stage(float* base, int f, int r, int d, const float* __restrict__ g_mr, const float* __restrict__ g_wr,
+                        const float* __restrict__ g_wl, const float* __restrict__ g_mat, const float* __restrict__ g_br,
+                        const float* __restrict__ g_cv, const float* __restrict__ g_fr) {
+    const int s = pnap_stride(f);
+    mr = base;
+    wr = mr + f * s;
+    wl = wr + r * f;
+    ma = wl + r * f;
+    br = ma + d * f;
+    cv = br + f;
+    fr = cv + f;
+    end = fr + r;
+    for (int t = threadIdx.x; t < f * f; t += blockDim.x) mr[(t / f) * s + t % f] = __ldg(g_mr + t);
+    for (int t = threadIdx.x; t < r * f; t += blockDim.x) {
+      const int k = t / f, c = t % f;
+      wr[t] = __ldg(g_wr + c * r + k);
+      wl[t] = __ldg(g_wl + c * r + k);
+    }
+    for (int t = threadIdx.x; t < d * f; t += blockDim.x) ma[t] = __ldg(g_mat + t);
+    for (int t = threadIdx.x; t < f; t += blockDim.x) {
+      br[t] = __ldg(g_br + t);
+      cv[t] = g_cv ? __ldg(g_cv + t) : 0.f;
+    }
+    for (int t = threadIdx.x; t < r; t += blockDim.x) fr[t] = __ldg(g_fr + t);
+    __syncthreads();
+  }
+};
+
+// x = d / radius, env(x) and d env / dx (both 0 for x >= 1), rb[k] = env sin(freq_k x)
+__device__ __forceinline__ void pnap_basis(float dist, float radius, int expo, const float* fr, int r, float (&rb)[PNAP_MAX_R],
+                                           float& x, float& env, float& denv) {
+  x = dist / radius;
+  const int p = expo + 1;
+  const float a = -(float)((p + 1) * (p + 2)) / 2.f, b = (float)(p * (p + 2)), c = -(float)(p * (p + 1)) / 2.f;
+  float xp0 = 1.f;
+  for (int q = 0; q < p - 1; ++q) xp0 *= x;
+  const float xp1 = xp0 * x, xp2 = xp1 * x;
+  const bool in = x < 1.f;
+  env = in ? 1.f / x + a * xp0 + b * xp1 + c * xp2 : 0.f;
+  denv = in ? -1.f / (x * x) + a * (float)(p - 1) * (xp0 / x) + b * (float)p * xp0 + c * (float)(p + 1) * xp1 : 0.f;
+#pragma unroll
+  for (int k = 0; k < PNAP_MAX_R; ++k) rb[k] = (k < r && in) ? env * sinf(fr[k] * x) : 0.f;
+}
+
+// upre = W_r rb + b_r, gate = W_l rb, h = base + Q[j] + M_r relu(upre) + M_a a for the lane's channels.  The forward and the
+// backward both call this, so the backward sees the forward's m_e = h * gate bit for bit.  u_s: the warp's [f] row.
+template <int NC>
+__device__ __forceinline__ void pnap_message(const PnapParams& s, int f, int r, int d, int lane, float* u_s, const float (&base)[NC],
+                                             const float* __restrict__ q_row, const float* __restrict__ a_row,
+                                             const float (&rb)[PNAP_MAX_R], float (&upre)[NC], float (&gate)[NC], float (&h)[NC]) {
+  const int sr = pnap_stride(f);
+  __syncwarp();                                           // the previous edge's reads of u_s are done
+#pragma unroll
+  for (int t = 0; t < NC; ++t) {
+    const int c = lane + 32 * t;
+    float ub = 0.f, g = 0.f;
+    if (c < f) {
+      ub = s.br[c];
+#pragma unroll
+      for (int k = 0; k < PNAP_MAX_R; ++k) {
+        if (k < r) {
+          ub = fmaf(s.wr[k * f + c], rb[k], ub);
+          g = fmaf(s.wl[k * f + c], rb[k], g);
+        }
+      }
+      u_s[c] = fmaxf(ub, 0.f);
+    }
+    upre[t] = ub;
+    gate[t] = g;
+  }
+  __syncwarp();
+#pragma unroll
+  for (int t = 0; t < NC; ++t) {
+    const int c = lane + 32 * t;
+    float acc = 0.f;
+    if (c < f) {
+      acc = base[t] + __ldg(q_row + c);
+      const float* mrow = s.mr + c * sr;
+      for (int m = 0; m < f; ++m) acc = fmaf(mrow[m], u_s[m], acc);
+      for (int k = 0; k < d; ++k) acc = fmaf(s.ma[k * f + c], __ldg(a_row + k), acc);
+    }
+    h[t] = acc;
+  }
+}
+
+template <int NC>
+__global__ void __launch_bounds__(256) pnaplus_conv_fwd_kernel(
+    const float* __restrict__ pq, const float* __restrict__ dist, const int32_t* __restrict__ rowptr,
+    const int32_t* __restrict__ perm, const int32_t* __restrict__ src, const float* __restrict__ eattr, int d,
+    const float* __restrict__ freq, int r, float radius, int expo, const float* __restrict__ wr, const float* __restrict__ br,
+    const float* __restrict__ wl, const float* __restrict__ mr, const float* __restrict__ mat, const float* __restrict__ cvec,
+    int n, int f, float* __restrict__ out, int32_t* __restrict__ amin, int32_t* __restrict__ amax) {
+  extern __shared__ float smem[];
+  PnapParams s;
+  s.stage(smem, f, r, d, mr, wr, wl, mat, br, cvec, freq);
+  const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  float* u_s = s.end + warp * f;
+  for (int row = blockIdx.x * warps + warp; row < n; row += gridDim.x * warps) {
+    const int lo = rowptr[row], hi = rowptr[row + 1];
+    const float inv = 1.f / (float)max(hi - lo, 1);
+    float base[NC];
+#pragma unroll
+    for (int t = 0; t < NC; ++t) {
+      const int c = lane + 32 * t;
+      base[t] = c < f ? __ldg(pq + (int64_t)row * 2 * f + c) + s.cv[c] : 0.f;
+    }
+    PnaAcc acc[NC];
+    for (int p = lo; p < hi; ++p) {
+      const int e = perm ? perm[p] : p;
+      float rb[PNAP_MAX_R], x, env, denv, upre[NC], gate[NC], h[NC];
+      pnap_basis(__ldg(dist + e), radius, expo, s.fr, r, rb, x, env, denv);
+      pnap_message<NC>(s, f, r, d, lane, u_s, base, pq + (int64_t)src[p] * 2 * f + f, eattr + (int64_t)e * d, rb, upre, gate, h);
+#pragma unroll
+      for (int t = 0; t < NC; ++t)
+        if (lane + 32 * t < f) acc[t].push(h[t] * gate[t], e);
+    }
+#pragma unroll
+    for (int t = 0; t < NC; ++t) {
+      const int c = lane + 32 * t;
+      if (c < f) acc[t].store(inv, out + (int64_t)row * 4 * f + c, f, amin + (int64_t)row * f + c, amax + (int64_t)row * f + c);
+    }
+  }
+}
+
+// Parameter-gradient layout (the order of g_params): c [f] | M_a^T [d][f] | M_r [f][f] | W_r^T [r][f] | b_r [f] | W_l^T [r][f] |
+// freq [r].  Per warp the accumulators live in shared memory in the same order, M_r with the odd row stride.
+struct PnapGrad {
+  float *c, *ma, *mr, *wr, *br, *wl, *fr;
+  static __host__ __device__ int64_t floats(int f, int r, int d) { return (int64_t)f + d * f + (int64_t)f * f + 2 * r * f + f + r; }
+  static __host__ __device__ int64_t smem_floats(int f, int r, int d) { return floats(f, r, d) + (int64_t)f * (pnap_stride(f) - f); }
+  __device__ void carve(float* base, int f, int r, int d) {
+    c = base;
+    ma = c + f;
+    mr = ma + d * f;
+    wr = mr + f * pnap_stride(f);
+    br = wr + r * f;
+    wl = br + f;
+    fr = wl + r * f;
+  }
+};
+
+// g_m = g_mean / deg + [e = amin] g_min + [e = amax] g_max + g_std (m - mean) / (deg std), as pna_conv_bwd_kernel; then
+// g_h = g_m * gate, g_gate = g_m * h, g_u = M_r^T g_h, g_upre = [upre > 0] g_u, g_rbf = W_r^T g_upre + W_l^T g_gate.
+// g_p[i] summed in registers; g_h written once per edge; g_dist / g_eattr per edge when asked; with `grads` the parameter
+// sums go to per-warp shared accumulators, summed over the CTA's warps in order into part [gridDim.x, PnapGrad::floats].
+template <int NC>
+__global__ void __launch_bounds__(256) pnaplus_conv_bwd_kernel(
+    const float* __restrict__ g_out, const float* __restrict__ pq, const float* __restrict__ dist, const int32_t* __restrict__ rowptr,
+    const int32_t* __restrict__ perm, const int32_t* __restrict__ src, const float* __restrict__ eattr, int d,
+    const float* __restrict__ freq, int r, float radius, int expo, const float* __restrict__ wr, const float* __restrict__ br,
+    const float* __restrict__ wl, const float* __restrict__ mr, const float* __restrict__ mat, const float* __restrict__ cvec,
+    const float* __restrict__ agg, const int32_t* __restrict__ amin, const int32_t* __restrict__ amax, int n, int f,
+    float* __restrict__ g_p, int ldgp, float* __restrict__ g_h, float* __restrict__ g_dist, float* __restrict__ g_eattr,
+    bool grads, float* __restrict__ part) {
+  extern __shared__ float smem[];
+  PnapParams s;
+  s.stage(smem, f, r, d, mr, wr, wl, mat, br, cvec, freq);
+  const int warps = blockDim.x >> 5, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int sr = pnap_stride(f);
+  const int64_t per_warp = 2 * f + (grads ? PnapGrad::smem_floats(f, r, d) : 0);
+  float* u_s = s.end + warp * per_warp;
+  float* gh_s = u_s + f;
+  PnapGrad A;
+  A.carve(gh_s + f, f, r, d);
+  if (grads)
+    for (int64_t q = lane; q < PnapGrad::smem_floats(f, r, d); q += 32) A.c[q] = 0.f;
+  const bool want_rbf = grads || g_dist;
+  float gfreq = 0.f;                                      // lane k < r: sum of g_freq[k]
+  for (int row = blockIdx.x * warps + warp; row < n; row += gridDim.x * warps) {
+    const int lo = rowptr[row], hi = rowptr[row + 1];
+    const float inv = 1.f / (float)max(hi - lo, 1);
+    float base[NC], gmean[NC], gmin[NC], gmax[NC], kstd[NC], mean[NC], gp[NC];
+    int imin[NC], imax[NC];
+#pragma unroll
+    for (int t = 0; t < NC; ++t) {
+      const int c = lane + 32 * t;
+      const bool on = c < f;
+      const float* g = g_out + (int64_t)row * 4 * f + c;
+      const float* o = agg + (int64_t)row * 4 * f + c;
+      base[t] = on ? __ldg(pq + (int64_t)row * 2 * f + c) + s.cv[c] : 0.f;
+      gmean[t] = on ? g[0] * inv : 0.f;
+      gmin[t] = on ? g[f] : 0.f;
+      gmax[t] = on ? g[2 * f] : 0.f;
+      mean[t] = on ? o[0] : 0.f;
+      const float sd = on ? o[3 * f] : 0.f;
+      kstd[t] = sd > 0.f ? g[3 * f] * inv / sd : 0.f;
+      imin[t] = on ? amin[(int64_t)row * f + c] : -1;
+      imax[t] = on ? amax[(int64_t)row * f + c] : -1;
+      gp[t] = 0.f;
+    }
+    for (int p = lo; p < hi; ++p) {
+      const int e = perm ? perm[p] : p;
+      const float* a_row = eattr + (int64_t)e * d;
+      float rb[PNAP_MAX_R], x, env, denv, upre[NC], gate[NC], h[NC], gh[NC], gg[NC];
+      pnap_basis(__ldg(dist + e), radius, expo, s.fr, r, rb, x, env, denv);
+      pnap_message<NC>(s, f, r, d, lane, u_s, base, pq + (int64_t)src[p] * 2 * f + f, a_row, rb, upre, gate, h);
+#pragma unroll
+      for (int t = 0; t < NC; ++t) {
+        const int c = lane + 32 * t;
+        gh[t] = gg[t] = 0.f;
+        if (c < f) {
+          float gm = gmean[t];
+          if (imin[t] == e) gm += gmin[t];
+          if (imax[t] == e) gm += gmax[t];
+          if (kstd[t] != 0.f) gm = fmaf(kstd[t], h[t] * gate[t] - mean[t], gm);
+          gh[t] = gm * gate[t];
+          gg[t] = gm * h[t];
+          gp[t] += gh[t];
+          g_h[(int64_t)e * f + c] = gh[t];
+          gh_s[c] = gh[t];
+          if (grads) {
+            A.c[c] += gh[t];
+            for (int k = 0; k < d; ++k) A.ma[k * f + c] = fmaf(gh[t], __ldg(a_row + k), A.ma[k * f + c]);
+#pragma unroll
+            for (int k = 0; k < PNAP_MAX_R; ++k)
+              if (k < r) A.wl[k * f + c] = fmaf(gg[t], rb[k], A.wl[k * f + c]);
+            float* arow = A.mr + c * sr;
+            for (int m = 0; m < f; ++m) arow[m] = fmaf(gh[t], u_s[m], arow[m]);
+          }
+        }
+      }
+      __syncwarp();                                       // gh_s complete
+      float grbf[PNAP_MAX_R];
+#pragma unroll
+      for (int k = 0; k < PNAP_MAX_R; ++k) grbf[k] = 0.f;
+#pragma unroll
+      for (int t = 0; t < NC; ++t) {
+        const int c = lane + 32 * t;
+        if (c < f) {
+          float gu = 0.f;
+          for (int q = 0; q < f; ++q) gu = fmaf(s.mr[q * sr + c], gh_s[q], gu);
+          const float gpre = upre[t] > 0.f ? gu : 0.f;
+          if (grads) {
+            A.br[c] += gpre;
+#pragma unroll
+            for (int k = 0; k < PNAP_MAX_R; ++k)
+              if (k < r) A.wr[k * f + c] = fmaf(gpre, rb[k], A.wr[k * f + c]);
+          }
+          if (want_rbf) {
+#pragma unroll
+            for (int k = 0; k < PNAP_MAX_R; ++k)
+              if (k < r) grbf[k] = fmaf(s.wr[k * f + c], gpre, fmaf(s.wl[k * f + c], gg[t], grbf[k]));
+          }
+        }
+      }
+      if (want_rbf) {
+        float gx = 0.f;
+#pragma unroll
+        for (int k = 0; k < PNAP_MAX_R; ++k) {
+          if (k < r) {
+            const float gk = hgb_warp_sum(grbf[k]);
+            if (x < 1.f) {
+              float sn, cs;
+              sincosf(s.fr[k] * x, &sn, &cs);
+              gx = fmaf(gk, fmaf(denv, sn, env * s.fr[k] * cs), gx);
+              if (lane == k) gfreq = fmaf(gk, env * x * cs, gfreq);
+            }
+          }
+        }
+        if (g_dist && lane == 0) g_dist[e] = gx / radius;
+      }
+      if (g_eattr) {
+        for (int k = 0; k < d; ++k) {
+          float v = 0.f;
+#pragma unroll
+          for (int t = 0; t < NC; ++t)
+            if (lane + 32 * t < f) v = fmaf(s.ma[k * f + lane + 32 * t], gh[t], v);
+          v = hgb_warp_sum(v);
+          if (lane == 0) g_eattr[(int64_t)e * d + k] = v;
+        }
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < NC; ++t) {
+      const int c = lane + 32 * t;
+      if (c < f) g_p[(int64_t)row * ldgp + c] = gp[t];
+    }
+  }
+  if (!grads) return;                                     // grid-uniform: no CTA skips the barrier below alone
+  if (lane < r) A.fr[lane] = gfreq;
+  __syncthreads();
+  // fixed-order sum over the CTA's warps, written unpadded
+  const int64_t total = PnapGrad::floats(f, r, d), mr0 = f + (int64_t)d * f, mr1 = mr0 + (int64_t)f * f;
+  for (int64_t q = threadIdx.x; q < total; q += blockDim.x) {
+    const int64_t qs = q < mr0 ? q : (q < mr1 ? mr0 + ((q - mr0) / f) * sr + (q - mr0) % f : q + (int64_t)f * (sr - f));
+    float v = 0.f;
+    for (int w = 0; w < warps; ++w) v += s.end[w * per_warp + 2 * f + qs];
+    part[(int64_t)blockIdx.x * total + q] = v;
+  }
+}
+
+namespace {
+// warps per CTA and dynamic shared bytes; the backward's per-warp accumulators grow as f^2, so wide rows run 4 warps
+struct PnapLaunch {
+  int warps;
+  size_t fwd_smem, bwd_smem;
+};
+
+PnapLaunch pnap_launch(int f, int r, int d, bool grads) {
+  PnapLaunch L;
+  const int64_t params = PnapParams::floats(f, r, d);
+  const int64_t per_warp = 2 * f + (grads ? PnapGrad::smem_floats(f, r, d) : 0);
+  L.warps = (params + 8 * per_warp) * 4 <= 200 * 1024 ? 8 : 4;
+  L.fwd_smem = (size_t)(params + 8 * f) * 4;
+  L.bwd_smem = (size_t)(params + L.warps * per_warp) * 4;
+  return L;
+}
+}  // namespace
+
+extern "C" int hgb_pnaplus_conv_supported(int32_t f, int32_t r, int32_t d) {
+  return f >= 1 && f <= PNAP_MAX_F && r >= 1 && r <= PNAP_MAX_R && d >= 0 && d <= PNAP_MAX_D;
+}
+
+extern "C" int64_t hgb_pnaplus_conv_workspace_bytes(int32_t f, int32_t r, int32_t d) {
+  if (!hgb_pnaplus_conv_supported(f, r, d)) return -1;
+  return (int64_t)PNAP_BWD_MAX_BLOCKS * PnapGrad::floats(f, r, d) * (int64_t)sizeof(float);
+}
+
+#define PNAP_CHECK_ARGS(name)                                                                                                \
+  HGB_REQUIRE(n >= 0 && hgb_pnaplus_conv_supported(f, r, d) && radius > 0.f && expo >= 0,                                  \
+              name ": bad sizes (n %d, f %d, r %d, d %d, radius %g, exponent %d; f <= %d, r <= %d, d <= %d)", n, f, r, d,     \
+              (double)radius, expo, PNAP_MAX_F, PNAP_MAX_R, PNAP_MAX_D);                                                     \
+  HGB_REQUIRE(pq && dist && rowptr && src && freq && wr && br && wl && mr && cvec, name ": null argument");                  \
+  HGB_REQUIRE(d == 0 || (eattr && mat), name ": d > 0 needs edge attributes and M_a")
+
+extern "C" int hgb_pnaplus_conv_fwd(const float* pq, const float* dist, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                                    const float* eattr, int32_t d, const float* freq, int32_t r, float radius, int32_t expo,
+                                    const float* wr, const float* br, const float* wl, const float* mr, const float* mat,
+                                    const float* cvec, int32_t n, int32_t f, float* out, int32_t* argmin, int32_t* argmax,
+                                    hgb_stream_t stream) {
+  PNAP_CHECK_ARGS("pnaplus_conv_fwd");
+  HGB_REQUIRE(out && argmin && argmax, "pnaplus_conv_fwd: null output");
+  if (n == 0) return HGB_OK;
+  const PnapLaunch L = pnap_launch(f, r, d, false);
+  const int grid = hgb_grid_for(n, 8);
+#define PNAP_FWD(NC)                                                                                                         \
+  do {                                                                                                                       \
+    cudaFuncSetAttribute(pnaplus_conv_fwd_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.fwd_smem);        \
+    pnaplus_conv_fwd_kernel<NC><<<grid, 256, L.fwd_smem, (cudaStream_t)stream>>>(pq, dist, rowptr, perm, src, eattr, d, freq, \
+                                                                                 r, radius, expo, wr, br, wl, mr, mat, cvec, \
+                                                                                 n, f, out, argmin, argmax);                 \
+  } while (0)
+  if (f <= 32) PNAP_FWD(1);
+  else PNAP_FWD(2);
+#undef PNAP_FWD
+  HGB_LAUNCH_CHECK("pnaplus_conv_fwd");
+  return HGB_OK;
+}
+
+extern "C" int hgb_pnaplus_conv_bwd(const float* g_out, const float* pq, const float* dist, const int32_t* rowptr, const int32_t* perm,
+                                    const int32_t* src, const float* eattr, int32_t d, const float* freq, int32_t r, float radius,
+                                    int32_t expo, const float* wr, const float* br, const float* wl, const float* mr, const float* mat,
+                                    const float* cvec, const float* out, const int32_t* argmin, const int32_t* argmax, int32_t n,
+                                    int32_t f, float* g_p, int32_t ldgp, float* g_h, float* g_dist, float* g_eattr, float* g_params,
+                                    void* workspace, hgb_stream_t stream) {
+  PNAP_CHECK_ARGS("pnaplus_conv_bwd");
+  HGB_REQUIRE(ldgp >= f, "pnaplus_conv_bwd: ldgp %d < f %d", ldgp, f);
+  HGB_REQUIRE(g_out && out && argmin && argmax && g_p && g_h, "pnaplus_conv_bwd: null argument");
+  HGB_REQUIRE(!g_params || workspace, "pnaplus_conv_bwd: parameter gradients need the workspace");
+  HGB_REQUIRE(!g_eattr || d > 0, "pnaplus_conv_bwd: g_eattr needs d > 0");
+  const bool grads = g_params != nullptr;
+  const int64_t rows = PnapGrad::floats(f, r, d);
+  if (n == 0) {
+    if (grads) cudaMemsetAsync(g_params, 0, sizeof(float) * (size_t)rows, (cudaStream_t)stream);
+    HGB_LAUNCH_CHECK("pnaplus_conv_bwd");
+    return HGB_OK;
+  }
+  const PnapLaunch L = pnap_launch(f, r, d, grads);
+  const int grid = hgb_grid_for(n, L.warps, PNAP_BWD_MAX_BLOCKS);
+  float* part = static_cast<float*>(workspace);
+#define PNAP_BWD(NC)                                                                                                          \
+  do {                                                                                                                        \
+    cudaFuncSetAttribute(pnaplus_conv_bwd_kernel<NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.bwd_smem);         \
+    pnaplus_conv_bwd_kernel<NC><<<grid, L.warps * 32, L.bwd_smem, (cudaStream_t)stream>>>(                                    \
+        g_out, pq, dist, rowptr, perm, src, eattr, d, freq, r, radius, expo, wr, br, wl, mr, mat, cvec, out, argmin, argmax, n, \
+        f, g_p, ldgp, g_h, g_dist, g_eattr, grads, part);                                                                     \
+  } while (0)
+  if (f <= 32) PNAP_BWD(1);
+  else PNAP_BWD(2);
+#undef PNAP_BWD
+  HGB_LAUNCH_CHECK("pnaplus_conv_bwd");
+  if (grads) {
+    pna_conv_reduce_kernel<<<hgb_grid_for(rows, 256), 256, 0, (cudaStream_t)stream>>>(part, grid, (int)rows, g_params);
+    HGB_LAUNCH_CHECK("pnaplus_conv_reduce");
+  }
+  return HGB_OK;
+}

@@ -1197,6 +1197,82 @@ class PnaConvFn(torch.autograd.Function):
         return g_pq, g_eattr, g_mt, g_cm[0], None
 
 
+def pnaplus_conv_supported(f, r, d):
+    """Shapes ``PnaPlusConvFn`` takes: 1 <= f <= 64, 1 <= num_radial <= 16, edge input width d <= 16."""
+    return bool(_lib.query("hgb_pnaplus_conv_supported", int(f), int(r), int(d)))
+
+
+def raw_pnaplus_conv_fwd(pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec, radius, expo, plan):
+    """-> (agg [n, 4f], argmin, argmax [n, f] int32): hgb_pnaplus_conv_fwd over the by-target CSR of ``plan``."""
+    n, f = pq.shape[0], pq.shape[1] // 2
+    d, r = (0 if eattr is None else eattr.shape[1]), freq.numel()
+    col = plan.by_col
+    agg = torch.empty(n, 4 * f, dtype=pq.dtype, device=pq.device)
+    amin = torch.empty(n, f, dtype=torch.int32, device=pq.device)
+    amax = torch.empty_like(amin)
+    _lib.call("hgb_pnaplus_conv_fwd", _p(pq), _p(dist), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col")), _p(eattr), d, _p(freq), r,
+              float(radius), int(expo), _p(wr), _p(br), _p(wl), _p(mr), _p(mat), _p(cvec), n, f, _p(agg), _p(amin), _p(amax), _stream())
+    return agg, amin, amax
+
+
+def raw_pnaplus_conv_bwd(g_agg, pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec, radius, expo, agg, amin, amax, plan,
+                         need_dist=True, need_eattr=True, need_params=True):
+    """-> (g_pq [n, 2f], g_dist [e] or None, g_eattr [e, d] or None, g_params or None); g_params is laid out as
+    [c f | mat d*f | mr f*f | wr^T r*f | br f | wl^T r*f | freq r] (include/hgb.h)."""
+    n, f = pq.shape[0], pq.shape[1] // 2
+    d, r, e = (0 if eattr is None else eattr.shape[1]), freq.numel(), plan.num_edges
+    dev = pq.device
+    g_pq = torch.empty(n, 2 * f, dtype=pq.dtype, device=dev)
+    g_h = torch.empty(e, f, dtype=pq.dtype, device=dev)
+    g_dist = torch.empty(e, dtype=pq.dtype, device=dev) if need_dist else None
+    g_eattr = torch.empty(e, d, dtype=pq.dtype, device=dev) if (need_eattr and d > 0) else None
+    g_params = torch.empty(f + d * f + f * f + 2 * r * f + f + r, dtype=pq.dtype, device=dev) if need_params else None
+    ws = _ws(_lib.query("hgb_pnaplus_conv_workspace_bytes", f, r, d), dev) if need_params else None
+    col = plan.by_col
+    _lib.call("hgb_pnaplus_conv_bwd", _p(g_agg), _p(pq), _p(dist), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col")), _p(eattr), d,
+              _p(freq), r, float(radius), int(expo), _p(wr), _p(br), _p(wl), _p(mr), _p(mat), _p(cvec), _p(agg), _p(amin), _p(amax),
+              n, f, _p(g_pq), 2 * f, _p(g_h), _p(g_dist), _p(g_eattr), _p(g_params), _p(ws), _stream())
+    row = plan.by_row          # Q was gathered by the source of every edge: g_Q is the by-source segment sum of g_h
+    _lib.call("hgb_segment_sum_strided", _p(g_h), _p(row.rowptr), _p(row.perm), n, f, _p(g_pq[:, f:]), 2 * f, _stream())
+    return g_pq, g_dist, g_eattr, g_params
+
+
+class PnaPlusConvFn(torch.autograd.Function):
+    """agg = [mean | min | max | std] over the targets i = edge_index[1] of PNAPlus's message (hydragnn/models/PNAPlusStack.py
+    :233-263) m_e = (P[i] + Q[j] + M_r relu(W_r rbf_e + b_r) + M_a a_e + c) * (W_l rbf_e), with rbf_e the Bessel basis of the
+    edge length ``dist`` [e] (torch_geometric 2.6.1 BesselBasisLayer: ``freq`` [r], ``radius``, envelope exponent ``expo``).
+    [P | Q] = ``pq`` [n, 2f]; ``wr`` / ``wl`` [f, r], ``br`` [f], ``mr`` [f, f], ``mat`` = M_a^T [d, f] (None without edge
+    input), ``cvec`` [f].  One kernel each way; neither the basis, the embedding nor the message reaches memory."""
+
+    @staticmethod
+    def forward(ctx, pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec, radius, expo, plan):
+        pq, dist, freq, wr, br, wl, mr, cvec = (_chk(t) for t in (pq, dist, freq, wr, br, wl, mr, cvec))
+        eattr = _chk(eattr) if eattr is not None else None
+        mat = _chk(mat) if eattr is not None else None
+        agg, amin, amax = raw_pnaplus_conv_fwd(pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec, radius, expo, plan)
+        ctx.save_for_backward(pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec, agg, amin, amax)
+        ctx.radius, ctx.expo, ctx.plan = float(radius), int(expo), plan
+        return agg
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_agg):
+        pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec, agg, amin, amax = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        need_params = any(need[3:10]) and not _DATA_ONLY["on"]
+        g_pq, g_dist, g_eattr, gp = raw_pnaplus_conv_bwd(_chk(g_agg.contiguous()), pq, dist, eattr, freq, wr, br, wl, mr, mat, cvec,
+                                                         ctx.radius, ctx.expo, agg, amin, amax, ctx.plan, need_dist=need[1],
+                                                         need_eattr=eattr is not None and need[2], need_params=need_params)
+        if gp is None:
+            return g_pq, g_dist, g_eattr, None, None, None, None, None, None, None, None, None, None
+        f, r = pq.shape[1] // 2, freq.numel()
+        d = 0 if eattr is None else eattr.shape[1]
+        sizes = [f, d * f, f * f, r * f, f, r * f, r]
+        g_c, g_mat, g_mr, g_wrt, g_br, g_wlt, g_freq = torch.split(gp, sizes)
+        return (g_pq, g_dist, g_eattr, g_freq, g_wrt.view(r, f).t(), g_br, g_wlt.view(r, f).t(), g_mr.view(f, f),
+                g_mat.view(d, f) if eattr is not None else None, g_c, None, None, None)
+
+
 def cfconv_supported(g, nf, d):
     """Shapes ``CfConvFn`` takes: 1 <= num_gaussians <= 64, 1 <= num_filters <= 128, raw edge input width <= 16."""
     return bool(_lib.query("hgb_cfconv_supported", int(g), int(nf), int(d)))

@@ -30,6 +30,9 @@ WORKLOADS = {
     "eam_pna": dict(n=32, rho=0.085, species=[28, 41], radius=3.0, max_neighbours=20, pbc_box=True),
     # PNA on examples/ogb (ogb_gap): molecule-sized graphs of 9 to 30 atoms, k = 20
     "ogb_pna": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    # PNAPlus on examples/LennardJones (LJ.json: periodic cells, r = 5, k = 5) and on the ogb_pna graphs
+    "lj_pnaplus": dict(n=27, lattice=3.8, radius=5.0, max_neighbours=5, pbc=True),
+    "ogb_pnaplus": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
     # SchNet on examples/qm9 and examples/md17 (GPS: the positional encodings pe, rel_pe = |pe[row] - pe[col]| once the edges
     # exist, see add_rel_pe), and without GPS at the CI widths, building its radius graphs in the layers
     "qm9_schnet": dict(n=9, rho=0.10, species=[1, 6, 7, 8, 9], radius=7.0, max_neighbours=5, pe_dim=2),
@@ -87,6 +90,14 @@ ARCH["ogb_pna"] = dict(mpnn_type="PNA", input_dim=1, hidden_dim=55, num_conv_lay
                        output_heads={"graph": {"num_sharedlayers": 1, "dim_sharedlayers": 55, "num_headlayers": 2,
                                                "dim_headlayers": [55, 55]}},
                        activation_function="relu", loss_function_type="mse", graph_pooling="mean")
+# PNAPlus (PNAPlusStack.py): examples/LennardJones/LJ.json (4 layers at 32, 5 radial functions, envelope 5, MLIP with energy,
+# per-atom energy and force losses) and the ogb_pna widths with the same basis; pna_deg is filled in by the caller
+ARCH["lj_pnaplus"] = dict(mpnn_type="PNAPlus", input_dim=1, hidden_dim=32, num_conv_layers=4, num_radial=5, envelope_exponent=5,
+                          radius=5.0, max_neighbours=5, output_dim=[1], output_type=["node"], task_weights=[1.0],
+                          output_heads={"node": {"num_headlayers": 2, "dim_headlayers": [60, 20], "type": "mlp"}},
+                          activation_function="relu", loss_function_type="mse", enable_interatomic_potential=True,
+                          energy_weight=1.0, energy_peratom_weight=1.0, force_weight=1.0)
+ARCH["ogb_pnaplus"] = dict(ARCH["ogb_pna"], mpnn_type="PNAPlus", num_radial=5, envelope_exponent=5)
 # SchNet (SCFStack.py): examples/qm9/qm9.json exactly, examples/md17/md17.json (6 layers, pe_dim 6), and the in-layer branch at
 # the widths of tests/inputs/ci.json (num_filters 126, num_gaussians 50) with hidden 64 and three layers
 ARCH["qm9_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_conv_layers=2, num_gaussians=10, num_filters=8,

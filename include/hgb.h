@@ -529,6 +529,30 @@ int hgb_pna_conv_bwd(const float* g_out, const float* pq, const int32_t* rowptr,
                      const int32_t* argmax, int32_t n, int32_t f, float* g_p, int32_t ldgp, float* g_h, float* g_cm,
                      void* workspace, hgb_stream_t stream);
 
+/* PNAPlus conv fused (hydragnn/models/PNAPlusStack.py:144-279, message :233-263; torch_geometric 2.6.1 BesselBasisLayer /
+ * Envelope).  For the edge e (CSR slot of the target i, source src[slot]) with length dist[e]: x = dist / radius,
+ * env(x) = (1/x + a x^(p-1) + b x^p + c x^(p+1)) [x < 1] with p = expo + 1, rbf_k = env(x) sin(freq[k] x),
+ * u = relu(wr rbf + br), h = P[i] + Q[src] + mr u + mat^T a_e + cvec, m = h * (wl rbf).  pq [n, 2f] = [P | Q];
+ * wr / wl [f, r] (rbf_emb.0 / rbf_lin weights), br [f], mr [f, f], mat [d, f] (NULL when d = 0), cvec [f].  out [n, 4f] and
+ * argmin / argmax [n, f] are those of hgb_pna_aggregate_fwd on the messages m, which are never written.  1 <= f <= 64,
+ * 1 <= r <= 16, 0 <= d <= 16 (hgb_pnaplus_conv_supported).
+ * Backward recomputes m through the same device code: g_p [n, f] (row stride ldgp); g_h [e, f] = dL/dh in edge order (g_Q =
+ * hgb_segment_sum of it over the CSR of the sources); g_dist [e] and g_eattr [e, d] when non-NULL; g_params (NULL: not
+ * computed) = [c f | mat d*f | mr f*f | wr^T r*f | br f | wl^T r*f | freq r] from per-CTA partials reduced in fixed order in
+ * fp64.  Deterministic: no atomics.  workspace: hgb_pnaplus_conv_workspace_bytes(f, r, d) bytes (-1: unsupported).        */
+int hgb_pnaplus_conv_supported(int32_t f, int32_t r, int32_t d);
+int64_t hgb_pnaplus_conv_workspace_bytes(int32_t f, int32_t r, int32_t d);
+int hgb_pnaplus_conv_fwd(const float* pq, const float* dist, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                         const float* eattr, int32_t d, const float* freq, int32_t r, float radius, int32_t expo, const float* wr,
+                         const float* br, const float* wl, const float* mr, const float* mat, const float* cvec, int32_t n,
+                         int32_t f, float* out, int32_t* argmin, int32_t* argmax, hgb_stream_t stream);
+int hgb_pnaplus_conv_bwd(const float* g_out, const float* pq, const float* dist, const int32_t* rowptr, const int32_t* perm,
+                         const int32_t* src, const float* eattr, int32_t d, const float* freq, int32_t r, float radius,
+                         int32_t expo, const float* wr, const float* br, const float* wl, const float* mr, const float* mat,
+                         const float* cvec, const float* out, const int32_t* argmin, const int32_t* argmax, int32_t n, int32_t f,
+                         float* g_p, int32_t ldgp, float* g_h, float* g_dist, float* g_eattr, float* g_params, void* workspace,
+                         hgb_stream_t stream);
+
 /* SchNet continuous-filter convolution fused (hydragnn/models/SCFStack.py:267-301, CFConv.forward / message with aggr "add",
  * filter network of get_conv :97-103, PyG GaussianSmearing / ShiftedSoftplus).  For the edge e = (row[e] -> col[e]):
  * d_e = |pos[col] - pos[row]|, a_e = [exp(coeff (d_e - mu_k)^2), k < g | r_e] with r [e, d] (NULL when d = 0),
