@@ -224,7 +224,7 @@ extern "C" int hgb_mace_chan_contract(int32_t mode, const float* p0, const float
 // MACE edge embedding (SURVEY K2): edge vector -> real spherical harmonics (component normalisation, e3nn axis convention:
 // polar axis y; hydragnn/models/MACEStack.py:455-466 via o3.SphericalHarmonics) and Bessel basis x polynomial cutoff
 // (mace_utils/modules/radial.py:18-60,110-148, blocks.py:164-177) in ONE pass per edge, with the analytic gradient
-// d/d vec in the backward.  l <= 3, num_bessel <= 16.  vec = pos[col] - pos[row] + shift.
+// d/d vec in the backward.  l <= 3, num_bessel <= 64 (a loop bound: nothing is sized by it).  vec = pos[col] - pos[row] + shift.
 // ------------------------------------------------------------------------------------------------------------------
 namespace {
 

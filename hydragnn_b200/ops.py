@@ -1622,10 +1622,14 @@ class MaceTpScatterFn(torch.autograd.Function):
         d = 0 if eattr is None else eattr.shape[1]
         n, f = up.shape[0], up.shape[2]
         nacc = _lib.query("hgb_mace_tp_num_acc", lin, lsh)
-        out = torch.empty(nacc * n * f, dtype=up.dtype, device=up.device)
-        csr = plan.by_col
-        _lib.call("hgb_mace_tp_scatter_fwd", _p(up), _p(sh), _p(tpw), _p(csr.rowptr), _p(csr.perm), _p(plan.nbr("col")), n, f, lin, lsh,
-                  sh.shape[1], _p(eattr), d, _p(out), _stream())
+        if n == 0 or tpw.shape[0] == 0:
+            # no edge: every sum is empty, and an empty per-edge array has no address to hand to the kernel
+            out = torch.zeros(nacc * n * f, dtype=up.dtype, device=up.device)
+        else:
+            out = torch.empty(nacc * n * f, dtype=up.dtype, device=up.device)
+            csr = plan.by_col
+            _lib.call("hgb_mace_tp_scatter_fwd", _p(up), _p(sh), _p(tpw), _p(csr.rowptr), _p(csr.perm), _p(plan.nbr("col")), n, f, lin,
+                      lsh, sh.shape[1], _p(eattr), d, _p(out), _stream())
         ctx.save_for_backward(up, sh, tpw, eattr)
         ctx.plan, ctx.cfg = plan, (lin, lsh)
         return out
@@ -1638,6 +1642,9 @@ class MaceTpScatterFn(torch.autograd.Function):
         d = 0 if eattr is None else eattr.shape[1]
         n, s_in, f = up.shape
         e = tpw.shape[0]
+        if n == 0 or e == 0:
+            return (torch.zeros_like(up) if ctx.needs_input_grad[0] else None, torch.zeros_like(sh) if ctx.needs_input_grad[1] else None,
+                    torch.zeros_like(tpw), None, None, None, None)
         g = _chk(g.contiguous())
         g_tpw = torch.empty_like(tpw)
         g_up_e = torch.empty(e, s_in * f, dtype=up.dtype, device=up.device)
@@ -1663,7 +1670,8 @@ class MaceSymContractFn(torch.autograd.Function):
         n, _, f = x.shape
         assert wall.shape[1] == _lib.query("hgb_mace_symcontract_num_weights", lin, lout)
         out = torch.empty(n, (lout + 1) ** 2, f, dtype=x.dtype, device=x.device)
-        _lib.call("hgb_mace_symcontract_fwd", _p(x), _p(wall), _p(zcsr.idx), n, f, lin, lout, _p(out), _stream())
+        if n:
+            _lib.call("hgb_mace_symcontract_fwd", _p(x), _p(wall), _p(zcsr.idx), n, f, lin, lout, _p(out), _stream())
         ctx.save_for_backward(x, wall)
         ctx.zcsr, ctx.cfg = zcsr, (lin, lout)
         return out
@@ -1674,6 +1682,8 @@ class MaceSymContractFn(torch.autograd.Function):
         x, wall = ctx.saved_tensors
         zcsr, (lin, lout) = ctx.zcsr, ctx.cfg
         n, _, f = x.shape
+        if n == 0:
+            return torch.empty_like(x), torch.zeros_like(wall), None, None, None
         gx = torch.empty_like(x)
         gw_node = torch.empty(n, wall.shape[1] * f, dtype=x.dtype, device=x.device)
         _lib.call("hgb_mace_symcontract_bwd", _p(_chk(g.contiguous())), _p(x), _p(wall), _p(zcsr.idx), n, f, lin, lout, _p(gx), _p(gw_node),
@@ -1688,7 +1698,8 @@ def _tp_call(mode, p0, p1, p2, cg, out_shape):
     ni, nj, nk = cg.shape
     e, f = p0.shape[0], p0.shape[2]
     out = torch.empty(out_shape, dtype=p0.dtype, device=p0.device)
-    _lib.call("hgb_mace_tp_path", mode, _p(p0), _p(p1), _p(p2), _p(cg), e, f, ni, nj, nk, _p(out), _stream())
+    if e:                    # an empty operand has no address
+        _lib.call("hgb_mace_tp_path", mode, _p(p0), _p(p1), _p(p2), _p(cg), e, f, ni, nj, nk, _p(out), _stream())
     return out
 
 
@@ -1791,7 +1802,8 @@ class EdgeMixT(torch.autograd.Function):
 def _chan_call(mode, p0, p1, n, f, p, ni, out_shape):
     p0, p1 = _chk(p0.contiguous()), _chk(p1.contiguous())
     out = torch.empty(out_shape, dtype=p0.dtype, device=p0.device)
-    _lib.call("hgb_mace_chan_contract", mode, _p(p0), _p(p1), n, f, p, ni, _p(out), _stream())
+    if n:
+        _lib.call("hgb_mace_chan_contract", mode, _p(p0), _p(p1), n, f, p, ni, _p(out), _stream())
     return out
 
 
