@@ -13,7 +13,7 @@ from torch import nn
 from . import ops
 from .stacks import EGCLStack, PAINNStack, cached, graph_sum
 
-SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet")
+SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet", "CGCNN")
 
 
 def get_device(use_gpu=True):
@@ -131,6 +131,9 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
         assert radius is not None, "SchNet requires radius input."
         from .schnet import SCFStack
         model = SCFStack(num_filters, edge_dim, num_gaussians, radius, max_neighbours=max_neighbours, **common)
+    elif mpnn_type == "CGCNN":
+        from .cgcnn import CGCNNStack
+        model = CGCNNStack(edge_dim, **common)
     else:
         raise ValueError("Unknown mpnn_type: {0}".format(mpnn_type))
     if enable_interatomic_potential:

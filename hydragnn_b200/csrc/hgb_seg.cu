@@ -989,3 +989,310 @@ extern "C" int hgb_pnaplus_conv_bwd(const float* g_out, const float* pq, const f
   }
   return HGB_OK;
 }
+
+// ---- CGConv (torch_geometric 2.6.1 CGConv(channels, dim, aggr="add", batch_norm=False, bias=True),
+// hydragnn/models/CGCNNStack.py:60-80).  For the edge e = (j -> i), z_e = [x_i | x_j | a_e]:
+//   m_e = sigmoid(W_f z_e + b_f) * softplus(W_s z_e + b_s),   out_i = x_i + sum_{e: target i} m_e.
+// Both Linears are affine in the blocks of z, so with one per-node Linear [P_f | P_s | Q_f | Q_s] = x [A_f; A_s; B_f; B_s]^T
+// the pre-activations are f_e = P_f[i] + Q_f[j] + C_f a_e + b_f (s_e alike) and are formed in registers: no [E, 2F + D] z,
+// no [E, F] pre-activation and no message reach memory.
+//
+// Thread mapping: a group of G lanes owns one target node, G the power of two >= F up to 32, so a warp serves 32 / G targets
+// at F <= 32 (at F = 1, the update_config shape without GPS, all 32 lanes work on 32 targets).  Above 32 a warp owns one
+// target and lane l the channels l + 32 t, t < CPT.  A lane's channel set is fixed, so its sums run in CSR order (ascending
+// edge id, as scatter_add_ does) with no atomics.  mt [d, 2F] and cvec [2F] are staged in shared memory once per CTA.
+#define CGC_MAX_F 128
+#define CGC_MAX_D 16
+#define CGC_BWD_MAX_BLOCKS (HGB_NUM_SMS * 4)
+
+// torch's sigmoid and softplus (beta 1, threshold 20) with the accurate exp / log1p: the fp32 configs are held to fp64
+__device__ __forceinline__ float cgc_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
+__device__ __forceinline__ float cgc_softplus(float z) { return z > 20.f ? z : log1pf(expf(z)); }
+
+// f_e and s_e of the lane's channels cc[t] (clamped to f - 1 where the lane has no channel, so every load stays in range):
+// base = P[i] + b per node, then + Q[j] + sum_k mt[k, .] a_e[k].  Forward and backward both call this, so the backward's
+// softplus branch sees the forward's pre-activation bit for bit.
+template <int CPT>
+__device__ __forceinline__ void cgc_pre(const float* smt, int f, int d, const int (&cc)[CPT], const float (&bf)[CPT],
+                                        const float (&bs)[CPT], const float* __restrict__ q, const float* __restrict__ a_row,
+                                        float (&zf)[CPT], float (&zs)[CPT]) {
+#pragma unroll
+  for (int t = 0; t < CPT; ++t) {
+    zf[t] = bf[t] + __ldg(q + cc[t]);
+    zs[t] = bs[t] + __ldg(q + f + cc[t]);
+  }
+  for (int k = 0; k < d; ++k) {
+    const float a = __ldg(a_row + k);
+    const float* m = smt + k * 2 * f;
+#pragma unroll
+    for (int t = 0; t < CPT; ++t) {
+      zf[t] = fmaf(m[cc[t]], a, zf[t]);
+      zs[t] = fmaf(m[f + cc[t]], a, zs[t]);
+    }
+  }
+}
+
+__device__ __forceinline__ void cgc_stage(float* sm, const float* __restrict__ mt, const float* __restrict__ cvec, int f, int d) {
+  const int nm = d * 2 * f;
+  for (int t = threadIdx.x; t < nm + 2 * f; t += blockDim.x) sm[t] = t < nm ? __ldg(mt + t) : __ldg(cvec + t - nm);
+}
+
+template <int CPT>
+__global__ void __launch_bounds__(256) cgconv_fwd_kernel(
+    const float* __restrict__ pq, const int32_t* __restrict__ rowptr, const int32_t* __restrict__ perm,
+    const int32_t* __restrict__ src, const float* __restrict__ eattr, int d, const float* __restrict__ mt,
+    const float* __restrict__ cvec, const float* __restrict__ x, int n, int f, int gl2, float* __restrict__ out) {
+  extern __shared__ float cgc_sm[];
+  const float* smt = cgc_sm;
+  const float* scv = cgc_sm + d * 2 * f;
+  cgc_stage(cgc_sm, mt, cvec, f, d);
+  __syncthreads();
+  const int sub = threadIdx.x & ((1 << gl2) - 1);
+  const int gpb = blockDim.x >> gl2;
+  const int64_t ld = 4 * (int64_t)f;
+  int cc[CPT];
+  bool ok[CPT];
+#pragma unroll
+  for (int t = 0; t < CPT; ++t) {
+    ok[t] = sub + 32 * t < f;
+    cc[t] = min(sub + 32 * t, f - 1);
+  }
+  for (int row = blockIdx.x * gpb + (threadIdx.x >> gl2); row < n; row += gridDim.x * gpb) {
+    const int lo = rowptr[row], hi = rowptr[row + 1];
+    float bf[CPT], bs[CPT], acc[CPT];
+#pragma unroll
+    for (int t = 0; t < CPT; ++t) {
+      bf[t] = __ldg(pq + row * ld + cc[t]) + scv[cc[t]];
+      bs[t] = __ldg(pq + row * ld + f + cc[t]) + scv[f + cc[t]];
+      acc[t] = 0.f;
+    }
+    for (int p = lo; p < hi; ++p) {
+      const int e = perm ? perm[p] : p;
+      float zf[CPT], zs[CPT];
+      cgc_pre<CPT>(smt, f, d, cc, bf, bs, pq + (int64_t)src[p] * ld + 2 * f, eattr + (int64_t)e * d, zf, zs);
+#pragma unroll
+      for (int t = 0; t < CPT; ++t) acc[t] += cgc_sigmoid(zf[t]) * cgc_softplus(zs[t]);
+    }
+#pragma unroll
+    for (int t = 0; t < CPT; ++t)
+      if (ok[t]) out[(int64_t)row * f + cc[t]] = acc[t] + __ldg(x + (int64_t)row * f + cc[t]);    // residual, as PyG adds it
+  }
+}
+
+// Per edge, g = g_out[i]:  g_f = g softplus(s) sigma(f) (1 - sigma(f)),  g_s = g sigma(f) softplus'(s) with softplus'(s) = 1
+// above the threshold and e^s / (e^s + 1) below (ATen's softplus_backward).  g_h [e, 2f] = [g_f | g_s] in edge order; g_p[i]
+// its segment sum; g_eattr[e] = g_h mt^T (a fixed xor tree over the group) when non-NULL.  With part non-NULL the lane adds
+// g_h and a_e g_h into its own shared slots (warp w, entry (k, half, t) at ((k * 2 + half) * CPT + t) * 32 + lane), which
+// are then summed over the CTA's warps and groups in index order into part [gridDim.x, 1 + d, 2f].  The row loop and the
+// edge loop are warp-uniform, so the g_eattr shuffles see every lane.
+template <int CPT>
+__global__ void __launch_bounds__(256) cgconv_bwd_kernel(
+    const float* __restrict__ g_out, const float* __restrict__ pq, const int32_t* __restrict__ rowptr,
+    const int32_t* __restrict__ perm, const int32_t* __restrict__ src, const float* __restrict__ eattr, int d,
+    const float* __restrict__ mt, const float* __restrict__ cvec, int n, int f, int gl2, float* __restrict__ g_p, int ldgp,
+    float* __restrict__ g_h, float* __restrict__ g_eattr, float* __restrict__ part) {
+  extern __shared__ float cgc_sm[];
+  const float* smt = cgc_sm;
+  const float* scv = cgc_sm + d * 2 * f;
+  float* sacc = cgc_sm + (d + 1) * 2 * f;
+  const int slots = (d + 1) * 2 * CPT * 32;
+  const int nwarps = blockDim.x >> 5;
+  cgc_stage(cgc_sm, mt, cvec, f, d);
+  if (part)
+    for (int t = threadIdx.x; t < nwarps * slots; t += blockDim.x) sacc[t] = 0.f;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int G = 1 << gl2, sub = lane & (G - 1), gpw = 32 >> gl2;
+  float* wacc = sacc + warp * slots + lane;
+  const int64_t ld = 4 * (int64_t)f;
+  int cc[CPT];
+  bool ok[CPT];
+#pragma unroll
+  for (int t = 0; t < CPT; ++t) {
+    ok[t] = sub + 32 * t < f;
+    cc[t] = min(sub + 32 * t, f - 1);
+  }
+  for (int first = (blockIdx.x * nwarps + warp) * gpw; first < n; first += gridDim.x * nwarps * gpw) {
+    const int row = first + (lane >> gl2);
+    const bool rv = row < n;
+    const int lo = rv ? rowptr[row] : 0, len = rv ? rowptr[row + 1] - lo : 0;
+    const int maxlen = (int)__reduce_max_sync(0xffffffffu, (unsigned)len);
+    float bf[CPT], bs[CPT], g[CPT], gpf[CPT], gps[CPT];
+#pragma unroll
+    for (int t = 0; t < CPT; ++t) {
+      bf[t] = rv ? __ldg(pq + row * ld + cc[t]) + scv[cc[t]] : 0.f;
+      bs[t] = rv ? __ldg(pq + row * ld + f + cc[t]) + scv[f + cc[t]] : 0.f;
+      g[t] = (rv && ok[t]) ? __ldg(g_out + (int64_t)row * f + cc[t]) : 0.f;
+      gpf[t] = gps[t] = 0.f;
+    }
+    for (int it = 0; it < maxlen; ++it) {
+      const bool ev = it < len;
+      const int p = lo + it;
+      const int e = ev ? (perm ? perm[p] : p) : 0;
+      const float* a_row = eattr + (int64_t)e * d;
+      float gf[CPT], gs[CPT];
+      if (ev) {
+        float zf[CPT], zs[CPT];
+        cgc_pre<CPT>(smt, f, d, cc, bf, bs, pq + (int64_t)src[p] * ld + 2 * f, a_row, zf, zs);
+#pragma unroll
+        for (int t = 0; t < CPT; ++t) {
+          const float sg = cgc_sigmoid(zf[t]);
+          float dsp = 1.f;
+          if (!(zs[t] > 20.f)) {
+            const float ez = expf(zs[t]);
+            dsp = ez / (ez + 1.f);
+          }
+          gf[t] = g[t] * cgc_softplus(zs[t]) * (sg * (1.f - sg));
+          gs[t] = g[t] * sg * dsp;
+          gpf[t] += gf[t];
+          gps[t] += gs[t];
+          if (ok[t]) {
+            g_h[(int64_t)e * 2 * f + cc[t]] = gf[t];
+            g_h[(int64_t)e * 2 * f + f + cc[t]] = gs[t];
+          }
+        }
+        if (part) {
+#pragma unroll
+          for (int t = 0; t < CPT; ++t) {
+            wacc[(0 * CPT + t) * 32] += gf[t];
+            wacc[(1 * CPT + t) * 32] += gs[t];
+          }
+          for (int k = 0; k < d; ++k) {
+            const float a = __ldg(a_row + k);
+#pragma unroll
+            for (int t = 0; t < CPT; ++t) {
+              float* s = wacc + ((k + 1) * 2 * CPT + t) * 32;
+              s[0] = fmaf(a, gf[t], s[0]);
+              s[CPT * 32] = fmaf(a, gs[t], s[CPT * 32]);
+            }
+          }
+        }
+      } else {
+#pragma unroll
+        for (int t = 0; t < CPT; ++t) gf[t] = gs[t] = 0.f;
+      }
+      if (g_eattr) {
+        for (int k = 0; k < d; ++k) {
+          const float* m = smt + k * 2 * f;
+          float v = 0.f;
+#pragma unroll
+          for (int t = 0; t < CPT; ++t) v = fmaf(gf[t], m[cc[t]], fmaf(gs[t], m[f + cc[t]], v));
+          for (int o = G >> 1; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+          if (ev && sub == 0) g_eattr[(int64_t)e * d + k] = v;
+        }
+      }
+    }
+    if (rv) {
+#pragma unroll
+      for (int t = 0; t < CPT; ++t)
+        if (ok[t]) {
+          g_p[(int64_t)row * ldgp + cc[t]] = gpf[t];
+          g_p[(int64_t)row * ldgp + f + cc[t]] = gps[t];
+        }
+    }
+  }
+  if (!part) return;
+  __syncthreads();
+  const int rows = (d + 1) * 2 * f;
+  for (int r = threadIdx.x; r < rows; r += blockDim.x) {
+    const int k = r / (2 * f), half = (r / f) & 1, c = r % f;
+    const int slot = ((k * 2 + half) * CPT + (c >> 5)) * 32 + (c & 31);
+    float s = 0.f;
+    for (int w = 0; w < nwarps; ++w)
+      for (int grp = 0; grp < gpw; ++grp) s += sacc[w * slots + slot + grp * G];
+    part[(int64_t)blockIdx.x * rows + r] = s;
+  }
+}
+
+namespace {
+struct CgcLaunch {
+  int cpt, gl2, warps;
+  size_t fwd_smem, bwd_smem;
+};
+
+CgcLaunch cgc_launch(int f, int d, bool grads) {
+  CgcLaunch L;
+  L.cpt = f <= 32 ? 1 : (f <= 64 ? 2 : 4);
+  L.gl2 = 0;
+  while ((1 << L.gl2) < f && L.gl2 < 5) ++L.gl2;
+  const size_t params = (size_t)(d + 1) * 2 * f;
+  const size_t slots = grads ? (size_t)(d + 1) * 2 * L.cpt * 32 : 0;
+  L.warps = (params + 8 * slots) * 4 <= 160 * 1024 ? 8 : 4;
+  L.fwd_smem = params * 4;
+  L.bwd_smem = (params + L.warps * slots) * 4;
+  return L;
+}
+}  // namespace
+
+extern "C" int hgb_cgconv_supported(int32_t f, int32_t d) { return f >= 1 && f <= CGC_MAX_F && d >= 0 && d <= CGC_MAX_D; }
+
+extern "C" int64_t hgb_cgconv_workspace_bytes(int32_t f, int32_t d) {
+  if (!hgb_cgconv_supported(f, d)) return -1;
+  return (int64_t)CGC_BWD_MAX_BLOCKS * (d + 1) * 2 * f * (int64_t)sizeof(float);
+}
+
+#define CGC_CHECK_ARGS(name)                                                                                                 \
+  HGB_REQUIRE(n >= 0 && e >= 0 && hgb_cgconv_supported(f, d),                                                               \
+              name ": bad sizes (n %d, e %d, f %d, d %d; 1 <= f <= %d, 0 <= d <= %d)", n, e, f, d, CGC_MAX_F, CGC_MAX_D);      \
+  HGB_REQUIRE(rowptr && (n == 0 || (pq && cvec)) && (e == 0 || src) && (d == 0 || (mt && (e == 0 || eattr))),               \
+              name ": null argument")
+
+extern "C" int hgb_cgconv_fwd(const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src, const float* eattr,
+                              int32_t d, const float* mt, const float* cvec, const float* x, int32_t n, int32_t e, int32_t f,
+                              float* out, hgb_stream_t stream) {
+  CGC_CHECK_ARGS("cgconv_fwd");
+  HGB_REQUIRE(n == 0 || (x && out), "cgconv_fwd: null argument");
+  if (n == 0) return HGB_OK;
+  if (e == 0) {                              // no messages: out = x
+    cudaMemcpyAsync(out, x, sizeof(float) * (size_t)n * f, cudaMemcpyDeviceToDevice, (cudaStream_t)stream);
+    return cudaPeekAtLastError() == cudaSuccess ? HGB_OK : HGB_ECUDA;
+  }
+  const CgcLaunch L = cgc_launch(f, d, false);
+  const int grid = hgb_grid_for(n, (256 >> L.gl2));
+#define CGC_FWD(CPT)                                                                                                         \
+  cgconv_fwd_kernel<CPT><<<grid, 256, L.fwd_smem, (cudaStream_t)stream>>>(pq, rowptr, perm, src, eattr, d, mt, cvec, x, n, f, \
+                                                                          L.gl2, out)
+  if (L.cpt == 1) CGC_FWD(1);
+  else if (L.cpt == 2) CGC_FWD(2);
+  else CGC_FWD(4);
+#undef CGC_FWD
+  HGB_LAUNCH_CHECK("cgconv_fwd");
+  return HGB_OK;
+}
+
+extern "C" int hgb_cgconv_bwd(const float* g_out, const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                              const float* eattr, int32_t d, const float* mt, const float* cvec, int32_t n, int32_t e, int32_t f,
+                              float* g_p, int32_t ldgp, float* g_h, float* g_eattr, float* g_params, void* workspace,
+                              hgb_stream_t stream) {
+  CGC_CHECK_ARGS("cgconv_bwd");
+  HGB_REQUIRE(ldgp >= 2 * f, "cgconv_bwd: ldgp %d < 2 f = %d", ldgp, 2 * f);
+  HGB_REQUIRE((n == 0 || (g_out && g_p)) && (e == 0 || g_h), "cgconv_bwd: null argument");
+  HGB_REQUIRE(!g_params || workspace, "cgconv_bwd: parameter gradients need the workspace");
+  HGB_REQUIRE(!g_eattr || d > 0, "cgconv_bwd: g_eattr needs d > 0");
+  const bool grads = g_params != nullptr;
+  const int rows = (d + 1) * 2 * f;
+  if (n == 0 || e == 0) {                    // no messages: every gradient the kernel writes is zero
+    if (grads) cudaMemsetAsync(g_params, 0, sizeof(float) * (size_t)rows, (cudaStream_t)stream);
+    if (n > 0) cudaMemset2DAsync(g_p, sizeof(float) * (size_t)ldgp, 0, sizeof(float) * 2 * (size_t)f, n, (cudaStream_t)stream);
+    return cudaPeekAtLastError() == cudaSuccess ? HGB_OK : HGB_ECUDA;
+  }
+  const CgcLaunch L = cgc_launch(f, d, grads);
+  const int grid = hgb_grid_for(n, L.warps * (32 >> L.gl2), CGC_BWD_MAX_BLOCKS);
+  float* part = grads ? static_cast<float*>(workspace) : nullptr;
+#define CGC_BWD(CPT)                                                                                                         \
+  do {                                                                                                                       \
+    cudaFuncSetAttribute(cgconv_bwd_kernel<CPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.bwd_smem);             \
+    cgconv_bwd_kernel<CPT><<<grid, L.warps * 32, L.bwd_smem, (cudaStream_t)stream>>>(                                        \
+        g_out, pq, rowptr, perm, src, eattr, d, mt, cvec, n, f, L.gl2, g_p, ldgp, g_h, g_eattr, part);                       \
+  } while (0)
+  if (L.cpt == 1) CGC_BWD(1);
+  else if (L.cpt == 2) CGC_BWD(2);
+  else CGC_BWD(4);
+#undef CGC_BWD
+  HGB_LAUNCH_CHECK("cgconv_bwd");
+  if (grads) {
+    pna_conv_reduce_kernel<<<hgb_grid_for(rows, 256), 256, 0, (cudaStream_t)stream>>>(part, grid, rows, g_params);
+    HGB_LAUNCH_CHECK("cgconv_reduce");
+  }
+  return HGB_OK;
+}

@@ -1273,6 +1273,80 @@ class PnaPlusConvFn(torch.autograd.Function):
                 g_mat.view(d, f) if eattr is not None else None, g_c, None, None, None)
 
 
+def cgconv_supported(f, d):
+    """Shapes ``CgConvFn`` takes: 1 <= f <= 128 channels, edge input width 0 <= d <= 16."""
+    return bool(_lib.query("hgb_cgconv_supported", int(f), int(d)))
+
+
+def raw_cgconv_fwd(pq, eattr, mt, cvec, x, plan):
+    """-> out [n, f] = x + sum over the targets of sigmoid(f_e) * softplus(s_e): hgb_cgconv_fwd over the by-target CSR."""
+    n, f = x.shape
+    d = 0 if eattr is None else eattr.shape[1]
+    col = plan.by_col
+    out = torch.empty_like(x)
+    _lib.call("hgb_cgconv_fwd", _p(pq), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col")), _p(eattr), d, _p(mt), _p(cvec), _p(x),
+              n, plan.num_edges, f, _p(out), _stream())
+    return out
+
+
+def raw_cgconv_bwd(g_out, pq, eattr, mt, cvec, plan, need_eattr=True, need_params=True):
+    """-> (g_pq [n, 4f], g_eattr [e, d] or None, g_params [1 + d, 2f] = [g_cvec ; g_mt] or None)."""
+    n, f = g_out.shape
+    d, e = (0 if eattr is None else eattr.shape[1]), plan.num_edges
+    dev = g_out.device
+    g_pq = torch.empty(n, 4 * f, dtype=g_out.dtype, device=dev)
+    g_h = torch.empty(e, 2 * f, dtype=g_out.dtype, device=dev)
+    g_eattr = torch.empty(e, d, dtype=g_out.dtype, device=dev) if (need_eattr and d > 0) else None
+    g_params = torch.empty(1 + d, 2 * f, dtype=g_out.dtype, device=dev) if need_params else None
+    ws = _ws(_lib.query("hgb_cgconv_workspace_bytes", f, d), dev) if need_params else None
+    col = plan.by_col
+    _lib.call("hgb_cgconv_bwd", _p(g_out), _p(pq), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col")), _p(eattr), d, _p(mt), _p(cvec),
+              n, e, f, _p(g_pq), 4 * f, _p(g_h), _p(g_eattr), _p(g_params), _p(ws), _stream())
+    row = plan.by_row          # Q was gathered by the source of every edge: g_Q is the by-source segment sum of g_h
+    _lib.call("hgb_segment_sum_strided", _p(g_h), _p(row.rowptr), _p(row.perm), n, 2 * f, _p(g_pq[:, 2 * f:]), 4 * f, _stream())
+    return g_pq, g_eattr, g_params
+
+
+class CgConvFn(torch.autograd.Function):
+    """out = x + sum over the targets i = edge_index[1] of m_e = sigmoid(f_e) * softplus(s_e) -- torch_geometric 2.6.1 CGConv
+    (aggr "add", batch_norm=False; hydragnn/models/CGCNNStack.py:60-80) with f_e = P_f[i] + Q_f[j] + C_f a_e + b_f and s_e
+    alike.  ``pq`` [n, 4f] = [P_f | P_s | Q_f | Q_s], ``mt`` [d, 2f] = [C_f | C_s]^T (None without edge input), ``cvec`` [2f]
+    = [b_f | b_s], ``x`` [n, f] the residual.  One kernel each way; neither z, the pre-activations nor the message reach
+    memory.  Without nodes or edges no kernel runs."""
+
+    @staticmethod
+    def forward(ctx, pq, eattr, mt, cvec, x, plan):
+        pq, cvec, x = _chk(pq), _chk(cvec), _chk(x)
+        eattr = _chk(eattr) if eattr is not None else None
+        mt = _chk(mt) if eattr is not None else None
+        ctx.save_for_backward(pq, eattr, mt, cvec)
+        ctx.plan = plan
+        if x.shape[0] == 0 or plan.num_edges == 0:
+            return x.clone()
+        return raw_cgconv_fwd(pq, eattr, mt, cvec, x, plan)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out):
+        pq, eattr, mt, cvec = ctx.saved_tensors
+        plan = ctx.plan
+        need = ctx.needs_input_grad
+        need_params = (need[2] or need[3]) and not _DATA_ONLY["on"]
+        g_out = _chk(g_out.contiguous())
+        n, f = g_out.shape
+        d = 0 if eattr is None else eattr.shape[1]
+        if n == 0 or plan.num_edges == 0:
+            g_pq = torch.zeros_like(pq)
+            g_eattr = torch.zeros_like(eattr) if (eattr is not None and need[1]) else None
+            g_params = torch.zeros(1 + d, 2 * f, dtype=g_out.dtype, device=g_out.device) if need_params else None
+        else:
+            g_pq, g_eattr, g_params = raw_cgconv_bwd(g_out, pq, eattr, mt, cvec, plan, need_eattr=eattr is not None and need[1],
+                                                     need_params=need_params)
+        if g_params is None:
+            return g_pq, g_eattr, None, None, g_out, None
+        return g_pq, g_eattr, (g_params[1:] if eattr is not None else None), g_params[0], g_out, None
+
+
 def cfconv_supported(g, nf, d):
     """Shapes ``CfConvFn`` takes: 1 <= num_gaussians <= 64, 1 <= num_filters <= 128, raw edge input width <= 16."""
     return bool(_lib.query("hgb_cfconv_supported", int(g), int(nf), int(d)))

@@ -39,6 +39,11 @@ WORKLOADS = {
     "md17_schnet": dict(n=21, rho=0.08, species=[6] * 9 + [1] * 8 + [8] * 4, radius=7.0, max_neighbours=5, fixed_species=True,
                         pe_dim=6),
     "ci_schnet": dict(n=9, rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    # CGCNN on Materials-Project-like crystals: periodic cells of 8 to 64 atoms, any species, CGCNN's 12-neighbour graphs
+    # (r = 8 A); the GPS variant adds the positional encodings
+    "mp_cgcnn": dict(sizes=list(range(8, 65)), rho=0.06, species=list(range(1, 84)), radius=8.0, max_neighbours=12, pbc_box=True),
+    "mp_cgcnn_gps": dict(sizes=list(range(8, 65)), rho=0.06, species=list(range(1, 84)), radius=8.0, max_neighbours=12,
+                         pbc_box=True, pe_dim=6),
 }
 
 ARCH = {
@@ -115,6 +120,15 @@ ARCH["ci_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_con
 ARCH["oc20_mace_80"] = ARCH["oc20_mace"]
 ARCH["gfm_pnaeq_mini"] = dict(ARCH["gfm_pnaeq"], output_dim=[1], output_type=["graph"], task_weights=[1.0], loss_function_type="mse",
                               output_heads={"graph": ARCH["gfm_pnaeq"]["output_heads"]["graph"]})
+# CGCNN (CGCNNStack.py): the edge length as the one edge feature, and input_dim = hidden_dim = 1 as update_config makes them
+# without GPS, with the graph head widths of tests/inputs/ci.json; with GPS (8 heads, pe_dim 6) at hidden 64
+ARCH["mp_cgcnn"] = dict(mpnn_type="CGCNN", input_dim=1, hidden_dim=1, num_conv_layers=3, edge_dim=1, radius=8.0, max_neighbours=12,
+                        output_dim=[1], output_type=["graph"], task_weights=[1.0],
+                        output_heads={"graph": {"num_sharedlayers": 2, "dim_sharedlayers": 4, "num_headlayers": 2,
+                                                "dim_headlayers": [10, 10]}},
+                        activation_function="relu", loss_function_type="mse", graph_pooling="mean")
+ARCH["mp_cgcnn_gps"] = dict(ARCH["mp_cgcnn"], hidden_dim=64, global_attn_engine="GPS", global_attn_type="multihead",
+                            global_attn_heads=8, pe_dim=6)
 
 
 def _cube_positions(gen, num_graphs, n, box, min_sep, max_iter=200):

@@ -553,6 +553,26 @@ int hgb_pnaplus_conv_bwd(const float* g_out, const float* pq, const float* dist,
                          float* g_p, int32_t ldgp, float* g_h, float* g_dist, float* g_eattr, float* g_params, void* workspace,
                          hgb_stream_t stream);
 
+/* CGConv fused (hydragnn/models/CGCNNStack.py:60-80; torch_geometric 2.6.1 CGConv(channels, dim, aggr="add",
+ * batch_norm=False, bias=True), message with z = [x_i | x_j | a_e]).  For the edge e (CSR slot of the target i, source
+ * src[slot]): f_e = P_f[i] + Q_f[j] + mt[:, :f]^T a_e + cvec[:f], s_e = P_s[i] + Q_s[j] + mt[:, f:]^T a_e + cvec[f:],
+ * m_e = sigmoid(f_e) * softplus(s_e) (beta 1, threshold 20), out[i] = x[i] + sum_e m_e summed in CSR order.
+ * pq [n, 4f] = [P_f | P_s | Q_f | Q_s]; mt [d, 2f] (NULL when d = 0); cvec [2f] = [b_f | b_s]; x, out [n, f].
+ * 1 <= f <= 128, 0 <= d <= 16 (hgb_cgconv_supported); e is the number of edges (perm / src have e entries).
+ * Backward recomputes f_e, s_e through the same device code: g_p [n, 2f] (row stride ldgp) = segment sum of g_h;
+ * g_h [e, 2f] = [dL/df | dL/ds] in edge order (g_Q = hgb_segment_sum_strided of it over the CSR of the sources);
+ * g_eattr [e, d] = g_h mt^T when non-NULL; g_params (NULL: not computed) [1 + d, 2f] = [g_cvec ; g_mt] from per-CTA
+ * partials reduced in fixed order in fp64.  The residual's gradient is g_out itself and is not written.  Deterministic: no
+ * atomics.  n = 0 or e = 0 launch no kernel.  workspace: hgb_cgconv_workspace_bytes(f, d) bytes (-1: unsupported).     */
+int hgb_cgconv_supported(int32_t f, int32_t d);
+int64_t hgb_cgconv_workspace_bytes(int32_t f, int32_t d);
+int hgb_cgconv_fwd(const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src, const float* eattr, int32_t d,
+                   const float* mt, const float* cvec, const float* x, int32_t n, int32_t e, int32_t f, float* out,
+                   hgb_stream_t stream);
+int hgb_cgconv_bwd(const float* g_out, const float* pq, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                   const float* eattr, int32_t d, const float* mt, const float* cvec, int32_t n, int32_t e, int32_t f, float* g_p,
+                   int32_t ldgp, float* g_h, float* g_eattr, float* g_params, void* workspace, hgb_stream_t stream);
+
 /* SchNet continuous-filter convolution fused (hydragnn/models/SCFStack.py:267-301, CFConv.forward / message with aggr "add",
  * filter network of get_conv :97-103, PyG GaussianSmearing / ShiftedSoftplus).  For the edge e = (row[e] -> col[e]):
  * d_e = |pos[col] - pos[row]|, a_e = [exp(coeff (d_e - mu_k)^2), k < g | r_e] with r [e, d] (NULL when d = 0),
