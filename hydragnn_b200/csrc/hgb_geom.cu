@@ -21,8 +21,9 @@ __global__ void edge_geom_fwd_kernel(const float* __restrict__ pos, const int32_
 
 extern "C" int hgb_edge_geom_fwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, int64_t e,
                                  float eps, float* vec, float* len, float* unit, hgb_stream_t stream) {
-  HGB_REQUIRE(e >= 0 && pos && row && col, "edge_geom_fwd: bad arguments");
-  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(e >= 0, "edge_geom_fwd: bad arguments");
+  if (e == 0) return HGB_OK;   // no edges: no kernel runs (the arrays may then be NULL)
+  HGB_REQUIRE(pos && row && col, "edge_geom_fwd: bad arguments");
   edge_geom_fwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, e, eps, vec, len, unit);
   HGB_LAUNCH_CHECK("edge_geom_fwd");
   return HGB_OK;
@@ -51,8 +52,9 @@ __global__ void edge_geom_bwd_kernel(const float* __restrict__ vec, const float*
 
 extern "C" int hgb_edge_geom_bwd(const float* vec, const float* len, float eps, const float* g_vec_in, const float* g_len,
                                  const float* g_unit, int64_t e, float* g_vec, hgb_stream_t stream) {
-  HGB_REQUIRE(e >= 0 && vec && len && g_vec, "edge_geom_bwd: bad arguments");
+  HGB_REQUIRE(e >= 0, "edge_geom_bwd: bad arguments");
   if (e == 0) return HGB_OK;
+  HGB_REQUIRE(vec && len && g_vec, "edge_geom_bwd: bad arguments");
   edge_geom_bwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(vec, len, eps, g_vec_in, g_len, g_unit, e, g_vec);
   HGB_LAUNCH_CHECK("edge_geom_bwd");
   return HGB_OK;
@@ -80,8 +82,9 @@ __global__ void painn_edge_embed_fwd_kernel(const float* __restrict__ unit, cons
 
 extern "C" int hgb_painn_edge_embed_fwd(const float* unit, const float* len, int64_t e, int32_t r, float cutoff, float* epack,
                                         hgb_stream_t stream) {
-  HGB_REQUIRE(e >= 0 && r > 0 && r <= 8 && unit && len && epack, "painn_edge_embed_fwd: bad arguments (num_radial <= 8)");
-  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(e >= 0 && r > 0 && r <= 8, "painn_edge_embed_fwd: bad arguments (0 < num_radial <= 8, got %d)", r);
+  if (e == 0) return HGB_OK;   // no edges: no kernel runs (the arrays may then be NULL)
+  HGB_REQUIRE(unit && len && epack && (uintptr_t)epack % 16 == 0, "painn_edge_embed_fwd: null pointer or epack not 16-byte aligned");
   painn_edge_embed_fwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(unit, len, e, r, cutoff, epack);
   HGB_LAUNCH_CHECK("painn_edge_embed_fwd");
   return HGB_OK;
@@ -116,8 +119,9 @@ __global__ void painn_edge_embed_bwd_kernel(const float* __restrict__ unit, cons
 
 extern "C" int hgb_painn_edge_embed_bwd(const float* unit, const float* len, const float* g_epack, int64_t e, int32_t r, float cutoff,
                                         float* g_unit, float* g_len, hgb_stream_t stream) {
-  HGB_REQUIRE(e >= 0 && r > 0 && r <= 8 && unit && len && g_epack && g_unit && g_len, "painn_edge_embed_bwd: bad arguments");
+  HGB_REQUIRE(e >= 0 && r > 0 && r <= 8, "painn_edge_embed_bwd: bad arguments (0 < num_radial <= 8, got %d)", r);
   if (e == 0) return HGB_OK;
+  HGB_REQUIRE(unit && len && g_epack && g_unit && g_len, "painn_edge_embed_bwd: null pointer");
   painn_edge_embed_bwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(unit, len, g_epack, e, r, cutoff, g_unit, g_len);
   HGB_LAUNCH_CHECK("painn_edge_embed_bwd");
   return HGB_OK;

@@ -139,7 +139,7 @@ __global__ void painn_edge_records_kernel(const float* __restrict__ epack, const
 extern "C" int hgb_painn_edge_records(const float* epack, const int32_t* perm, const int32_t* nbr, int64_t e, float* rec,
                                       hgb_stream_t stream) {
   if (e == 0) return HGB_OK;
-  HGB_REQUIRE(epack && nbr && rec, "painn_edge_records: null pointer");
+  HGB_REQUIRE(epack && nbr && rec && ((uintptr_t)epack | (uintptr_t)rec) % 16 == 0, "painn_edge_records: null or misaligned pointer");
   painn_edge_records_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(epack, perm, nbr, e, rec);
   HGB_LAUNCH_CHECK("painn_edge_records");
   return HGB_OK;
@@ -404,7 +404,9 @@ painn_message_fwd_tiled_kernel(const float* __restrict__ phi, const float* __res
 }
 
 static int painn_group(int f) { int g = 32; if (f < 32) { g = 1; while (g < f) g <<= 1; } return g; }
-static int painn_cpl(int f) { return (f >= 64 && f % 2 == 0) ? 2 : 1; }
+// CPL = 2 moves channel pairs with 8-byte loads and stores: only when every row it touches that way is 8-byte aligned
+// (`rows` = the OR of those addresses; a view that starts 4 bytes into an allocation takes CPL = 1)
+static int painn_cpl(int f, uintptr_t rows) { return (f >= 64 && f % 2 == 0 && rows % 8 == 0) ? 2 : 1; }
 
 extern "C" int hgb_painn_message_affine_v_supported(int32_t n, int32_t f) { return (f == 64 && n >= 256) ? 1 : 0; }
 
@@ -413,15 +415,19 @@ extern "C" int hgb_painn_message_fwd(const float* phi, const float* s, const flo
                                      const float* epack, const float* rec, const float* wf, const float* bf, const float* efilt,
                                      int32_t n, int32_t f, int32_t r, float* s_out, float* v_out, hgb_stream_t stream) {
   HGB_REQUIRE(n >= 0 && f > 0 && r > 0 && r <= RMAX, "painn_message_fwd: need 0 < num_radial <= %d (got %d)", RMAX, r);
+  if (n == 0) return HGB_OK;   // no nodes: no kernel runs (the arrays may then be NULL)
   const bool av = v_in != nullptr;
   HGB_REQUIRE(phi && s && (av ? (v_w && v_b && !v) : v != nullptr) && rowptr && nbr && epack && wf && bf && s_out && v_out,
               "painn_message_fwd: null pointer (or both v and v_in)");
-  HGB_REQUIRE(!av || (hgb_painn_message_affine_v_supported(n, f) && rec &&
+  HGB_REQUIRE(((uintptr_t)epack | (uintptr_t)rec) % 16 == 0, "painn_message_fwd: epack and rec must be 16-byte aligned");
+  // the tiled kernels store s_out / v_out and gather efilt (and out-of-tile rows) in 8-byte channel pairs
+  const bool pairs8 = (((uintptr_t)efilt | (uintptr_t)s_out | (uintptr_t)v_out) % 8) == 0;
+  HGB_REQUIRE(!av || (hgb_painn_message_affine_v_supported(n, f) && rec && pairs8 &&
                       (((uintptr_t)phi | (uintptr_t)s | (uintptr_t)rec | (uintptr_t)v_in) % 16 == 0)),
-              "painn_message_fwd: affine v needs f = 64, n >= 256, edge records and 16-byte aligned rows (n=%d f=%d)", n, f);
-  if (n == 0) return HGB_OK;
+              "painn_message_fwd: affine v needs f = 64, n >= 256, edge records and aligned rows (n=%d f=%d)", n, f);
   cudaStream_t st = (cudaStream_t)stream;
-  if (rec && f % 64 == 0 && f <= 256 && n >= 256 && (((uintptr_t)phi | (uintptr_t)v | (uintptr_t)s | (uintptr_t)rec) % 16 == 0)) {
+  if (rec && f % 64 == 0 && f <= 256 && n >= 256 && pairs8 &&
+      (((uintptr_t)phi | (uintptr_t)v | (uintptr_t)s | (uintptr_t)rec) % 16 == 0)) {
     // tiled path: two double-buffered [tn x 3f] fp32 tiles of phi and of v (affine v: of phi and of the [tn x 3] v_in)
     const size_t fixed = TWPB * 1536 + 64, row = av ? (size_t)2 * 3 * f * 4 + 2 * 12 : (size_t)4 * 3 * f * 4;
     const int step = av ? 2 * TWPB : TWPB;                     // whole nodes per warp; affine v: tile starts 16-byte aligned in v_in
@@ -449,7 +455,8 @@ extern "C" int hgb_painn_message_fwd(const float* phi, const float* s, const flo
     HGB_LAUNCH_CHECK("painn_message_fwd_tiled");
     return HGB_OK;
   }
-  const int cpl = painn_cpl(f), group = painn_group(f);
+  const int cpl = painn_cpl(f, (uintptr_t)phi | (uintptr_t)s | (uintptr_t)v | (uintptr_t)efilt | (uintptr_t)s_out | (uintptr_t)v_out);
+  const int group = painn_group(f);
   dim3 grid(hgb_grid_for(n, WPB * (32 / group), HGB_NUM_SMS * 8), (f + group * cpl - 1) / (group * cpl));
 #define LAUNCH(C, E, G, R) painn_message_fwd_kernel<C, E, G, R><<<grid, WPB * 32, 0, st>>>(phi, s, v, rowptr, perm, nbr, epack, wf, bf, efilt, n, f, r, s_out, v_out)
 #define LAUNCH_R(C, E, G) do { if (r <= 5) LAUNCH(C, E, G, 5); else LAUNCH(C, E, G, 8); } while (0)
@@ -479,7 +486,7 @@ painn_message_bwd_kernel(const float* __restrict__ gs_out, const float* __restri
                          const int32_t* __restrict__ nbr, const float* __restrict__ epack, const float* __restrict__ wf,
                          const float* __restrict__ bf, const float* __restrict__ efilt, int n, int f, int r,
                          float* __restrict__ gphi, float* __restrict__ gv, float* __restrict__ part, float* __restrict__ g_epack,
-                         float* __restrict__ g_efilt, int multi_cb) {
+                         float* __restrict__ g_efilt, int64_t ep_stride) {
   __shared__ float red[WPB * 32];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   constexpr int NPW = 32 / GROUP;
@@ -574,22 +581,13 @@ painn_message_bwd_kernel(const float* __restrict__ gs_out, const float* __restri
         e_fc = hgb_group_sum<GROUP>(e_fc, gmask);
 #pragma unroll
         for (int k = 0; k < 3; ++k) e_d[k] = hgb_group_sum<GROUP>(e_d[k], gmask);
-        if (sub == 0) {
-          float* ge = g_epack + (int64_t)e * EPK;
-          if (multi_cb) {   // several channel blocks add into the same (zero-initialised) record
+        if (sub == 0) {   // several channel blocks: this block's partial record, summed in block order by painn_epack_reduce
+          float o[EPK];
 #pragma unroll
-            for (int q = 0; q < RT; ++q) atomicAdd(ge + q, e_rb[q]);
-            atomicAdd(ge + 8, e_fc);
-#pragma unroll
-            for (int k = 0; k < 3; ++k) atomicAdd(ge + 9 + k, e_d[k]);
-          } else {
-            float o[EPK];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) o[q] = q < RT ? e_rb[q < RT ? q : 0] : 0.f;
-            o[8] = e_fc; o[9] = e_d[0]; o[10] = e_d[1]; o[11] = e_d[2];
-            float4* gp = reinterpret_cast<float4*>(ge);
-            gp[0] = make_float4(o[0], o[1], o[2], o[3]); gp[1] = make_float4(o[4], o[5], o[6], o[7]); gp[2] = make_float4(o[8], o[9], o[10], o[11]);
-          }
+          for (int q = 0; q < 8; ++q) o[q] = q < RT ? e_rb[q < RT ? q : 0] : 0.f;
+          o[8] = e_fc; o[9] = e_d[0]; o[10] = e_d[1]; o[11] = e_d[2];
+          float4* gp = reinterpret_cast<float4*>(g_epack + blockIdx.y * ep_stride + (int64_t)e * EPK);
+          gp[0] = make_float4(o[0], o[1], o[2], o[3]); gp[1] = make_float4(o[4], o[5], o[6], o[7]); gp[2] = make_float4(o[8], o[9], o[10], o[11]);
         }
       }
     }
@@ -642,7 +640,7 @@ painn_message_bwd_tiled_kernel(const float* __restrict__ gs_out, const float* __
                                const float* __restrict__ v_b, const int32_t* __restrict__ rowptr, const float* __restrict__ rec,
                                const float* __restrict__ wf, const float* __restrict__ bf, const float* __restrict__ efilt, int n,
                                int f_rt, int r, int tn, float* __restrict__ gphi, float* __restrict__ gv, float* __restrict__ part,
-                               float* __restrict__ g_epack, float* __restrict__ g_efilt, int multi_cb) {
+                               float* __restrict__ g_epack, float* __restrict__ g_efilt, int64_t ep_stride) {
   static_assert(!AV || FT == 64, "affine v: one 64-channel block");
   extern __shared__ __align__(128) uint8_t pm_smem[];
   const int f = FT ? FT : f_rt;
@@ -840,22 +838,13 @@ painn_message_bwd_tiled_kernel(const float* __restrict__ gs_out, const float* __
           e_fc = hgb_warp_sum(e_fc);
 #pragma unroll
           for (int k = 0; k < 3; ++k) e_d[k] = hgb_warp_sum(e_d[k]);
-          if (lane == 0) {
-            float* ge = g_epack + (int64_t)e * EPK;
-            if (multi_cb) {
+          if (lane == 0) {   // several channel blocks: this block's partial record, as in the SIMT kernel
+            float o[EPK];
 #pragma unroll
-              for (int q = 0; q < RT; ++q) atomicAdd(ge + q, e_rb[q]);
-              atomicAdd(ge + 8, e_fc);
-#pragma unroll
-              for (int k = 0; k < 3; ++k) atomicAdd(ge + 9 + k, e_d[k]);
-            } else {
-              float o[EPK];
-#pragma unroll
-              for (int q = 0; q < 8; ++q) o[q] = q < RT ? e_rb[q < RT ? q : 0] : 0.f;
-              o[8] = e_fc; o[9] = e_d[0]; o[10] = e_d[1]; o[11] = e_d[2];
-              float4* gp = reinterpret_cast<float4*>(ge);
-              gp[0] = make_float4(o[0], o[1], o[2], o[3]); gp[1] = make_float4(o[4], o[5], o[6], o[7]); gp[2] = make_float4(o[8], o[9], o[10], o[11]);
-            }
+            for (int q = 0; q < 8; ++q) o[q] = q < RT ? e_rb[q < RT ? q : 0] : 0.f;
+            o[8] = e_fc; o[9] = e_d[0]; o[10] = e_d[1]; o[11] = e_d[2];
+            float4* gp = reinterpret_cast<float4*>(g_epack + blockIdx.y * ep_stride + (int64_t)e * EPK);
+            gp[0] = make_float4(o[0], o[1], o[2], o[3]); gp[1] = make_float4(o[4], o[5], o[6], o[7]); gp[2] = make_float4(o[8], o[9], o[10], o[11]);
           }
         }
       }
@@ -924,35 +913,72 @@ __global__ void painn_wgrad_reduce_kernel(const float* __restrict__ part, int nb
 // narrow layers: the per-block reduction of the filter-weight gradient dominates, so fewer / longer-lived blocks
 static int painn_bwd_grid(int n, int f) { return hgb_grid_for(n, WPB * (32 / painn_group(f)), HGB_NUM_SMS * (f < 32 ? 2 : 4)); }
 
-extern "C" int64_t hgb_painn_message_bwd_workspace_bytes(int32_t n, int32_t f, int32_t r) {
-  return (int64_t)painn_bwd_grid(n, f) * 3 * f * (r + 1) * 4;
+// g_epack of a launch with several channel blocks: block y stores its partial record in epart[y][e][12] and this kernel sums
+// them in block order (one float4 per thread), so the result does not depend on which block finishes first
+__global__ void painn_epack_reduce_kernel(const float4* __restrict__ epart, int ncb, int64_t e, float4* __restrict__ g_epack) {
+  const int64_t m = e * (EPK / 4);
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += (int64_t)gridDim.x * blockDim.x) {
+    float4 a = epart[t];
+    for (int y = 1; y < ncb; ++y) {
+      const float4 b = epart[y * m + t];
+      a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+    }
+    g_epack[t] = a;
+  }
+}
+
+// workspace: part[grid][3f][r+1] (column r holds the bias gradient), then, 16-byte aligned, room for the partial edge records
+// of up to ceil(f / group) channel blocks (CPL = 1, the most any launch uses)
+static int64_t painn_part_bytes(int32_t n, int32_t f, int32_t r) {
+  return (((int64_t)painn_bwd_grid(n, f) * 3 * f * (r + 1) * 4) + 15) & ~(int64_t)15;
+}
+
+extern "C" int64_t hgb_painn_message_bwd_workspace_bytes(int32_t n, int32_t f, int32_t r, int64_t e) {
+  const int64_t ncb = (f + painn_group(f) - 1) / painn_group(f);
+  return painn_part_bytes(n, f, r) + (ncb > 1 ? ncb * e * EPK * 4 : 0);
 }
 
 extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, const float* phi, const float* v, const float* v_in,
                                      const float* v_w, const float* v_b, const int32_t* rowptr_src, const int32_t* perm_src,
                                      const int32_t* nbr_agg, const float* epack, const float* rec, const float* wf, const float* bf,
-                                     const float* efilt, int32_t n, int32_t f, int32_t r, float* gphi, float* gv, float* gwf, float* gbf,
-                                     float* g_epack, float* g_efilt, void* workspace, int64_t workspace_bytes, hgb_stream_t stream) {
-  HGB_REQUIRE(n >= 0 && f > 0 && r > 0 && r <= RMAX, "painn_message_bwd: need 0 < num_radial <= %d (got %d)", RMAX, r);
-  const bool av = v_in != nullptr;
-  HGB_REQUIRE(gs_out && gv_out && phi && (av ? (v_w && v_b && !v) : v != nullptr) && rowptr_src && nbr_agg && epack && wf && bf &&
-              gphi && gv && gwf && gbf && workspace,
-              "painn_message_bwd: null pointer (or both v and v_in)");
-  HGB_REQUIRE(!av || (hgb_painn_message_affine_v_supported(n, f) && rec &&
-                      (((uintptr_t)gs_out | (uintptr_t)gv_out | (uintptr_t)phi | (uintptr_t)rec) % 16 == 0)),
-              "painn_message_bwd: affine v needs f = 64, n >= 256, edge records and 16-byte aligned rows (n=%d f=%d)", n, f);
-  const bool need_edge = g_epack != nullptr;
-  HGB_REQUIRE((efilt != nullptr) == (g_efilt != nullptr), "painn_message_bwd: g_efilt iff efilt");
-  HGB_REQUIRE(workspace_bytes >= hgb_painn_message_bwd_workspace_bytes(n, f, r), "painn_message_bwd: workspace too small");
+                                     const float* efilt, int32_t n, int32_t f, int32_t r, int64_t e, float* gphi, float* gv, float* gwf,
+                                     float* gbf, float* g_epack, float* g_efilt, void* workspace, int64_t workspace_bytes,
+                                     hgb_stream_t stream) {
+  HGB_REQUIRE(n >= 0 && e >= 0 && f > 0 && r > 0 && r <= RMAX, "painn_message_bwd: need 0 < num_radial <= %d (got %d)", RMAX, r);
   cudaStream_t st = (cudaStream_t)stream;
   const int f3 = 3 * f;
-  if (n == 0) {
+  if (n == 0) {   // no nodes: no kernel runs, the filter gradients are zero
+    HGB_REQUIRE(gwf && gbf, "painn_message_bwd: null pointer");
     cudaMemsetAsync(gwf, 0, (size_t)f3 * r * 4, st);
     cudaMemsetAsync(gbf, 0, (size_t)f3 * 4, st);
     return HGB_OK;
   }
+  const bool av = v_in != nullptr;
+  HGB_REQUIRE(gs_out && gv_out && phi && (av ? (v_w && v_b && !v) : v != nullptr) && rowptr_src && nbr_agg && epack && wf && bf &&
+              gphi && gv && gwf && gbf && workspace,
+              "painn_message_bwd: null pointer (or both v and v_in)");
+  HGB_REQUIRE(((uintptr_t)epack | (uintptr_t)rec | (uintptr_t)g_epack | (uintptr_t)workspace) % 16 == 0,
+              "painn_message_bwd: epack, rec, g_epack and the workspace must be 16-byte aligned");
+  // the tiled kernels store gphi / gv and gather efilt (and out-of-tile rows) in 8-byte channel pairs
+  const bool pairs8 = (((uintptr_t)efilt | (uintptr_t)gphi | (uintptr_t)gv) % 8) == 0;
+  HGB_REQUIRE(!av || (hgb_painn_message_affine_v_supported(n, f) && rec && pairs8 &&
+                      (((uintptr_t)gs_out | (uintptr_t)gv_out | (uintptr_t)phi | (uintptr_t)rec) % 16 == 0)),
+              "painn_message_bwd: affine v needs f = 64, n >= 256, edge records and aligned rows (n=%d f=%d)", n, f);
+  const bool need_edge = g_epack != nullptr;
+  HGB_REQUIRE((efilt != nullptr) == (g_efilt != nullptr), "painn_message_bwd: g_efilt iff efilt");
+  HGB_REQUIRE(workspace_bytes >= hgb_painn_message_bwd_workspace_bytes(n, f, r, e), "painn_message_bwd: workspace too small");
   float* part = (float*)workspace;
-  if (rec && f % 64 == 0 && f <= 256 && n >= 256 && (((uintptr_t)gs_out | (uintptr_t)gv_out | (uintptr_t)phi | (uintptr_t)v | (uintptr_t)rec) % 16 == 0)) {
+  float* epart = (float*)((char*)workspace + painn_part_bytes(n, f, r));
+  // g_epack: stored directly by a single channel block, else per-block partial records in the workspace reduced in block order
+  auto edge_out = [&](int ncb) { return ncb > 1 ? epart : g_epack; };
+  auto edge_stride = [&](int ncb) { return ncb > 1 ? e * EPK : (int64_t)0; };
+  auto reduce_edges = [&](int ncb) {   // true when it launched
+    if (!need_edge || ncb == 1 || e == 0) return false;
+    painn_epack_reduce_kernel<<<hgb_grid_for(e * (EPK / 4), 256), 256, 0, st>>>((const float4*)epart, ncb, e, (float4*)g_epack);
+    return true;
+  };
+  if (rec && f % 64 == 0 && f <= 256 && n >= 256 && pairs8 &&
+      (((uintptr_t)gs_out | (uintptr_t)gv_out | (uintptr_t)phi | (uintptr_t)v | (uintptr_t)rec) % 16 == 0)) {
     // two double-buffered [tn x 4f] fp32 tiles + per-warp scratch; two blocks per SM
     const size_t fixed = 32 + WPB * 32 * 4 + WPB * 4096;
     int tn = (int)((110 * 1024 - fixed) / ((size_t)2 * 4 * f * 4));
@@ -976,7 +1002,9 @@ extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, c
     if (gx > 2 * HGB_NUM_SMS) gx = 2 * HGB_NUM_SMS;
     const int ncb2 = f / 64;
     dim3 grid2(gx, ncb2);
-#define LAUNCH_F(E, G, R, F, A) painn_message_bwd_tiled_kernel<E, G, R, F, A><<<grid2, WPB * 32, smem, st>>>(gs_out, gv_out, phi, v, v_in, v_w, v_b, rowptr_src, rec, wf, bf, efilt, n, f, r, tn, gphi, gv, part, g_epack, g_efilt, ncb2 > 1)
+    float* ge = edge_out(ncb2);
+    const int64_t ges = edge_stride(ncb2);
+#define LAUNCH_F(E, G, R, F, A) painn_message_bwd_tiled_kernel<E, G, R, F, A><<<grid2, WPB * 32, smem, st>>>(gs_out, gv_out, phi, v, v_in, v_w, v_b, rowptr_src, rec, wf, bf, efilt, n, f, r, tn, gphi, gv, part, ge, g_efilt, ges)
 #define LAUNCH_T(E, G, R) do { if (av) LAUNCH_F(E, G, R, 64, true); else if (f == 64) LAUNCH_F(E, G, R, 64, false); else LAUNCH_F(E, G, R, 0, false); } while (0)
 #define LAUNCH_TR(E, G) do { if (r <= 5) LAUNCH_T(E, G, 5); else LAUNCH_T(E, G, 8); } while (0)
     if (efilt) { if (need_edge) LAUNCH_TR(true, true); else LAUNCH_TR(true, false); }
@@ -984,14 +1012,19 @@ extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, c
 #undef LAUNCH_TR
 #undef LAUNCH_T
     HGB_LAUNCH_CHECK("painn_message_bwd_tiled");
+    if (reduce_edges(ncb2)) HGB_LAUNCH_CHECK("painn_epack_reduce");
     painn_wgrad_reduce_kernel<<<(f3 * (r + 1) + 31) / 32, dim3(32, 8), 0, st>>>(part, gx, f3, r, gwf, gbf);
     HGB_LAUNCH_CHECK("painn_wgrad_reduce");
     return HGB_OK;
   }
-  const int cpl = painn_cpl(f), group = painn_group(f);
+  const int cpl = painn_cpl(f, (uintptr_t)gs_out | (uintptr_t)gv_out | (uintptr_t)phi | (uintptr_t)v | (uintptr_t)efilt |
+                                   (uintptr_t)gphi | (uintptr_t)gv);
+  const int group = painn_group(f);
   const int ncb = (f + group * cpl - 1) / (group * cpl);
   dim3 grid(painn_bwd_grid(n, f), ncb);
-#define LAUNCH(C, E, G, W, R) painn_message_bwd_kernel<C, E, G, W, R><<<grid, WPB * 32, 0, st>>>(gs_out, gv_out, phi, v, rowptr_src, perm_src, nbr_agg, epack, wf, bf, efilt, n, f, r, gphi, gv, part, g_epack, g_efilt, ncb > 1)
+  float* ge = edge_out(ncb);
+  const int64_t ges = edge_stride(ncb);
+#define LAUNCH(C, E, G, W, R) painn_message_bwd_kernel<C, E, G, W, R><<<grid, WPB * 32, 0, st>>>(gs_out, gv_out, phi, v, rowptr_src, perm_src, nbr_agg, epack, wf, bf, efilt, n, f, r, gphi, gv, part, ge, g_efilt, ges)
 #define LAUNCH_R(C, E, G, W) do { if (r <= 5) LAUNCH(C, E, G, W, 5); else LAUNCH(C, E, G, W, 8); } while (0)
 #define LAUNCH_G(E, G)                                                           \
   switch (group) {                                                               \
@@ -1008,6 +1041,7 @@ extern "C" int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, c
 #undef LAUNCH_R
 #undef LAUNCH
   HGB_LAUNCH_CHECK("painn_message_bwd");
+  if (reduce_edges(ncb)) HGB_LAUNCH_CHECK("painn_epack_reduce");
   painn_wgrad_reduce_kernel<<<(f3 * (r + 1) + 31) / 32, dim3(32, 8), 0, st>>>(part, grid.x, f3, r, gwf, gbf);
   HGB_LAUNCH_CHECK("painn_wgrad_reduce");
   return HGB_OK;

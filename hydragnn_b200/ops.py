@@ -742,7 +742,8 @@ def mlp2(x, w1, b1, act1, p1, w2, b2, act2=None, p2=0.0):
 
 class EdgeGeomFn(torch.autograd.Function):
     """(vec, len, unit) of hydragnn/utils/model/operations.py:21-36 in one pass; the backward turns the
-    three edge gradients into one [E,3] vector and scatters it to both endpoints with segment sums."""
+    three edge gradients into one [E,3] vector and scatters it to both endpoints with segment sums.  Without edges no
+    kernel runs."""
 
     @staticmethod
     def forward(ctx, pos, shifts, plan, eps):
@@ -751,8 +752,9 @@ class EdgeGeomFn(torch.autograd.Function):
         vec = torch.empty(e, 3, dtype=pos.dtype, device=pos.device)
         ln = torch.empty(e, 1, dtype=pos.dtype, device=pos.device)
         unit = torch.empty(e, 3, dtype=pos.dtype, device=pos.device)
-        _lib.call("hgb_edge_geom_fwd", _p(pos), _p(plan.row), _p(plan.col), _p(_chk(shifts)), e, float(eps), _p(vec), _p(ln),
-                  _p(unit), _stream())
+        if e > 0:
+            _lib.call("hgb_edge_geom_fwd", _p(pos), _p(plan.row), _p(plan.col), _p(_chk(shifts)), e, float(eps), _p(vec), _p(ln),
+                      _p(unit), _stream())
         ctx.save_for_backward(vec, ln)
         ctx.plan, ctx.eps = plan, float(eps)
         return vec, ln, unit
@@ -763,9 +765,12 @@ class EdgeGeomFn(torch.autograd.Function):
         vec, ln = ctx.saved_tensors
         plan = ctx.plan
         gv = torch.empty_like(vec)
+        g_pos = g_shift = None
+        if plan.num_edges == 0:
+            return (vec.new_zeros(plan.num_nodes, 3) if ctx.needs_input_grad[0] else None), \
+                (gv if ctx.needs_input_grad[1] else None), None, None
         _lib.call("hgb_edge_geom_bwd", _p(vec), _p(ln), ctx.eps, _p(_chk(g_vec)), _p(_chk(g_len)), _p(_chk(g_unit)),
                   plan.num_edges, _p(gv), _stream())
-        g_pos = g_shift = None
         if ctx.needs_input_grad[0]:
             # vec = pos[col] - pos[row] + shift
             g_pos = raw_segment_sum(gv, plan.by_col.rowptr, plan.by_col.perm, plan.num_nodes) - \
@@ -777,13 +782,14 @@ class EdgeGeomFn(torch.autograd.Function):
 
 class PainnEdgeEmbedFn(torch.autograd.Function):
     """len/unit -> one 12-float record per edge {rbf*cutoff (8, zero padded), cutoff, dir = unit/len [quirk Q2]}
-    (hydragnn/models/PAINNStack.py:239-242,257)."""
+    (hydragnn/models/PAINNStack.py:239-242,257).  Without edges no kernel runs."""
 
     @staticmethod
     def forward(ctx, unit, ln, num_radial, cutoff):
         e = unit.shape[0]
         epack = torch.empty(e, 12, dtype=unit.dtype, device=unit.device)
-        _lib.call("hgb_painn_edge_embed_fwd", _p(unit), _p(ln), e, num_radial, float(cutoff), _p(epack), _stream())
+        if e > 0:
+            _lib.call("hgb_painn_edge_embed_fwd", _p(unit), _p(ln), e, num_radial, float(cutoff), _p(epack), _stream())
         ctx.save_for_backward(unit, ln)
         ctx.r, ctx.cutoff = num_radial, float(cutoff)
         return epack
@@ -795,7 +801,8 @@ class PainnEdgeEmbedFn(torch.autograd.Function):
         e = unit.shape[0]
         g_unit = torch.empty_like(unit)
         g_len = torch.empty_like(ln)
-        _lib.call("hgb_painn_edge_embed_bwd", _p(unit), _p(ln), _p(_chk(g_epack)), e, ctx.r, ctx.cutoff, _p(g_unit), _p(g_len), _stream())
+        if e > 0:
+            _lib.call("hgb_painn_edge_embed_bwd", _p(unit), _p(ln), _p(_chk(g_epack)), e, ctx.r, ctx.cutoff, _p(g_unit), _p(g_len), _stream())
         return g_unit, g_len, None, None
 
 
@@ -820,7 +827,7 @@ def painn_affine_v_ok(v, s, rec_row):
 class PainnMessageFn(torch.autograd.Function):
     """Fused PaiNN message (hydragnn/models/PAINNStack.py:239-270): returns (s + ds, v + dv).  The input v is either a
     [n, 3, f] tensor (``v0 = vw = vb = None``) or, with ``v = None``, the affine v0 [n, 3, 1], vw [f, 1], vb [f] of an
-    ``AffineV`` (``painn_affine_v_ok``)."""
+    ``AffineV`` (``painn_affine_v_ok``).  Without nodes or edges no kernel runs: s and v pass through unchanged."""
 
     @staticmethod
     def forward(ctx, phi, s, v, epack, wf, bf, efilt, plan, rec_row=None, v0=None, vw=None, vb=None):
@@ -830,15 +837,18 @@ class PainnMessageFn(torch.autograd.Function):
         av = v0 is not None
         if av:
             v, v0, vw, vb = None, _chk(v0), _chk(vw), _chk(vb)
-            v_out = torch.empty(n, 3, f, dtype=s.dtype, device=s.device)
         else:
             v = _chk(v)
-            v_out = torch.empty_like(v)
-        s_out = torch.empty_like(s)
         agg = plan.by_row     # messages are summed into edge[:,0] = edge_index[0]
-        _lib.call("hgb_painn_message_fwd", _p(phi), _p(s), _p(v), _p(v0), _p(vw), _p(vb), _p(agg.rowptr), _p(agg.perm),
-                  _p(plan.nbr("row")), _p(epack), _p(rec_row), _p(_chk(wf)), _p(_chk(bf)), _p(_chk(efilt)), n, f, r, _p(s_out),
-                  _p(v_out), _stream())
+        if n == 0 or plan.num_edges == 0:
+            s_out = s.clone()
+            v_out = linear_act(v0, vw, vb) if av else v.clone()
+        else:
+            s_out = torch.empty_like(s)
+            v_out = torch.empty(n, 3, f, dtype=s.dtype, device=s.device)
+            _lib.call("hgb_painn_message_fwd", _p(phi), _p(s), _p(v), _p(v0), _p(vw), _p(vb), _p(agg.rowptr), _p(agg.perm),
+                      _p(plan.nbr("row")), _p(epack), _p(rec_row), _p(_chk(wf)), _p(_chk(bf)), _p(_chk(efilt)), n, f, r, _p(s_out),
+                      _p(v_out), _stream())
         ctx.save_for_backward(phi, v, epack, wf, bf, efilt, v0, vw, vb)
         ctx.plan, ctx.use_rec = plan, rec_row is not None
         return s_out, v_out
@@ -852,15 +862,18 @@ class PainnMessageFn(torch.autograd.Function):
         r = wf.shape[1]
         gs_out, gv_out = _chk(gs_out), _chk(gv_out)
         need_edge = ctx.needs_input_grad[3]
-        av = v0 is not None
+        e = plan.num_edges
+        if n == 0 or e == 0:
+            g_epack = torch.zeros_like(epack) if need_edge else None
+            g_ef = torch.zeros_like(efilt) if efilt is not None else None
+            return PainnMessageFn._grads(ctx, torch.zeros_like(phi), gs_out, gv_out, g_epack, torch.zeros_like(wf),
+                                         torch.zeros_like(bf), g_ef, v0, vw)
         gphi = torch.empty_like(phi)
         gv = torch.empty(n, 3, f, dtype=phi.dtype, device=phi.device)
         gwf, gbf = torch.empty_like(wf), torch.empty_like(bf)
-        cpl = 2 if (f >= 64 and f % 2 == 0) else 1          # mirrors painn_cpl / painn_group in csrc/hgb_painn.cu
-        multi = f > 32 * cpl                                # several channel blocks accumulate into g_epack
-        g_epack = (torch.zeros_like(epack) if multi else torch.empty_like(epack)) if need_edge else None
+        g_epack = torch.empty_like(epack) if need_edge else None
         g_ef = torch.empty_like(efilt) if efilt is not None else None
-        nbytes = _lib.query("hgb_painn_message_bwd_workspace_bytes", n, f, r)
+        nbytes = _lib.query("hgb_painn_message_bwd_workspace_bytes", n, f, r, e)
         ws = _ws(nbytes, phi.device)
         src = plan.by_col     # the gather side: edge[:,1] = edge_index[1]
         rec_col = None
@@ -872,9 +885,14 @@ class PainnMessageFn(torch.autograd.Function):
                 cache[key] = painn_edge_records(epack, plan, "col")
             rec_col = cache[key]
         _lib.call("hgb_painn_message_bwd", _p(gs_out), _p(gv_out), _p(phi), _p(v), _p(v0), _p(vw), _p(vb), _p(src.rowptr),
-                  _p(src.perm), _p(plan.nbr("col")), _p(epack), _p(rec_col), _p(wf), _p(bf), _p(efilt), n, f, r, _p(gphi), _p(gv),
-                  _p(gwf), _p(gbf), _p(g_epack), _p(g_ef), _p(ws), nbytes, _stream())
-        if not av:
+                  _p(src.perm), _p(plan.nbr("col")), _p(epack), _p(rec_col), _p(wf), _p(bf), _p(efilt), n, f, r, e, _p(gphi),
+                  _p(gv), _p(gwf), _p(gbf), _p(g_epack), _p(g_ef), _p(ws), nbytes, _stream())
+        return PainnMessageFn._grads(ctx, gphi, gs_out, gv, g_epack, gwf, gbf, g_ef, v0, vw)
+
+    @staticmethod
+    def _grads(ctx, gphi, gs_out, gv, g_epack, gwf, gbf, g_ef, v0, vw):
+        n, f = gs_out.shape
+        if v0 is None:
             return gphi, gs_out, gv, g_epack, gwf, gbf, g_ef, None, None, None, None, None
         # v = Linear(1, f)(v0): the same small-k backward LinearAct runs on a stored v, so all three gradients keep its bits
         g_v0, g_vw, g_vb = raw_smallk_bwd(gv.reshape(3 * n, f), None, None, v0.reshape(3 * n, 1), vw, 0, 0.0,

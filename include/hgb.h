@@ -241,7 +241,8 @@ int64_t hgb_colsum_workspace_bytes(int32_t m, int32_t n);
  * hydragnn/models/PAINNStack.py:331-352)
  * ------------------------------------------------------------------------------------------ */
 
-/* vec = pos[col] - pos[row] + shift; len = |vec|; unit = vec / (len + eps).  Any output may be NULL. */
+/* vec = pos[col] - pos[row] + shift; len = |vec|; unit = vec / (len + eps).  Any output may be NULL; with e = 0
+ * nothing runs and every pointer may be NULL (as for the backward and the PaiNN embedding below).        */
 int hgb_edge_geom_fwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts,
                       int64_t e, float eps, float* vec, float* len, float* unit, hgb_stream_t stream);
 /* g_vec = g_vec_in + g_len * vec/len + d(unit)/d(vec)^T g_unit   (NULL gradients are zero).       */
@@ -249,7 +250,7 @@ int hgb_edge_geom_bwd(const float* vec, const float* len, float eps, const float
                       const float* g_len, const float* g_unit, int64_t e, float* g_vec,
                       hgb_stream_t stream);
 /* PaiNN edge embedding: one 48-byte record per edge, epack [e,12] = { sin(n pi d/rc)/d * fcut(d) for n = 1..r
- * (zero padded to 8), fcut(d), dir = unit/len (quirk Q2, PAINNStack.py:257) }.  r <= 8.                     */
+ * (zero padded to 8), fcut(d), dir = unit/len (quirk Q2, PAINNStack.py:257) }.  0 < r <= 8; epack 16-byte aligned. */
 int hgb_painn_edge_embed_fwd(const float* unit, const float* len, int64_t e, int32_t r, float cutoff,
                              float* epack, hgb_stream_t stream);
 /* backward of the above: g_epack [e,12] -> (g_unit [e,3], g_len [e])                                       */
@@ -269,7 +270,9 @@ int hgb_painn_edge_embed_bwd(const float* unit, const float* len, const float* g
  * phi [n,3f], s [n,f], v [n,3,f], wf [3f,r], bf [3f], efilt [e,3f] or NULL.
  * Affine v: with v = NULL and v_in [n,3], v_w [f], v_b [f] set, v[i,k,c] = fmaf(v_in[i,k], v_w[c], v_b[c]) (a
  * Linear(1, f) of a [n,3,1] tensor, PaiNN's first vec_embed_out) is formed on chip and never stored; only when
- * hgb_painn_message_affine_v_supported(n, f), `rec` is given and phi, s, rec, v_in are 16-byte aligned.       */
+ * hgb_painn_message_affine_v_supported(n, f), `rec` is given and phi, s, rec, v_in are 16-byte aligned.
+ * epack and rec are 16-byte aligned; with n = 0 nothing runs.  Rows that are not 8-byte aligned take the narrower
+ * one-channel-per-lane kernels.                                                                                 */
 int hgb_painn_message_fwd(const float* phi, const float* s, const float* v, const float* v_in, const float* v_w,
                           const float* v_b, const int32_t* rowptr, const int32_t* perm, const int32_t* nbr,
                           const float* epack, const float* rec, const float* wf, const float* bf, const float* efilt,
@@ -285,17 +288,20 @@ int hgb_painn_edge_records(const float* epack, const int32_t* perm, const int32_
 /* Backward of the fused message, as a segmented reduction over the CSR of edge[:,1] (the gather side);
  * nbr_agg [e] = edge[:,0] of every slot of that CSR.  gs_out [n,f], gv_out [n,3,f] are the incoming gradients.
  * Outputs: gphi [n,3f]; gv [n,3,f] (= gv_out + gathered part; gs_in == gs_out is the caller's); gwf [3f,r],
- * gbf [3f] (via workspace partials); optional g_epack [e,12] (zero-initialised by the caller when f > 64) and
- * g_efilt [e,3f] (iff efilt).  `rec` (optional): by-col CSR edge records -> shared-memory-tiled kernel.
+ * gbf [3f] (via workspace partials); optional g_epack [e,12] (16-byte aligned, every column written, 0 from r to 7;
+ * when several channel blocks share an edge their partial records go to the workspace and are summed in block
+ * order) and g_efilt [e,3f] (iff efilt).  `rec` (optional): by-col CSR edge records -> shared-memory-tiled kernel.
+ * With n = 0 only gwf = gbf = 0 are written.
  * Affine v (v = NULL, v_in / v_w / v_b as in the forward): v is formed on chip, gv is written as usual; the caller
  * reduces gv to the gradients of v_in, v_w, v_b with hgb_linear_smallk_bwd, as for a stored Linear(1, f) output.  */
 int hgb_painn_message_bwd(const float* gs_out, const float* gv_out, const float* phi, const float* v, const float* v_in,
                           const float* v_w, const float* v_b, const int32_t* rowptr_src, const int32_t* perm_src,
                           const int32_t* nbr_agg, const float* epack, const float* rec, const float* wf, const float* bf,
-                          const float* efilt, int32_t n, int32_t f, int32_t r, float* gphi, float* gv, float* gwf,
-                          float* gbf, float* g_epack, float* g_efilt, void* workspace, int64_t workspace_bytes,
-                          hgb_stream_t stream);
-int64_t hgb_painn_message_bwd_workspace_bytes(int32_t n, int32_t f, int32_t r);
+                          const float* efilt, int32_t n, int32_t f, int32_t r, int64_t e, float* gphi, float* gv,
+                          float* gwf, float* gbf, float* g_epack, float* g_efilt, void* workspace,
+                          int64_t workspace_bytes, hgb_stream_t stream);
+/* 16-byte aligned workspace of hgb_painn_message_bwd for n nodes and e edges                                   */
+int64_t hgb_painn_message_bwd_workspace_bytes(int32_t n, int32_t f, int32_t r, int64_t e);
 
 /* Update block glue (PAINNStack.py:298-328).  uv, vv are update_U(v), update_V(v) as [3n, f] matrices with row
  * stride `ld` (ld = f: two separate tensors; ld = 2f: the two halves of ONE [3n, 2f] matrix produced by a single
