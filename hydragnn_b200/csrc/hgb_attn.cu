@@ -192,9 +192,14 @@ __global__ void __launch_bounds__(ATT_TQ) mha_bwd_kv_kernel(const float* __restr
     default: hgb_set_error("mha: head_dim %d not supported (1,2,4,8,16,32)", d); return HGB_EINVAL; \
   }
 
+static bool mha_head_dim_ok(int d) { return d == 1 || d == 2 || d == 4 || d == 8 || d == 16 || d == 32; }
+
+// Sizes are checked first, pointers only when there is a row: the data pointer of an empty tensor may be NULL.
 extern "C" int hgb_mha_fwd(const float* qkv, int32_t n, int32_t f, int32_t heads, float* out, float* lse, hgb_stream_t stream) {
-  HGB_REQUIRE(qkv && out && lse && n >= 0 && heads > 0 && f % heads == 0, "mha_fwd: bad arguments");
+  HGB_REQUIRE(n >= 0 && heads > 0 && f % heads == 0 && mha_head_dim_ok(f / heads),
+              "mha_fwd: bad sizes (n %d, f %d, heads %d; head_dim must be 1, 2, 4, 8, 16 or 32)", n, f, heads);
   if (n == 0) return HGB_OK;
+  HGB_REQUIRE(qkv && out && lse, "mha_fwd: NULL pointer");
   const int d = f / heads;
   const float scale = 1.f / sqrtf((float)d);
   dim3 grid((n + ATT_QPB - 1) / ATT_QPB, heads);
@@ -206,8 +211,10 @@ extern "C" int hgb_mha_fwd(const float* qkv, int32_t n, int32_t f, int32_t heads
 
 extern "C" int hgb_mha_bwd(const float* qkv, const float* out, const float* lse, const float* gout, int32_t n, int32_t f,
                            int32_t heads, float* gqkv, hgb_stream_t stream) {
-  HGB_REQUIRE(qkv && out && lse && gout && gqkv && n >= 0 && heads > 0 && f % heads == 0, "mha_bwd: bad arguments");
+  HGB_REQUIRE(n >= 0 && heads > 0 && f % heads == 0 && mha_head_dim_ok(f / heads),
+              "mha_bwd: bad sizes (n %d, f %d, heads %d; head_dim must be 1, 2, 4, 8, 16 or 32)", n, f, heads);
   if (n == 0) return HGB_OK;
+  HGB_REQUIRE(qkv && out && lse && gout && gqkv, "mha_bwd: NULL pointer");
   const int d = f / heads;
   const float scale = 1.f / sqrtf((float)d);
   dim3 grid((n + ATT_QPB - 1) / ATT_QPB, heads);

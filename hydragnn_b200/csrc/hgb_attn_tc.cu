@@ -238,7 +238,10 @@ __global__ void __launch_bounds__(WARPS * 32) mha_tc_bwd_q_kernel(const float* _
   if (rb < n) *reinterpret_cast<float2*>(gqkv + (int64_t)rb * f3 + h * D + 2 * t) = make_float2(dq[2] * scale, dq[3] * scale);
 }
 
-// dK, dV: a warp owns 16 key rows and walks every query
+// dK, dV: a warp owns 16 key rows and walks every query.  Q is staged with the forward's base-2 scale, so S^T is built from the
+// same split operands as the forward's S and P = exp2(s - lse log2 e) matches the forward's p to a few ulp of the score; Q
+// staged with 1/sqrt(d) alone would round differently and, at the TF32 split, shift p by ~2^-11 |s| (15 % at |s| = 600).
+// dK = dS^T Q / sqrt(d) is then the accumulated dS^T (Q scale log2 e) times ln 2.
 template <int SPLIT>
 __global__ void __launch_bounds__(WARPS * 32) mha_tc_bwd_kv_kernel(const float* __restrict__ qkv, const float* __restrict__ lse,
                                                                    const float* __restrict__ delta, const float* __restrict__ gout,
@@ -257,7 +260,7 @@ __global__ void __launch_bounds__(WARPS * 32) mha_tc_bwd_kv_kernel(const float* 
   float dk[4] = {0.f, 0.f, 0.f, 0.f}, dv[4] = {0.f, 0.f, 0.f, 0.f};
   for (int i0 = 0; i0 < n; i0 += CH) {
     __syncthreads();
-    stage<SPLIT>(sq, qkv, f3, h * D, i0, n, scale);
+    stage<SPLIT>(sq, qkv, f3, h * D, i0, n, scale * LOG2E);
     stage<SPLIT>(sg, gout, f, h * D, i0, n, 1.f);
     for (int i = threadIdx.x; i < CH; i += WARPS * 32) {
       sl[i] = i0 + i < n ? lse[(int64_t)(i0 + i) * nh + h] * LOG2E : 0.f;
@@ -266,7 +269,7 @@ __global__ void __launch_bounds__(WARPS * 32) mha_tc_bwd_kv_kernel(const float* 
     __syncthreads();
 #pragma unroll
     for (int qb = 0; qb < CH / 8; ++qb) {
-      float st[4] = {0.f, 0.f, 0.f, 0.f}, dpt[4] = {0.f, 0.f, 0.f, 0.f};      // S^T, dP^T: rows = keys, cols = queries
+      float st[4] = {0.f, 0.f, 0.f, 0.f}, dpt[4] = {0.f, 0.f, 0.f, 0.f};      // S^T (base 2), dP^T: rows = keys, cols = queries
       mma_sm<SPLIT>(st, kh, kl, sq, (qb * 8 + g) * RS + t, (qb * 8 + g) * RS + t + 4);
       mma_sm<SPLIT>(dpt, vh, vl, sg, (qb * 8 + g) * RS + t, (qb * 8 + g) * RS + t + 4);
       const int qi = qb * 8 + 2 * t;
@@ -274,8 +277,8 @@ __global__ void __launch_bounds__(WARPS * 32) mha_tc_bwd_kv_kernel(const float* 
       const float lq0 = sl[qi], lq1 = sl[qi + 1], dq0 = sd[qi], dq1 = sd[qi + 1];
       float p[4], ds[4], ph[4], pl[4], dsh[4], dsl[4];
       // permuted A order: (key g, query 2t), (key g+8, query 2t), (key g, query 2t+1), (key g+8, query 2t+1)
-      p[0] = v0 ? exp2f(fmaf(st[0], LOG2E, -lq0)) : 0.f; p[1] = v0 ? exp2f(fmaf(st[2], LOG2E, -lq0)) : 0.f;
-      p[2] = v1 ? exp2f(fmaf(st[1], LOG2E, -lq1)) : 0.f; p[3] = v1 ? exp2f(fmaf(st[3], LOG2E, -lq1)) : 0.f;
+      p[0] = v0 ? exp2f(st[0] - lq0) : 0.f; p[1] = v0 ? exp2f(st[2] - lq0) : 0.f;
+      p[2] = v1 ? exp2f(st[1] - lq1) : 0.f; p[3] = v1 ? exp2f(st[3] - lq1) : 0.f;
       ds[0] = p[0] * (dpt[0] - dq0); ds[1] = p[1] * (dpt[2] - dq0);
       ds[2] = p[2] * (dpt[1] - dq1); ds[3] = p[3] * (dpt[3] - dq1);
       split4<SPLIT>(p, ph, pl);
@@ -285,11 +288,11 @@ __global__ void __launch_bounds__(WARPS * 32) mha_tc_bwd_kv_kernel(const float* 
     }
   }
   if (ra < n) {
-    *reinterpret_cast<float2*>(gqkv + (int64_t)ra * f3 + f + h * D + 2 * t) = make_float2(dk[0], dk[1]);
+    *reinterpret_cast<float2*>(gqkv + (int64_t)ra * f3 + f + h * D + 2 * t) = make_float2(dk[0] * LN2, dk[1] * LN2);
     *reinterpret_cast<float2*>(gqkv + (int64_t)ra * f3 + 2 * f + h * D + 2 * t) = make_float2(dv[0], dv[1]);
   }
   if (rb < n) {
-    *reinterpret_cast<float2*>(gqkv + (int64_t)rb * f3 + f + h * D + 2 * t) = make_float2(dk[2], dk[3]);
+    *reinterpret_cast<float2*>(gqkv + (int64_t)rb * f3 + f + h * D + 2 * t) = make_float2(dk[2] * LN2, dk[3] * LN2);
     *reinterpret_cast<float2*>(gqkv + (int64_t)rb * f3 + 2 * f + h * D + 2 * t) = make_float2(dv[2], dv[3]);
   }
 }
@@ -300,10 +303,18 @@ extern "C" int32_t hgb_mha_tc_supported(int32_t f, int32_t heads) {
   return (heads > 0 && f % heads == 0 && f / heads == D && f % 4 == 0) ? 1 : 0;
 }
 
+static bool aligned(const void* p, uintptr_t bytes) { return ((uintptr_t)p & (bytes - 1)) == 0; }
+
+// Sizes are checked first, pointers only when there is a row: the data pointer of an empty tensor may be NULL.  Rows are read
+// with float4 loads (stage, delta) and written with float2 stores; the row strides 3f and f are multiples of 4 floats, so the
+// base pointers decide the alignment.
 extern "C" int hgb_mha_tc_fwd(const float* qkv, int32_t n, int32_t f, int32_t heads, int32_t exact, float* out, float* lse,
                               hgb_stream_t stream) {
-  HGB_REQUIRE(qkv && out && lse && n >= 0 && hgb_mha_tc_supported(f, heads), "mha_tc_fwd: bad arguments (head_dim must be 8)");
+  HGB_REQUIRE(n >= 0 && hgb_mha_tc_supported(f, heads), "mha_tc_fwd: bad sizes (n %d, f %d, heads %d; head_dim must be 8)",
+              n, f, heads);
   if (n == 0) return HGB_OK;
+  HGB_REQUIRE(qkv && out && lse, "mha_tc_fwd: NULL pointer");
+  HGB_REQUIRE(aligned(qkv, 16) && aligned(out, 8), "mha_tc_fwd: qkv must be 16-byte and out 8-byte aligned");
   const float scale = 1.f / sqrtf((float)D);
   dim3 grid((n + ROWS - 1) / ROWS, heads);
   cudaStream_t st = (cudaStream_t)stream;
@@ -315,9 +326,12 @@ extern "C" int hgb_mha_tc_fwd(const float* qkv, int32_t n, int32_t f, int32_t he
 
 extern "C" int hgb_mha_tc_bwd(const float* qkv, const float* out, const float* lse, const float* gout, int32_t n, int32_t f,
                               int32_t heads, int32_t exact, float* delta_ws, float* gqkv, hgb_stream_t stream) {
-  HGB_REQUIRE(qkv && out && lse && gout && gqkv && delta_ws && n >= 0 && hgb_mha_tc_supported(f, heads),
-              "mha_tc_bwd: bad arguments (head_dim must be 8)");
+  HGB_REQUIRE(n >= 0 && hgb_mha_tc_supported(f, heads), "mha_tc_bwd: bad sizes (n %d, f %d, heads %d; head_dim must be 8)",
+              n, f, heads);
   if (n == 0) return HGB_OK;
+  HGB_REQUIRE(qkv && out && lse && gout && gqkv && delta_ws, "mha_tc_bwd: NULL pointer");
+  HGB_REQUIRE(aligned(qkv, 16) && aligned(out, 16) && aligned(gout, 16) && aligned(gqkv, 8),
+              "mha_tc_bwd: qkv, out and gout must be 16-byte and gqkv 8-byte aligned");
   const float scale = 1.f / sqrtf((float)D);
   dim3 grid((n + ROWS - 1) / ROWS, heads);
   cudaStream_t st = (cudaStream_t)stream;

@@ -37,10 +37,13 @@ class MhaFn(torch.autograd.Function):
         f = f3 // 3
         out = torch.empty(n, f, dtype=qkv.dtype, device=qkv.device)
         lse = torch.empty(n, heads, dtype=qkv.dtype, device=qkv.device)
-        # head_dim 8: tensor-core kernels (3xTF32 = fp32-level accuracy in fp32 mode, plain TF32 under precision="bf16")
-        ctx.tc = bool(_lib.query("hgb_mha_tc_supported", f, heads))
+        # head_dim 8: tensor-core kernels (3xTF32 = fp32-level accuracy in fp32 mode, plain TF32 under precision="bf16").  They
+        # move rows as float4, so a view that does not start on a 16-byte boundary takes the SIMT kernels (scalar accesses).
+        ctx.tc = bool(_lib.query("hgb_mha_tc_supported", f, heads)) and qkv.data_ptr() % 16 == 0
         ctx.exact = 0 if ops._TC["enabled"] else 1
-        if ctx.tc:
+        if n == 0:
+            pass
+        elif ctx.tc:
             _lib.call("hgb_mha_tc_fwd", _p(qkv), n, f, heads, ctx.exact, _p(out), _p(lse), _stream())
         else:
             _lib.call("hgb_mha_fwd", _p(qkv), n, f, heads, _p(out), _p(lse), _stream())
@@ -54,12 +57,14 @@ class MhaFn(torch.autograd.Function):
         qkv, out, lse = ctx.saved_tensors
         n, f = out.shape
         gqkv = torch.empty_like(qkv)
-        if ctx.tc:
+        gout = _chk(gout)
+        if n == 0:
+            pass
+        elif ctx.tc and gout.data_ptr() % 16 == 0:
             ws = torch.empty(n * ctx.heads, dtype=qkv.dtype, device=qkv.device)
-            _lib.call("hgb_mha_tc_bwd", _p(qkv), _p(out), _p(lse), _p(_chk(gout.contiguous())), n, f, ctx.heads, ctx.exact, _p(ws), _p(gqkv),
-                      _stream())
-        else:
-            _lib.call("hgb_mha_bwd", _p(qkv), _p(out), _p(lse), _p(_chk(gout)), n, f, ctx.heads, _p(gqkv), _stream())
+            _lib.call("hgb_mha_tc_bwd", _p(qkv), _p(out), _p(lse), _p(gout), n, f, ctx.heads, ctx.exact, _p(ws), _p(gqkv), _stream())
+        else:       # either backward takes either forward's out and lse (include/hgb.h)
+            _lib.call("hgb_mha_bwd", _p(qkv), _p(out), _p(lse), _p(gout), n, f, ctx.heads, _p(gqkv), _stream())
         return gqkv, None
 
 

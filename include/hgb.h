@@ -351,7 +351,8 @@ int hgb_painn_update_tc_bwd(const float* v, const float* gs_out, const float* gv
 /* Dense multi-head self-attention over ONE sequence of n tokens (quirk Q1: the reference never passes
  * graph_batch, so the whole mini-batch attends to itself).  qkv [n,3f] is the packed in-projection
  * [q | k | v], head h owns columns h*d..h*d+d-1 (d = f/heads in {1,2,4,8,16,32}); out [n,f]; lse [n,heads]
- * (log-sum-exp of the scaled scores, kept for the backward).  Flash-style: no [n,n] matrix reaches HBM.    */
+ * (natural-log log-sum-exp of the scaled scores, kept for the backward).  Flash-style: no [n,n] matrix reaches HBM.
+ * Sizes are checked before pointers: with n = 0 nothing runs and every pointer may be NULL.  Any float alignment.          */
 int hgb_mha_fwd(const float* qkv, int32_t n, int32_t f, int32_t heads, float* out, float* lse,
                 hgb_stream_t stream);
 int hgb_mha_bwd(const float* qkv, const float* out, const float* lse, const float* gout, int32_t n, int32_t f,
@@ -361,7 +362,10 @@ int hgb_mha_bwd(const float* qkv, const float* out, const float* lse, const floa
  * mma.sync m16n8k8 TF32 with fp32 accumulation; one score block of 16 queries x 8 keys per instruction, the accumulator
  * layout of S re-used as the A operand of P V through a key permutation (no shuffles).  exact != 0: every product as three
  * TF32 products of a hi/lo split (fp32-level accuracy, the fp32 configs); exact == 0: plain TF32 (precision="bf16").
- * delta_ws: n * heads floats of scratch.  Same lse / layout contract as hgb_mha_fwd / hgb_mha_bwd.                       */
+ * delta_ws: n * heads floats of scratch.  Same lse / layout contract as hgb_mha_fwd / hgb_mha_bwd, so either backward takes
+ * either forward's out and lse.  With n = 0 nothing runs and every pointer may be NULL.  Rows move as float4 / float2: the
+ * forward needs qkv 16-byte and out 8-byte aligned, the backward qkv, out and gout 16-byte and gqkv 8-byte aligned; other
+ * pointers are refused before any launch (the SIMT entries above take any alignment).                                   */
 int32_t hgb_mha_tc_supported(int32_t f, int32_t heads);
 int hgb_mha_tc_fwd(const float* qkv, int32_t n, int32_t f, int32_t heads, int32_t exact, float* out, float* lse,
                    hgb_stream_t stream);
