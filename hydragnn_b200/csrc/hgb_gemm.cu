@@ -23,65 +23,69 @@ __global__ void __launch_bounds__(256) gemm_kernel(const float* __restrict__ a, 
   __shared__ __align__(16) float As[BK][BM + 4];
   __shared__ __align__(16) float Bs[BK][BN + 4];
   const int tid = threadIdx.x;
-  const int m0 = blockIdx.y * BM, n0 = blockIdx.x * BN;
+  const int n0 = blockIdx.x * BN;
   const int kbeg = blockIdx.z * k_per_split;
   const int kend = min(k, kbeg + k_per_split);
   const int tx = tid % 16, ty = tid / 16;  // 16 x 16 threads, each TM x TN
-  float acc[TM][TN];
+  // row tiles stride over grid.y, which holds at most 65,535 of them (4,194,240 rows); each tile is summed as before
+  for (int64_t mt = blockIdx.y; mt * BM < m; mt += gridDim.y) {
+    const int m0 = (int)mt * BM;
+    float acc[TM][TN];
 #pragma unroll
-  for (int i = 0; i < TM; ++i)
+    for (int i = 0; i < TM; ++i)
 #pragma unroll
-    for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
+      for (int j = 0; j < TN; ++j) acc[i][j] = 0.f;
 
-  for (int kk = kbeg; kk < kend; kk += BK) {
-    // load A tile (BM x BK) and B tile (BK x BN): 1024 elements each, 4 per thread
+    for (int kk = kbeg; kk < kend; kk += BK) {
+      // load A tile (BM x BK) and B tile (BK x BN): 1024 elements each, 4 per thread
 #pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const int l = tid + t * 256;
-      int am, ak;
-      if (TA) { am = l % BM; ak = l / BM; } else { ak = l % BK; am = l / BK; }   // contiguous index fastest
-      const int gm = m0 + am, gk = kk + ak;
-      float v = 0.f;
-      if (gm < m && gk < kend) v = TA ? a[(int64_t)gk * lda + gm] : a[(int64_t)gm * lda + gk];
-      As[ak][am] = v;
-      int bn, bk;
-      if (TB) { bk = l % BK; bn = l / BK; } else { bn = l % BN; bk = l / BN; }
-      const int gn = n0 + bn, gk2 = kk + bk;
-      float w = 0.f;
-      if (gn < n && gk2 < kend) w = TB ? b[(int64_t)gn * ldb + gk2] : b[(int64_t)gk2 * ldb + gn];
-      Bs[bk][bn] = w;
+      for (int t = 0; t < 4; ++t) {
+        const int l = tid + t * 256;
+        int am, ak;
+        if (TA) { am = l % BM; ak = l / BM; } else { ak = l % BK; am = l / BK; }   // contiguous index fastest
+        const int gm = m0 + am, gk = kk + ak;
+        float v = 0.f;
+        if (gm < m && gk < kend) v = TA ? a[(int64_t)gk * lda + gm] : a[(int64_t)gm * lda + gk];
+        As[ak][am] = v;
+        int bn, bk;
+        if (TB) { bk = l % BK; bn = l / BK; } else { bn = l % BN; bk = l / BN; }
+        const int gn = n0 + bn, gk2 = kk + bk;
+        float w = 0.f;
+        if (gn < n && gk2 < kend) w = TB ? b[(int64_t)gn * ldb + gk2] : b[(int64_t)gk2 * ldb + gn];
+        Bs[bk][bn] = w;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int q = 0; q < BK; ++q) {
+        // one 16-byte shared-memory load per operand (TM = TN = 4; rows of As / Bs are 272 B apart: 16-byte aligned)
+        const float4 a4 = *reinterpret_cast<const float4*>(&As[q][ty * TM]);
+        const float4 b4 = *reinterpret_cast<const float4*>(&Bs[q][tx * TN]);
+        const float ra[TM] = {a4.x, a4.y, a4.z, a4.w}, rb[TN] = {b4.x, b4.y, b4.z, b4.w};
+#pragma unroll
+        for (int i = 0; i < TM; ++i)
+#pragma unroll
+          for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(ra[i], rb[j], acc[i][j]);
+      }
+      __syncthreads();
     }
-    __syncthreads();
 #pragma unroll
-    for (int q = 0; q < BK; ++q) {
-      // one 16-byte shared-memory load per operand (TM = TN = 4; rows of As / Bs are 272 B apart: 16-byte aligned)
-      const float4 a4 = *reinterpret_cast<const float4*>(&As[q][ty * TM]);
-      const float4 b4 = *reinterpret_cast<const float4*>(&Bs[q][tx * TN]);
-      const float ra[TM] = {a4.x, a4.y, a4.z, a4.w}, rb[TN] = {b4.x, b4.y, b4.z, b4.w};
+    for (int i = 0; i < TM; ++i) {
+      const int gm = m0 + ty * TM + i;
+      if (gm >= m) continue;
 #pragma unroll
-      for (int i = 0; i < TM; ++i)
-#pragma unroll
-        for (int j = 0; j < TN; ++j) acc[i][j] = fmaf(ra[i], rb[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < TM; ++i) {
-    const int gm = m0 + ty * TM + i;
-    if (gm >= m) continue;
-#pragma unroll
-    for (int j = 0; j < TN; ++j) {
-      const int gn = n0 + tx * TN + j;
-      if (gn >= n) continue;
-      if (part) {
-        part[((int64_t)blockIdx.z * m + gm) * n + gn] = acc[i][j];
-      } else {
-        float v = acc[i][j];
-        if (bias) v += bias[gn];
-        if (zout) zout[(int64_t)gm * ldc + gn] = v;
-        v = hgb_act(v, act, act_param);
-        if (beta_one) v += c[(int64_t)gm * ldc + gn];
-        c[(int64_t)gm * ldc + gn] = v;
+      for (int j = 0; j < TN; ++j) {
+        const int gn = n0 + tx * TN + j;
+        if (gn >= n) continue;
+        if (part) {
+          part[((int64_t)blockIdx.z * m + gm) * n + gn] = acc[i][j];
+        } else {
+          float v = acc[i][j];
+          if (bias) v += bias[gn];
+          if (zout) zout[(int64_t)gm * ldc + gn] = v;
+          v = hgb_act(v, act, act_param);
+          if (beta_one) v += c[(int64_t)gm * ldc + gn];
+          c[(int64_t)gm * ldc + gn] = v;
+        }
       }
     }
   }
@@ -236,7 +240,8 @@ static int launch_gemm(const float* a, const float* b, float* c, int m, int n, i
   kps = ((kps + BK - 1) / BK) * BK;
   splits = (k + kps - 1) / kps;
   if (splits < 1) splits = 1;
-  dim3 grid((n + BN - 1) / BN, (m + BM - 1) / BM, splits);
+  const int mtiles = (m + BM - 1) / BM;
+  dim3 grid((n + BN - 1) / BN, mtiles < 65535 ? mtiles : 65535, splits);
   gemm_kernel<TA, TB><<<grid, 256, 0, st>>>(a, b, c, m, n, k, lda, ldb, ldc, beta_one, kps, splits > 1 ? (float*)ws : nullptr,
                                             bias, act, act_param, z);
   HGB_LAUNCH_CHECK("gemm");
@@ -350,21 +355,25 @@ extern "C" int hgb_act_deriv(const float* x, int64_t count, int32_t act, float a
 // ---- column sums (bias gradients): two deterministic stages -------------------------------------
 #define CS_ROWS 512  // rows per block in stage 1
 __global__ void colsum_stage1(const float* __restrict__ x, int m, int n, float* __restrict__ part) {
-  // block (32 x 8): lanes over columns, 8 row-walkers; partial [blockIdx.y, n]
+  // block (32 x 8): lanes over columns, 8 row-walkers; partial [row block, n].  Row blocks stride over grid.y (at most 65,535).
   __shared__ float sm[8][33];
   const int col = blockIdx.x * 32 + threadIdx.x;
-  const int r0 = blockIdx.y * CS_ROWS;
-  const int r1 = min(m, r0 + CS_ROWS);
-  float acc = 0.f;
-  if (col < n)
-    for (int r = r0 + threadIdx.y; r < r1; r += 8) acc += x[(int64_t)r * n + col];
-  sm[threadIdx.y][threadIdx.x] = acc;
-  __syncthreads();
-  if (threadIdx.y == 0 && col < n) {
-    float t = 0.f;
+  const int nb = (m + CS_ROWS - 1) / CS_ROWS;
+  for (int rb = blockIdx.y; rb < nb; rb += gridDim.y) {
+    const int r0 = rb * CS_ROWS;
+    const int r1 = min(m, r0 + CS_ROWS);
+    float acc = 0.f;
+    if (col < n)
+      for (int r = r0 + threadIdx.y; r < r1; r += 8) acc += x[(int64_t)r * n + col];
+    sm[threadIdx.y][threadIdx.x] = acc;
+    __syncthreads();
+    if (threadIdx.y == 0 && col < n) {
+      float t = 0.f;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x];
-    part[(int64_t)blockIdx.y * n + col] = t;
+      for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x];
+      part[(int64_t)rb * n + col] = t;
+    }
+    __syncthreads();
   }
 }
 __global__ void colsum_stage2(const float* __restrict__ part, int nb, int n, float* __restrict__ out) {
@@ -387,7 +396,7 @@ extern "C" int hgb_colsum(const float* x, int32_t m, int32_t n, float* out, void
     return HGB_OK;
   }
   const int nb = (m + CS_ROWS - 1) / CS_ROWS;
-  colsum_stage1<<<dim3((n + 31) / 32, nb), dim3(32, 8), 0, st>>>(x, m, n, (float*)workspace);
+  colsum_stage1<<<dim3((n + 31) / 32, nb < 65535 ? nb : 65535), dim3(32, 8), 0, st>>>(x, m, n, (float*)workspace);
   HGB_LAUNCH_CHECK("colsum_stage1");
   colsum_stage2<<<(n + 127) / 128, 128, 0, st>>>((const float*)workspace, nb, n, out);
   HGB_LAUNCH_CHECK("colsum_stage2");

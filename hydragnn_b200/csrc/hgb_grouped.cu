@@ -7,8 +7,8 @@
 //   fwd / dgrad   C[r, :] = act(A[r, :] op(W_g) + bias_g)      for r in [rowptr[g], rowptr[g+1])
 //   wgrad         dW_g = sum_{r in g} dY[r, :]^T X[r, :],  db_g = sum_{r in g} dY[r, :]
 //
-// Exact fp32 FMAs (heads are small: 50 / 25 / 200-wide), no host read of the group sizes: the grid is sized for the worst case
-// (ceil(M / 64) + groups tiles) and surplus tiles exit.
+// Exact fp32 FMAs (heads are small: 50 / 25 / 200-wide), no host read of the group sizes: the launch covers the worst case
+// (ceil(M / 64) + groups tiles, strided over grid.y) and surplus tiles are skipped.
 #include "hgb_common.cuh"
 
 namespace {
@@ -37,61 +37,64 @@ __device__ __forceinline__ bool locate_tile(const int32_t* __restrict__ rowptr, 
 template <bool TB>
 __global__ void __launch_bounds__(256) grouped_rows_kernel(const float* __restrict__ a, int64_t lda, const float* __restrict__ w,
                                                            const float* __restrict__ bias, const int32_t* __restrict__ rowptr,
-                                                           int groups, int n, int k, int act, float act_param,
+                                                           int groups, int tiles, int n, int k, int act, float act_param,
                                                            float* __restrict__ c, float* __restrict__ z) {
   __shared__ float As[GBK][GBM + 4];
   __shared__ float Bs[GBK][GBN + 4];
-  int g, row0, rows;
-  if (!locate_tile(rowptr, groups, blockIdx.y, g, row0, rows)) return;
-  const float* wg = w + (int64_t)g * n * k;
   const int tid = threadIdx.x, n0 = blockIdx.x * GBN;
   const int tx = tid % 16, ty = tid / 16;
-  float acc[GTM][GTN];
+  // tiles stride over grid.y, which holds at most 65,535 of them; each tile is summed as before
+  for (int tile = blockIdx.y; tile < tiles; tile += gridDim.y) {
+    int g, row0, rows;
+    if (!locate_tile(rowptr, groups, tile, g, row0, rows)) continue;   // surplus tile (uniform across the block)
+    const float* wg = w + (int64_t)g * n * k;
+    float acc[GTM][GTN];
 #pragma unroll
-  for (int i = 0; i < GTM; ++i)
+    for (int i = 0; i < GTM; ++i)
 #pragma unroll
-    for (int j = 0; j < GTN; ++j) acc[i][j] = 0.f;
-  for (int kk = 0; kk < k; kk += GBK) {
+      for (int j = 0; j < GTN; ++j) acc[i][j] = 0.f;
+    for (int kk = 0; kk < k; kk += GBK) {
 #pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const int l = tid + t * 256;
-      const int ak = l % GBK, am = l / GBK;
-      float v = 0.f;
-      if (am < rows && kk + ak < k) v = a[(int64_t)(row0 + am) * lda + kk + ak];
-      As[ak][am] = v;
-      int bn, bk;
-      if (TB) { bk = l % GBK; bn = l / GBK; } else { bn = l % GBN; bk = l / GBN; }
-      float u = 0.f;
-      if (n0 + bn < n && kk + bk < k) u = TB ? wg[(int64_t)(n0 + bn) * k + kk + bk] : wg[(int64_t)(kk + bk) * n + n0 + bn];
-      Bs[bk][bn] = u;
+      for (int t = 0; t < 4; ++t) {
+        const int l = tid + t * 256;
+        const int ak = l % GBK, am = l / GBK;
+        float v = 0.f;
+        if (am < rows && kk + ak < k) v = a[(int64_t)(row0 + am) * lda + kk + ak];
+        As[ak][am] = v;
+        int bn, bk;
+        if (TB) { bk = l % GBK; bn = l / GBK; } else { bn = l % GBN; bk = l / GBN; }
+        float u = 0.f;
+        if (n0 + bn < n && kk + bk < k) u = TB ? wg[(int64_t)(n0 + bn) * k + kk + bk] : wg[(int64_t)(kk + bk) * n + n0 + bn];
+        Bs[bk][bn] = u;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int q = 0; q < GBK; ++q) {
+        float ra[GTM], rb[GTN];
+#pragma unroll
+        for (int i = 0; i < GTM; ++i) ra[i] = As[q][ty * GTM + i];
+#pragma unroll
+        for (int j = 0; j < GTN; ++j) rb[j] = Bs[q][tx * GTN + j];
+#pragma unroll
+        for (int i = 0; i < GTM; ++i)
+#pragma unroll
+          for (int j = 0; j < GTN; ++j) acc[i][j] = fmaf(ra[i], rb[j], acc[i][j]);
+      }
+      __syncthreads();
     }
-    __syncthreads();
 #pragma unroll
-    for (int q = 0; q < GBK; ++q) {
-      float ra[GTM], rb[GTN];
+    for (int i = 0; i < GTM; ++i) {
+      const int lm = ty * GTM + i;
+      if (lm >= rows) continue;
 #pragma unroll
-      for (int i = 0; i < GTM; ++i) ra[i] = As[q][ty * GTM + i];
-#pragma unroll
-      for (int j = 0; j < GTN; ++j) rb[j] = Bs[q][tx * GTN + j];
-#pragma unroll
-      for (int i = 0; i < GTM; ++i)
-#pragma unroll
-        for (int j = 0; j < GTN; ++j) acc[i][j] = fmaf(ra[i], rb[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < GTM; ++i) {
-    const int lm = ty * GTM + i;
-    if (lm >= rows) continue;
-#pragma unroll
-    for (int j = 0; j < GTN; ++j) {
-      const int gn = n0 + tx * GTN + j;
-      if (gn >= n) continue;
-      float v = acc[i][j];
-      if (bias) v += bias[(int64_t)g * n + gn];
-      if (z) z[(int64_t)(row0 + lm) * n + gn] = v;
-      c[(int64_t)(row0 + lm) * n + gn] = hgb_act(v, act, act_param);
+      for (int j = 0; j < GTN; ++j) {
+        const int gn = n0 + tx * GTN + j;
+        if (gn >= n) continue;
+        float v = acc[i][j];
+        if (bias) v += bias[(int64_t)g * n + gn];
+        if (z) z[(int64_t)(row0 + lm) * n + gn] = v;
+        c[(int64_t)(row0 + lm) * n + gn] = hgb_act(v, act, act_param);
+      }
     }
   }
 }
@@ -174,10 +177,11 @@ extern "C" int hgb_grouped_linear(const float* x, int64_t ldx, const float* w, c
                                   float* y, float* z, hgb_stream_t stream) {
   HGB_REQUIRE(x && w && rowptr && y && groups >= 1 && m >= 0 && n >= 1 && k >= 1 && ldx >= k, "grouped_linear: bad arguments");
   if (m == 0) return HGB_OK;
-  dim3 grid((n + GBN - 1) / GBN, (m + GBM - 1) / GBM + groups);
+  const int tiles = (m + GBM - 1) / GBM + groups;
+  dim3 grid((n + GBN - 1) / GBN, tiles < 65535 ? tiles : 65535);
   cudaStream_t st = (cudaStream_t)stream;
-  if (trans_w) grouped_rows_kernel<false><<<grid, 256, 0, st>>>(x, ldx, w, bias, rowptr, groups, n, k, act, act_param, y, z);
-  else grouped_rows_kernel<true><<<grid, 256, 0, st>>>(x, ldx, w, bias, rowptr, groups, n, k, act, act_param, y, z);
+  if (trans_w) grouped_rows_kernel<false><<<grid, 256, 0, st>>>(x, ldx, w, bias, rowptr, groups, tiles, n, k, act, act_param, y, z);
+  else grouped_rows_kernel<true><<<grid, 256, 0, st>>>(x, ldx, w, bias, rowptr, groups, tiles, n, k, act, act_param, y, z);
   HGB_LAUNCH_CHECK("grouped_linear");
   return HGB_OK;
 }

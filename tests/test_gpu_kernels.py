@@ -94,19 +94,6 @@ def test_gather_segment_sum_any_order_autograd():
     torch.testing.assert_close(he.cpu(), hr, rtol=1e-3, atol=1e-3)
 
 
-@pytest.mark.parametrize("ta,tb", [(False, False), (False, True), (True, False), (True, True)])
-@pytest.mark.parametrize("m,n,k", [(1, 1, 1), (65, 63, 17), (200, 192, 64), (3, 5, 20000), (130, 70, 9000)])
-def test_gemm(ta, tb, m, n, k):
-    g = gen(m * n + k)
-    a = torch.randn((k, m) if ta else (m, k), generator=g)
-    b = torch.randn((n, k) if tb else (k, n), generator=g)
-    ref = (a.t() if ta else a).double() @ (b.t() if tb else b).double()
-    out = ops.raw_gemm(a.to(DEV), b.to(DEV), ta, tb).cpu()
-    torch.testing.assert_close(out.double(), ref, rtol=2e-5, atol=2e-5 * k ** 0.5)
-    out2 = ops.raw_gemm(a.to(DEV), b.to(DEV), ta, tb, out=torch.ones(m, n, device=DEV), beta_one=True).cpu()
-    torch.testing.assert_close(out2.double(), ref + 1, rtol=2e-5, atol=2e-5 * k ** 0.5)
-
-
 def test_matmul_any_order():
     g = gen(3)
     a, b = torch.randn(7, 5, generator=g), torch.randn(4, 5, generator=g)
@@ -152,26 +139,6 @@ def test_linear_act_strided_weight_block_and_3d_input():
     wfull = torch.randn(5, 20, generator=g)
     ye = ops.linear_act(x.to(DEV), wfull.to(DEV)[:, 4:12], None)
     torch.testing.assert_close(ye.cpu(), x @ wfull[:, 4:12].t(), **TOL)
-
-
-@pytest.mark.parametrize("order", [0, 1, 2])
-def test_act_deriv(order):
-    x = torch.linspace(-4, 4, 401).requires_grad_(True)
-    codes = {"relu": 1, "silu": 2, "tanh": 3, "sigmoid": 4, "lrelu": 5, "elu": 6, "selu": 7}
-    for name, code in codes.items():
-        y = ACTS[name](x)
-        ref = y
-        for _ in range(order):
-            ref, = torch.autograd.grad(ref.sum(), x, create_graph=True)
-        out = torch.empty(401, device=DEV)
-        _lib.call("hgb_act_deriv", x.detach().to(DEV).data_ptr(), 401, code, 0.1, order, out.data_ptr(), ops._stream())
-        mask = x.detach().abs() > 1e-3        # kinks at 0
-        torch.testing.assert_close(out.cpu()[mask], ref.detach()[mask], rtol=1e-4, atol=1e-5)
-
-
-def test_colsum():
-    x = torch.randn(5000, 70, generator=gen(4))
-    torch.testing.assert_close(ops.raw_colsum(x.to(DEV)).cpu(), x.sum(0), rtol=1e-5, atol=1e-4)
 
 
 @pytest.mark.parametrize("mode", ["add", "mean", "max"])

@@ -416,33 +416,6 @@ def test_train_fast_path_equals_eager_on_variable_batches(name, mlip, build):
     assert o1._hgb_fast.recaptures >= 1
 
 
-# ---- SIMT fp32 GEMMs: the shapes the tensor-core Linear and weight gradient do not take ---------------------------------------
-@pytest.mark.parametrize("m,n,k", [(5000, 64, 64), (4097, 200, 128), (20000, 24, 8), (513, 64, 16), (3000, 192, 64)])
-def test_simt_rows_forms_match_fp64(m, n, k):
-    g = torch.Generator().manual_seed(m + n + k)
-    x, w, b = torch.randn(m, k, generator=g), torch.randn(n, k, generator=g) * 0.3, torch.randn(n, generator=g)
-    xd, wd, bd = x.to(DEV), w.to(DEV), b.to(DEV)
-    y, z = ops.raw_linear(xd, wd, bd, ops.ACT_CODES["silu"], 0.0, want_z=True)          # x W^T + b, SiLU, pre-activation kept
-    zr = x.double() @ w.double().t() + b.double()
-    assert rel_l2(z, zr) < 5e-7 and rel_l2(y, torch.nn.functional.silu(zr)) < 5e-7
-    gy = torch.randn(m, n, generator=g)
-    dx = ops.raw_gemm(gy.to(DEV), wd, False, False)                                        # dgrad: g W
-    assert rel_l2(dx, gy.double() @ w.double()) < 5e-7
-    # strided operand (a column block of a wider matrix), accumulate into the output
-    wide = torch.randn(m, k + 8, generator=g).to(DEV)
-    out = torch.ones(m, n, device=DEV)
-    ops.raw_gemm(wide[:, 4:4 + k], wd, False, True, out=out, beta_one=True)
-    assert rel_l2(out, 1.0 + wide[:, 4:4 + k].double().cpu() @ w.double().t()) < 5e-7
-
-
-@pytest.mark.parametrize("r,mo,no", [(50000, 64, 64), (4099, 192, 64), (100000, 64, 128), (9000, 16, 8)])
-def test_simt_weight_gradient_form_matches_fp64(r, mo, no):
-    g = torch.Generator().manual_seed(r + mo)
-    dz, x = torch.randn(r, mo, generator=g), torch.randn(r, no, generator=g)
-    dw = ops.raw_gemm(dz.to(DEV), x.to(DEV), True, False)
-    assert rel_l2(dw, dz.double().t() @ x.double()) < 5e-6
-
-
 def test_pna_aggregate_kernel_hand_computed_cases():
     """hgb_pna_aggregate_fwd on the hand-worked segments of tests/test_oracle_golden.py (two values, single edge, EMPTY segment,
     equal values): [mean | min | max | std] with PyG's std convention (sqrt(relu(var) + 1e-5), forced to 0 at the floor)."""
