@@ -13,7 +13,7 @@ from torch import nn
 from . import ops
 from .stacks import EGCLStack, PAINNStack, cached, graph_sum
 
-SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet", "CGCNN")
+SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet", "CGCNN", "GAT")
 
 
 def get_device(use_gpu=True):
@@ -134,6 +134,12 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
     elif mpnn_type == "CGCNN":
         from .cgcnn import CGCNNStack
         model = CGCNNStack(edge_dim, **common)
+    elif mpnn_type == "GAT":
+        # hydragnn/models/create.py:261-264: the attention heads and the slope are fixed there, and so here
+        heads = 6
+        negative_slope = 0.05
+        from .gat import GATStack
+        model = GATStack(heads, negative_slope, edge_dim, **common)
     else:
         raise ValueError("Unknown mpnn_type: {0}".format(mpnn_type))
     if enable_interatomic_potential:

@@ -1365,6 +1365,104 @@ class CgConvFn(torch.autograd.Function):
         return g_pq, g_eattr, (g_params[1:] if eattr is not None else None), g_params[0], g_out, None
 
 
+def gat_supported(heads, c, d):
+    """Shapes ``GatConvFn`` takes: 1 <= heads <= 8, heads * c <= 512 (<= 256 when c is not a multiple of 4), 0 <= d <= 16."""
+    return bool(_lib.query("hgb_gat_supported", int(heads), int(c), int(d)))
+
+
+def gat_dropout_seed(device):
+    """The attention-dropout seed of one training forward: one int64 drawn on the device from torch's CUDA generator, so
+    ``torch.manual_seed`` reproduces the mask and a captured step draws a new one at every replay."""
+    return torch.randint(0, 2 ** 62, (1,), dtype=torch.int64, device=device)
+
+
+def raw_gat_dropout_keep(n, e, heads, p, seed):
+    """-> uint8 [e + n, heads], 1 where attention coefficient (edge id, head) is kept (self-loop of node i: edge id e + i)."""
+    keep = torch.empty(e + n, heads, dtype=torch.uint8, device=seed.device)
+    _lib.call("hgb_gat_dropout_keep", int(n), int(e), int(heads), float(p), _p(seed), _p(keep), _stream())
+    return keep
+
+
+def _al16(t):
+    return t if t is None or t.data_ptr() % 16 == 0 else t.clone()
+
+
+def raw_gat_fwd(xlr, eattr, mt, att, bias, plan, heads, c, concat, slope, p=0.0, seed=None):
+    """-> (out [n, heads c] (concat) or [n, c], lse [n, heads]): hgb_gat_fwd over the by-target CSR."""
+    n, e = xlr.shape[0], plan.num_edges
+    d = 0 if eattr is None else eattr.shape[1]
+    col = plan.by_col
+    out = torch.empty(n, heads * c if concat else c, dtype=xlr.dtype, device=xlr.device)
+    lse = torch.empty(n, heads, dtype=xlr.dtype, device=xlr.device)
+    _lib.call("hgb_gat_fwd", _p(xlr), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col") if e else None), _p(eattr), d, _p(mt),
+              _p(att), _p(bias), n, e, heads, c, int(bool(concat)), float(slope), float(p), _p(seed), _p(out), _p(lse), _stream())
+    return out, lse
+
+
+def raw_gat_bwd(g_out, xlr, eattr, mt, att, lse, plan, heads, c, concat, slope, p=0.0, seed=None, need_eattr=True,
+                need_params=True):
+    """-> (g_xlr [n, 2 heads c], g_eattr [e, d] or None, g_params [1 + d, heads c] = [g_att ; g_mt] or None)."""
+    n, e = xlr.shape[0], plan.num_edges
+    d = 0 if eattr is None else eattr.shape[1]
+    dev = xlr.device
+    g_xlr = torch.empty_like(xlr)
+    g_eattr = torch.empty(e, d, dtype=xlr.dtype, device=dev) if (need_eattr and d > 0) else None
+    g_params = torch.empty(1 + d, heads * c, dtype=xlr.dtype, device=dev) if need_params else None
+    ws = _ws(_lib.query("hgb_gat_workspace_bytes", n, e, heads, c, d), dev)
+    col, row = plan.by_col, plan.by_row
+    _lib.call("hgb_gat_bwd", _p(g_out), _p(xlr), _p(col.rowptr), _p(col.perm), _p(plan.nbr("col") if e else None), _p(row.rowptr),
+              _p(row.perm), _p(plan.nbr("row") if e else None), _p(eattr), d, _p(mt), _p(att), _p(lse), n, e, heads, c,
+              int(bool(concat)), float(slope), float(p), _p(seed), _p(g_xlr), _p(g_eattr), _p(g_params), _p(ws), _stream())
+    return g_xlr, g_eattr, g_params
+
+
+class GatConvFn(torch.autograd.Function):
+    """torch_geometric 2.6.1 GATv2Conv (add_self_loops=True, fill_value="mean", share_weights=False; hydragnn/models/
+    GATStack.py:175-205) after its two Linears: ``xlr`` [n, 2 heads c] = [x_l | x_r], ``eattr`` [e, d] the edge input (None
+    without one) and ``mt`` [d, heads c] the (folded) lin_edge weight transposed, ``att`` [heads c], ``bias`` [heads c] (concat)
+    or [c] (mean over the heads).  Attention dropout with probability ``p`` keyed by the device ``seed``.  One kernel forward
+    writes only out and the per-head log-sum-exp; the backward is two kernels (by target, by source) and no atomics."""
+
+    @staticmethod
+    def forward(ctx, xlr, eattr, mt, att, bias, plan, heads, c, concat, slope, p, seed):
+        xlr, att, bias = _al16(_chk(xlr)), _chk(att), _chk(bias)
+        eattr = _chk(eattr) if eattr is not None else None
+        mt = _chk(mt) if eattr is not None else None
+        n = xlr.shape[0]
+        if n == 0:
+            out = xlr.new_empty(0, heads * c if concat else c)
+            lse = xlr.new_empty(0, heads)
+        else:
+            out, lse = raw_gat_fwd(xlr, eattr, mt, att, bias, plan, heads, c, concat, slope, p, seed)
+        ctx.save_for_backward(xlr, eattr, mt, att, lse, seed)
+        ctx.plan, ctx.cfg = plan, (heads, c, bool(concat), float(slope), float(p))
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out):
+        xlr, eattr, mt, att, lse, seed = ctx.saved_tensors
+        heads, c, concat, slope, p = ctx.cfg
+        need = ctx.needs_input_grad
+        data_only = _DATA_ONLY["on"]
+        need_params = (need[2] or need[3]) and not data_only
+        g_out = _al16(_chk(g_out.contiguous()))
+        n = xlr.shape[0]
+        d = 0 if eattr is None else eattr.shape[1]
+        if n == 0:
+            g_xlr = torch.zeros_like(xlr)
+            g_eattr = torch.zeros_like(eattr) if (eattr is not None and need[1]) else None
+            g_params = torch.zeros(1 + d, heads * c, dtype=xlr.dtype, device=xlr.device) if need_params else None
+            g_bias = torch.zeros(g_out.shape[1], dtype=xlr.dtype, device=xlr.device)
+        else:
+            g_xlr, g_eattr, g_params = raw_gat_bwd(g_out, xlr, eattr, mt, att, lse, ctx.plan, heads, c, concat, slope, p, seed,
+                                                   need_eattr=eattr is not None and need[1], need_params=need_params)
+            g_bias = raw_colsum(g_out) if (need[4] and not data_only) else None
+        g_att = g_params[0] if g_params is not None else None
+        g_mt = g_params[1:] if (g_params is not None and eattr is not None) else None
+        return (g_xlr, g_eattr, g_mt, g_att, None if data_only else g_bias) + (None,) * 7
+
+
 def cfconv_supported(g, nf, d):
     """Shapes ``CfConvFn`` takes: 1 <= num_gaussians <= 64, 1 <= num_filters <= 128, raw edge input width <= 16."""
     return bool(_lib.query("hgb_cfconv_supported", int(g), int(nf), int(d)))

@@ -33,6 +33,9 @@ WORKLOADS = {
     # PNAPlus on examples/LennardJones (LJ.json: periodic cells, r = 5, k = 5) and on the ogb_pna graphs
     "lj_pnaplus": dict(n=27, lattice=3.8, radius=5.0, max_neighbours=5, pbc=True),
     "ogb_pnaplus": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    # GAT on the ogb_pna graphs; the GPS variant adds the positional encodings
+    "ogb_gat": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    "ogb_gat_gps": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20, pe_dim=6),
     # SchNet on examples/qm9 and examples/md17 (GPS: the positional encodings pe, rel_pe = |pe[row] - pe[col]| once the edges
     # exist, see add_rel_pe), and without GPS at the CI widths, building its radius graphs in the layers
     "qm9_schnet": dict(n=9, rho=0.10, species=[1, 6, 7, 8, 9], radius=7.0, max_neighbours=5, pe_dim=2),
@@ -103,6 +106,11 @@ ARCH["lj_pnaplus"] = dict(mpnn_type="PNAPlus", input_dim=1, hidden_dim=32, num_c
                           activation_function="relu", loss_function_type="mse", enable_interatomic_potential=True,
                           energy_weight=1.0, energy_peratom_weight=1.0, force_weight=1.0)
 ARCH["ogb_pnaplus"] = dict(ARCH["ogb_pna"], mpnn_type="PNAPlus", num_radial=5, envelope_exponent=5)
+# GAT (GATStack.py, 6 attention heads as create.py fixes them): the ogb_pna graphs and graph head with the edge length as the one
+# edge feature, 3 layers at hidden 64 (the concat layers are 6 x 64 = 384 wide; the reference ships no GAT example, 64 is the
+# width of the other GPS workloads); the GPS variant adds 8 attention heads and pe_dim 6
+ARCH["ogb_gat"] = dict(ARCH["ogb_pna"], mpnn_type="GAT", hidden_dim=64, num_conv_layers=3, edge_dim=1)
+ARCH["ogb_gat_gps"] = dict(ARCH["ogb_gat"], global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=8, pe_dim=6)
 # SchNet (SCFStack.py): examples/qm9/qm9.json exactly, examples/md17/md17.json (6 layers, pe_dim 6), and the in-layer branch at
 # the widths of tests/inputs/ci.json (num_filters 126, num_gaussians 50) with hidden 64 and three layers
 ARCH["qm9_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_conv_layers=2, num_gaussians=10, num_filters=8,

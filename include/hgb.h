@@ -583,6 +583,34 @@ int hgb_cgconv_bwd(const float* g_out, const float* pq, const int32_t* rowptr, c
                    const float* eattr, int32_t d, const float* mt, const float* cvec, int32_t n, int32_t e, int32_t f, float* g_p,
                    int32_t ldgp, float* g_h, float* g_eattr, float* g_params, void* workspace, hgb_stream_t stream);
 
+/* GATv2Conv fused (hydragnn/models/GATStack.py:175-205; torch_geometric 2.6.1 GATv2Conv(in, c, heads, concat,
+ * negative_slope, dropout, add_self_loops=True, edge_dim, fill_value="mean", share_weights=False, residual=False)).
+ * xlr [n, 2 hc] = [x_l | x_r] (hc = heads c); the by-target CSR (rowptr, perm, src = source of every slot).  For the edge
+ * j -> i with attribute a (d wide): z = x_r[i] + x_l[j] + mt^T a (mt [d, hc], NULL when d = 0), s_h = sum_c leaky_relu(z_hc,
+ * negative_slope) att_hc, alpha = softmax of s over the in-edges of i and its self-loop (max subtracted), dropped with
+ * probability p after normalisation (kept ones scaled by 1 / (1 - p)), out[i] = sum alpha x_l[j]: [n, hc] (concat) or the
+ * mean over the heads [n, c], + bias.  Input edges with src == dst are skipped; the self-loop of i has the mean attribute of
+ * i's remaining in-edges (0 without any) and edge id e + i.  lse [n, heads] = log-sum-exp of s per target and head.
+ * Dropout keep(seed, edge id, head) is one Philox4x32-10 draw, seed read from device memory (NULL when p = 0);
+ * hgb_gat_dropout_keep writes the same mask as uint8 [e + n, heads] into keep (1 = kept).
+ * Backward (by target, then by source through the second CSR row_rowptr / row_perm / row_dst = target of every slot):
+ * g_xlr [n, 2 hc]; g_eattr [e, d] when non-NULL (input self-loops get 0; every in-edge receives its share of its target's
+ * self-loop mean); g_params (NULL: not computed) [1 + d, hc] = [g_att ; g_mt] from per-CTA partials reduced in fixed order
+ * in fp64.  The bias gradient is the column sum of g_out and is not formed here.  Deterministic: no atomics.
+ * 1 <= heads <= 8, 1 <= c, heads c <= 1024, 0 <= d <= 16 (hgb_gat_supported); 0 <= p < 1.  n = 0 launches nothing; e = 0
+ * runs the self-loops only.  workspace: hgb_gat_workspace_bytes(n, e, heads, c, d) bytes (-1: unsupported).             */
+int hgb_gat_supported(int32_t heads, int32_t c, int32_t d);
+int64_t hgb_gat_workspace_bytes(int32_t n, int32_t e, int32_t heads, int32_t c, int32_t d);
+int hgb_gat_fwd(const float* xlr, const int32_t* rowptr, const int32_t* perm, const int32_t* src, const float* eattr, int32_t d,
+                const float* mt, const float* att, const float* bias, int32_t n, int32_t e, int32_t heads, int32_t c,
+                int32_t concat, float negative_slope, float p, const int64_t* seed, float* out, float* lse, hgb_stream_t stream);
+int hgb_gat_dropout_keep(int32_t n, int32_t e, int32_t heads, float p, const int64_t* seed, void* keep, hgb_stream_t stream);
+int hgb_gat_bwd(const float* g_out, const float* xlr, const int32_t* rowptr, const int32_t* perm, const int32_t* src,
+                const int32_t* row_rowptr, const int32_t* row_perm, const int32_t* row_dst, const float* eattr, int32_t d,
+                const float* mt, const float* att, const float* lse, int32_t n, int32_t e, int32_t heads, int32_t c,
+                int32_t concat, float negative_slope, float p, const int64_t* seed, float* g_xlr, float* g_eattr,
+                float* g_params, void* workspace, hgb_stream_t stream);
+
 /* SchNet continuous-filter convolution fused (hydragnn/models/SCFStack.py:267-301, CFConv.forward / message with aggr "add",
  * filter network of get_conv :97-103, PyG GaussianSmearing / ShiftedSoftplus).  For the edge e = (row[e] -> col[e]):
  * d_e = |pos[col] - pos[row]|, a_e = [exp(coeff (d_e - mu_k)^2), k < g | r_e] with r [e, d] (NULL when d = 0),
