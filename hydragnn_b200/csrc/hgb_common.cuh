@@ -62,6 +62,9 @@ __device__ __forceinline__ float hgb_act(float x, int act, float p) {
   }
 }
 
+// gradient g through a ReLU with output y, bit for bit ATen's threshold_backward: +0 where y <= 0, g elsewhere (NaN y included)
+__device__ __forceinline__ float hgb_relu_select(float g, float y) { return y <= 0.f ? 0.f : g; }
+
 // derivative of act at pre-activation z, given y = act(z) (z is only read for SiLU)
 __device__ __forceinline__ float hgb_act_grad(float y, float z, int act, float p) {
   switch (act) {

@@ -297,7 +297,7 @@ extern "C" int hgb_linear_fwd(const float* x, const float* w, const float* b, in
 __global__ void act_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, const float* __restrict__ z,
                                int64_t count, int act, float p, float* __restrict__ dz) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x)
-    dz[i] = dy[i] * hgb_act_grad(y ? y[i] : 0.f, z ? z[i] : 0.f, act, p);
+    dz[i] = act == HGB_ACT_RELU_SELECT ? hgb_relu_select(dy[i], y[i]) : dy[i] * hgb_act_grad(y ? y[i] : 0.f, z ? z[i] : 0.f, act, p);
 }
 
 extern "C" int hgb_act_bwd(const float* dy, const float* y, const float* z, int64_t count, int32_t act, float act_param,

@@ -131,8 +131,9 @@ __global__ void pool_fwd_kernel(const float* __restrict__ x, const int32_t* __re
   }
 }
 
-__global__ void pool_bwd_kernel(const float* __restrict__ gout, const int32_t* __restrict__ gptr,
-                                const int32_t* __restrict__ argmax, int n, int g, int c, int mode, float* __restrict__ gx) {
+// relu_y (add / mean, may be NULL): the pooled rows were ReLU outputs, gx is masked by hgb_relu_select on the way out
+__global__ void pool_bwd_kernel(const float* __restrict__ gout, const int32_t* __restrict__ gptr, const int32_t* __restrict__ argmax,
+                                const float* __restrict__ relu_y, int n, int g, int c, int mode, float* __restrict__ gx) {
   const int wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
   for (int k = blockIdx.x * wpb + (threadIdx.x >> 5); k < g; k += gridDim.x * wpb) {
     const int lo = gptr[k], hi = gptr[k + 1];
@@ -142,6 +143,8 @@ __global__ void pool_bwd_kernel(const float* __restrict__ gout, const int32_t* _
       if (mode == HGB_POOL_MAX) {
         const int arg = argmax[(int64_t)k * c + ch];
         for (int i = lo; i < hi; ++i) gx[(int64_t)i * c + ch] = (i == arg) ? gv : 0.f;
+      } else if (relu_y) {
+        for (int i = lo; i < hi; ++i) gx[(int64_t)i * c + ch] = hgb_relu_select(gv, relu_y[(int64_t)i * c + ch]);
       } else {
         for (int i = lo; i < hi; ++i) gx[(int64_t)i * c + ch] = gv;
       }
@@ -159,12 +162,13 @@ extern "C" int hgb_pool_fwd(const float* x, const int32_t* graph_ptr, int32_t g,
   return HGB_OK;
 }
 
-extern "C" int hgb_pool_bwd(const float* gout, const int32_t* graph_ptr, const int32_t* argmax, int32_t n, int32_t g,
-                            int32_t c, int32_t mode, float* gx, hgb_stream_t stream) {
+extern "C" int hgb_pool_bwd(const float* gout, const int32_t* graph_ptr, const int32_t* argmax, const float* relu_y, int32_t n,
+                            int32_t g, int32_t c, int32_t mode, float* gx, hgb_stream_t stream) {
   HGB_REQUIRE(g >= 0 && c > 0 && graph_ptr && gx && mode >= 0 && mode <= 2, "pool_bwd: bad arguments");
   HGB_REQUIRE(mode != HGB_POOL_MAX || argmax, "pool_bwd: max pooling needs the argmax buffer");
+  HGB_REQUIRE(mode != HGB_POOL_MAX || !relu_y, "pool_bwd: the ReLU mask is for add / mean pooling");
   if (g == 0) return HGB_OK;
-  pool_bwd_kernel<<<hgb_grid_for(g, 8), 256, 0, (cudaStream_t)stream>>>(gout, graph_ptr, argmax, n, g, c, mode, gx);
+  pool_bwd_kernel<<<hgb_grid_for(g, 8), 256, 0, (cudaStream_t)stream>>>(gout, graph_ptr, argmax, relu_y, n, g, c, mode, gx);
   HGB_LAUNCH_CHECK("pool_bwd");
   return HGB_OK;
 }

@@ -91,7 +91,7 @@ enum { EPI_NONE, EPI_RELU, EPI_SILU, EPI_SILU_ZD, EPI_TANH, EPI_OTHER };
 template <int K>
 __device__ __forceinline__ float lin_epilogue1(const LinParams& p, float v, float& z, float a, float g) {
   z = v;
-  if (K == EPI_RELU) v = fmaxf(v, 0.f);
+  if (K == EPI_RELU) v = isnan(v) ? v : fmaxf(v, 0.f);     // torch.relu (clamp_min): NaN propagates
   if (K == EPI_SILU) v = __fdividef(v, 1.f + __expf(-v));
   if (K == EPI_SILU_ZD) {     // z receives silu'(pre) = s + y (1 - s): the backward then needs one multiply per element
     const float s = __fdividef(1.f, 1.f + __expf(-v));
@@ -101,7 +101,10 @@ __device__ __forceinline__ float lin_epilogue1(const LinParams& p, float v, floa
   if (K == EPI_TANH) v = tanhf(v);
   if (K == EPI_OTHER) v = hgb_act(v, p.act, p.act_param);
   if (p.addend) v += a;
-  if (p.gsrc) v *= p.gact == HGB_ACT_DERIV ? g : hgb_act_grad(g, g, p.gact, p.act_param);   // DERIV: gsrc already holds act'(.)
+  if (p.gsrc) {
+    if (p.gact == HGB_ACT_RELU_SELECT) v = hgb_relu_select(v, g);
+    else v *= p.gact == HGB_ACT_DERIV ? g : hgb_act_grad(g, g, p.gact, p.act_param);   // DERIV: gsrc already holds act'(.)
+  }
   return v;
 }
 

@@ -302,6 +302,7 @@ def raw_smallk_bwd(dy, y, z, x2, w, code=0, param=0.0, need_x=True, need_w=True,
 
 
 ACT_DERIV = 100   # HGB_ACT_DERIV: "the tensor already holds act'(.)"
+RELU_SELECT = 101  # HGB_ACT_RELU_SELECT: the gradient through a ReLU as threshold_backward's select
 
 
 def linear_fwd_dispatch(x2, w, b, code=0, param=0.0, want_z=False):
@@ -666,6 +667,34 @@ def linear_act(x, weight, bias=None, act=None, act_param=0.0):
     return LinearAct.apply(x, weight, bias, act, act_param)
 
 
+def _mlp2_fwd(x2, w1, b1, c1, p1, w2, b2, c2, p2):
+    """act2(act1(x2 W1^T + b1) W2^T + b2) -> (y, tensors to save, act1 config), the forward of Mlp2Fn and of the nodes that fold an
+    activation next to it."""
+    w1 = w1 if w1.stride(1) == 1 else w1.contiguous()
+    w2 = w2 if w2.stride(1) == 1 else w2.contiguous()
+    silu = ACT_CODES["silu"]
+    h, z1, deriv = linear_fwd_dispatch_ex(x2, w1, _chk(b1), c1, p1, want_z=(c1 == silu), z_deriv=True)
+    y, z2 = linear_fwd_dispatch(h, w2, _chk(b2), c2, p2, want_z=(c2 == silu))
+    return y, [x2, w1, w2, h, z1, y if c2 not in (0, silu) else None, z2], (ACT_DERIV if deriv else c1, float(p1))
+
+
+def _mlp2_bwd(dz2, saved, act1, need, leaves1, leaves2, dx_addend=None, dx_gsrc=None, dx_gact=0):
+    """Backward of ``_mlp2_fwd`` from dz2 (the gradient at the second layer's pre-activation) -> (gx, gw1, gb1, gw2, gb2); the
+    gradient through act1 runs in the epilogue of the second layer's data gradient.  need = (x, w1, b1, w2, b2); dx_*: as in
+    linear_bwd_dispatch, for gx."""
+    x2, w1, w2, h, z1 = saved[:5]
+    c1, p1 = act1
+    dz1, gw2, gb2 = linear_bwd_dispatch(dz2, h, w2, True, need[3], need[4], dx_gsrc=(z1 if c1 in (ACT_CODES["silu"], ACT_DERIV) else h),
+                                        dx_gact=c1, dx_gparam=p1, leaves=leaves2)
+    gx, gw1, gb1 = linear_bwd_dispatch(dz1, x2, w1, need[0], need[1], need[2], dx_addend=dx_addend, dx_gsrc=dx_gsrc, dx_gact=dx_gact,
+                                       leaves=leaves1)
+    return gx, gw1, gb1, gw2, gb2
+
+
+def _leaves(w, b):
+    return [w] + ([b] if b is not None else [])
+
+
 class Mlp2Fn(torch.autograd.Function):
     """``act2(act1(x W1^T + b1) W2^T + b2)`` as one node: in the backward the gradient through act1 is applied in the epilogue of
     the second layer's data-gradient GEMM (no separate activation-backward pass over the hidden tensor)."""
@@ -673,36 +702,105 @@ class Mlp2Fn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w1, b1, act1, p1, w2, b2, act2, p2):
         shp = x.shape
-        x2 = _row_major_2d(x)
-        w1_in, w2_in = w1, w2
-        w1 = w1 if w1.stride(1) == 1 else w1.contiguous()
-        w2 = w2 if w2.stride(1) == 1 else w2.contiguous()
-        c1, c2 = ACT_CODES[act1], ACT_CODES[act2]
-        silu = ACT_CODES["silu"]
-        h, z1, deriv = linear_fwd_dispatch_ex(x2, w1, _chk(b1), c1, p1, want_z=(c1 == silu), z_deriv=True)
-        y, z2 = linear_fwd_dispatch(h, w2, _chk(b2), c2, p2, want_z=(c2 == silu))
-        ctx.save_for_backward(x2, w1, w2, h, z1, y if c2 not in (0, silu) else None, z2)
-        ctx.cfg = (ACT_DERIV if deriv else c1, float(p1), c2, float(p2), shp, b1 is not None, b2 is not None)
+        c2 = ACT_CODES[act2]
+        y, saved, ctx.act1 = _mlp2_fwd(_row_major_2d(x), w1, b1, ACT_CODES[act1], p1, w2, b2, c2, p2)
+        ctx.save_for_backward(*saved)
+        ctx.cfg = (c2, float(p2), shp, b1 is not None, b2 is not None)
         ctx.tc = _TC["enabled"]
-        ctx.leaves1 = [w1_in] + ([b1] if b1 is not None else [])
-        ctx.leaves2 = [w2_in] + ([b2] if b2 is not None else [])
+        ctx.leaves1, ctx.leaves2 = _leaves(w1, b1), _leaves(w2, b2)
         return y.reshape(shp[:-1] + (w2.shape[0],))
 
     @staticmethod
     @once_differentiable
     def backward(ctx, gy):
-        x2, w1, w2, h, z1, y, z2 = ctx.saved_tensors
-        c1, p1, c2, p2, shp, has_b1, has_b2 = ctx.cfg
-        m = x2.shape[0]
-        gy2 = _chk(gy.reshape(m, w2.shape[0]))
+        saved = ctx.saved_tensors
+        x2, w2, y, z2 = saved[0], saved[2], saved[5], saved[6]
+        c2, p2, shp, has_b1, has_b2 = ctx.cfg
+        gy2 = _chk(gy.reshape(x2.shape[0], w2.shape[0]))
         dz2 = raw_act_bwd(gy2, y, z2, c2, p2) if c2 != 0 else gy2
+        nig = ctx.needs_input_grad
         with tensor_cores(ctx.tc):
-            dz1, gw2, gb2 = linear_bwd_dispatch(dz2, h, w2, True, ctx.needs_input_grad[5], has_b2 and ctx.needs_input_grad[6],
-                                                dx_gsrc=(z1 if c1 in (ACT_CODES["silu"], ACT_DERIV) else h), dx_gact=c1, dx_gparam=p1,
-                                                leaves=ctx.leaves2)
-            gx, gw1, gb1 = linear_bwd_dispatch(dz1, x2, w1, ctx.needs_input_grad[0], ctx.needs_input_grad[1],
-                                               has_b1 and ctx.needs_input_grad[2], leaves=ctx.leaves1)
+            gx, gw1, gb1, gw2, gb2 = _mlp2_bwd(dz2, saved, ctx.act1, (nig[0], nig[1], has_b1 and nig[2], nig[5], has_b2 and nig[6]),
+                                               ctx.leaves1, ctx.leaves2)
         return (gx.reshape(shp) if gx is not None else None), gw1, gb1, None, None, gw2, gb2, None, None
+
+
+# ---- a PaiNN layer's closing ReLU folded into the passes next to it (C2: node_embed_out - ReLU - {next message | mean pool}) ----
+def relu_embed_fold_ok(x, w1, w2):
+    """True when relu(Linear - act - Linear) of x can run with the ReLU in the second Linear's tensor-core epilogue (TF32 mode),
+    which gives torch.relu's bits."""
+    m, k = x.shape
+    return (_TC["enabled"] and x.is_cuda and x.dtype == torch.float32 and not smallk_ok(w2.shape[0], w1.shape[0])
+            and tc_ok(m, w2.shape[0], w1.shape[0]) and w1.shape[0] <= 256)
+
+
+class ReluMlp2PhiFn(torch.autograd.Function):
+    """(s, phi) with s = relu(act1a(x W1a^T + b1a) W2a^T + b2a) -- a PaiNN layer's node_embed_out and the encoder's ReLU -- and
+    phi = act1b(s W1b^T + b1b) W2b^T + b2b, the next layer's scalar-message MLP, as one node.  The ReLU runs in the epilogue of
+    the Linear that writes s; in the backward the data gradient of phi's first Linear adds g_s (the message's passthrough
+    gradient of s) and applies the ReLU's select in its epilogue, which is the gradient at s's pre-activation.  Every value has
+    the bits of Mlp2Fn - torch.relu - Mlp2Fn with autograd's sum of the two gradients of s."""
+
+    @staticmethod
+    def forward(ctx, x, w1a, b1a, act1a, p1a, w2a, b2a, w1b, b1b, act1b, p1b, w2b, b2b):
+        x2 = _row_major_2d(x)
+        s, saved_a, ctx.act_a = _mlp2_fwd(x2, w1a, b1a, ACT_CODES[act1a], p1a, w2a, b2a, ACT_CODES["relu"], 0.0)
+        phi, saved_b, ctx.act_b = _mlp2_fwd(s, w1b, b1b, ACT_CODES[act1b], p1b, w2b, b2b, 0, 0.0)
+        ctx.save_for_backward(*saved_a, *saved_b)
+        ctx.cfg = (x.shape, b1a is not None, b2a is not None, b1b is not None, b2b is not None)
+        ctx.tc = _TC["enabled"]
+        ctx.leaves = (_leaves(w1a, b1a), _leaves(w2a, b2a), _leaves(w1b, b1b), _leaves(w2b, b2b))
+        return s, phi
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_s, g_phi):
+        saved = ctx.saved_tensors
+        saved_a, saved_b = saved[:7], saved[7:]
+        s = saved_a[5]
+        shp, hb1a, hb2a, hb1b, hb2b = ctx.cfg
+        nig = ctx.needs_input_grad
+        la1, la2, lb1, lb2 = ctx.leaves
+        with tensor_cores(ctx.tc):
+            dz2a, gw1b, gb1b, gw2b, gb2b = _mlp2_bwd(_chk(g_phi), saved_b, ctx.act_b, (True, nig[7], hb1b and nig[8], nig[11], hb2b and nig[12]),
+                                                     lb1, lb2, dx_addend=_chk(g_s), dx_gsrc=s, dx_gact=RELU_SELECT)
+            gx, gw1a, gb1a, gw2a, gb2a = _mlp2_bwd(dz2a, saved_a, ctx.act_a, (nig[0], nig[1], hb1a and nig[2], nig[5], hb2a and nig[6]),
+                                                   la1, la2)
+        return ((gx.reshape(shp) if gx is not None else None), gw1a, gb1a, None, None, gw2a, gb2a, gw1b, gb1b, None, None, gw2b, gb2b)
+
+
+class ReluMlp2MeanPoolFn(torch.autograd.Function):
+    """mean_pool(relu(act1(x W1^T + b1) W2^T + b2)) over the graphs of a sorted batch as one node: the ReLU runs in the second
+    Linear's epilogue, and the pool's backward applies the ReLU's select while it broadcasts, which is the gradient at the second
+    Linear's pre-activation; from there the backward is Mlp2Fn's.  Bits of Mlp2Fn - torch.relu - PoolFn."""
+
+    @staticmethod
+    def forward(ctx, x, w1, b1, act1, p1, w2, b2, gcsr):
+        x2 = _row_major_2d(x)
+        y, saved, ctx.act1 = _mlp2_fwd(x2, w1, b1, ACT_CODES[act1], p1, w2, b2, ACT_CODES["relu"], 0.0)
+        g, c = gcsr.n, y.shape[1]
+        out = torch.empty(g, c, dtype=y.dtype, device=y.device)
+        _lib.call("hgb_pool_fwd", _p(y), _p(gcsr.rowptr), g, c, POOL_CODES["mean"], _p(out), None, _stream())
+        ctx.save_for_backward(*saved)
+        ctx.gcsr, ctx.cfg, ctx.tc = gcsr, (x.shape, b1 is not None, b2 is not None), _TC["enabled"]
+        ctx.leaves1, ctx.leaves2 = _leaves(w1, b1), _leaves(w2, b2)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        saved = ctx.saved_tensors
+        y = saved[5]
+        shp, has_b1, has_b2 = ctx.cfg
+        g = _chk(g)
+        dz2 = torch.empty_like(y)
+        _lib.call("hgb_pool_bwd", _p(g), _p(ctx.gcsr.rowptr), None, _p(y), y.shape[0], ctx.gcsr.n, y.shape[1], POOL_CODES["mean"],
+                  _p(dz2), _stream())
+        nig = ctx.needs_input_grad
+        with tensor_cores(ctx.tc):
+            gx, gw1, gb1, gw2, gb2 = _mlp2_bwd(dz2, saved, ctx.act1, (nig[0], nig[1], has_b1 and nig[2], nig[5], has_b2 and nig[6]),
+                                               ctx.leaves1, ctx.leaves2)
+        return (gx.reshape(shp) if gx is not None else None), gw1, gb1, None, None, gw2, gb2, None
 
 
 class Mlp2ScalarFn(torch.autograd.Function):
@@ -1102,7 +1200,8 @@ class PoolFn(torch.autograd.Function):
     def backward(ctx, g):
         g = _chk(g)
         gx = torch.empty(ctx.n, g.shape[1], dtype=g.dtype, device=g.device)
-        _lib.call("hgb_pool_bwd", _p(g), _p(ctx.gcsr.rowptr), _p(ctx.arg), ctx.n, ctx.gcsr.n, g.shape[1], ctx.code, _p(gx), _stream())
+        _lib.call("hgb_pool_bwd", _p(g), _p(ctx.gcsr.rowptr), _p(ctx.arg), None, ctx.n, ctx.gcsr.n, g.shape[1], ctx.code, _p(gx),
+                  _stream())
         return gx, None, None
 
 

@@ -13,6 +13,8 @@ Every conv has two execution modes, selected per forward call:
   differentiated again -- hydragnn/models/create.py:718-724 with ``create_graph=True``): the same math
   composed from the closed primitives GatherRows / SegmentSum / MatMul, with ATen only for elementwise glue.
 """
+from typing import NamedTuple
+
 import torch
 import torch.nn.functional as F
 from torch import nn
@@ -273,6 +275,18 @@ class E_GCL(nn.Module):
 # ------------------------------------------------------------------------------------------------
 # PaiNN  (hydragnn/models/PAINNStack.py:194-328)
 # ------------------------------------------------------------------------------------------------
+class ReluEmbed(NamedTuple):
+    """s = relu(node_embed_out(x)) of a PaiNN layer (Linear - act - Linear, then the encoder's ReLU), kept unevaluated like
+    ``ops.AffineV``: the next layer's message (``ops.ReluMlp2PhiFn``) or the mean pool (``ops.ReluMlp2MeanPoolFn``) runs it with
+    the ReLU in an epilogue and its gradient folded into a backward pass they make anyway.  ``materialize`` makes the calls of
+    the unfused loop."""
+    x: torch.Tensor
+    seq: nn.Sequential
+
+    def materialize(self):
+        return torch.relu(run_mlp(self.seq, self.x))
+
+
 class PainnMessage(nn.Module):
     def __init__(self, node_size, num_radial, cutoff, edge_dim=None):
         super().__init__()
@@ -302,7 +316,17 @@ class PainnMessage(nn.Module):
             g_v, g_e, m_s = torch.split(fo, f, dim=1)
             m_v = GatherRows.apply(v, plan.by_col) * g_v.unsqueeze(1) + g_e.unsqueeze(1) * (diff / dist).unsqueeze(-1)
             return s + SegmentSum.apply(m_s, plan.by_row), v + SegmentSum.apply(m_v, plan.by_row)
-        phi = run_mlp(self.scalar_message_mlp, s)
+        if isinstance(s, ReluEmbed):
+            l1, a1, l2 = s.seq
+            m1, m2 = self.scalar_message_mlp[0], self.scalar_message_mlp[2]
+            if ops.relu_embed_fold_ok(s.x, l1.weight, l2.weight):
+                s, phi = ops.ReluMlp2PhiFn.apply(s.x, l1.weight, l1.bias, *_act_code(a1), l2.weight, l2.bias, m1.weight, m1.bias,
+                                                 *_act_code(self.scalar_message_mlp[1]), m2.weight, m2.bias)
+            else:
+                s = s.materialize()
+                phi = run_mlp(self.scalar_message_mlp, s)
+        else:
+            phi = run_mlp(self.scalar_message_mlp, s)
         efilt = run_mlp(self.edge_filter, edge_attr) if edge_attr is not None else None
         if "rec_row" not in geom and self.node_size % 64 == 0:      # built once per batch, reused by every layer
             geom["rec_row"] = ops.painn_edge_records(geom["epack"], plan, "row")
@@ -366,10 +390,13 @@ class PainnConv(nn.Module):
             self.module_3 = vec_embed_out
         self.last = vec_embed_out is None
 
-    def forward(self, inv_node_feat, equiv_node_feat, plan, edge_attr=None, edge_shifts=None, geom=None, higher_order=False):
+    def forward(self, inv_node_feat, equiv_node_feat, plan, edge_attr=None, edge_shifts=None, geom=None, higher_order=False,
+                relu_after=False):
+        """``relu_after``: the caller applies a ReLU to s next and hands s to a consumer that takes a ``ReluEmbed`` -- s is then
+        returned as that record, node_embed_out unevaluated."""
         s, v = self.module_0(inv_node_feat, equiv_node_feat, plan, geom, edge_attr, higher_order)
         s, v_new = self.module_1(s, v, higher_order)
-        s = run_mlp(self.module_2, s, higher_order)
+        s = ReluEmbed(s, self.module_2) if relu_after else run_mlp(self.module_2, s, higher_order)
         if self.last:
             return s, v          # PAINNStack.py:124-147: v passes through unchanged in the last layer
         lin = self.module_3
@@ -657,12 +684,23 @@ class Base(nn.Module):
         """Encoder loop, pooling and heads (Base.py:697-846); ``higher``: any-order differentiable path."""
         plan = self._edge_plan(data)
         inv, equiv, conv_args = self._embedding(data, plan, higher)
-        for conv, feat in zip(self.graph_convs, self.feature_layers):
+        defer = self._relu_embed_plan(higher)
+        for conv, feat, d in zip(self.graph_convs, self.feature_layers, defer):
+            if d:                                                            # s = relu(node_embed_out(.)) stays a ReluEmbed
+                inv, equiv = conv(inv_node_feat=inv, equiv_node_feat=equiv, plan=plan, higher_order=higher, relu_after=True, **conv_args)
+                continue
             inv, equiv = conv(inv_node_feat=inv, equiv_node_feat=equiv, plan=plan, higher_order=higher, **conv_args)
             inv = self.activation_function(feat(inv))                        # Base.py:726
         x = inv
         batch, num_graphs, gcsr = self.graph_index(data)
-        x_graph = self.pool(x, gcsr, higher)                                  # Base.py:733-738
+        if isinstance(x, ReluEmbed):                                          # only graph heads follow: x itself is not needed
+            l1, a1, l2 = x.seq
+            if ops.relu_embed_fold_ok(x.x, l1.weight, l2.weight):
+                x_graph = ops.ReluMlp2MeanPoolFn.apply(x.x, l1.weight, l1.bias, *_act_code(a1), l2.weight, l2.bias, gcsr)
+            else:
+                x_graph = self.pool(x.materialize(), gcsr, higher)
+        else:
+            x_graph = self.pool(x, gcsr, higher)                              # Base.py:733-738
         ds = getattr(data, "dataset_name", None)
         outputs = []
         for hd, head, kind in zip(self.head_dims, self.heads_NN, self.head_type):
@@ -686,6 +724,23 @@ class Base(nn.Module):
                 out = decode_branches(kind, head, self.graph_shared, ids, x, x_graph, batch, hd, num_graphs, higher)
             outputs.append(out)
         return outputs
+
+    def _relu_embed_plan(self, higher):
+        """Per conv: hand its s on as a ``ReluEmbed``?  Only where the encoder's step after a PaiNN layer is a plain ReLU
+        (identity feature layer) on the first-order TF32 path and the consumer can take the record: the next PaiNN layer's
+        message, or after the last layer a mean pool that feeds graph heads only.  GPS-wrapped convs and PNAEq's layers (other
+        message modules) are never deferred."""
+        n = len(self.graph_convs)
+        if higher or not ops._TC["enabled"] or type(self.activation_function) is not nn.ReLU:
+            return [False] * n
+
+        def painn(i):
+            conv = self.graph_convs[i]
+            return (type(conv) is PainnConv and type(conv.module_0) is PainnMessage and type(self.feature_layers[i]) is nn.Identity
+                    and _act_code(conv.module_2[1]) is not None)
+
+        readout = self.graph_pooling == "mean" and all(k == "graph" for k in self.head_type)
+        return [painn(i) and (painn(i + 1) if i + 1 < n else readout) for i in range(n)]
 
     def _grouped_decode(self, kind, head, ids, x, x_graph, batch, hd, num_graphs):
         """Branch decoding as grouped GEMMs (SURVEY 8f-4): rows are sorted by dataset branch on the device (CSR over the branch

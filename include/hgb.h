@@ -33,6 +33,10 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 
 /* activation codes (hydragnn/utils/model/model.py:30-46 plus the ones hard-wired in the stacks) */
 #define HGB_ACT_DERIV 100 /* not an activation: "the tensor already holds act'(.)" (hgb_tc_linear, hgb_act_bwd) */
+/* not an activation: the gradient through a ReLU whose OUTPUT is y, as ATen's threshold_backward computes it -- the select
+ * (y <= 0 ? +0 : g), not the product g * relu'(y), which gives -0 for a negative g and NaN for g = inf (hgb_tc_linear's gact,
+ * hgb_act_bwd) */
+#define HGB_ACT_RELU_SELECT 101
 #define HGB_ACT_NONE 0
 #define HGB_ACT_RELU 1
 #define HGB_ACT_SILU 2
@@ -47,6 +51,7 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 #define HGB_POOL_MEAN 1
 #define HGB_POOL_MAX 2
 
+/* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -159,11 +164,13 @@ int hgb_segment_sum_strided(const float* m, const int32_t* rowptr, const int32_t
 int hgb_segment_argminmax(const float* m, const int32_t* rowptr, const int32_t* perm, int32_t n, int32_t c,
                           int64_t* argmin, int64_t* argmax, hgb_stream_t stream);
 /* graph pooling over sorted `batch` (graph_ptr [g+1]); mode HGB_POOL_*.  argmax [g,c] int32 is
- * written for HGB_POOL_MAX (may be NULL otherwise).  -- PyG global_*_pool, Base.py:147-170.     */
+ * written for HGB_POOL_MAX (may be NULL otherwise).  -- PyG global_*_pool, Base.py:147-170.
+ * bwd: `relu_y` [n,c] (optional, add / mean only) is the ReLU output that was pooled: gx is then
+ * also the gradient through that ReLU, masked with HGB_ACT_RELU_SELECT's select (no separate pass). */
 int hgb_pool_fwd(const float* x, const int32_t* graph_ptr, int32_t g, int32_t c, int32_t mode,
                  float* out, int32_t* argmax, hgb_stream_t stream);
-int hgb_pool_bwd(const float* gout, const int32_t* graph_ptr, const int32_t* argmax, int32_t n,
-                 int32_t g, int32_t c, int32_t mode, float* gx, hgb_stream_t stream);
+int hgb_pool_bwd(const float* gout, const int32_t* graph_ptr, const int32_t* argmax, const float* relu_y,
+                 int32_t n, int32_t g, int32_t c, int32_t mode, float* gx, hgb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Dense layers: the cuBLAS call sites behind every nn.Linear of the path -- hydragnn/models/EGCLStack.py:207-240
@@ -206,8 +213,9 @@ int64_t hgb_linear_smallk_bwd_workspace_bytes(int32_t m, int32_t n, int32_t k);
  * (optional) is added after the activation: gradient accumulation without an extra pass.  `gsrc` [m,n_out]
  * (optional): the result is multiplied by act'(gsrc) with activation code `gact` -- the GEMM is then the data
  * gradient THROUGH the activation that produced this layer's input (gsrc = its saved pre-activation for SiLU,
- * its output for the others; gact = HGB_ACT_DERIV: gsrc already holds act'), which removes the separate
- * activation-backward pass.  Forward calls with gsrc = NULL, gact = HGB_ACT_DERIV, act = SiLU and z != NULL store
+ * its output for the others; gact = HGB_ACT_DERIV: gsrc already holds act'; gact = HGB_ACT_RELU_SELECT: gsrc is
+ * a ReLU output and the result is masked by a select, after the addend), which removes the separate
+ * activation-backward pass.  A ReLU epilogue (act = HGB_ACT_RELU) passes NaN through, as torch.relu does.  Forward calls with gsrc = NULL, gact = HGB_ACT_DERIV, act = SiLU and z != NULL store
  * silu'(pre-activation) in z instead of the pre-activation.  n_out, k_red up to 1024 are cut into <= 256 pieces.
  * exact != 0: fp32-accurate mode for the fp32 configs -- every operand is split in shared memory into a TF32 hi / lo
  * pair (three producer-side warps split each A stage as the TMA lands it) and each k-step issues hi*hi + lo*hi + hi*lo
@@ -226,7 +234,8 @@ int hgb_tc_wgrad(const float* dz, int64_t lddz, const float* x, int64_t ldx, int
                  int32_t k_out, float* dw, int64_t lddw, float* db, int32_t accumulate, int32_t exact,
                  void* workspace, int64_t workspace_bytes, hgb_stream_t stream);
 int64_t hgb_tc_wgrad_workspace_bytes(int32_t n_out, int32_t k_out);
-/* dz = dy * act'(.) evaluated from y (or from z for SiLU, which must then be non-NULL).           */
+/* dz = dy * act'(.) evaluated from y (or from z for SiLU, which must then be non-NULL);
+ * HGB_ACT_RELU_SELECT: dz = y <= 0 ? +0 : dy.                                                      */
 int hgb_act_bwd(const float* dy, const float* y, const float* z, int64_t count, int32_t act,
                 float act_param, float* dz, hgb_stream_t stream);
 /* elementwise activation value (order 0) or its order-th derivative (1..2) at x                   */
