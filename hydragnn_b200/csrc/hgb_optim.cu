@@ -10,10 +10,10 @@ __global__ void loss_fwd_bwd_kernel(const float* __restrict__ pred, const float*
   const int64_t total = count;
   if (valid_rows) {          // capacity-padded batch: only the first *valid_rows rows are real (hydragnn_b200/padded.py)
     const int64_t v = (int64_t)valid_rows[0] * row_width;
-    count = v < count ? (v > 0 ? v : 1) : count;
+    count = v < count ? (v > 0 ? v : 0) : count;    // no real row: loss 0, gpred all zero
     for (int64_t i = count + threadIdx.x; gpred && i < total; i += blockDim.x) gpred[i] = 0.f;
   }
-  const float inv = 1.f / (float)count;
+  const float inv = 1.f / (float)(count > 0 ? count : 1);
   for (int64_t i = threadIdx.x; i < count; i += blockDim.x) {
     const float d = pred[i] - target[i];
     if (mode == 0) {

@@ -131,12 +131,21 @@ __global__ void pool_fwd_kernel(const float* __restrict__ x, const int32_t* __re
   }
 }
 
-// relu_y (add / mean, may be NULL): the pooled rows were ReLU outputs, gx is masked by hgb_relu_select on the way out
+// one warp zeroes gx rows [lo, hi)
+__device__ __forceinline__ void pool_zero_rows(float* __restrict__ gx, int lo, int hi, int c, int lane) {
+  for (int64_t t = lane; t < (int64_t)(hi - lo) * c; t += 32) gx[(int64_t)lo * c + t] = 0.f;
+}
+
+// relu_y (add / mean, may be NULL): the pooled rows were ReLU outputs, gx is masked by hgb_relu_select on the way out.
+// Rows outside [gptr[0], gptr[g]) belong to no graph: the warps of the first and last graph zero them.
 __global__ void pool_bwd_kernel(const float* __restrict__ gout, const int32_t* __restrict__ gptr, const int32_t* __restrict__ argmax,
                                 const float* __restrict__ relu_y, int n, int g, int c, int mode, float* __restrict__ gx) {
   const int wpb = blockDim.x >> 5, lane = threadIdx.x & 31;
+  if (g == 0 && blockIdx.x == 0 && threadIdx.x < 32) pool_zero_rows(gx, 0, n, c, lane);
   for (int k = blockIdx.x * wpb + (threadIdx.x >> 5); k < g; k += gridDim.x * wpb) {
     const int lo = gptr[k], hi = gptr[k + 1];
+    if (k == 0) pool_zero_rows(gx, 0, lo, c, lane);
+    if (k == g - 1) pool_zero_rows(gx, hi, n, c, lane);
     const float scale = mode == HGB_POOL_MEAN ? 1.f / (float)max(hi - lo, 1) : 1.f;
     for (int ch = lane; ch < c; ch += 32) {
       const float gv = gout[(int64_t)k * c + ch] * scale;
@@ -167,7 +176,8 @@ extern "C" int hgb_pool_bwd(const float* gout, const int32_t* graph_ptr, const i
   HGB_REQUIRE(g >= 0 && c > 0 && graph_ptr && gx && mode >= 0 && mode <= 2, "pool_bwd: bad arguments");
   HGB_REQUIRE(mode != HGB_POOL_MAX || argmax, "pool_bwd: max pooling needs the argmax buffer");
   HGB_REQUIRE(mode != HGB_POOL_MAX || !relu_y, "pool_bwd: the ReLU mask is for add / mean pooling");
-  if (g == 0) return HGB_OK;
+  HGB_REQUIRE(n >= 0, "pool_bwd: bad row count");
+  if (g == 0 && n == 0) return HGB_OK;
   pool_bwd_kernel<<<hgb_grid_for(g, 8), 256, 0, (cudaStream_t)stream>>>(gout, graph_ptr, argmax, relu_y, n, g, c, mode, gx);
   HGB_LAUNCH_CHECK("pool_bwd");
   return HGB_OK;

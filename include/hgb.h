@@ -51,7 +51,8 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 #define HGB_POOL_MEAN 1
 #define HGB_POOL_MAX 2
 
-/* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd) */
+/* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd);
+ * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -166,7 +167,16 @@ int hgb_segment_argminmax(const float* m, const int32_t* rowptr, const int32_t* 
 /* graph pooling over sorted `batch` (graph_ptr [g+1]); mode HGB_POOL_*.  argmax [g,c] int32 is
  * written for HGB_POOL_MAX (may be NULL otherwise).  -- PyG global_*_pool, Base.py:147-170.
  * bwd: `relu_y` [n,c] (optional, add / mean only) is the ReLU output that was pooled: gx is then
- * also the gradient through that ReLU, masked with HGB_ACT_RELU_SELECT's select (no separate pass). */
+ * also the gradient through that ReLU, masked with HGB_ACT_RELU_SELECT's select (no separate pass).
+ * All n rows of gx are written: rows outside [graph_ptr[0], graph_ptr[g]) belong to no graph and get 0.
+ * mean: out = (sum in row order) / cnt, one division; gx = gout * (1.f / cnt), cnt = max(rows of the graph, 1).
+ * max ties: argmax is the FIRST row holding the maximum, and the backward gives that row the whole gradient
+.  ATen's scatter_reduce("amax") backward instead splits it evenly among
+ * the tied rows.  Both are subgradients of max with the same sum over the tied rows, and they agree wherever
+ * the maximum is unique.  They differ only where distinct rows hold exactly the same maximum: after a ReLU
+ * whose output is 0 in every row the ReLU's own backward zeroes every tied row either way, but equal positive
+ * values (e.g. symmetric atoms of one graph) send the gradient along different rows, so a parameter gradient
+ * can differ from ATen's by the difference of those rows' Jacobians.  An empty graph pools to 0 with argmax -1. */
 int hgb_pool_fwd(const float* x, const int32_t* graph_ptr, int32_t g, int32_t c, int32_t mode,
                  float* out, int32_t* argmax, hgb_stream_t stream);
 int hgb_pool_bwd(const float* gout, const int32_t* graph_ptr, const int32_t* argmax, const float* relu_y,
@@ -483,7 +493,8 @@ int hgb_edge_vec_scatter(const float* gvec, const int32_t* col_rowptr, const int
 /* loss[0] = mean((pred - target)^2) (mode 0) or mean(|pred - target|) (mode 1);
  * gpred = d loss / d pred * gscale.  Single-block deterministic reduction.
  * valid_rows (optional, device int32): capacity-padded batches -- only the first *valid_rows rows of
- * row_width entries are real: the mean runs over them and gpred is zero beyond.                      */
+ * row_width entries are real: the mean runs over them and gpred is exactly zero beyond.  With
+ * *valid_rows <= 0 no row is real: loss[0] = 0 and gpred is zero everywhere.                          */
 int hgb_loss_fwd_bwd(const float* pred, const float* target, int64_t count, int32_t mode, float gscale,
                      float* loss, float* gpred, const int32_t* valid_rows, int32_t row_width,
                      hgb_stream_t stream);
