@@ -22,6 +22,11 @@ Parity pin status (see DESIGN.md "Oracle"):
   tests (H2: 1/2 neighbours, BCC Cr 5x5x5: 14/15) and the rotational-invariance
   test pin counts and edge sets.  Ordering under ``max_neighbours`` truncation
   is "parity unpinned" (no golden vectors exist in the reference).
+* The PNA, PNAPlus, CGCNN, GAT and SchNet stacks (``pna``, ``pnaplus``, ``cgcnn``, ``gat``,
+  ``schnet``) are PINNED by ``tests/golden/models_{pna,pnaplus,cgcnn,gat,schnet}.pt``,
+  produced by the reference's own stack, ``Base.py`` and ``gps.py`` with the PyG convs
+  restated here standing in for PyG's; each restated conv is pinned by hand-computed
+  cases in ``tests/test_oracle_*.py``.
 """
 
 from . import geometry, radius_graph, egnn, painn, base, mlip  # noqa: F401

@@ -1,11 +1,13 @@
 """Oracle: model assembly (encoder loop, pooling, multi-head decoder).
 
-Test infrastructure only.  Restates ``Base`` (hydragnn/models/Base.py:36-982),
-``EGCLStack`` (hydragnn/models/EGCLStack.py:22-152), ``PAINNStack``
-(hydragnn/models/PAINNStack.py:27-191) and the ``create_model`` dispatch
-(hydragnn/models/create.py:112-584) for the EGNN and PAINN stacks without GPS.
-Parameter names follow the reference (PyG ``Sequential`` names its children
-``module_<i>`` [3P-memory B.5]) so state dicts interchange with the engine.
+Test infrastructure only.  Restates ``Base`` (hydragnn/models/Base.py:36-982) once, as
+``StackOracle``, which every oracle stack subclasses; ``EGCLStack``
+(hydragnn/models/EGCLStack.py:22-152), ``PAINNStack`` (hydragnn/models/PAINNStack.py:27-191)
+and ``PNAEqStack`` as ``OracleModel``; and the ``create_model`` dispatch
+(hydragnn/models/create.py:112-584).  The PNA, PNAPlus, CGCNN, GAT and SchNet stacks are
+in oracle/{pna,pnaplus,cgcnn,gat,schnet}.py.  Parameter names follow the reference (PyG
+``Sequential`` names its children ``module_<i>`` [3P-memory B.5]) so state dicts
+interchange with the engine.
 """
 import torch
 from torch import nn
@@ -14,7 +16,7 @@ from .egnn import EGCL
 from .geometry import edge_vectors_and_lengths, graph_pool
 from .painn import PainnMessage, PainnUpdate
 from . import pnaeq
-from .gps import GPSConv
+from .gps import GPSConv, PyGBatchNorm
 
 
 def activation(name):
@@ -51,31 +53,38 @@ class _Conv(nn.Module):
     """Stand-in for the PyG ``Sequential`` built by ``get_conv``; holds children under
     the names PyG would give them."""
 
-    def __init__(self, kind, mods):
+    def __init__(self, mods):
         super().__init__()
-        self.kind = kind
         for i, m in enumerate(mods):
             if m is not None:
                 self.add_module("module_%d" % i, m)
 
 
-class OracleModel(nn.Module):
-    def __init__(self, mpnn_type, input_dim, hidden_dim, output_dim, output_type, output_heads,
-                 activation_function="relu", loss_function_type="mse", task_weights=None,
-                 num_conv_layers=2, num_nodes=None, edge_dim=None, num_radial=None, radius=None,
-                 equivariance=False, graph_pooling="mean", pna_deg=None, global_attn_engine=None,
-                 global_attn_type=None, global_attn_heads=0, pe_dim=0, dropout=0.25, **_unused):
+class StackOracle(nn.Module):
+    """``Base`` (hydragnn/models/Base.py:36-982): loss weights and pooling, the GPS node and edge embeddings, the encoder loop,
+    ``graph_shared``, the graph heads, the ``mlp`` / ``mlp_per_node`` / ``conv`` node heads, single- and multi-branch decoding and
+    ``loss_hpweighted``.  A stack sets its own attributes (``edge_dim`` first of all) before calling this constructor and supplies
+    the hooks the reference's stacks override:
+
+    * ``_get_conv(fin, fout, last, edge_dim=None)``: one conv under the reference's child names;
+    * ``_feature_layer(width)``: what follows every encoder conv (Identity here, a BatchNorm in ``Base._init_conv``);
+    * ``_conv_width(fout, last)``: what a conv built for ``fout`` outputs (GAT's concat convs: ``fout`` times its heads);
+    * ``_embedding(data) -> (x, equiv, ctx)``: the per-forward node features, equivariant features and context every conv reads;
+    * ``_run_conv(conv, x, equiv, ctx) -> (x, equiv)``: one conv, unwrapped from GPS.
+
+    ``_init_conv`` and ``_init_node_conv`` are overridden where the reference's stack overrides them.
+    """
+
+    def __init__(self, input_dim, hidden_dim, output_dim, output_type, output_heads, activation_function="relu",
+                 loss_function_type="mse", task_weights=None, num_conv_layers=2, num_nodes=None, equivariance=False,
+                 graph_pooling="mean", global_attn_engine=None, global_attn_type=None, global_attn_heads=0, pe_dim=0, dropout=0.25,
+                 **_unused):
         super().__init__()
         self.use_global_attn = bool(global_attn_engine)
         if self.use_global_attn and (global_attn_engine != "GPS" or global_attn_type != "multihead"):
             raise ValueError("oracle supports global_attn_engine='GPS' with global_attn_type='multihead'")
         self.global_attn_heads, self.pe_dim, self.dropout = global_attn_heads, pe_dim, dropout
-        if mpnn_type == "PNAEq":
-            assert pna_deg is not None, "PNAEq requires degree input."
-            self.deg = pnaeq.sanitize_degree(pna_deg)
-        if mpnn_type not in ("EGNN", "PAINN", "PNAEq"):
-            raise ValueError("Unknown mpnn_type: {0}".format(mpnn_type))
-        self.mpnn_type, self.input_dim, self.hidden_dim = mpnn_type, input_dim, hidden_dim
+        self.input_dim, self.hidden_dim = input_dim, hidden_dim
         self.head_dims, self.head_type = list(output_dim), list(output_type)
         self.num_heads = len(self.head_dims)
         self.config_heads = normalize_heads(output_heads)
@@ -88,12 +97,8 @@ class OracleModel(nn.Module):
         self.loss_weights = [t / tot for t in w]                           # Base.py:121-132
         mode = graph_pooling.lower()
         self.graph_pooling = "add" if mode == "sum" else mode
-        self.num_conv_layers, self.num_radial, self.radius = num_conv_layers, num_radial, radius
+        self.num_conv_layers, self.num_nodes = num_conv_layers, num_nodes
         self.equivariance = bool(equivariance)
-        if mpnn_type == "EGNN":
-            self.edge_dim = 0 if edge_dim is None else edge_dim            # EGCLStack.py:33-35
-        else:
-            self.edge_dim = edge_dim                                        # PAINNStack.py:43
         self.use_edge_attr = self.edge_dim is not None and self.edge_dim > 0   # Base.py:135-141
         if self.use_global_attn:                                               # Base.py:179-215
             self.embed_dim = self.edge_embed_dim = hidden_dim
@@ -107,17 +112,27 @@ class OracleModel(nn.Module):
                 self.edge_lin = nn.Linear(2 * hidden_dim, hidden_dim, bias=False)
         else:
             self.embed_dim, self.edge_embed_dim = input_dim, self.edge_dim
+        self.graph_convs, self.feature_layers = nn.ModuleList(), nn.ModuleList()
+        self._init_conv()
+        self._multihead()
 
-        # --- conv stack: first layer at embed_dim (= input_dim without GPS, Q4), last layer flagged (EGCLStack.py:45-70)
-        self.graph_convs = nn.ModuleList()
-        for i in range(num_conv_layers):
-            last = i == num_conv_layers - 1
-            conv = self._get_conv(self.embed_dim if i == 0 else hidden_dim, hidden_dim, last)
-            if self.use_global_attn:                                           # Base._apply_global_attn :234-247
-                conv = GPSConv(hidden_dim, conv, heads=global_attn_heads, dropout=dropout)
-            self.graph_convs.append(conv)
+    def _wrap(self, conv):
+        """Base._apply_global_attn (:234-247)."""
+        return GPSConv(self.hidden_dim, conv, heads=self.global_attn_heads, dropout=self.dropout) if self.use_global_attn else conv
 
-        # --- decoder (Base.py:590-691), single or multi branch
+    def _init_conv(self):
+        """First layer at embed_dim (= input_dim without GPS, Q4), last layer flagged (EGCLStack.py:45-70, Base.py:446-463)."""
+        for i in range(self.num_conv_layers):
+            last = i == self.num_conv_layers - 1
+            conv = self._get_conv(self.embed_dim if i == 0 else self.hidden_dim, self.hidden_dim, last, edge_dim=self.edge_embed_dim)
+            self.graph_convs.append(self._wrap(conv))
+            self.feature_layers.append(self._feature_layer(self.hidden_dim))
+
+    def _feature_layer(self, width):
+        return nn.Identity()
+
+    def _multihead(self):
+        """Base._multihead (:590-691), single or multi branch."""
         act = self.activation_function
         self.heads_NN = nn.ModuleList()          # registered before graph_shared, as in Base.__init__:83
         self.convs_node_hidden, self.batch_norms_node_hidden = nn.ModuleDict(), nn.ModuleDict()       # Base.py:88-91
@@ -128,12 +143,12 @@ class OracleModel(nn.Module):
             self.num_branches = len(self.config_heads["graph"])
             for br in self.config_heads["graph"]:
                 a = br["architecture"]
-                layers = [nn.Linear(hidden_dim, a["dim_sharedlayers"]), act]
+                layers = [nn.Linear(self.hidden_dim, a["dim_sharedlayers"]), act]
                 for _ in range(a["num_sharedlayers"] - 1):
                     layers += [nn.Linear(a["dim_sharedlayers"], a["dim_sharedlayers"]), act]
                 self.graph_shared[br["type"]] = nn.Sequential(*layers)
         if "node" in self.config_heads:
-            self._init_node_conv(num_nodes)
+            self._init_node_conv()
         inode = 0
         for ih in range(self.num_heads):
             head = nn.ModuleDict()
@@ -152,9 +167,9 @@ class OracleModel(nn.Module):
                     if a["type"] in ("mlp", "mlp_per_node"):                       # Base.py:648-664
                         per_node = a["type"] == "mlp_per_node"
                         if per_node:
-                            assert num_nodes is not None, "num_nodes must be provided for mlp_per_node; use 'mlp' for variable-size graphs"
-                        head[br["type"]] = _MLPNode(hidden_dim, self.head_dims[ih], a["dim_headlayers"], act,
-                                                    num_mlp=num_nodes if per_node else 1, num_nodes=num_nodes if per_node else None)
+                            assert self.num_nodes is not None, "num_nodes must be provided for mlp_per_node; use 'mlp' for variable-size graphs"
+                        head[br["type"]] = _MLPNode(self.hidden_dim, self.head_dims[ih], a["dim_headlayers"], act,
+                                                    num_mlp=self.num_nodes if per_node else 1, num_nodes=self.num_nodes if per_node else None)
                     elif a["type"] == "conv":                                       # Base.py:665-680: the SAME modules, listed again
                         key, mods = br["type"], nn.ModuleList()
                         for conv, bn in zip(self.convs_node_hidden[key], self.batch_norms_node_hidden[key]):
@@ -170,9 +185,8 @@ class OracleModel(nn.Module):
                 raise ValueError("Unknown head type" + str(self.head_type[ih]))
             self.heads_NN.append(head)
 
-    def _init_node_conv(self, num_nodes):
+    def _init_node_conv(self):
         """Base._init_node_conv (:508-588): conv-type node heads share their hidden convolutions between heads."""
-        from .gps import PyGBatchNorm
         cfgs = self.config_heads["node"]
         if any(br["architecture"]["type"] != "conv" for br in cfgs):
             return
@@ -183,94 +197,52 @@ class OracleModel(nn.Module):
             a = br["architecture"]
             hid = a["dim_headlayers"]
             ch, bh, co, bo = nn.ModuleList(), nn.ModuleList(), nn.ModuleList(), nn.ModuleList()
+            w = self._conv_width
             ch.append(self._get_conv(self.hidden_dim, hid[0], False))
-            bh.append(PyGBatchNorm(hid[0]))
+            bh.append(PyGBatchNorm(w(hid[0], False)))
             for k in range(a["num_headlayers"] - 1):
-                ch.append(self._get_conv(hid[k], hid[k + 1], False))
-                bh.append(PyGBatchNorm(hid[k + 1]))
+                ch.append(self._get_conv(w(hid[k], False), hid[k + 1], False))
+                bh.append(PyGBatchNorm(w(hid[k + 1], False)))
             for ih in node_heads:
-                co.append(self._get_conv(hid[-1], self.head_dims[ih], True))
-                bo.append(PyGBatchNorm(self.head_dims[ih]))
+                co.append(self._get_conv(w(hid[-1], False), self.head_dims[ih], True))
+                bo.append(PyGBatchNorm(w(self.head_dims[ih], True)))
             key = br["type"]
             self.convs_node_hidden[key], self.batch_norms_node_hidden[key] = ch, bh
             self.convs_node_output[key], self.batch_norms_node_output[key] = co, bo
 
-    # EGCLStack.get_conv :72-109 / PAINNStack.get_conv :76-147
-    def _get_conv(self, fin, fout, last):
-        ed = self.edge_embed_dim                                        # hidden_dim under GPS, else the stack's edge_dim
-        if self.mpnn_type == "EGNN":
-            return _Conv("egnn", [EGCL(fin, fout, self.hidden_dim, edge_attr_dim=ed or self.edge_dim,
-                                       equivariant=self.equivariance and not last)])
-        if self.mpnn_type == "PNAEq":                                   # PNAEqStack.get_conv :119-192
-            msg = pnaeq.PainnMessage(fin, self.deg, ed, self.num_radial)
-            upd = pnaeq.PainnUpdate(fin, last_layer=last)
-        else:
-            msg = PainnMessage(fin, self.num_radial, self.radius, edge_dim=ed)
-            upd = PainnUpdate(fin, last_layer=last)
-        s_out = nn.Sequential(nn.Linear(fin, fout), nn.Tanh(), nn.Linear(fout, fout))
-        v_out = None if last else nn.Linear(fin, fout)
-        return _Conv("painn", [msg, upd, s_out, v_out])
+    def _conv_width(self, fout, last):
+        """Width of what a conv built for ``fout`` outputs."""
+        return fout
+
+    def _node_edge_features(self, data):
+        """(x, edge_attr) entering the first conv: the input features, or the GPS node and edge embeddings (Base._embedding
+        :477-491)."""
+        eattr = data.edge_attr if self.use_edge_attr else None
+        if not self.use_global_attn:
+            return data.x, eattr
+        x = self.pos_emb(data.pe)
+        if self.input_dim:
+            x = self.node_lin(torch.cat((self.node_emb(data.x.to(x.dtype)), x), 1))
+        e = self.rel_pos_emb(data.rel_pe)
+        if self.use_edge_attr:
+            e = self.edge_lin(torch.cat((self.edge_emb(eattr), e), 1))
+        return x, e
+
+    def _embedding(self, data):
+        x, eattr = self._node_edge_features(data)
+        return x, None, {"edge_index": data.edge_index, "edge_attr": eattr}
+
+    def _layer(self, conv, x, equiv, ctx):
+        """One encoder conv, through GPSConv when global attention is on."""
+        if self.use_global_attn:
+            return conv(x, equiv, lambda a, b: self._run_conv(conv.conv, a, b, ctx))
+        return self._run_conv(conv, x, equiv, ctx)
 
     def forward(self, data):
-        x, pos, ei = data.x, data.pos, data.edge_index.to(torch.long)
-        shifts = getattr(data, "edge_shifts", None)
-        if shifts is None:                                                   # Base.py:466-469
-            shifts = torch.zeros(ei.shape[1], 3, dtype=pos.dtype, device=pos.device)
-        eattr = data.edge_attr if self.use_edge_attr else None
-        if self.use_global_attn:                                               # Base._embedding :477-491
-            xe = self.pos_emb(data.pe)
-            if self.input_dim:
-                xe = self.node_lin(torch.cat((self.node_emb(x.float()), xe), 1))
-            e = self.rel_pos_emb(data.rel_pe)
-            if self.use_edge_attr:
-                e = self.edge_lin(torch.cat((self.edge_emb(eattr), e), 1))
-            x, eattr = xe, e
-
-        def layer(conv, fn):
-            """run one conv, through GPSConv when global attention is on"""
-            if self.use_global_attn:
-                return lambda x_, q_: conv(x_, q_, lambda a, b: fn(conv.conv, a, b))
-            return lambda x_, q_: fn(conv, x_, q_)
-
-        if self.mpnn_type == "EGNN":
-            equiv = pos
-            run_conv = lambda c, a, b: c.module_0(a, b, ei, eattr, shifts)
-            for conv in self.graph_convs:
-                x, equiv = layer(conv, run_conv)(x, equiv)
-                x = self.activation_function(x)                              # Base.py:726
-        elif self.mpnn_type == "PNAEq":
-            vec, dist = edge_vectors_and_lengths(pos, ei, shifts, normalize=True)    # PNAEqStack.py:202-205
-            rbf = pnaeq.rbf_basis(dist.squeeze(-1), self.num_radial, self.radius)
-            edge = ei.t()
-            v = torch.zeros(x.shape[0], 3, x.shape[1], dtype=x.dtype, device=x.device)
-
-            def pna_conv(c, a, b):
-                a, b2 = c.module_0(a, b, edge, rbf, vec, eattr)
-                a, b3 = c.module_1(a, b2)
-                a = c.module_2(a)
-                return a, (c.module_3(b3) if b3 is not None else b2)
-
-            run_conv = pna_conv
-            for conv in self.graph_convs:
-                x, v = layer(conv, pna_conv)(x, v)
-                x = self.activation_function(x)
-            equiv = v
-        else:
-            diff, dist = edge_vectors_and_lengths(pos, ei, shifts, normalize=True)   # PAINNStack.py:157-159
-            edge = ei.t()
-            v = torch.zeros(x.shape[0], 3, x.shape[1], dtype=x.dtype, device=x.device)
-
-            def painn_conv(c, a, b):
-                a, b2 = c.module_0(a, b, edge, diff, dist, eattr)
-                a, b3 = c.module_1(a, b2)
-                a = c.module_2(a)
-                return a, (c.module_3(b3) if b3 is not None else b2)
-
-            run_conv = painn_conv
-            for conv in self.graph_convs:
-                x, v = layer(conv, painn_conv)(x, v)
-                x = self.activation_function(x)
-            equiv = v
+        x, equiv, ctx = self._embedding(data)
+        for conv, feat in zip(self.graph_convs, self.feature_layers):
+            x, equiv = self._layer(conv, x, equiv, ctx)
+            x = self.activation_function(feat(x))                             # Base.py:726
         batch = getattr(data, "batch", None)
         if batch is None:
             batch = torch.zeros(x.shape[0], dtype=torch.long, device=x.device)
@@ -286,7 +258,7 @@ class OracleModel(nn.Module):
                     a, b = x, equiv
                     mods = head["branch-0"]
                     for conv, bn in zip(mods[0::2], mods[1::2]):
-                        a, b = run_conv(conv, a, b)
+                        a, b = self._run_conv(conv, a, b, ctx)
                         a = self.activation_function(bn(a))
                     outs.append(a[:, :hd])
                 else:
@@ -314,11 +286,72 @@ class OracleModel(nn.Module):
         """``loss_hpweighted`` (Base.py:879-906)."""
         tot, tasks = 0, []
         for ih in range(self.num_heads):
-            tgt = value[head_index[ih]].reshape(pred[ih].shape)
+            tgt = value[head_index[ih]].reshape(pred[ih].shape).to(pred[ih].dtype)
             li = self.loss_function(pred[ih], tgt)
             tot = tot + li * self.loss_weights[ih]
             tasks.append(li)
         return tot, tasks
+
+
+class OracleModel(StackOracle):
+    """``EGCLStack`` (hydragnn/models/EGCLStack.py:22-152), ``PAINNStack`` (hydragnn/models/PAINNStack.py:27-191) and
+    ``PNAEqStack`` (hydragnn/models/PNAEqStack.py) on the skeleton, chosen by ``mpnn_type``."""
+
+    def __init__(self, mpnn_type, input_dim, hidden_dim, output_dim, output_type, output_heads, edge_dim=None, num_radial=None,
+                 radius=None, pna_deg=None, **kw):
+        if mpnn_type == "PNAEq":
+            assert pna_deg is not None, "PNAEq requires degree input."
+            self.deg = pnaeq.sanitize_degree(pna_deg)
+        if mpnn_type not in ("EGNN", "PAINN", "PNAEq"):
+            raise ValueError("Unknown mpnn_type: {0}".format(mpnn_type))
+        self.mpnn_type, self.num_radial, self.radius = mpnn_type, num_radial, radius
+        if mpnn_type == "EGNN":
+            self.edge_dim = 0 if edge_dim is None else edge_dim            # EGCLStack.py:33-35
+        else:
+            self.edge_dim = edge_dim                                        # PAINNStack.py:43
+        super().__init__(input_dim, hidden_dim, output_dim, output_type, output_heads, **kw)
+
+    # EGCLStack.get_conv :72-109 / PAINNStack.get_conv :76-147
+    def _get_conv(self, fin, fout, last, edge_dim=None):
+        ed = self.edge_embed_dim                                        # hidden_dim under GPS, else the stack's edge_dim
+        if self.mpnn_type == "EGNN":
+            return _Conv([EGCL(fin, fout, self.hidden_dim, edge_attr_dim=ed or self.edge_dim,
+                               equivariant=self.equivariance and not last)])
+        if self.mpnn_type == "PNAEq":                                   # PNAEqStack.get_conv :119-192
+            msg = pnaeq.PainnMessage(fin, self.deg, ed, self.num_radial)
+            upd = pnaeq.PainnUpdate(fin, last_layer=last)
+        else:
+            msg = PainnMessage(fin, self.num_radial, self.radius, edge_dim=ed)
+            upd = PainnUpdate(fin, last_layer=last)
+        s_out = nn.Sequential(nn.Linear(fin, fout), nn.Tanh(), nn.Linear(fout, fout))
+        v_out = None if last else nn.Linear(fin, fout)
+        return _Conv([msg, upd, s_out, v_out])
+
+    def _embedding(self, data):
+        x, eattr = self._node_edge_features(data)
+        pos, ei = data.pos, data.edge_index.to(torch.long)
+        shifts = getattr(data, "edge_shifts", None)
+        if shifts is None:                                                   # Base.py:466-469
+            shifts = torch.zeros(ei.shape[1], 3, dtype=pos.dtype, device=pos.device)
+        ctx = {"edge_index": ei, "edge": ei.t(), "edge_attr": eattr, "shifts": shifts}
+        if self.mpnn_type == "EGNN":
+            return x, pos, ctx
+        # PAINNStack.py:157-159 / PNAEqStack.py:202-205
+        ctx["vec"], ctx["dist"] = edge_vectors_and_lengths(pos, ei, shifts, normalize=True)
+        if self.mpnn_type == "PNAEq":
+            ctx["rbf"] = pnaeq.rbf_basis(ctx["dist"].squeeze(-1), self.num_radial, self.radius)
+        return x, torch.zeros(x.shape[0], 3, x.shape[1], dtype=x.dtype, device=x.device), ctx
+
+    def _run_conv(self, c, a, b, ctx):
+        if self.mpnn_type == "EGNN":
+            return c.module_0(a, b, ctx["edge_index"], ctx["edge_attr"], ctx["shifts"])
+        if self.mpnn_type == "PNAEq":
+            a, b2 = c.module_0(a, b, ctx["edge"], ctx["rbf"], ctx["vec"], ctx["edge_attr"])
+        else:
+            a, b2 = c.module_0(a, b, ctx["edge"], ctx["vec"], ctx["dist"], ctx["edge_attr"])
+        a, b3 = c.module_1(a, b2)
+        a = c.module_2(a)
+        return a, (c.module_3(b3) if b3 is not None else b2)
 
 
 class _MLPNode(nn.Module):
@@ -344,6 +377,20 @@ class _MLPNode(nn.Module):
         for i in range(self.num_nodes):
             outs[i::self.num_nodes] = self.mlp[i](x[i::self.num_nodes])
         return outs
+
+
+def oracle_from_case(cls, case, state=None, dtype=torch.float64):
+    """The oracle stack ``cls`` built from a case of tests/golden/models_*.pt, with ``state`` (the case's own by default) loaded
+    strictly, in ``dtype``.  The cases' GPS runs use 4 attention heads and 4-wide encodings, and their train-mode steps were
+    recorded with dropout off."""
+    cfg = dict(case["cfg"])
+    if cfg.pop("gps"):
+        cfg.update(global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=4, pe_dim=4)
+    if "deg" in case:
+        cfg["pna_deg"] = case["deg"]
+    m = cls(**cfg, task_weights=[1.0] * len(cfg["output_type"]), dropout=0.0)
+    m.load_state_dict(case["state"] if state is None else state, strict=True)
+    return m.to(dtype)
 
 
 def create_model(**kw):

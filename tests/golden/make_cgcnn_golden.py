@@ -6,7 +6,7 @@ on the GPU machines.
 
 What the golden pins: everything in CGCNNStack.py / Base.py / gps.py that runs -- the layer loop with its BatchNorm feature
 layers, the GPS embedding and wrapper, pooling, heads, losses, the conv-head refusals -- EXCEPT PyG's ``CGConv`` itself, which is
-the restatement in tests/cgcnn_oracle.py [3P-memory]; test_oracle_cgcnn.py pins it by hand-computed cases.
+the restatement in oracle/cgcnn.py [3P-memory]; test_oracle_cgcnn.py pins it by hand-computed cases.
 
 Each case of models_cgcnn.pt stores the state dict, the inputs, the eval-mode predictions, and one train-mode step (batch
 statistics, dropout off): predictions, the reference's own loss, every parameter gradient and the BatchNorm running statistics
@@ -52,7 +52,7 @@ ERROR_CASES = {
 
 
 def install_cgcnn_stubs():
-    from cgcnn_oracle import CGConv
+    from oracle.cgcnn import CGConv
     from oracle.gps import PyGBatchNorm
     mg.install_stubs()
     tg = sys.modules["torch_geometric.nn"]

@@ -6,11 +6,11 @@ the GPU machines.
 
 What the golden pins: everything in GATStack.py / Base.py / gps.py that runs -- GAT's own _init_conv (head-multiplied BatchNorm
 widths, the two-conv quirk at num_conv_layers = 1, out_lin under GPS) and _init_node_conv, the GPS embedding and wrapper,
-pooling, heads, losses -- EXCEPT PyG's ``GATv2Conv`` itself, which is the restatement in tests/gat_oracle.py [3P-memory];
+pooling, heads, losses -- EXCEPT PyG's ``GATv2Conv`` itself, which is the restatement in oracle/gat.py [3P-memory];
 test_oracle_gat.py pins it by hand-computed cases.
 
-Each case of models_gat.pt stores the seeded state dict as its names in order with one SHA-256 per entry (gat_oracle.state_digest;
-the engine's own seeded construction reproduces the values, gat_oracle.seeded_state checks it), the inputs, the eval-mode
+Each case of models_gat.pt stores the seeded state dict as its names in order with one SHA-256 per entry (stack_support.state_digest;
+the engine's own seeded construction reproduces the values, stack_support.seeded_state checks it), the inputs, the eval-mode
 predictions, and one train-mode step (batch statistics, every dropout off, the attention dropout of the convs included):
 predictions, the reference's own loss, every parameter gradient (the conv-head case: those of its head modules) and the BatchNorm
 running statistics afterwards.  "errors" stores what the reference raises for a conv-type
@@ -27,7 +27,7 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
 import make_golden as mg  # noqa: E402
-from gat_oracle import state_digest  # noqa: E402
+from stack_support import state_digest  # noqa: E402
 import make_pna_golden as mp  # noqa: E402
 
 
@@ -65,7 +65,7 @@ CASES = {
 
 
 def install_gat_stubs():
-    from gat_oracle import GATv2Conv
+    from oracle.gat import GATv2Conv
     from oracle.gps import PyGBatchNorm
     mg.install_stubs()
     tg = sys.modules["torch_geometric.nn"]

@@ -6,7 +6,7 @@ exist on the GPU machines.
 
 What the golden pins: everything in PNAStack.py / Base.py / gps.py that runs -- the layer loop with its BatchNorm feature
 layers, the GPS embedding and wrapper, pooling, heads, losses -- EXCEPT PyG's ``PNAConv`` itself.  That class is third-party
-and absent here, so the generator uses the restatement in tests/pna_oracle.py [3P-memory]; test_oracle_pna.py pins it by
+and absent here, so the generator uses the restatement in oracle/pna.py [3P-memory]; test_oracle_pna.py pins it by
 hand-computed cases instead.  PyG's ``BatchNorm`` is ``PyGBatchNorm`` (a module holding ``.module = BatchNorm1d``), as in
 make_golden.py.
 
@@ -65,7 +65,7 @@ def install_pna_stubs():
     """PNAStack.py imports PNAConv / BatchNorm / Sequential from torch_geometric.nn: PNAConv is the restatement, BatchNorm the PyG
     wrapper; gps.py for the GPS case."""
     from oracle.gps import PyGBatchNorm
-    from pna_oracle import PNAConv
+    from oracle.pna import PNAConv
     mg.install_stubs()
     tg = sys.modules["torch_geometric.nn"]
     tg.PNAConv, tg.BatchNorm = PNAConv, PyGBatchNorm
@@ -153,7 +153,7 @@ def make_dropin(pna):
     create_model_config, _ = md._reference_create()
     # _reference_create re-installs the stubs: put the PNA pieces back and hand PNAStack to the reference's create_model
     from oracle.gps import PyGBatchNorm
-    from pna_oracle import PNAConv
+    from oracle.pna import PNAConv
     sys.modules["torch_geometric.nn"].PNAConv = PNAConv
     sys.modules["hydragnn.models.Base"].BatchNorm = PyGBatchNorm
     pna = mg._load("hydragnn.models.PNAStack", mg.REF + "/hydragnn/models/PNAStack.py")

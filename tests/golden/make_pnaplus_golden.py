@@ -6,7 +6,7 @@ reference tree does not exist on the GPU machines.
 
 What the golden pins: everything in PNAPlusStack.py (its own PNAConv included), Base.py and gps.py that runs.  The PyG pieces it
 imports -- BesselBasisLayer / Envelope, MessagePassing.propagate, DegreeScalerAggregation, Linear, reset -- are the restatements
-in tests/pnaplus_oracle.py [3P-memory]; test_oracle_pnaplus.py pins the basis by hand-computed values.
+in oracle/pnaplus.py and in this file [3P-memory]; test_oracle_pnaplus.py pins the basis by hand-computed values.
 
 Each case of models_pnaplus.pt stores the state dict, the inputs, the eval-mode predictions, and one train-mode step (batch
 statistics, dropout off): predictions, the reference's own loss, every parameter gradient and the BatchNorm running statistics
@@ -25,6 +25,7 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import make_golden as mg  # noqa: E402
 import make_pna_golden as mp  # noqa: E402
+from oracle.pnaeq import DegreeScalerAggregation as _DSA  # noqa: E402
 
 HEAD_CONV = {"node": [{"type": "branch-0", "architecture": {"num_headlayers": 2, "dim_headlayers": [6, 5], "type": "conv"}}]}
 R, EXPO, RADIUS = 5, 5, 3.0
@@ -41,24 +42,62 @@ CASES = {
 }
 
 
+class DegreeScalerAggregation(_DSA):
+    """oracle.pnaeq's restatement, taking PyG's [E, towers, F] messages."""
+
+    def __init__(self, aggr, scaler, deg, train_norm=False):
+        assert not train_norm, "PNAConv's default train_norm=False only"
+        super().__init__(aggr, scaler, deg)
+
+    def forward(self, x, index=None, dim_size=None, **kw):
+        out = super().forward(x.reshape(x.shape[0], -1), index, dim_size)
+        return out.view(out.shape[0], 1, -1)
+
+
+class MessagePassing(torch.nn.Module):
+    """The part of PyG's base class the reference's PNAConv uses: ``aggr_module`` registered first, ``propagate`` gathering
+    x_i = x[edge_index[1]] (target) and x_j = x[edge_index[0]] and aggregating ``message`` at the targets."""
+
+    def __init__(self, aggr=None, node_dim=0, **kw):
+        super().__init__()
+        self.aggr_module = aggr
+
+    def reset_parameters(self):
+        pass
+
+    def propagate(self, edge_index, size=None, x=None, edge_attr=None, rbf=None):
+        src, dst = edge_index[0], edge_index[1]
+        m = self.message(x[dst], x[src], rbf=rbf, edge_attr=edge_attr)
+        return self.aggr_module(m, dst, x.shape[0])
+
+
+def reset(value):
+    """torch_geometric.nn.inits.reset."""
+    if hasattr(value, "reset_parameters"):
+        value.reset_parameters()
+    else:
+        for child in value.children() if hasattr(value, "children") else []:
+            reset(child)
+
+
 def install_pnaplus_stubs():
-    import pnaplus_oracle as po
+    from oracle.pnaplus import BesselBasisLayer
     from oracle.gps import PyGBatchNorm
     mg.install_stubs()
     sys.modules["hydragnn.models.Base"].BatchNorm = PyGBatchNorm
     gps = mg.install_gps_stubs()
     tg = sys.modules["torch_geometric.nn"]
     tg.BatchNorm = PyGBatchNorm
-    mg._mod("torch_geometric.nn.aggr", DegreeScalerAggregation=po.DegreeScalerAggregation)
-    mg._mod("torch_geometric.nn.conv", MessagePassing=po.MessagePassing)
+    mg._mod("torch_geometric.nn.aggr", DegreeScalerAggregation=DegreeScalerAggregation)
+    mg._mod("torch_geometric.nn.conv", MessagePassing=MessagePassing)
     mg._mod("torch_geometric.nn.dense")
     mg._mod("torch_geometric.nn.dense.linear", Linear=torch.nn.Linear)
-    mg._mod("torch_geometric.nn.inits", reset=po.reset)
+    mg._mod("torch_geometric.nn.inits", reset=reset)
     sys.modules["torch_geometric.nn.resolver"].activation_resolver = lambda act, **kw: {"relu": torch.nn.ReLU}[act]()
     sys.modules["torch_geometric.typing"].Adj = object
     sys.modules["torch_geometric.utils"].degree = None
     mg._mod("torch_geometric.nn.models")
-    mg._mod("torch_geometric.nn.models.dimenet", BesselBasisLayer=po.BesselBasisLayer)
+    mg._mod("torch_geometric.nn.models.dimenet", BesselBasisLayer=BesselBasisLayer)
     mod = mg._load("hydragnn.models.PNAPlusStack", mg.REF + "/hydragnn/models/PNAPlusStack.py")
     return mod, gps
 

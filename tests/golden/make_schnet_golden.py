@@ -8,7 +8,7 @@ What the golden pins: everything in SCFStack.py / Base.py / gps.py that runs -- 
 equivariant coordinate update, the GPS embedding, pooling, heads (including conv-type node heads), losses.  The PyG pieces
 SCFStack.py imports (MessagePassing with aggr "add", GaussianSmearing, ShiftedSoftplus, RadiusInteractionGraph on
 oracle/radius_graph.py, which SCFStack.py reaches as RadiusInteractionGraphCPU without CUDA) are the restatements in
-tests/schnet_oracle.py [3P-memory].
+oracle/schnet.py and in this file [3P-memory].
 
 Each case of models_schnet.pt stores the state dict, the inputs, the eval-mode predictions, and one train-mode step (dropout
 off): predictions, the reference's own loss and every parameter gradient, plus the radius graph of every in-layer conv.
@@ -41,18 +41,46 @@ CASES = {
 }
 
 
+class RadiusInteractionGraph(torch.nn.Module):
+    """edge_index = radius_graph(pos, cutoff, batch, max_num_neighbors) (torch_cluster's ordering and truncation,
+    ``oracle.radius_graph``), edge_weight = |pos[row] - pos[col]|."""
+
+    def __init__(self, cutoff=10.0, max_num_neighbors=32):
+        super().__init__()
+        self.cutoff, self.max_num_neighbors = cutoff, max_num_neighbors
+
+    def forward(self, pos, batch):
+        from oracle.radius_graph import radius_graph
+        edge_index = radius_graph(pos, r=self.cutoff, batch=batch, max_num_neighbors=self.max_num_neighbors).to(pos.device)
+        row, col = edge_index
+        return edge_index, (pos[row] - pos[col]).norm(dim=-1)
+
+
+class MessagePassing(torch.nn.Module):
+    """aggr "add", flow source_to_target; ``propagate(edge_index, **kw)`` lifts every ``*_j`` argument of ``message`` to
+    the sources and sums the messages at the targets."""
+
+    def __init__(self, aggr="add", **kw):
+        super().__init__()
+        assert aggr == "add"
+
+    def propagate(self, edge_index, x, W):
+        m = self.message(x[edge_index[0]], W)
+        return m.new_zeros((x.shape[0],) + tuple(m.shape[1:])).index_add_(0, edge_index[1], m)
+
+
 def install_schnet_stubs():
-    import schnet_oracle as so
+    from oracle import schnet as so
     from oracle.gps import PyGBatchNorm
     mg.install_stubs()
     tg = sys.modules["torch_geometric.nn"]
-    tg.MessagePassing = so.MessagePassing
+    tg.MessagePassing = MessagePassing
     sys.modules["torch_geometric"].nn = tg
     mg._mod("torch_geometric.nn.models")
     mg._mod("torch_geometric.nn.models.schnet", GaussianSmearing=so.GaussianSmearing, ShiftedSoftplus=so.ShiftedSoftplus,
-            RadiusInteractionGraph=so.RadiusInteractionGraph)
+            RadiusInteractionGraph=RadiusInteractionGraph)
     mg._mod("hydragnn.preprocess")
-    mg._mod("hydragnn.preprocess.graph_samples_checks_and_updates", RadiusInteractionGraphCPU=so.RadiusInteractionGraph)
+    mg._mod("hydragnn.preprocess.graph_samples_checks_and_updates", RadiusInteractionGraphCPU=RadiusInteractionGraph)
     sys.modules["hydragnn.models.Base"].BatchNorm = PyGBatchNorm
     gps = mg.install_gps_stubs()
     scf = mg._load("hydragnn.models.SCFStack", mg.REF + "/hydragnn/models/SCFStack.py")

@@ -2,7 +2,7 @@
 configurations that went through update_config (hidden_dim = input_dim = 1 without GPS, edge_dim 0 or 1; and GPS with edge_dim
 0), and that model is interchangeable with the reference's own CGCNNStack: same state-dict names, shapes and seeded values, same
 plugin attributes and ``str``, and a reference checkpoint loads into it strictly.  tests/golden/make_cgcnn_golden.py wrote
-dropin_cgcnn.pt by running the reference's code; PyG's CGConv is restated there (tests/cgcnn_oracle.py).  CPU test."""
+dropin_cgcnn.pt by running the reference's code; PyG's CGConv is restated there (oracle/cgcnn.py).  CPU test."""
 import pytest
 import torch
 

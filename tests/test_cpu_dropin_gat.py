@@ -2,7 +2,7 @@
 configurations that went through update_config (edge_dim None without edge features, 1 with the edge length; and GPS without
 edge features), and that model is interchangeable with the reference's own GATStack: same state-dict names, shapes and seeded values, same
 plugin attributes and ``str``, and a reference checkpoint loads into it strictly.  tests/golden/make_gat_golden.py wrote
-dropin_gat.pt by running the reference's code; PyG's GATv2Conv is restated there (tests/gat_oracle.py).  CPU test."""
+dropin_gat.pt by running the reference's code; PyG's GATv2Conv is restated there (oracle/gat.py).  CPU test."""
 import pytest
 import torch
 

@@ -2,7 +2,7 @@
 configurations (EAM-like: 1-wide edge attribute, node head; and without edge attributes, graph head), and that model is
 interchangeable with the reference's own PNAStack: same state-dict names, shapes and seeded values, same plugin attributes and
 ``str``, and a reference checkpoint loads into it strictly.  tests/golden/make_pna_golden.py wrote dropin_pna.pt by running the
-reference's code; PyG's PNAConv is restated there (tests/pna_oracle.py).  CPU test."""
+reference's code; PyG's PNAConv is restated there (oracle/pna.py).  CPU test."""
 import pytest
 import torch
 

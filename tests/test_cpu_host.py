@@ -11,7 +11,7 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import _lib, ops
 from hydragnn_b200.synthetic import ARCH, make_samples
-from test_oracle_golden import GPS_KW, HEAD_KW, MODEL_KW, PNAEQ_KW
+from stack_support import GPS_KW, HEAD_KW, MACE_KW, MODEL_KW, PNAEQ_KW
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -90,7 +90,6 @@ def test_mace_initialisation_matches_oracle_and_tables_agree():
     consumption is pinned to the oracle's restatement, and the engine's coupling tables to the oracle's."""
     from oracle import e3 as oe3, mace as omace
     from hydragnn_b200 import e3 as pe3
-    from test_oracle_mace import MACE_KW
     for extra in ({}, {"max_ell": 3, "node_max_ell": 2, "correlation": 3, "hidden_dim": 4, "num_conv_layers": 3}):
         kw = dict(MACE_KW, **extra)
         torch.manual_seed(0)

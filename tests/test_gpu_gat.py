@@ -1,9 +1,9 @@
 """GAT on the GPU: the fused kernels (hgb_gat_{fwd,bwd}) against an fp64 restatement written here, the attention dropout, the
 raw C-ABI, the fused path against the composed one, the engine's GATStack against models_gat.pt (the reference's own
 GATStack.py + Base.py + gps.py), and one training step at the ogb_gat / ogb_gat_gps shapes against the fp64 oracle of
-tests/gat_oracle.py.
+oracle/gat.py.
 
-Kernel graph (test_gpu_pna._graph): runs of isolated nodes, a target of in-degree 1000, targets of in-degree 1 and 2, random
+Kernel graph (stack_support._graph): runs of isolated nodes, a target of in-degree 1000, targets of in-degree 1 and 2, random
 sources (input self-loops and duplicate pairs included) and shuffled edge ids.  Every output of the backward is checked on its
 own."""
 import math
@@ -18,10 +18,10 @@ import hydragnn_b200 as hb  # noqa: E402
 from hydragnn_b200 import _lib, ops  # noqa: E402
 from hydragnn_b200.gat import gat_composed  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
-from gat_oracle import GATStackOracle, check_grads, engine_kwargs, seeded_state  # noqa: E402
-from pna_oracle import tf32_linears  # noqa: E402
-from test_oracle_golden import _zero_dropout  # noqa: E402
-from test_gpu_pna import _graph, rel_l2, _batch, _bench_batch  # noqa: E402
+from oracle.gat import GATStackOracle  # noqa: E402
+from oracle.tf32 import tf32_linears  # noqa: E402
+from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, _zero_dropout,  # noqa: E402
+                           check_grads, golden_engine, rel_l2, seeded_state)
 
 DEV = "cuda"
 SLOPE = 0.05
@@ -195,26 +195,10 @@ def test_gat_raw_abi_errors_and_empty_sizes():
     assert _lib.query("hgb_gat_workspace_bytes", 1, 1, 9, 1, 0) == -1
 
 
-def _model(c, device=DEV):
-    m = hb.create_model(**engine_kwargs(c))
-    m.load_state_dict(seeded_state(c), strict=True)
-    return m
-
-
-def _train_step(m, c):
-    m.train()
-    _zero_dropout(m)
-    m.zero_grad(set_to_none=True)
-    pred = m(_batch(c["inputs"]))
-    loss, _ = m.loss(pred, c["value"].to(DEV), [i.to(DEV) for i in c["head_index"]])
-    loss.backward()
-    return pred, loss
-
-
 @pytest.mark.parametrize("name", CASES)
 def test_gat_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_gat.pt")[name]
-    m = _model(c).eval()
+    m = golden_engine("GAT", c, seeded_state(c)).eval()
     _lib.trace_begin()
     with torch.no_grad():
         pred = m(_batch(c["inputs"]))
@@ -245,7 +229,7 @@ def test_gat_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_gat.pt")[name]
     res = []
     for composed in (False, True):
-        m = _model(c)
+        m = golden_engine("GAT", c, seeded_state(c))
         m.force_higher_order = composed
         _lib.trace_begin()
         pred, loss = _train_step(m, c)
@@ -261,34 +245,6 @@ def test_gat_fused_path_equals_composed_path(golden_dir, name):
         torch.testing.assert_close(gf[n], gc[n], rtol=1e-3, atol=1e-5 * gmax, msg=lambda s, n=n: n + ": " + s)
 
 
-class _Data:
-    def __init__(self, b, dtype):
-        for k in ("x", "pos", "edge_index", "edge_attr", "batch", "y", "pe", "rel_pe"):
-            v = getattr(b, k, None)
-            setattr(self, k, v.to(dtype) if v is not None and v.is_floating_point() else v)
-
-
-def _oracle_step(kw, state, b, dtype):
-    om = GATStackOracle(**{k: v for k, v in kw.items() if k != "mpnn_type"})
-    om.load_state_dict(state, strict=True)
-    om = om.to(dtype).train()
-    _zero_dropout(om)
-    od = _Data(b, dtype)
-    pred = om(od)
-    loss = om.loss(pred, od.y, [torch.arange(b.y.shape[0])])
-    grads = dict(zip([n for n, _ in om.named_parameters()], torch.autograd.grad(loss, list(om.parameters()))))
-    return [p.detach() for p in pred], loss.detach(), grads
-
-
-def _errors(pred, loss, grads, ref):
-    rpred, rloss, rgrads = ref
-    names = sorted(rgrads)
-    g = torch.cat([grads[n].double().cpu().reshape(-1) for n in names])
-    r = torch.cat([rgrads[n].double().reshape(-1) for n in names])
-    return {"pred": max(rel_l2(p.cpu(), q) for p, q in zip(pred, rpred)),
-            "loss": abs(float(loss) - float(rloss)) / abs(float(rloss)), "grad": rel_l2(g, r)}
-
-
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 @pytest.mark.parametrize("name,graphs", [("ogb_gat", 128), ("ogb_gat_gps", 64)])
 def test_gat_training_step_at_benchmark_shape_matches_oracle(name, graphs, precision):
@@ -299,12 +255,12 @@ def test_gat_training_step_at_benchmark_shape_matches_oracle(name, graphs, preci
     kw = {k: v for k, v in kw.items() if k not in ("pna_deg", "radius", "max_neighbours")}
     em = hb.set_precision(hb.create_model(**kw), precision)
     state = {k: v.detach().cpu().clone() for k, v in em.state_dict().items()}
-    ref64 = _oracle_step(kw, state, b, torch.float64)
+    ref64 = _oracle_step(GATStackOracle, kw, state, b, torch.float64)
     if precision == "fp32":
-        ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+        ref32 = _errors(*_oracle_step(GATStackOracle, kw, state, b, torch.float32), ref64)
     else:
         with tf32_linears():
-            ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+            ref32 = _errors(*_oracle_step(GATStackOracle, kw, state, b, torch.float32), ref64)
     em.train()
     _zero_dropout(em)
     d = b.clone().to(DEV)
@@ -315,7 +271,7 @@ def test_gat_training_step_at_benchmark_shape_matches_oracle(name, graphs, preci
     loss.backward()
     calls = {t[0] for t in _lib.trace_end()}
     assert "hgb_gat_fwd" in calls and "hgb_gat_bwd" in calls
-    eng = _errors([p.detach() for p in pred], loss.detach(), {n: p.grad for n, p in em.named_parameters()}, ref64)
+    eng = _errors([p.detach() for p in pred], loss.detach(), {n: p.grad for n, p in em.named_parameters()}, em.state_dict(), ref64)
     if precision == "fp32":
         # gradients: 4x rather than 2x.  At input width 1 the first conv's lin_l / lin_r bias gradients are sums over every atom
         # that cancel to about 1e-3 of their terms, and the engine's fp32 reductions (its Linear backward, not the attention

@@ -9,7 +9,7 @@ pytestmark = pytest.mark.gpu
 import hydragnn_b200 as hb  # noqa: E402
 from oracle import mace as omace  # noqa: E402
 from oracle.mlip import MLIPWrapper  # noqa: E402
-from test_oracle_mace import MACE_KW, mace_batch, random_rotation  # noqa: E402
+from stack_support import MACE_KW, mace_batch, random_rotation  # noqa: E402
 
 DEV = "cuda"
 

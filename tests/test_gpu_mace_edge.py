@@ -15,8 +15,7 @@ from hydragnn_b200.synthetic import ARCH, make_samples  # noqa: E402
 from mace_edge_oracle import MACEEdgeOracle  # noqa: E402
 from oracle.mlip import MLIPWrapper  # noqa: E402
 from oracle.workloads import add_edges_cpu, arch_for  # noqa: E402
-from test_gpu_round2 import _gpu_batch, _grad_rel, _loader  # noqa: E402
-from test_oracle_mace import MACE_KW, mace_batch, random_rotation  # noqa: E402
+from stack_support import MACE_KW, _gpu_batch, _grad_rel, _loader, mace_batch, random_rotation  # noqa: E402
 
 DEV = "cuda"
 PAIRS = [(lin, lsh) for lsh in (1, 2, 3) for lin in (0, 1, 2) if lin <= lsh]

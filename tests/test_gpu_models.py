@@ -16,7 +16,7 @@ from hydragnn_b200 import ops  # noqa: E402
 from hydragnn_b200.synthetic import ARCH, make_samples  # noqa: E402
 import oracle  # noqa: E402
 from oracle.workloads import add_edges_cpu  # noqa: E402
-from test_oracle_golden import GPS_KW, HEAD_KW, MODEL_KW, PNAEQ_KW, _zero_dropout  # noqa: E402
+from stack_support import GPS_KW, HEAD_KW, MODEL_KW, PNAEQ_KW, _zero_dropout  # noqa: E402
 
 DEV = "cuda"
 

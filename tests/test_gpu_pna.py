@@ -1,6 +1,6 @@
 """PNA on the GPU: the fused PNAConv kernels (hgb_pna_conv_{fwd,bwd}) against an fp64 restatement written here, the raw C-ABI,
 the fused path against the composed one, and the engine's PNAStack against models_pna.pt (the reference's own PNAStack.py +
-Base.py + gps.py, PyG's PNAConv restated in tests/pna_oracle.py).
+Base.py + gps.py, PyG's PNAConv restated in oracle/pna.py).
 
 Kernel cases: widths F in {1, 5, 50, 55, 64, 200} (scalar and float4 paths, widths that are not multiples of 4 or 32), edge
 attribute widths D in {0, 1, 3, 16} (all three register capacities), on a graph with runs of isolated nodes, a target of
@@ -9,7 +9,7 @@ With dyadic inputs fp32 is exact, so ties are real: the first edge in CSR order 
 equal hgb_pna_aggregate_fwd on the materialised messages bit for bit.
 
 At the benchmark shapes (eam_pna: 10 layers at F = 50 with a 1-wide edge attribute; ogb_pna: 6 layers at F = 55) one training
-step is checked against the CPU oracle stack of tests/pna_oracle.py in fp64, on edges built by the oracle's own radius graph:
+step is checked against the CPU oracle stack of oracle/pna.py in fp64, on edges built by the oracle's own radius graph:
 in fp32 and under precision "bf16" (TF32 Linears); and the captured GraphedTrainStep must reproduce the eager steps."""
 import copy
 import math
@@ -22,28 +22,12 @@ pytestmark = pytest.mark.gpu
 import hydragnn_b200 as hb  # noqa: E402
 from hydragnn_b200 import _lib, ops  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
-from hydragnn_b200.synthetic import ARCH, make_samples  # noqa: E402
-from oracle.workloads import add_edges_cpu  # noqa: E402
-from pna_oracle import PNAStackOracle, tf32_linears  # noqa: E402
-from test_oracle_golden import _zero_dropout  # noqa: E402
+from oracle.pna import PNAStackOracle  # noqa: E402
+from oracle.tf32 import tf32_linears  # noqa: E402
+from stack_support import _batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, golden_engine, rel_l2  # noqa: E402
 
 DEV = "cuda"
 CASES = ["pna_graph_noedge", "pna_node_edge_len", "pna_multihead_h5", "pna_gps", "pna_add_pool_edge3"]
-
-
-def rel_l2(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp(min=1e-30))
-
-
-def _graph(seed=0, n=3000):
-    """Nodes 0..99 and 300..399 receive nothing, node 7 receives 1000 edges, 100..199 one each, 200..299 two each, 400.. random."""
-    g = torch.Generator().manual_seed(seed)
-    dst = torch.cat([torch.full((1000,), 7), torch.arange(100, 200), torch.arange(200, 300).repeat(2),
-                     torch.randint(400, n, (3000,), generator=g)])
-    dst[:1000] = 7
-    src = torch.randint(0, n, (dst.numel(),), generator=g)
-    perm = torch.randperm(dst.numel(), generator=g)
-    return torch.stack([src[perm], dst[perm]]).to(DEV), n
 
 
 def _inputs(n, e, f, d, seed, dyadic=False):
@@ -229,39 +213,10 @@ def test_pna_conv_raw_abi_errors_and_empty_sizes():
     torch.cuda.synchronize()
 
 
-def _model(c, device=DEV):
-    cfg = c["cfg"]
-    m = hb.create_model(mpnn_type="PNA", input_dim=cfg["input_dim"], hidden_dim=cfg["hidden_dim"], output_dim=cfg["output_dim"],
-                        output_type=cfg["output_type"], output_heads=cfg["output_heads"], activation_function="relu",
-                        loss_function_type="mse", task_weights=[1.0] * len(cfg["output_type"]), num_conv_layers=cfg["num_conv_layers"],
-                        edge_dim=cfg["edge_dim"], pna_deg=c["deg"], graph_pooling=cfg["graph_pooling"],
-                        pe_dim=4 if cfg["gps"] else 0, global_attn_engine="GPS" if cfg["gps"] else None,
-                        global_attn_type="multihead" if cfg["gps"] else None, global_attn_heads=4 if cfg["gps"] else 0)
-    m.load_state_dict(c["state"], strict=True)
-    return m
-
-
-def _batch(inputs):
-    d = hb.Batch(**{k: v.clone().to(DEV) for k, v in inputs.items()})
-    d._num_graphs = int(inputs["batch"].max()) + 1
-    return d
-
-
-def _train_step(m, c):
-    m.train()
-    _zero_dropout(m)
-    m.zero_grad(set_to_none=True)
-    d = _batch(c["inputs"])
-    pred = m(d)
-    loss, _ = m.loss(pred, c["value"].to(DEV), [i.to(DEV) for i in c["head_index"]])
-    loss.backward()
-    return pred, loss
-
-
 @pytest.mark.parametrize("name", CASES)
 def test_pna_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_pna.pt")[name]
-    m = _model(c).eval()
+    m = golden_engine("PNA", c).eval()
     _lib.trace_begin()
     with torch.no_grad():
         pred = m(_batch(c["inputs"]))
@@ -288,7 +243,7 @@ def test_pna_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_pna.pt")[name]
     res = []
     for composed in (False, True):
-        m = _model(c)
+        m = golden_engine("PNA", c)
         m.force_higher_order = composed
         pred, loss = _train_step(m, c)
         res.append(([p.detach() for p in pred], {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}))
@@ -299,54 +254,6 @@ def test_pna_fused_path_equals_composed_path(golden_dir, name):
     gmax = max(float(g.abs().max()) for g in gc.values())
     for n in gf:
         torch.testing.assert_close(gf[n], gc[n], rtol=1e-3, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-
-
-def _bench_batch(name, graphs):
-    """A synthetic batch of the benchmark workload with the oracle's CPU radius graph, edge lengths as the edge attribute where the
-    architecture reads one, per-atom targets for a node head, and the batch's in-degree histogram."""
-    b = add_edges_cpu(make_samples(name, graphs), name)
-    n = b.pos.shape[0]
-    if ARCH[name].get("edge_dim"):
-        b.edge_attr = (b.pos[b.edge_index[1]] - b.pos[b.edge_index[0]] + b.edge_shifts).norm(dim=1, keepdim=True).contiguous()
-    if ARCH[name]["output_type"] == ["node"]:
-        b.y = torch.randn(n, 1, generator=torch.Generator().manual_seed(11))
-    deg = torch.bincount(torch.bincount(b.edge_index[1], minlength=n)).tolist()
-    return b, dict(ARCH[name], pna_deg=deg)
-
-
-class _Data:
-    def __init__(self, b):
-        for k in ("x", "edge_index", "edge_attr", "batch", "y"):
-            v = getattr(b, k, None)
-            setattr(self, k, v.double() if v is not None and v.is_floating_point() else v)
-
-
-def _oracle_step(kw, state, b, dtype):
-    """One train-mode forward + loss + gradient of the oracle stack in ``dtype`` on the CPU -> (preds, loss, {name: grad}, state)."""
-    om = PNAStackOracle(**kw)
-    om.load_state_dict(state, strict=True)
-    om = om.to(dtype).train()
-    od = _Data(b)
-    for k in ("x", "edge_attr", "y"):
-        if getattr(od, k) is not None:
-            setattr(od, k, getattr(od, k).to(dtype))
-    pred = om(od)
-    loss = om.loss(pred, od.y, [torch.arange(b.y.shape[0])])
-    grads = dict(zip([n for n, _ in om.named_parameters()], torch.autograd.grad(loss, list(om.parameters()))))
-    return [p.detach() for p in pred], loss.detach(), grads, om.state_dict()
-
-
-def _errors(pred, loss, grads, state, ref):
-    """rel-L2 of predictions, loss, all parameter gradients together and the BatchNorm running statistics against ``ref``."""
-    rpred, rloss, rgrads, rstate = ref
-    names = sorted(rgrads)
-    g = torch.cat([grads[n].double().cpu().reshape(-1) for n in names])
-    r = torch.cat([rgrads[n].double().reshape(-1) for n in names])
-    keys = [k for k in rstate if "running" in k]
-    return {"pred": max(rel_l2(p.cpu(), q) for p, q in zip(pred, rpred)),
-            "loss": abs(float(loss) - float(rloss)) / abs(float(rloss)),
-            "grad": rel_l2(g, r),
-            "bn_stats": max(rel_l2(state[k].cpu(), rstate[k]) for k in keys)}
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
@@ -367,12 +274,12 @@ def test_pna_training_step_at_benchmark_shape_matches_oracle(name, graphs, hidde
         kw["hidden_dim"] = hidden
     em = hb.set_precision(hb.create_model(**kw), precision)
     state = {k: v.detach().cpu().clone() for k, v in em.state_dict().items()}
-    ref64 = _oracle_step(kw, state, b, torch.float64)
+    ref64 = _oracle_step(PNAStackOracle, kw, state, b, torch.float64)
     if precision == "fp32":
-        ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+        ref32 = _errors(*_oracle_step(PNAStackOracle, kw, state, b, torch.float32), ref64, bn_stats=True)
     else:
         with tf32_linears():
-            ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+            ref32 = _errors(*_oracle_step(PNAStackOracle, kw, state, b, torch.float32), ref64, bn_stats=True)
     n_atoms, mean_deg = b.pos.shape[0], float(torch.bincount(b.edge_index[1]).float().mean())
     assert n_atoms > 2000 and mean_deg > 8                                    # thousands of atoms, realistic in-degrees
     em.train()
@@ -386,7 +293,7 @@ def test_pna_training_step_at_benchmark_shape_matches_oracle(name, graphs, hidde
     assert "hgb_pna_conv_fwd" in calls and "hgb_pna_conv_bwd" in calls
     if precision == "bf16" and hidden == 64:
         assert any(c.startswith("hgb_tc_linear") for c in calls), sorted(calls)
-    eng = _errors([p.detach() for p in pred], loss.detach(), {n: p.grad for n, p in em.named_parameters()}, em.state_dict(), ref64)
+    eng = _errors([p.detach() for p in pred], loss.detach(), {n: p.grad for n, p in em.named_parameters()}, em.state_dict(), ref64, bn_stats=True)
     if precision == "fp32":
         bound = {"pred": max(1e-5, 2 * ref32["pred"]), "grad": max(1e-4, 2 * ref32["grad"]), "loss": 1e-5, "bn_stats": 1e-5}
     else:

@@ -1,7 +1,7 @@
 """PNAPlus on the GPU: the fused kernels (hgb_pnaplus_conv_{fwd,bwd}) against an fp64 restatement written here, the raw C-ABI,
 the fused path against the composed one, the engine's PNAPlusStack against models_pnaplus.pt (the reference's own
 PNAPlusStack.py + Base.py + gps.py), forces, and one training step at the lj_pnaplus / ogb_pnaplus shapes against the fp64
-oracle of tests/pnaplus_oracle.py.
+oracle of oracle/pnaplus.py.
 
 Kernel graph: runs of isolated nodes, a target of in-degree 1000, targets of in-degree 1 and 2, shuffled edge ids; every
 target's first edge lies past the cutoff (its message is exactly 0, the other messages are continuous, so there are no ties).
@@ -17,10 +17,9 @@ import hydragnn_b200 as hb  # noqa: E402
 from hydragnn_b200 import _lib, ops  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.pnaeq import DegreeScalerAggregation as ODSA  # noqa: E402
-from pna_oracle import tf32_linears  # noqa: E402
-from pnaplus_oracle import PNAPlusStackOracle  # noqa: E402
-from test_oracle_golden import _zero_dropout  # noqa: E402
-from test_gpu_pna import _graph, rel_l2, _batch, _bench_batch  # noqa: E402
+from oracle.pnaplus import PNAPlusStackOracle  # noqa: E402
+from oracle.tf32 import tf32_linears  # noqa: E402
+from stack_support import _batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, golden_engine, rel_l2  # noqa: E402
 
 DEV = "cuda"
 RADIUS, EXPO = 2.0, 5
@@ -131,20 +130,6 @@ def test_pnaplus_conv_raw_abi_errors_and_empty_sizes():
     torch.cuda.synchronize()
 
 
-def _model(c, device=DEV):
-    cfg = c["cfg"]
-    m = hb.create_model(mpnn_type="PNAPlus", input_dim=cfg["input_dim"], hidden_dim=cfg["hidden_dim"], output_dim=cfg["output_dim"],
-                        output_type=cfg["output_type"], output_heads=cfg["output_heads"], activation_function="relu",
-                        loss_function_type="mse", task_weights=[1.0] * len(cfg["output_type"]),
-                        num_conv_layers=cfg["num_conv_layers"], edge_dim=cfg["edge_dim"], pna_deg=c["deg"],
-                        graph_pooling=cfg["graph_pooling"], num_radial=cfg["num_radial"], radius=cfg["radius"],
-                        envelope_exponent=cfg["envelope_exponent"], pe_dim=4 if cfg["gps"] else 0,
-                        global_attn_engine="GPS" if cfg["gps"] else None, global_attn_type="multihead" if cfg["gps"] else None,
-                        global_attn_heads=4 if cfg["gps"] else 0)
-    m.load_state_dict(c["state"], strict=True)
-    return m
-
-
 def _before_batch_norm(name):
     """The biases of a conv's post Linear and last Linear shift every row alike ahead of a BatchNorm with batch statistics, which
     subtracts the mean: their gradients are 0 up to rounding in train mode (largest behind the 1-wide output of a conv head),
@@ -152,20 +137,10 @@ def _before_batch_norm(name):
     return name.endswith(("module_0.lin.bias", "module_0.post_nns.0.0.bias"))
 
 
-def _train_step(m, c):
-    m.train()
-    _zero_dropout(m)
-    m.zero_grad(set_to_none=True)
-    pred = m(_batch(c["inputs"]))
-    loss, _ = m.loss(pred, c["value"].to(DEV), [i.to(DEV) for i in c["head_index"]])
-    loss.backward()
-    return pred, loss
-
-
 @pytest.mark.parametrize("name", CASES)
 def test_pnaplus_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
-    m = _model(c).eval()
+    m = golden_engine("PNAPlus", c).eval()
     _lib.trace_begin()
     with torch.no_grad():
         pred = m(_batch(c["inputs"]))
@@ -196,7 +171,7 @@ def test_pnaplus_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
     res = []
     for composed in (False, True):
-        m = _model(c)
+        m = golden_engine("PNAPlus", c)
         m.force_higher_order = composed
         pred, loss = _train_step(m, c)
         res.append(([p.detach() for p in pred], {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}))
@@ -228,7 +203,7 @@ def test_pnaplus_mlip_matches_reference_golden_and_forces(golden_dir):
     """The MLIP case (eval mode): the loss through the composed any-order path against the reference's energy_force_loss with its
     second-order parameter gradients; the fused first-order path predicts the same forces as -autograd.grad on the composed one."""
     c = torch.load(golden_dir + "/models_pnaplus.pt")["pnaplus_mlip"]
-    m = hb.create.EnhancedModelWrapper(_model(c), 1.0, 1.0, 1.0).eval()
+    m = hb.create.EnhancedModelWrapper(golden_engine("PNAPlus", c), 1.0, 1.0, 1.0).eval()
     d = _batch(c["inputs"])
     d.pos.requires_grad_(True)
     m.model.force_higher_order = True
@@ -251,36 +226,6 @@ def test_pnaplus_mlip_matches_reference_golden_and_forces(golden_dir):
     torch.testing.assert_close(forces[False], forces[True], rtol=1e-4, atol=1e-5)
 
 
-class _Data:
-    def __init__(self, b):
-        for k in ("x", "pos", "edge_index", "edge_shifts", "edge_attr", "batch", "y"):
-            v = getattr(b, k, None)
-            setattr(self, k, v.double() if v is not None and v.is_floating_point() else v)
-
-
-def _oracle_step(kw, state, b, dtype):
-    om = PNAPlusStackOracle(**{k: v for k, v in kw.items() if k != "mpnn_type"})
-    om.load_state_dict(state, strict=True)
-    om = om.to(dtype).train()
-    od = _Data(b)
-    for k in ("x", "pos", "edge_shifts", "edge_attr", "y"):
-        if getattr(od, k) is not None:
-            setattr(od, k, getattr(od, k).to(dtype))
-    pred = om(od)
-    loss = om.loss(pred, od.y, [torch.arange(b.y.shape[0])])
-    grads = dict(zip([n for n, _ in om.named_parameters()], torch.autograd.grad(loss, list(om.parameters()))))
-    return [p.detach() for p in pred], loss.detach(), grads
-
-
-def _errors(pred, loss, grads, ref):
-    rpred, rloss, rgrads = ref
-    names = sorted(rgrads)
-    g = torch.cat([grads[n].double().cpu().reshape(-1) for n in names])
-    r = torch.cat([rgrads[n].double().reshape(-1) for n in names])
-    return {"pred": max(rel_l2(p.cpu(), q) for p, q in zip(pred, rpred)),
-            "loss": abs(float(loss) - float(rloss)) / abs(float(rloss)), "grad": rel_l2(g, r)}
-
-
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 @pytest.mark.parametrize("name,graphs", [("lj_pnaplus", 96), ("ogb_pnaplus", 128)])
 def test_pnaplus_training_step_at_benchmark_shape_matches_oracle(name, graphs, precision):
@@ -300,12 +245,12 @@ def test_pnaplus_training_step_at_benchmark_shape_matches_oracle(name, graphs, p
         b.y = torch.randn(b.pos.shape[0], 1, generator=torch.Generator().manual_seed(11))
     em = hb.set_precision(hb.create_model(**kw), precision)
     state = {k: v.detach().cpu().clone() for k, v in em.state_dict().items()}
-    ref64 = _oracle_step(kw, state, b, torch.float64)
+    ref64 = _oracle_step(PNAPlusStackOracle, kw, state, b, torch.float64)
     if precision == "fp32":
-        ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+        ref32 = _errors(*_oracle_step(PNAPlusStackOracle, kw, state, b, torch.float32), ref64)
     else:
         with tf32_linears():
-            ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+            ref32 = _errors(*_oracle_step(PNAPlusStackOracle, kw, state, b, torch.float32), ref64)
     em.train()
     d = b.clone().to(DEV)
     d._num_graphs = graphs
@@ -315,7 +260,7 @@ def test_pnaplus_training_step_at_benchmark_shape_matches_oracle(name, graphs, p
     loss.backward()
     calls = {t[0] for t in _lib.trace_end()}
     assert "hgb_pnaplus_conv_fwd" in calls and "hgb_pnaplus_conv_bwd" in calls
-    eng = _errors([p.detach() for p in pred], loss.detach(), {n: p.grad for n, p in em.named_parameters()}, ref64)
+    eng = _errors([p.detach() for p in pred], loss.detach(), {n: p.grad for n, p in em.named_parameters()}, em.state_dict(), ref64)
     if precision == "fp32":
         bound = {"pred": max(1e-4, 2 * ref32["pred"]), "grad": max(1e-3, 2 * ref32["grad"]), "loss": max(1e-5, 2 * ref32["loss"])}
     else:

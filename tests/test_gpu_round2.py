@@ -16,26 +16,13 @@ from hydragnn_b200 import ops, radius, stacks  # noqa: E402
 from hydragnn_b200.synthetic import ARCH, WORKLOADS, make_samples  # noqa: E402
 import oracle  # noqa: E402
 from oracle.workloads import add_edges_cpu, arch_for  # noqa: E402
+from stack_support import _gpu_batch, _grad_rel, _loader  # noqa: E402
 
 DEV = "cuda"
 
 
 def rel_l2(a, b):
     return float((a.double().cpu() - b.double().cpu()).norm() / b.double().cpu().norm().clamp(min=1e-30))
-
-
-def _gpu_batch(cpu, name, g):
-    """device twin of a CPU batch with its edges built by the ENGINE's neighbour kernels"""
-    w = WORKLOADS[name]
-    d = make_samples(name, g).to(DEV)
-    d._num_graphs = g
-    if w.get("pbc") or w.get("pbc_box"):
-        d = hb.get_radius_graph_pbc(w["radius"], w["max_neighbours"])(d)
-    else:
-        d = hb.get_radius_graph(w["radius"], w["max_neighbours"])(d)
-    if w.get("pe_dim"):
-        d.rel_pe = (d.pe[d.edge_index[0]] - d.pe[d.edge_index[1]]).abs()
-    return d
 
 
 def _canon(ei, sh=None):
@@ -45,22 +32,6 @@ def _canon(ei, sh=None):
         key = key * 1e3 + (sh * torch.tensor([1.0, 3.0, 9.0], dtype=sh.dtype, device=sh.device)).sum(1).double() * 1e-2
     o = torch.argsort(key, stable=True)
     return o
-
-
-def _grad_rel(em_params, om_params):
-    """rel-L2 over all parameter gradients; accepts parameter lists (same order) or modules (matched by name)."""
-    if isinstance(em_params, torch.nn.Module):
-        en, on = dict(em_params.named_parameters()), dict(om_params.named_parameters())
-        assert set(en) == set(on)
-        em_params, om_params = [en[k] for k in on], [on[k] for k in on]
-    num = den = 0.0
-    for p, q in zip(em_params, om_params):
-        if q.grad is None:
-            continue
-        assert p.grad is not None
-        num += float((p.grad.double().cpu() - q.grad.double()).pow(2).sum())
-        den += float(q.grad.double().pow(2).sum())
-    return (num / max(den, 1e-300)) ** 0.5
 
 
 # ---- C4: periodic MACE at the oc20 shape -------------------------------------------------------------------------------
@@ -370,24 +341,6 @@ def test_tensor_core_attention_matches_fp64_reference(n, f, heads, mode, monkeyp
 
 
 # ---- the API path IS the fast path: capacity-padded captured step behind hb.train (rows a11 / f3) -------------------------------
-def _loader(name, sizes, with_edges, seed0=10):
-    w = WORKLOADS[name]
-    out = []
-    for i, g in enumerate(sizes):
-        b = make_samples(name, g, seed=seed0 + i)
-        if with_edges:
-            d = b.clone().to(DEV)
-            d._num_graphs = g
-            d = (hb.get_radius_graph_pbc if w.get("pbc") else hb.get_radius_graph)(w["radius"], w["max_neighbours"])(d)
-            b.edge_index = d.edge_index.cpu()
-            if d.edge_shifts is not None:
-                b.edge_shifts = d.edge_shifts.cpu()
-        for k in ("cell", "pbc", "ptr"):
-            b.__dict__.pop(k, None)
-        out.append(b)
-    return out
-
-
 @pytest.mark.parametrize("name,mlip,build", [("qm9_painn", False, False), ("qm9_painn", False, True), ("md17_egnn", True, False),
                                              ("md17_egnn", True, True), ("lj_egnn", True, False)])
 def test_train_fast_path_equals_eager_on_variable_batches(name, mlip, build):

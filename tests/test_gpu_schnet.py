@@ -5,14 +5,11 @@ import math
 import pytest
 import torch
 
-import schnet_oracle as so
+from oracle import schnet as so
+from stack_support import _OD, _errors, _oracle, _oracle_step, golden_engine, rel_l2 as _rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm().clamp(min=1e-30))
 
 
 def _graph(gen, n=1200):
@@ -105,21 +102,6 @@ def test_cfconv_rejects_out_of_range_arguments():
                   x.data_ptr(), x.data_ptr(), x.data_ptr(), x.data_ptr(), 4, 0, 10, 129, x.data_ptr(), None, 0)
 
 
-def _model(case, dev=DEV):
-    import hydragnn_b200 as hb
-    cfg = case["cfg"]
-    kw = dict(mpnn_type="SchNet", input_dim=cfg["input_dim"], hidden_dim=cfg["hidden_dim"], output_dim=cfg["output_dim"],
-              output_type=cfg["output_type"], output_heads=cfg["output_heads"], num_conv_layers=cfg["num_conv_layers"],
-              num_filters=cfg["num_filters"], num_gaussians=cfg["num_gaussians"], radius=cfg["radius"],
-              max_neighbours=cfg["max_neighbours"], edge_dim=cfg["edge_dim"], graph_pooling=cfg["graph_pooling"],
-              equivariance=cfg["equivariance"], task_weights=[1.0])
-    if cfg["gps"]:
-        kw.update(global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=4, pe_dim=4)
-    m = hb.create_model(**kw)
-    m.load_state_dict(case["state"], strict=True)
-    return m
-
-
 def _batch(case):
     from hydragnn_b200.data import Data
     d = Data(**{k: v.to(DEV) for k, v in case["inputs"].items()})
@@ -133,7 +115,7 @@ CASES = ["inlayer_graph", "inlayer_truncated", "equivariant_conv_head", "edge_le
 @pytest.mark.parametrize("name", CASES)
 def test_engine_matches_the_reference_stack(golden_dir, name, higher):
     case = torch.load(golden_dir + "/models_schnet.pt")[name]
-    m = _model(case)
+    m = golden_engine("SchNet", case)
     m.force_higher_order = higher
     m.eval()
     with torch.no_grad():
@@ -164,7 +146,7 @@ def test_engine_matches_the_reference_stack(golden_dir, name, higher):
 
 def test_nonzero_edge_shifts_do_not_change_the_result(golden_dir):
     case = torch.load(golden_dir + "/models_schnet.pt")["edge3"]
-    m = _model(case).eval()
+    m = golden_engine("SchNet", case).eval()
     b1, b2 = _batch(case), _batch(case)
     b2.edge_shifts = torch.zeros_like(b2.edge_shifts)
     with torch.no_grad():
@@ -174,7 +156,7 @@ def test_nonzero_edge_shifts_do_not_change_the_result(golden_dir):
 def test_equivariant_layers_rebuild_the_graph_on_the_moved_positions(golden_dir):
     from hydragnn_b200 import ops, radius
     case = torch.load(golden_dir + "/models_schnet.pt")["equivariant_conv_head"]
-    m = _model(case).eval()
+    m = golden_engine("SchNet", case).eval()
     b = _batch(case)
     seen = []
     orig = ops.EdgePlan.__init__
@@ -242,23 +224,7 @@ def test_cfconv_backward_without_parameter_gradients():
     assert torch.equal(gx, full["xl"]) and torch.equal(gr, full["r"]) and torch.equal(gp, full["pos"])
 
 
-# ---- the fp64 oracle stack (tests/schnet_oracle.py, itself checked against the reference's stack on the CPU) -----------------
-class _OD:
-    def __init__(self, b, dtype=torch.float64):
-        for k in ("x", "pos", "batch", "edge_index", "edge_attr", "pe", "rel_pe", "y", "energy", "forces"):
-            v = getattr(b, k, None)
-            if v is not None:
-                v = v.detach().cpu()
-                v = v.to(dtype) if v.is_floating_point() else v
-            setattr(self, k, v)
-
-
-def _oracle(kw, state, dtype=torch.float64):
-    m = so.SCFStackOracle(**kw)
-    m.load_state_dict(state, strict=True)
-    return m.to(dtype)
-
-
+# ---- the fp64 oracle stack (oracle/schnet.py, itself checked against the reference's stack on the CPU) ------------------------
 @pytest.mark.parametrize("nf,g", [(130, 10), (16, 65)])
 def test_shapes_outside_the_kernel_run_composed_and_match_fp64(golden_dir, nf, g):
     import hydragnn_b200 as hb
@@ -277,10 +243,10 @@ def test_shapes_outside_the_kernel_run_composed_and_match_fp64(golden_dir, nf, g
     loss.backward()
     calls = {c[0] for c in _lib.trace_end()}
     assert "hgb_cfconv_fwd" not in calls and "hgb_cfconv_bwd" not in calls
-    om = _oracle(kw, state).train()
+    om = _oracle(so.SCFStackOracle, kw, state).train()
     od = _OD(b)
     opred = om(od)
-    oloss = om.loss(opred, od.y.reshape(-1), [torch.arange(od.y.numel())])
+    oloss, _ = om.loss(opred, od.y.reshape(-1), [torch.arange(od.y.numel())])
     ograds = dict(zip([n for n, _ in om.named_parameters()], torch.autograd.grad(oloss, list(om.parameters()))))
     assert _rel(pred[0].detach().cpu(), opred[0].detach()) < 1e-5
     for n, p in em.named_parameters():
@@ -304,7 +270,7 @@ def test_mlip_forces_and_force_loss_gradients_match_fp64():
     d._num_graphs = 32
     d.pos.requires_grad_(True)
     f_eng = -torch.autograd.grad(w(d)[0].sum(), d.pos)[0]
-    om = _oracle(kw, state)
+    om = _oracle(so.SCFStackOracle, kw, state)
     od = _OD(b)
     od.pos.requires_grad_(True)
     f_ref = -torch.autograd.grad(om(od)[0].sum(), od.pos)[0]
@@ -341,24 +307,6 @@ def _workload(name, graphs):
     return b, dict(ARCH[name])
 
 
-def _errors(pred, loss, grads, ref):
-    rpred, rloss, rgrads = ref
-    names = sorted(rgrads)
-    g = torch.cat([grads[n].double().cpu().reshape(-1) for n in names])
-    r = torch.cat([rgrads[n].double().cpu().reshape(-1) for n in names])
-    return {"pred": max(_rel(p.detach().cpu(), q) for p, q in zip(pred, rpred)),
-            "loss": abs(float(loss) - float(rloss)) / abs(float(rloss)), "grad": _rel(g, r)}
-
-
-def _oracle_step(kw, state, b, dtype):
-    om = _oracle(kw, state, dtype).train()
-    od = _OD(b, dtype)
-    pred = om(od)
-    loss = om.loss(pred, od.y.reshape(-1), [torch.arange(od.y.numel())])
-    grads = torch.autograd.grad(loss, list(om.parameters()))
-    return [p.detach() for p in pred], loss.detach(), dict(zip([n for n, _ in om.named_parameters()], grads))
-
-
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
 @pytest.mark.parametrize("name,graphs", [("qm9_schnet", 128), ("md17_schnet", 64), ("ci_schnet", 128)])
 def test_training_step_at_workload_shape_matches_oracle(name, graphs, precision):
@@ -367,7 +315,7 @@ def test_training_step_at_workload_shape_matches_oracle(name, graphs, precision)
     fixed bounds (fp32: outputs and loss rel-L2 1e-5, gradients 1e-4; TF32: 2e-2)."""
     import hydragnn_b200 as hb
     from hydragnn_b200 import _lib
-    from pna_oracle import tf32_linears
+    from oracle.tf32 import tf32_linears
     b, kw = _workload(name, graphs)
     em = hb.set_precision(hb.create_model(**kw), precision)
     for mod in em.modules():
@@ -376,12 +324,12 @@ def test_training_step_at_workload_shape_matches_oracle(name, graphs, precision)
         if hasattr(mod, "dropout") and isinstance(mod.dropout, float):
             mod.dropout = 0.0
     state = {k: v.detach().cpu().clone() for k, v in em.state_dict().items()}
-    ref64 = _oracle_step(kw, state, b, torch.float64)
+    ref64 = _oracle_step(so.SCFStackOracle, kw, state, b, torch.float64)
     if precision == "fp32":
-        ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+        ref32 = _errors(*_oracle_step(so.SCFStackOracle, kw, state, b, torch.float32), ref64)
     else:
         with tf32_linears():
-            ref32 = _errors(*_oracle_step(kw, state, b, torch.float32), ref64)
+            ref32 = _errors(*_oracle_step(so.SCFStackOracle, kw, state, b, torch.float32), ref64)
     em.train()
     d = b.clone().to(DEV)
     d._num_graphs = graphs
@@ -393,7 +341,7 @@ def test_training_step_at_workload_shape_matches_oracle(name, graphs, precision)
     from hydragnn_b200.schnet import FUSED_MAX_FILTERS
     fused = kw["num_filters"] <= FUSED_MAX_FILTERS                   # ci_schnet (126 filters) runs the composed path
     assert ("hgb_cfconv_fwd" in calls and "hgb_cfconv_bwd" in calls) == fused, sorted(calls)
-    eng = _errors(pred, loss.detach(), {n: p.grad for n, p in em.named_parameters()}, ref64)
+    eng = _errors(pred, loss.detach(), {n: p.grad for n, p in em.named_parameters()}, em.state_dict(), ref64)
     if precision == "fp32":
         bound = {"pred": max(1e-5, 2 * ref32["pred"]), "grad": max(1e-4, 2 * ref32["grad"]), "loss": max(1e-5, 2 * ref32["loss"])}
     else:

@@ -1,4 +1,4 @@
-"""CGCNN on the CPU: the CGConv restatement (tests/cgcnn_oracle.py) by hand-computed cases, the oracle stack against the
+"""CGCNN on the CPU: the CGConv restatement (oracle/cgcnn.py) by hand-computed cases, the oracle stack against the
 reference's own CGCNNStack.py + Base.py + gps.py (tests/golden/models_cgcnn.pt), and the engine's construction: seeded state
 dict, names, ``str``, strict loading of the reference's checkpoint, and the refusals the reference shares."""
 import math
@@ -7,9 +7,11 @@ import pytest
 import torch
 
 import hydragnn_b200 as hb
-from cgcnn_oracle import CGConv, oracle_from_case
 from hydragnn_b200 import padded
 from hydragnn_b200.cgcnn import CGCNNStack
+from oracle.base import oracle_from_case
+from oracle.cgcnn import CGCNNStackOracle, CGConv
+from stack_support import engine_kwargs
 
 CASES = ["cgcnn_graph_edge0", "cgcnn_node_edge_len", "cgcnn_add_pool_edge3", "cgcnn_multihead", "cgcnn_mlp_per_node", "cgcnn_gps",
          "cgcnn_gps_edge2", "cgcnn_ci_width1"]
@@ -91,7 +93,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole CGCNN stack (fp64) against the reference's: eval and train-mode predictions, the loss, every parameter
     gradient and the BatchNorm running statistics."""
     c = _golden(golden_dir)[name]
-    m = oracle_from_case(c)
+    m = oracle_from_case(CGCNNStackOracle, c)
     d = _Data(c["inputs"])
     rel = lambda a, b: float((a - b.double()).norm() / b.double().norm())                # noqa: E731
     m.eval()
@@ -100,7 +102,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     m.train()
     pred = m(d)
     assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss = m.loss(pred, c["value"].double(), c["head_index"])
+    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
     torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
     grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
     gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
@@ -115,11 +117,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
 
 
 def engine_from_case(c, **kw):
-    cfg = dict(c["cfg"])
-    gps = cfg.pop("gps")
-    if gps:
-        cfg.update(pe_dim=4, global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=4)
-    return hb.create_model(mpnn_type="CGCNN", task_weights=[1.0] * len(cfg["output_type"]), use_gpu=False, **cfg, **kw)
+    return hb.create_model(**engine_kwargs("CGCNN", c), use_gpu=False, **kw)
 
 
 @pytest.mark.parametrize("name", CASES)

@@ -1,4 +1,4 @@
-"""GAT on the CPU: the GATv2Conv restatement (tests/gat_oracle.py) by hand-computed cases, the oracle stack against the
+"""GAT on the CPU: the GATv2Conv restatement (oracle/gat.py) by hand-computed cases, the oracle stack against the
 reference's own GATStack.py + Base.py + gps.py (tests/golden/models_gat.pt), and the engine's construction: seeded state dict,
 names, ``str``, strict loading of the reference's checkpoint, and the refusals."""
 import math
@@ -7,9 +7,11 @@ import pytest
 import torch
 
 import hydragnn_b200 as hb
-from gat_oracle import GATv2Conv, check_grads, engine_kwargs, oracle_from_case, seeded_state, state_digest
 from hydragnn_b200 import ops, padded
 from hydragnn_b200.gat import GATStack
+from oracle.base import oracle_from_case
+from oracle.gat import GATStackOracle, GATv2Conv
+from stack_support import check_grads, engine_kwargs, seeded_state, state_digest
 
 CASES = ["gat_graph_noedge", "gat_node_edge_len", "gat_multihead", "gat_add_pool_edge3", "gat_one_layer", "gat_input_ne_hidden",
          "gat_conv_head", "gat_gps", "gat_gps_edge2", "gat_loops_dups_isolated"]
@@ -118,7 +120,7 @@ def test_gatv2conv_hand_computed_gradients(concat):
 @pytest.mark.parametrize("name", CASES)
 def test_oracle_stack_matches_reference_golden(golden_dir, name):
     c = _golden(golden_dir)[name]
-    m = oracle_from_case(c)
+    m = oracle_from_case(GATStackOracle, c, seeded_state(c))
     d = _Data(c["inputs"])
     rel = lambda a, b: float((a - b.double()).norm() / max(float(b.double().norm()), 1e-12))  # noqa: E731
     m.eval()
@@ -127,7 +129,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     m.train()
     pred = m(d)
     assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss = m.loss(pred, c["value"].double(), c["head_index"])
+    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
     # the golden is the reference's fp32 arithmetic: the 120-wide head convs of gat_conv_head put its loss 1.2e-6 from fp64
     torch.testing.assert_close(float(loss), float(c["loss"]), rtol=5e-6, atol=0)
     grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
@@ -147,7 +149,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
 
 
 def engine_from_case(c, **kw):
-    return hb.create_model(**engine_kwargs(c), use_gpu=False, **kw)
+    return hb.create_model(**engine_kwargs("GAT", c), use_gpu=False, **kw)
 
 
 @pytest.mark.parametrize("name", CASES)

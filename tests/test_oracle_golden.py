@@ -9,6 +9,7 @@ import torch
 import oracle
 from oracle.base import OracleModel
 from oracle.mlip import MLIPWrapper
+from stack_support import GPS_KW, HEAD_KW, MODEL_KW, PNAEQ_KW, _zero_dropout
 
 TOL = dict(rtol=1e-5, atol=1e-6)
 
@@ -52,24 +53,6 @@ def test_painn_layer(golden_dir):
     s3, none = upl(s1, v1)
     assert none is None
     torch.testing.assert_close(s3, c["s3"], **TOL)
-
-
-HEADS_NODE = {"node": [{"type": "branch-0", "architecture": {"num_headlayers": 2, "dim_headlayers": [12, 6], "type": "mlp"}}]}
-HEADS_GRAPH = {"graph": [{"type": "branch-0", "architecture": {"num_sharedlayers": 2, "dim_sharedlayers": 5,
-                                                               "num_headlayers": 2, "dim_headlayers": [10, 7]}}]}
-
-MODEL_KW = {
-    "egnn_mlip": dict(mpnn_type="EGNN", input_dim=1, hidden_dim=16, output_dim=[1], output_type=["node"],
-                      output_heads=HEADS_NODE, activation_function="relu", num_conv_layers=3, task_weights=[1.0]),
-    "egnn_equiv_multihead": dict(mpnn_type="EGNN", input_dim=2, hidden_dim=12, output_dim=[1, 3],
-                                 output_type=["graph", "node"], output_heads=dict(HEADS_GRAPH, **HEADS_NODE),
-                                 activation_function="lrelu_01", num_conv_layers=3, task_weights=[1.0, 2.0],
-                                 equivariance=True, graph_pooling="add"),
-    "painn_graph_mean": dict(mpnn_type="PAINN", input_dim=1, hidden_dim=16, output_dim=[1], output_type=["graph"],
-                             output_heads=HEADS_GRAPH, activation_function="relu", num_conv_layers=2,
-                             task_weights=[1.0], num_radial=5, radius=7.0, graph_pooling="mean"),
-}
-MODEL_KW["painn_graph_max"] = dict(MODEL_KW["painn_graph_mean"], graph_pooling="max")
 
 
 def test_state_dict_keys_match_reference(golden_dir):
@@ -136,10 +119,6 @@ def test_pbc_limit_neighbors(golden_dir):
         assert np.array_equal(np.asarray(a), b.numpy())
 
 
-PNAEQ_KW = dict(mpnn_type="PNAEq", input_dim=1, hidden_dim=12, output_dim=[1], output_type=["graph"], output_heads=HEADS_GRAPH,
-                activation_function="relu", num_conv_layers=3, task_weights=[1.0], num_radial=6, radius=5.0)
-
-
 def test_pnaeq_matches_reference_golden(golden_dir):
     """Everything in PNAEqStack.py is the reference's own code; the PyG DegreeScalerAggregation inside it is the
     restated one (see tests/golden/make_golden.py)."""
@@ -159,24 +138,6 @@ def test_pnaeq_matches_reference_golden(golden_dir):
             assert (gr is None) == (ref is None), n
             if gr is not None:
                 torch.testing.assert_close(gr, ref, rtol=1e-4, atol=1e-6)
-
-
-GPS_KW = {
-    "gps_egnn": dict(mpnn_type="EGNN", input_dim=2, hidden_dim=16, output_dim=[1], output_type=["graph"], output_heads=HEADS_GRAPH,
-                     activation_function="relu", num_conv_layers=2, task_weights=[1.0], global_attn_engine="GPS",
-                     global_attn_type="multihead", global_attn_heads=4, pe_dim=4),
-    "gps_painn": dict(mpnn_type="PAINN", input_dim=2, hidden_dim=16, output_dim=[1], output_type=["graph"], output_heads=HEADS_GRAPH,
-                      activation_function="relu", num_conv_layers=2, task_weights=[1.0], num_radial=5, radius=7.0,
-                      global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=4, pe_dim=4),
-}
-
-
-def _zero_dropout(m):
-    for mod in m.modules():
-        if isinstance(mod, torch.nn.Dropout):
-            mod.p = 0.0
-        if hasattr(mod, "dropout") and isinstance(getattr(mod, "dropout"), float):
-            mod.dropout = 0.0
 
 
 def test_gps_matches_reference_golden(golden_dir):
@@ -207,18 +168,6 @@ def test_gps_matches_reference_golden(golden_dir):
         sd = m.state_dict()
         for k, v in c["state_after"].items():
             torch.testing.assert_close(sd[k], v, rtol=1e-4, atol=1e-6)
-
-
-HEADS_PERNODE = {"node": {"num_headlayers": 2, "dim_headlayers": [7, 5], "type": "mlp_per_node"}}
-HEADS_CONV = {"node": {"num_headlayers": 2, "dim_headlayers": [10, 6], "type": "conv"}}
-HEAD_KW = {
-    "egnn_mlp_per_node": dict(mpnn_type="EGNN", input_dim=1, hidden_dim=12, output_dim=[2], output_type=["node"], output_heads=HEADS_PERNODE,
-                              activation_function="relu", num_conv_layers=2, task_weights=[1.0], num_nodes=6),
-    "egnn_conv_head": dict(mpnn_type="EGNN", input_dim=1, hidden_dim=12, output_dim=[2], output_type=["node"], output_heads=HEADS_CONV,
-                           activation_function="relu", num_conv_layers=2, task_weights=[1.0]),
-    "painn_conv_head": dict(mpnn_type="PAINN", input_dim=1, hidden_dim=12, output_dim=[2], output_type=["node"], output_heads=HEADS_CONV,
-                            activation_function="relu", num_conv_layers=2, task_weights=[1.0], num_radial=5, radius=7.0),
-}
 
 
 def test_node_heads_mlp_per_node_and_conv_match_reference_golden(golden_dir):

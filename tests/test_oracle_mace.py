@@ -9,32 +9,7 @@ import torch
 
 import hydragnn_b200 as hb
 from oracle import e3, mace
-from oracle.radius_graph import radius_graph
-
-MACE_KW = dict(input_dim=1, hidden_dim=8, output_dim=[1, 3], output_type=["graph", "node"],
-               output_heads={"graph": {"num_sharedlayers": 2, "dim_sharedlayers": 5, "num_headlayers": 2, "dim_headlayers": [10, 6]},
-                             "node": {"num_headlayers": 2, "dim_headlayers": [12, 12], "type": "mlp"}},
-               activation_function="relu", loss_function_type="mae", task_weights=[1.0, 1.0], num_conv_layers=2, num_radial=8,
-               radius=6.0, max_ell=2, node_max_ell=1, avg_num_neighbors=10.0, envelope_exponent=5, correlation=2, graph_pooling="mean", num_nodes=9)
-
-
-def random_rotation(gen):
-    q = torch.randn(4, generator=gen, dtype=torch.float64)
-    a, b, c, d = (q / q.norm()).tolist()
-    return torch.tensor([[a * a + b * b - c * c - d * d, 2 * (b * c - a * d), 2 * (b * d + a * c)],
-                         [2 * (b * c + a * d), a * a - b * b + c * c - d * d, 2 * (c * d - a * b)],
-                         [2 * (b * d - a * c), 2 * (c * d + a * b), a * a - b * b - c * c + d * d]], dtype=torch.float64)
-
-
-def mace_batch(gen, sizes=(7, 9), box=4.0, radius=6.0):
-    pos = torch.cat([torch.rand(k, 3, generator=gen, dtype=torch.float64) * box for k in sizes])
-    batch = torch.cat([torch.full((k,), i) for i, k in enumerate(sizes)])
-    z = torch.randint(1, 10, (sum(sizes), 1), generator=gen).double()
-    ei = radius_graph(pos.float(), radius, batch, max_num_neighbors=100)
-    d = hb.Batch(x=z, pos=pos, edge_index=ei, batch=batch)
-    d._num_graphs = len(sizes)
-    return d
-
+from stack_support import MACE_KW, mace_batch, random_rotation
 
 def test_irreps_bookkeeping():
     ir = e3.Irreps("64x0e + 64x1o")

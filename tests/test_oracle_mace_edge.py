@@ -7,7 +7,7 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import padded
 from mace_edge_oracle import MACEEdgeOracle
-from test_oracle_mace import MACE_KW, mace_batch, random_rotation
+from stack_support import MACE_KW, mace_batch, random_rotation
 
 
 def _golden(golden_dir):

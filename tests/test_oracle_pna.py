@@ -1,4 +1,4 @@
-"""CPU checks of the PNAConv restatement (tests/pna_oracle.py) and of the engine's seeded construction.
+"""CPU checks of the PNAConv restatement (oracle/pna.py) and of the engine's seeded construction.
 
 models_pna.pt pins the reference's PNAStack / Base code with this restatement standing in for PyG's PNAConv, so the
 restatement itself is pinned here by hand-computed cases: x_i (the target, edge_index[1]) is the first block of the pre_nn
@@ -10,7 +10,8 @@ import pytest
 import torch
 
 from hydragnn_b200.pna import AGGREGATORS, SCALERS, PNAStack
-from pna_oracle import PNAConv
+from oracle.base import oracle_from_case
+from oracle.pna import PNAConv, PNAStackOracle
 
 # nodes 0..4, x = [1, 2, 4, 8, 16]; edges (source -> target): 1->0, 2->0 (two into 0), 0->3 (one), 2->4 twice (a tie);
 # nodes 1 and 2 receive nothing
@@ -122,13 +123,8 @@ class _Data:
 def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole PNA stack (fp64) against the reference's PNAStack.py + Base.py: eval and train-mode predictions, the loss,
     every parameter gradient and the BatchNorm running statistics after the step.  (GPS is the reference's gps.py, not restated.)"""
-    from pna_oracle import PNAStackOracle
     c = torch.load(golden_dir + "/models_pna.pt")[name]
-    cfg = c["cfg"]
-    m = PNAStackOracle(cfg["input_dim"], cfg["hidden_dim"], cfg["output_dim"], cfg["output_type"], cfg["output_heads"], c["deg"],
-                       edge_dim=cfg["edge_dim"], num_conv_layers=cfg["num_conv_layers"], graph_pooling=cfg["graph_pooling"])
-    m.load_state_dict(c["state"], strict=True)
-    m = m.double()
+    m = oracle_from_case(PNAStackOracle, c)
     d = _Data(c["inputs"])
     rel = lambda a, b: float((a - b.double()).norm() / b.double().norm())                # noqa: E731
     m.eval()
@@ -137,7 +133,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     m.train()
     pred = m(d)
     assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss = m.loss(pred, c["value"].double(), c["head_index"])
+    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
     torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
     grads = torch.autograd.grad(loss, list(m.parameters()))
     gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)

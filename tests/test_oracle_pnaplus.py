@@ -1,4 +1,4 @@
-"""CPU checks of the PNAPlus restatements (tests/pnaplus_oracle.py) and of the engine's seeded construction.
+"""CPU checks of the PNAPlus restatements (oracle/pnaplus.py) and of the engine's seeded construction.
 
 models_pnaplus.pt pins the reference's own PNAPlusStack.py / Base.py with PyG's BesselBasisLayer / Envelope restated, so the
 basis is pinned here by hand-computed values and derivatives (d/d dist and d/d freq), and the oracle stack is checked against
@@ -9,7 +9,8 @@ import math
 import pytest
 import torch
 
-from pnaplus_oracle import BesselBasisLayer, Envelope, PNAPlusStackOracle
+from oracle.base import oracle_from_case
+from oracle.pnaplus import BesselBasisLayer, Envelope, PNAPlusStackOracle
 
 CASES = ["pnaplus_graph_noedge", "pnaplus_node_edge_len", "pnaplus_multihead_h5", "pnaplus_gps", "pnaplus_edge_dim0",
          "pnaplus_add_pool_edge3", "pnaplus_conv_head"]
@@ -101,22 +102,13 @@ class _Data:
             self.edge_attr = None
 
 
-def _oracle(c):
-    cfg = c["cfg"]
-    m = PNAPlusStackOracle(cfg["input_dim"], cfg["hidden_dim"], cfg["output_dim"], cfg["output_type"], cfg["output_heads"], c["deg"],
-                           edge_dim=cfg["edge_dim"], num_conv_layers=cfg["num_conv_layers"], graph_pooling=cfg["graph_pooling"],
-                           num_radial=cfg["num_radial"], radius=cfg["radius"], envelope_exponent=cfg["envelope_exponent"])
-    m.load_state_dict(c["state"], strict=True)
-    return m.double()
-
-
 @pytest.mark.parametrize("name", ["pnaplus_graph_noedge", "pnaplus_node_edge_len", "pnaplus_multihead_h5", "pnaplus_edge_dim0",
                                   "pnaplus_add_pool_edge3"])
 def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole PNAPlus stack (fp64) against the reference's PNAPlusStack.py + Base.py: eval and train-mode predictions,
     the loss, every parameter gradient (None where the reference's is None) and the BatchNorm running statistics."""
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
-    m = _oracle(c)
+    m = oracle_from_case(PNAPlusStackOracle, c)
     d = _Data(c["inputs"])
     dist = (d.pos[d.edge_index[1]] - d.pos[d.edge_index[0]]).norm(dim=-1)
     assert float(dist.max()) > c["cfg"]["radius"] > float(dist.min())                    # edges on both sides of the cutoff
@@ -127,7 +119,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     m.train()
     pred = m(d)
     assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss = m.loss(pred, c["value"].double(), c["head_index"])
+    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
     torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
     grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
     gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
@@ -151,7 +143,7 @@ def test_edge_dim0_keeps_an_unused_edge_encoder(golden_dir):
 def test_oracle_mlip_matches_reference_golden(golden_dir):
     """Energy + per-atom energy + force loss in eval mode: forces and the second-order parameter gradients."""
     c = torch.load(golden_dir + "/models_pnaplus.pt")["pnaplus_mlip"]
-    m = _oracle(c)
+    m = oracle_from_case(PNAPlusStackOracle, c)
     m.eval()
     d = _Data(c["inputs"])
     d.pos.requires_grad_(True)

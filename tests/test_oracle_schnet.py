@@ -1,4 +1,4 @@
-"""tests/schnet_oracle.py pinned by hand-computed cases, and its CFConv checked against the reference's own stack
+"""oracle/schnet.py pinned by hand-computed cases, and its CFConv checked against the reference's own stack
 (models_schnet.pt, written by tests/golden/make_schnet_golden.py).  CPU test."""
 import math
 
@@ -6,7 +6,8 @@ import torch
 
 import pytest
 
-import schnet_oracle as so
+from oracle import schnet as so
+from oracle.base import oracle_from_case
 
 
 def test_gaussian_coefficient_and_values():
@@ -73,7 +74,7 @@ def test_oracle_stack_matches_the_reference(golden_dir, name):
     """The oracle stack at fp64 against the reference's own SCFStack (fp32): eval predictions, the train-mode loss and every
     parameter gradient."""
     case = torch.load(golden_dir + "/models_schnet.pt")[name]
-    m = so.oracle_from_case(case)
+    m = oracle_from_case(so.SCFStackOracle, case)
     d = _D(case["inputs"], torch.float64)
     m.eval()
     with torch.no_grad():
@@ -83,7 +84,7 @@ def test_oracle_stack_matches_the_reference(golden_dir, name):
     pred = m(d)
     for p, ref in zip(pred, case["pred_train"]):
         assert _rel(p, ref) < 1e-5, name
-    loss = m.loss(pred, case["value"].double(), [torch.arange(case["value"].numel())])
+    loss, _ = m.loss(pred, case["value"].double(), [torch.arange(case["value"].numel())])
     assert abs(float(loss) - float(case["loss"])) <= 1e-5 * abs(float(case["loss"]))
     grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
     for (n, _), g in zip(m.named_parameters(), grads):
