@@ -1018,6 +1018,7 @@ extern "C" int hgb_pnaplus_conv_bwd(const float* g_out, const float* pq, const f
 #define CGC_MAX_F 128
 #define CGC_MAX_D 16
 #define CGC_BWD_MAX_BLOCKS (HGB_NUM_SMS * 4)
+#define CGC_BWD_WARPS 8
 
 // torch's sigmoid and softplus (beta 1, threshold 20) with the accurate exp / log1p: the fp32 configs are held to fp64
 __device__ __forceinline__ float cgc_sigmoid(float z) { return 1.f / (1.f + expf(-z)); }
@@ -1220,9 +1221,14 @@ __global__ void __launch_bounds__(256) cgconv_bwd_kernel(
 
 namespace {
 struct CgcLaunch {
-  int cpt, gl2, warps;
+  int cpt, gl2;
   size_t fwd_smem, bwd_smem;
 };
+
+// The backward always runs 8 warps: at the largest shape (f = 128, d = 16, CPT 4) the staged parameters and the 8 warps'
+// accumulator slots take (17 * 256 + 8 * 17 * 2 * 4 * 32) * 4 = 156,672 bytes, within the 227 KB a CTA may opt into.
+static_assert(((CGC_MAX_D + 1) * 2 * CGC_MAX_F + CGC_BWD_WARPS * (CGC_MAX_D + 1) * 2 * 4 * 32) * 4 <= 227 * 1024,
+              "cgconv_bwd: the 8-warp shared memory must fit at every supported shape");
 
 CgcLaunch cgc_launch(int f, int d, bool grads) {
   CgcLaunch L;
@@ -1231,9 +1237,8 @@ CgcLaunch cgc_launch(int f, int d, bool grads) {
   while ((1 << L.gl2) < f && L.gl2 < 5) ++L.gl2;
   const size_t params = (size_t)(d + 1) * 2 * f;
   const size_t slots = grads ? (size_t)(d + 1) * 2 * L.cpt * 32 : 0;
-  L.warps = (params + 8 * slots) * 4 <= 160 * 1024 ? 8 : 4;
   L.fwd_smem = params * 4;
-  L.bwd_smem = (params + L.warps * slots) * 4;
+  L.bwd_smem = (params + CGC_BWD_WARPS * slots) * 4;
   return L;
 }
 }  // namespace
@@ -1291,12 +1296,12 @@ extern "C" int hgb_cgconv_bwd(const float* g_out, const float* pq, const int32_t
     return cudaPeekAtLastError() == cudaSuccess ? HGB_OK : HGB_ECUDA;
   }
   const CgcLaunch L = cgc_launch(f, d, grads);
-  const int grid = hgb_grid_for(n, L.warps * (32 >> L.gl2), CGC_BWD_MAX_BLOCKS);
+  const int grid = hgb_grid_for(n, CGC_BWD_WARPS * (32 >> L.gl2), CGC_BWD_MAX_BLOCKS);
   float* part = grads ? static_cast<float*>(workspace) : nullptr;
 #define CGC_BWD(CPT)                                                                                                         \
   do {                                                                                                                       \
     cudaFuncSetAttribute(cgconv_bwd_kernel<CPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.bwd_smem);             \
-    cgconv_bwd_kernel<CPT><<<grid, L.warps * 32, L.bwd_smem, (cudaStream_t)stream>>>(                                        \
+    cgconv_bwd_kernel<CPT><<<grid, CGC_BWD_WARPS * 32, L.bwd_smem, (cudaStream_t)stream>>>(                                        \
         g_out, pq, rowptr, perm, src, eattr, d, mt, cvec, n, f, L.gl2, g_p, ldgp, g_h, g_eattr, part);                       \
   } while (0)
   if (L.cpt == 1) CGC_BWD(1);

@@ -617,8 +617,9 @@ int hgb_cgconv_bwd(const float* g_out, const float* pq, const int32_t* rowptr, c
  * g_xlr [n, 2 hc]; g_eattr [e, d] when non-NULL (input self-loops get 0; every in-edge receives its share of its target's
  * self-loop mean); g_params (NULL: not computed) [1 + d, hc] = [g_att ; g_mt] from per-CTA partials reduced in fixed order
  * in fp64.  The bias gradient is the column sum of g_out and is not formed here.  Deterministic: no atomics.
- * 1 <= heads <= 8, 1 <= c, heads c <= 1024, 0 <= d <= 16 (hgb_gat_supported); 0 <= p < 1.  n = 0 launches nothing; e = 0
- * runs the self-loops only.  workspace: hgb_gat_workspace_bytes(n, e, heads, c, d) bytes (-1: unsupported).             */
+ * 1 <= heads <= 8, 1 <= c, heads c <= 512 when c % 4 == 0, else <= 256, 0 <= d <= 16 (hgb_gat_supported); 0 <= p < 1.
+ * heads c > 256 also needs 16-byte aligned xlr and out (forward) or xlr, g_out and g_xlr (backward): without it the call
+ * fails before any launch.  n = 0 launches nothing; e = 0 runs the self-loops only.  workspace: hgb_gat_workspace_bytes(n, e, heads, c, d) bytes (-1: unsupported).             */
 int hgb_gat_supported(int32_t heads, int32_t c, int32_t d);
 int64_t hgb_gat_workspace_bytes(int32_t n, int32_t e, int32_t heads, int32_t c, int32_t d);
 int hgb_gat_fwd(const float* xlr, const int32_t* rowptr, const int32_t* perm, const int32_t* src, const float* eattr, int32_t d,

@@ -9,7 +9,6 @@ import copy
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
@@ -18,6 +17,7 @@ from hydragnn_b200 import _lib, ops  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.cgcnn import CGCNNStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
+from conv_reference import cgconv as _ref  # noqa: E402
 from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, _zero_dropout,  # noqa: E402
                            golden_engine, rel_l2)
 
@@ -36,23 +36,6 @@ def _inputs(n, e, f, d, seed):
     cvec = torch.randn(2 * f, generator=g) * 0.5
     ea, mt = (torch.randn(e, d, generator=g), torch.randn(d, 2 * f, generator=g) * 0.5) if d else (None, None)
     return {k: (v.to(DEV) if v is not None else None) for k, v in dict(pq=pq, ea=ea, mt=mt, cvec=cvec, x=x).items()}
-
-
-def _ref(t, ei, g_out):
-    """fp64: out = x + sum at the targets of sigmoid(f) softplus(s), and the gradients of <out, g_out> by autograd."""
-    src, dst = ei[0].cpu(), ei[1].cpu()
-    leaves = {k: (v.detach().cpu().double().requires_grad_(True) if v is not None else None) for k, v in t.items()}
-    pq, ea, mt, cvec, x = (leaves[k] for k in ("pq", "ea", "mt", "cvec", "x"))
-    f = x.shape[1]
-    h = pq[dst, :2 * f] + pq[src, 2 * f:] + cvec
-    if ea is not None:
-        h = h + ea @ mt
-    m = torch.sigmoid(h[:, :f]) * F.softplus(h[:, f:])
-    out = x + torch.zeros_like(x).index_add(0, dst, m)
-    wrt = [v for v in (pq, ea, mt, cvec) if v is not None]
-    grads = torch.autograd.grad(out, wrt, g_out.cpu().double())
-    names = [k for k in ("pq", "ea", "mt", "cvec") if leaves[k] is not None]
-    return out.detach(), dict(zip(names, grads))
 
 
 @pytest.mark.parametrize("d", [0, 1, 7, 16])

@@ -10,7 +10,6 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 pytestmark = pytest.mark.gpu
 
@@ -20,6 +19,7 @@ from hydragnn_b200.gat import gat_composed  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.gat import GATStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
+from conv_reference import gat as _ref  # noqa: E402
 from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, _zero_dropout,  # noqa: E402
                            check_grads, golden_engine, rel_l2, seeded_state)
 
@@ -39,37 +39,6 @@ def _inputs(n, e, heads, c, d, concat, seed):
     return {k: (v.to(DEV) if v is not None else None) for k, v in dict(xlr=xlr, ea=ea, mt=mt, att=att, bias=bias).items()}
 
 
-def _ref(t, ei, heads, c, concat, g_out, keep=None, p=0.0):
-    """fp64 GATv2Conv after its Linears (remove / add self-loops with the mean attribute, softmax with the max detached), and the
-    gradients of <out, g_out> by autograd."""
-    src, dst = ei[0].cpu(), ei[1].cpu()
-    leaves = {k: (v.detach().cpu().double().requires_grad_(True) if v is not None else None) for k, v in t.items()}
-    xlr, ea, mt, att, bias = (leaves[k] for k in ("xlr", "ea", "mt", "att", "bias"))
-    n, hc = xlr.shape[0], heads * c
-    xl, xr = xlr[:, :hc], xlr[:, hc:]
-    e = src.numel()
-    other = src != dst
-    eid = torch.cat([torch.arange(e)[other], e + torch.arange(n)])
-    s_, d_ = torch.cat([src[other], torch.arange(n)]), torch.cat([dst[other], torch.arange(n)])
-    z = xr[d_] + xl[s_]
-    if ea is not None:
-        a = ea[other]
-        cnt = torch.zeros(n, dtype=a.dtype).index_add_(0, dst[other], torch.ones(a.shape[0], dtype=a.dtype)).clamp(min=1)
-        a = torch.cat([a, torch.zeros(n, a.shape[1], dtype=a.dtype).index_add(0, dst[other], a) / cnt[:, None]])
-        z = z + a @ mt
-    s = (F.leaky_relu(z, SLOPE).view(-1, heads, c) * att.view(1, heads, c)).sum(-1)
-    m = torch.full((n, heads), float("-inf"), dtype=s.dtype).scatter_reduce(0, d_[:, None].expand_as(s), s.detach(), "amax")
-    ex = (s - m[d_]).exp()
-    al = ex / (torch.zeros(n, heads, dtype=s.dtype).index_add(0, d_, ex) + 1e-16)[d_]
-    if keep is not None:
-        al = al * keep.cpu().double()[eid] / (1.0 - p)
-    out = torch.zeros(n, heads, c, dtype=s.dtype).index_add(0, d_, al[:, :, None] * xl[s_].view(-1, heads, c))
-    out = (out.reshape(n, hc) if concat else out.mean(1)) + bias
-    names = [k for k in ("xlr", "ea", "mt", "att", "bias") if leaves[k] is not None]
-    grads = torch.autograd.grad(out, [leaves[k] for k in names], g_out.cpu().double())
-    return out.detach(), dict(zip(names, grads))
-
-
 SHAPES = [(h, c) for h in (1, 2, 6, 8) for c in (1, 3, 20, 32, 64) if ops.gat_supported(h, c, 0)] + [(2, 128), (4, 128)]
 
 
@@ -83,7 +52,7 @@ def test_gat_kernels_match_fp64(heads, c, concat):
     g_out = torch.randn(n, heads * c if concat else c, generator=torch.Generator().manual_seed(3)).to(DEV)
     out, lse = ops.raw_gat_fwd(t["xlr"], t["ea"], t["mt"], t["att"], t["bias"], plan, heads, c, concat, SLOPE)
     g_xlr, g_ea, g_par = ops.raw_gat_bwd(g_out, t["xlr"], t["ea"], t["mt"], t["att"], lse, plan, heads, c, concat, SLOPE)
-    ref, rg = _ref(t, ei, heads, c, concat, g_out)
+    ref, rg = _ref(t, ei, heads, c, concat, g_out, SLOPE)
     assert rel_l2(out.cpu(), ref) < 1e-5
     assert rel_l2(g_xlr[:, :heads * c].cpu(), rg["xlr"][:, :heads * c]) < 1e-4        # g_x_l: pass B (by source)
     assert rel_l2(g_xlr[:, heads * c:].cpu(), rg["xlr"][:, heads * c:]) < 1e-4        # g_x_r: pass A (by target)
@@ -122,7 +91,7 @@ def test_gat_dropout_fused_equals_composed_and_is_seeded():
     assert rel_l2(fused.detach(), comp.detach()) < 1e-5
     for a, b in zip(gf, gc):
         assert rel_l2(a, b) < 1e-4
-    ref, rg = _ref(t, ei, heads, c, True, g_out, keep, p)
+    ref, rg = _ref(t, ei, heads, c, True, g_out, SLOPE, keep, p)
     assert rel_l2(fused.detach().cpu(), ref) < 1e-5
     assert rel_l2(gf[0].cpu(), rg["xlr"]) < 1e-4 and rel_l2(gf[1].cpu(), rg["ea"]) < 1e-4
     # another seed gives another mask; eval mode (p = 0) draws nothing

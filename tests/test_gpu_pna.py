@@ -1,4 +1,4 @@
-"""PNA on the GPU: the fused PNAConv kernels (hgb_pna_conv_{fwd,bwd}) against an fp64 restatement written here, the raw C-ABI,
+"""PNA on the GPU: the fused PNAConv kernels (hgb_pna_conv_{fwd,bwd}) against the fp64 restatement of conv_reference.py, the raw C-ABI,
 the fused path against the composed one, and the engine's PNAStack against models_pna.pt (the reference's own PNAStack.py +
 Base.py + gps.py, PyG's PNAConv restated in oracle/pna.py).
 
@@ -24,6 +24,7 @@ from hydragnn_b200 import _lib, ops  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.pna import PNAStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
+from conv_reference import pna_bwd as _ref_bwd, pna_fwd as _ref_fwd  # noqa: E402
 from stack_support import _batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, golden_engine, rel_l2  # noqa: E402
 
 DEV = "cuda"
@@ -39,49 +40,6 @@ def _inputs(n, e, f, d, seed, dyadic=False):
     pq, c = r(n, 2 * f), r(f)
     ea, mt = (r(e, d), r(d, f) * 0.5) if d else (None, None)
     return [t.to(DEV) if t is not None else None for t in (pq, ea, mt, c)]
-
-
-def _ref_fwd(pq, ea, mt, c, ei, n):
-    """fp64: (agg [n, 4f], first argmin / argmax in CSR order = smallest edge id, h [e, f])."""
-    f = pq.shape[1] // 2
-    src, dst = ei[0], ei[1]
-    h = pq[:, :f].double()[dst] + pq[:, f:].double()[src] + c.double()
-    if ea is not None:
-        h = h + ea.double() @ mt.double()
-    e = h.shape[0]
-    cnt = torch.bincount(dst, minlength=n).double()
-    inv = (1.0 / cnt.clamp(min=1))[:, None]
-    idx = dst[:, None].expand(-1, f)
-    mean = torch.zeros(n, f, dtype=torch.float64, device=DEV).index_add_(0, dst, h) * inv
-    var = torch.zeros(n, f, dtype=torch.float64, device=DEV).index_add_(0, dst, h * h) * inv - mean * mean
-    sd = var.clamp(min=1e-5).sqrt()
-    sd = sd.masked_fill(sd <= math.sqrt(1e-5), 0.0)
-    empty = (cnt == 0)[:, None]
-    mn = torch.full((n, f), math.inf, dtype=torch.float64, device=DEV).scatter_reduce(0, idx, h, "amin")
-    mx = torch.full((n, f), -math.inf, dtype=torch.float64, device=DEV).scatter_reduce(0, idx, h, "amax")
-    eid = torch.arange(e, device=DEV)[:, None].expand(-1, f)
-    big = torch.full((n, f), e, dtype=torch.int64, device=DEV)
-    amin = big.scatter_reduce(0, idx, torch.where(h == mn[dst], eid, e), "amin").masked_fill(empty, -1)
-    amax = big.scatter_reduce(0, idx, torch.where(h == mx[dst], eid, e), "amin").masked_fill(empty, -1)
-    agg = torch.cat([mean, mn.masked_fill(empty, 0), mx.masked_fill(empty, 0), sd], dim=1)
-    return agg, amin, amax, h
-
-
-def _ref_bwd(g, agg, amin, amax, h, ea, mt, ei, n):
-    f = h.shape[1]
-    src, dst = ei[0], ei[1]
-    g = g.double()
-    cnt = torch.bincount(dst, minlength=n).double().clamp(min=1)[:, None]
-    mean, sd = agg[:, :f], agg[:, 3 * f:]
-    e = torch.arange(h.shape[0], device=DEV)[:, None]
-    gh = g[:, :f][dst] / cnt[dst] + (amin.long()[dst] == e) * g[:, f:2 * f][dst] + (amax.long()[dst] == e) * g[:, 2 * f:3 * f][dst]
-    safe = torch.where(sd > 0, sd, torch.ones_like(sd))
-    gh = gh + torch.where(sd[dst] > 0, g[:, 3 * f:][dst] / (cnt[dst] * safe[dst]) * (h - mean[dst]), torch.zeros_like(h))
-    gp = torch.zeros(n, f, dtype=torch.float64, device=DEV).index_add_(0, dst, gh)
-    gq = torch.zeros(n, f, dtype=torch.float64, device=DEV).index_add_(0, src, gh)
-    gmt = ea.double().t() @ gh if ea is not None else None
-    gea = gh @ mt.double().t() if ea is not None else None
-    return gh, gp, gq, gh.sum(0), gmt, gea
 
 
 @pytest.mark.parametrize("d", [0, 1, 3, 16])

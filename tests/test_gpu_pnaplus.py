@@ -1,4 +1,4 @@
-"""PNAPlus on the GPU: the fused kernels (hgb_pnaplus_conv_{fwd,bwd}) against an fp64 restatement written here, the raw C-ABI,
+"""PNAPlus on the GPU: the fused kernels (hgb_pnaplus_conv_{fwd,bwd}) against the fp64 restatement of conv_reference.py, the raw C-ABI,
 the fused path against the composed one, the engine's PNAPlusStack against models_pnaplus.pt (the reference's own
 PNAPlusStack.py + Base.py + gps.py), forces, and one training step at the lj_pnaplus / ogb_pnaplus shapes against the fp64
 oracle of oracle/pnaplus.py.
@@ -16,9 +16,9 @@ pytestmark = pytest.mark.gpu
 import hydragnn_b200 as hb  # noqa: E402
 from hydragnn_b200 import _lib, ops  # noqa: E402
 from hydragnn_b200.ops import _p, _stream  # noqa: E402
-from oracle.pnaeq import DegreeScalerAggregation as ODSA  # noqa: E402
 from oracle.pnaplus import PNAPlusStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
+from conv_reference import pnaplus_agg  # noqa: E402
 from stack_support import _batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, golden_engine, rel_l2  # noqa: E402
 
 DEV = "cuda"
@@ -43,30 +43,13 @@ def _inputs(ei, n, f, d, r, seed):
 NAMES = ["pq", "dist", "eattr", "freq", "wr", "br", "wl", "mr", "mat", "cvec"]
 
 
-def _ref(t, ei, n):
-    """fp64 agg [n, 4f] = [mean | min | max | std] of m_e, written from the definitions."""
-    src, dst = ei[0].cpu(), ei[1].cpu()
-    f = t["pq"].shape[1] // 2
-    x = (t["dist"] / RADIUS)[:, None]
-    p = EXPO + 1
-    a, b, c = -(p + 1) * (p + 2) / 2, p * (p + 2), -p * (p + 1) / 2
-    env = (1 / x + a * x ** (p - 1) + b * x ** p + c * x ** (p + 1)) * (x < 1).double()
-    rbf = env * torch.sin(t["freq"] * x)
-    u = torch.relu(rbf @ t["wr"].t() + t["br"])
-    h = t["pq"][dst, :f] + t["pq"][src, f:] + u @ t["mr"].t() + t["cvec"]
-    if t["eattr"] is not None:
-        h = h + t["eattr"] @ t["mat"]
-    m = h * (rbf @ t["wl"].t())
-    return ODSA(["mean", "min", "max", "std"], ["identity"], torch.tensor([1.0]))(m, dst, n)
-
-
 @pytest.mark.parametrize("f,d,r", [(1, 0, 1), (5, 1, 5), (32, 0, 5), (32, 3, 16), (55, 16, 5), (64, 0, 16), (64, 16, 1)])
 def test_pnaplus_conv_kernels_match_fp64(f, d, r):
     ei, n = _graph(seed=1)
     plan = ops.EdgePlan(ei, n)
     t = _inputs(ei, n, f, d, r, seed=f * 100 + d * 10 + r)
     t64 = {k: (v.double().requires_grad_(True) if v is not None else None) for k, v in t.items()}
-    ref = _ref(t64, ei, n)
+    ref = pnaplus_agg(t64, ei, n, RADIUS, EXPO)
     gout = torch.randn(ref.shape, generator=torch.Generator().manual_seed(3), dtype=torch.float64)
     want = torch.autograd.grad((ref * gout).sum(), [t64[k] for k in NAMES if t64[k] is not None])
     want = dict(zip([k for k in NAMES if t64[k] is not None], want))

@@ -6,6 +6,7 @@ import pytest
 import torch
 
 from oracle import schnet as so
+from conv_reference import cfconv as _fp64
 from stack_support import _OD, _errors, _oracle, _oracle_step, golden_engine, rel_l2 as _rel
 
 pytestmark = pytest.mark.gpu
@@ -41,23 +42,6 @@ def _setup(nf, g, d, seed=0):
     coeff = -0.5 / (3.0 / max(g - 1, 1)) ** 2
     plan = ops.EdgePlan(ei.to(DEV), n)
     return ei, pos, t, offset, coeff, plan
-
-
-def _fp64(ei, pos, t, offset, coeff, cutoff=3.0):
-    leaves = {k: (v.clone().requires_grad_(True) if v is not None and k not in ("g_out", "g_we") else v) for k, v in t.items()}
-    p = pos.clone().requires_grad_(True)
-    g = offset.numel()
-    a = leaves["a1t"]
-    ea = leaves["r"]
-    w1 = a.t()
-    eye = torch.eye(a.shape[1], dtype=torch.float64)
-    # cfconv computes x @ lin1^T and agg @ lin2^T + b: identities here, so out = sum_e xl[j] W_e
-    out, w = so.cfconv(leaves["xl"], p, ei, eye, w1, leaves["b1"], leaves["w2"], leaves["b2"], eye, torch.zeros_like(leaves["b1"]),
-                       offset, coeff, cutoff, edge_attr=ea)
-    obj = (out * t["g_out"]).sum() + (w * t["g_we"]).sum()
-    names = ["xl", "a1t", "b1", "w2", "b2"] + (["r"] if ea is not None else [])
-    grads = torch.autograd.grad(obj, [leaves[k] for k in names] + [p])
-    return out, w, dict(zip(names + ["pos"], grads))
 
 
 def _engine(ei, pos, t, offset, coeff, plan, cutoff=3.0):
