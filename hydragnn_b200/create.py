@@ -13,7 +13,7 @@ from torch import nn
 from . import ops
 from .stacks import EGCLStack, PAINNStack, cached, graph_sum
 
-SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet", "CGCNN", "GAT")
+SUPPORTED = ("EGNN", "PAINN", "PNA", "PNAPlus", "PNAEq", "MACE", "SchNet", "CGCNN", "GAT", "SAGE", "MFC")
 
 
 def get_device(use_gpu=True):
@@ -140,6 +140,14 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
         negative_slope = 0.05
         from .gat import GATStack
         model = GATStack(heads, negative_slope, edge_dim, **common)
+    elif mpnn_type == "SAGE":
+        # hydragnn/models/create.py:348-370 does not pass initial_bias to SAGEStack
+        from .sage import SAGEStack
+        model = SAGEStack(**dict(common, initial_bias=None))
+    elif mpnn_type == "MFC":
+        assert max_neighbours is not None, "MFC requires max_neighbours input."
+        from .sage import MFCStack
+        model = MFCStack(max_neighbours, **common)
     else:
         raise ValueError("Unknown mpnn_type: {0}".format(mpnn_type))
     if enable_interatomic_potential:

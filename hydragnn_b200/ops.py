@@ -1687,6 +1687,137 @@ def grouped_mlp(seq_by_group, x, rowptr):
 
 
 # =====================================================================================================
+# SAGEConv / MFConv: neighbour aggregation gathered into a degree-grouped wgmma Linear (hgb_nbr.cu)
+# =====================================================================================================
+class DegreePlan:
+    """Nodes grouped by clamped in-degree (MFConv's weight index): ``order`` [n] row -> node (None: identity, one group),
+    ``grp_ptr`` [groups + 1], ``tiles`` the fused kernel's tile table (None when the kernel does not take this many groups), and
+    ``perm``, the CSR of ``order`` as a gather / scatter pair, built when the composed path first asks for it."""
+    __slots__ = ("order", "grp_ptr", "tiles", "groups", "n", "_perm")
+
+    def __init__(self, order, grp_ptr, tiles, groups, n):
+        self.order, self.grp_ptr, self.tiles, self.groups, self.n, self._perm = order, grp_ptr, tiles, groups, n, None
+
+    @property
+    def perm(self):
+        if self._perm is None:
+            self._perm = csr_build(self.order.to(torch.int64), self.n)
+        return self._perm
+
+
+NBR_MAX_GROUPS = 128        # the largest group count hgb_nbr_tiles and the fused kernels take
+
+
+def degree_plan(plan, groups):
+    """Counting sort of the nodes by min(in-degree, groups - 1), stable by node id, on the device: a CSR build over the clamped
+    degrees (no host read).  One group needs no sort: the order is the identity."""
+    col = plan.by_col
+    n = plan.num_nodes
+    dev = col.rowptr.device
+    if groups == 1:
+        order, grp_ptr = None, torch.full((2,), n, dtype=torch.int32, device=dev)
+        grp_ptr[0] = 0
+    else:
+        deg = (col.rowptr[1:] - col.rowptr[:-1]).clamp(max=groups - 1).to(torch.int64)
+        csr = csr_build(deg, groups)
+        order, grp_ptr = csr.perm, csr.rowptr
+    tiles = None
+    if groups <= NBR_MAX_GROUPS:
+        tiles = torch.empty(((n + 63) // 64 + groups) * 2, dtype=torch.int32, device=dev)
+        _lib.call("hgb_nbr_tiles", _p(grp_ptr), groups, n, _p(tiles), _stream())
+    return DegreePlan(order, grp_ptr, tiles, groups, n)
+
+
+def nbr_linear_supported(k, n_out, groups):
+    """Shapes ``NbrLinearFn`` takes: 1 <= k <= 128, 1 <= n_out <= 256, groups <= 128."""
+    return bool(_lib.query("hgb_nbr_linear_supported", int(k), int(n_out), int(groups)))
+
+
+def _r32(v):
+    return (v + 31) // 32 * 32
+
+
+class NbrLinearFn(torch.autograd.Function):
+    """out[i] = lin_l,g(h_i) + lin_r,g(x_i) with h_i the sum (``mean``: the mean, 0 without in-edges) of x_j over the in-edges
+    j -> i (i = edge_index[1]) and g the node's group in ``dp`` -- SAGEConv with one group and the mean, MFConv with a group per
+    clamped in-degree and the sum.  ``wl`` / ``wr`` [groups, n_out, k], ``bl`` [groups, n_out].  Forward: one hgb_nbr_linear_fwd
+    launch; h never reaches memory unless the weight gradient needs it (as part of the [h | x] operand).  Backward: the grouped
+    wgmma with the transposed weights gives [g_h | g_x root]; g_x = g_x root + the by-source segment sum of g_h; the weight
+    gradient is hgb_tc_wgrad (one group) or hgb_grouped_wgrad (rows in degree order), skipped under ``only_data_grads``."""
+
+    @staticmethod
+    def forward(ctx, x, wl, bl, wr, dp, plan, mean):
+        x = _chk(x.contiguous())
+        n, k = x.shape
+        groups, n_out, _ = wl.shape
+        kp = _r32(k)
+        w = x.new_zeros(groups, _r32(n_out), 2 * kp)                    # [W_l | 0 | W_r | 0], zero rows past n_out
+        w[:, :n_out, :k] = wl
+        w[:, :n_out, kp:kp + k] = wr
+        need_w = any(ctx.needs_input_grad[1:4])
+        hx = torch.empty(n, 2 * kp, dtype=x.dtype, device=x.device) if need_w else None
+        out = torch.empty(n, n_out, dtype=x.dtype, device=x.device)
+        ctx.tc, ctx.mean, ctx.dp, ctx.plan, ctx.k = _TC["enabled"], bool(mean), dp, plan, k
+        ctx.save_for_backward(w, hx)
+        col = plan.by_col
+        _lib.call("hgb_nbr_linear_fwd", _p(x), n, k, _p(col.rowptr), _p(plan.nbr("col")), plan.num_edges, int(mean), _p(dp.order),
+                  _p(dp.grp_ptr), _p(dp.tiles), groups, _p(w), _p(_chk(bl.contiguous())), n_out, _p(out), _p(hx),
+                  0 if ctx.tc else 1, _stream())
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_out):
+        w, hx = ctx.saved_tensors
+        dp, plan, k = ctx.dp, ctx.plan, ctx.k
+        g = _chk(g_out.contiguous())
+        n, n_out = g.shape
+        groups, kp = w.shape[0], w.shape[2] // 2
+        exact = 0 if ctx.tc else 1
+        need = ctx.needs_input_grad
+        g_x = g_wl = g_bl = g_wr = None
+        if need[0]:
+            g_h = torch.empty(n, k, dtype=g.dtype, device=g.device)
+            g_xr = torch.empty_like(g_h)
+            _lib.call("hgb_nbr_linear_bwd_data", _p(g), n, n_out, _p(plan.by_col.rowptr), int(ctx.mean), _p(dp.order), _p(dp.grp_ptr),
+                      _p(dp.tiles), groups, _p(w.transpose(1, 2).contiguous()), k, _p(g_h), _p(g_xr), exact, _stream())
+            # every node j receives g_h of the targets of its out-edges: the by-source CSR, gathering target rows
+            g_x = raw_segment_sum(g_h, plan.by_row.rowptr, plan.nbr("row"), n).add_(g_xr)
+        if any(need[1:4]) and not _DATA_ONLY["on"]:
+            if n == 0:
+                dw = g.new_zeros(groups, n_out, 2 * kp)
+                db = g.new_zeros(groups, n_out)
+            elif groups == 1:
+                with tensor_cores(ctx.tc):
+                    _, dw, db = linear_bwd_dispatch(g, hx, w[0, :n_out], need_x=False)
+                dw, db = dw[None], db[None]
+            else:
+                gs = raw_gather(g, dp.order)                               # g_out in degree order, as hx
+                dw = torch.empty(groups, n_out, 2 * kp, dtype=g.dtype, device=g.device)
+                db = torch.empty(groups, n_out, dtype=g.dtype, device=g.device)
+                _lib.call("hgb_grouped_wgrad", _p(gs), _p(hx), 2 * kp, _p(dp.grp_ptr), groups, n, n_out, 2 * kp, _p(dw), _p(db),
+                          _stream())
+            g_wl, g_bl, g_wr = dw[:, :, :k], db, dw[:, :, kp:kp + k]
+        return g_x, g_wl, g_bl, g_wr, None, None, None
+
+
+def nbr_linear_composed(x, wl, bl, wr, dp, plan, mean, higher_order=False):
+    """The same layer composed from GatherRows / SegmentSum, Linear and the grouped Linear over degree-sorted rows: the path of
+    higher-order passes and unsupported shapes, and the reference the fused path is tested against.  With more than one group
+    the grouped Linear is first-order only."""
+    h = SegmentSum.apply(GatherRows.apply(x, plan.by_row), plan.by_col)             # sum of x[edge_index[0]] at edge_index[1]
+    if mean:
+        col = plan.by_col
+        h = h / (col.rowptr[1:] - col.rowptr[:-1]).clamp(min=1).to(h.dtype)[:, None]
+    if dp.groups == 1:
+        lin = linear_any_order if higher_order else linear_act
+        return lin(h, wl[0], bl[0]) + lin(x, wr[0], None)
+    hx = GatherRows.apply(torch.cat([h, x], dim=1), dp.perm)                        # rows in degree order
+    y = GroupedLinearFn.apply(hx, torch.cat([wl, wr], dim=2), bl, dp.grp_ptr, None, 0.0)
+    return SegmentSum.apply(y, dp.perm)
+
+
+# =====================================================================================================
 # fused EGNN edge block + closed edge-length primitives (any order of differentiation the MLIP loss needs)
 # =====================================================================================================
 class only_data_grads:

@@ -132,9 +132,10 @@ def _padded_chain(mods, x):
 
 
 # Per-batch index plans, cached on the batch object: the CSR views of edge_index (ops.EdgePlan), the graph offsets, MACE's
-# element CSR, and the (edge_index, rowptr, graph_ptr) hint a radius build leaves.  A step that copies a new batch into the same
-# tensors must forget them (``forget_plans``).
-PLAN_KEYS = EDGE_PLAN, GRAPH_CSR, ELEMENT_CSR, COL_SORTED = ("_hgb_plan", "_hgb_gcsr", "_hgb_zcsr", "_hgb_col_sorted")
+# element CSR, the (edge_index, rowptr, graph_ptr) hint a radius build leaves, and the in-degree groupings of the SAGE / MFC
+# layers (ops.DegreePlan).  A step that copies a new batch into the same tensors must forget them (``forget_plans``).
+PLAN_KEYS = EDGE_PLAN, GRAPH_CSR, ELEMENT_CSR, COL_SORTED, DEGREE_PLAN = ("_hgb_plan", "_hgb_gcsr", "_hgb_zcsr", "_hgb_col_sorted",
+                                                                         "_hgb_degplan")
 
 
 def cached(data, key):

@@ -36,6 +36,10 @@ WORKLOADS = {
     # GAT on the ogb_pna graphs; the GPS variant adds the positional encodings
     "ogb_gat": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
     "ogb_gat_gps": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20, pe_dim=6),
+    # SAGE and MFC on the ogb_pna graphs; the GPS variant adds the positional encodings
+    "ogb_sage": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    "ogb_mfc": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20),
+    "ogb_sage_gps": dict(sizes=list(range(9, 31)), rho=0.10, species=[1, 6, 7, 8, 9], radius=5.0, max_neighbours=20, pe_dim=6),
     # SchNet on examples/qm9 and examples/md17 (GPS: the positional encodings pe, rel_pe = |pe[row] - pe[col]| once the edges
     # exist, see add_rel_pe), and without GPS at the CI widths, building its radius graphs in the layers
     "qm9_schnet": dict(n=9, rho=0.10, species=[1, 6, 7, 8, 9], radius=7.0, max_neighbours=5, pe_dim=2),
@@ -111,6 +115,11 @@ ARCH["ogb_pnaplus"] = dict(ARCH["ogb_pna"], mpnn_type="PNAPlus", num_radial=5, e
 # width of the other GPS workloads); the GPS variant adds 8 attention heads and pe_dim 6
 ARCH["ogb_gat"] = dict(ARCH["ogb_pna"], mpnn_type="GAT", hidden_dim=64, num_conv_layers=3, edge_dim=1)
 ARCH["ogb_gat_gps"] = dict(ARCH["ogb_gat"], global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=8, pe_dim=6)
+# SAGE (SAGEStack.py) and MFC (MFCStack.py, max_degree = max_neighbours = 20: 21 weight groups): the ogb_pna graphs and graph
+# head, 3 layers at hidden 64; the GPS variant adds 8 attention heads and pe_dim 6
+ARCH["ogb_sage"] = dict(ARCH["ogb_pna"], mpnn_type="SAGE", hidden_dim=64, num_conv_layers=3)
+ARCH["ogb_mfc"] = dict(ARCH["ogb_sage"], mpnn_type="MFC")
+ARCH["ogb_sage_gps"] = dict(ARCH["ogb_sage"], global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=8, pe_dim=6)
 # SchNet (SCFStack.py): examples/qm9/qm9.json exactly, examples/md17/md17.json (6 layers, pe_dim 6), and the in-layer branch at
 # the widths of tests/inputs/ci.json (num_filters 126, num_gaussians 50) with hidden 64 and three layers
 ARCH["qm9_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_conv_layers=2, num_gaussians=10, num_filters=8,

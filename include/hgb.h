@@ -52,7 +52,8 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 #define HGB_POOL_MAX 2
 
 /* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd);
- * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient */
+ * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient;
+ * 109: hgb_nbr_* (SAGEConv / MFConv) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -686,6 +687,29 @@ int hgb_mace_symcontract_fwd(const float* x, const float* wall, const int32_t* z
 /* gx [N,(lmax_in+1)^2,F]; gw_node [N,KTOT,F] (per-node weight gradients; reduce per element with hgb_segment_sum).       */
 int hgb_mace_symcontract_bwd(const float* g_out, const float* x, const float* wall, const int32_t* z, int32_t n, int32_t f,
                              int32_t lmax_in, int32_t lmax_out, float* gx, float* gw_node, hgb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Neighbour aggregation into a degree-grouped wgmma Linear (hgb_nbr.cu): torch_geometric 2.6.1 SAGEConv (aggr "mean",
+ * root_weight; hydragnn/models/SAGEStack.py) and MFConv (aggr "add", weights picked by min(in-degree, max_degree);
+ * hydragnn/models/MFCStack.py).  Rows are taken in an order in which the weight groups are contiguous: order [n] maps rows to
+ * nodes (NULL: identity), grp_ptr [groups + 1] (device) gives each group's rows, tiles [ceil(n / 64) + groups][2] is the tile
+ * table hgb_nbr_tiles writes from grp_ptr.  rowptr [n + 1] / src [e] are the by-target CSR (edge_index[1]) and the source of
+ * every CSR slot.  kpad = round32(k), npad = round32(n_out).  exact != 0: 3xTF32 (fp32-accurate), else TF32.
+ * Supported: 1 <= k <= 128, 1 <= n_out <= 256, 1 <= groups <= 128 (hgb_nbr_linear_supported).  n = 0 launches nothing.
+ * ------------------------------------------------------------------------------------------ */
+int hgb_nbr_linear_supported(int32_t k, int32_t n_out, int32_t groups);
+int hgb_nbr_tiles(const int32_t* grp_ptr, int32_t groups, int32_t n, int32_t* tiles, hgb_stream_t stream);
+/* out [n, n_out] = [h | x] [W_l | 0 | W_r | 0]_g^T + bias_g with h the sum (mean != 0: mean, 0 without in-edges) of x [n, k]
+ * over each node's in-edges in CSR order; w [groups, npad, 2 kpad], bias [groups, n_out] or NULL; hx [n, 2 kpad] (or NULL)
+ * receives the rows [h | 0 | x | 0] in row order (the weight gradient's operand). */
+int hgb_nbr_linear_fwd(const float* x, int32_t n, int32_t k, const int32_t* rowptr, const int32_t* src, int64_t e, int32_t mean,
+                       const int32_t* order, const int32_t* grp_ptr, const int32_t* tiles, int32_t groups, const float* w,
+                       const float* bias, int32_t n_out, float* out, float* hx, int32_t exact, hgb_stream_t stream);
+/* [g_h | g_xr] = g_out [n, n_out] . w_g with wt [groups, 2 kpad, npad] the transposed packed weights: g_h [n, k] (divided by
+ * max(in-degree, 1) when mean != 0) and g_xr [n, k], each in node order. */
+int hgb_nbr_linear_bwd_data(const float* g_out, int32_t n, int32_t n_out, const int32_t* rowptr, int32_t mean,
+                            const int32_t* order, const int32_t* grp_ptr, const int32_t* tiles, int32_t groups, const float* wt,
+                            int32_t k, float* g_h, float* g_xr, int32_t exact, hgb_stream_t stream);
 
 #ifdef __cplusplus
 }
