@@ -1,11 +1,11 @@
-"""Generate golden vectors by running the REFERENCE's own code (run in the build
-container only; /root/reference does not exist on the GPU box).
+"""Generate golden vectors by running the REFERENCE's own code, from the checkout
+record.REF names (HYDRAGNN_REF); the tests never read it.
 
     python tests/golden/make_golden.py            # writes tests/golden/*.pt
 
 What is real and what is stubbed
 --------------------------------
-Loaded verbatim from /root/reference (never copied into this repo):
+Loaded verbatim from the reference checkout (never copied into this repo):
   hydragnn/utils/model/operations.py, hydragnn/models/Base.py,
   hydragnn/models/EGCLStack.py, hydragnn/models/PAINNStack.py, plus (AST-extracted,
   because their modules import absent packages at top level)
@@ -31,9 +31,9 @@ import types
 import numpy as np
 import torch
 
-REF = "/root/reference"
+from record import REF, save, t2d
+
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 
 
 def _mod(name, **attrs):
@@ -251,10 +251,6 @@ def toy_batch(gen, sizes, box, input_dim=1, dtype=torch.float32):
     return Batch.from_data_list(samples)
 
 
-def t2d(batch):
-    return {k: v for k, v in batch.items() if torch.is_tensor(v)}
-
-
 def main():
     egcl, painn = install_stubs()
     gen = torch.Generator().manual_seed(20260921)
@@ -285,7 +281,7 @@ def main():
                           "x": b.x, "v": v0, "pos": b.pos, "edge_index": b.edge_index, "diff": diff, "dist": dist,
                           "sinc": painn.sinc_expansion(dist, 5, 7.0), "fcut": painn.cosine_cutoff(dist, 7.0),
                           "s1": s1.detach(), "v1": v1.detach(), "s2": s2.detach(), "v2": v2.detach(), "s3": s3.detach()}
-    torch.save(out, HERE + "/layers.pt")
+    save(out, HERE + "/layers.pt", compact=False)                # b.x, b.pos, b.edge_index: one tensor each, three times
 
     # ---- full models through the reference's Base.forward -----------------------------------
     models = {}
@@ -343,7 +339,7 @@ def main():
                                          "loss": loss.detach(),
                                          "grads": {n: (g.detach() if g is not None else None)
                                                    for (n, _), g in zip(m.named_parameters(), grads)}}
-    torch.save(models, HERE + "/models.pt")
+    save(models, HERE + "/models.pt")
 
     # ---- PNAEq through the reference's PNAEqStack (third-party DegreeScalerAggregation restated, see stub) ----
     pna = install_pnaeq_stubs()
@@ -363,7 +359,7 @@ def main():
                                           "loss": loss.detach(), "deg": last_deg,
                                           "grads": {n: (g.detach() if g is not None else None)
                                                     for (n, _), g in zip(m.named_parameters(), grads)}}
-    torch.save(pmodels, HERE + "/models_pnaeq.pt")
+    save(pmodels, HERE + "/models_pnaeq.pt", compact=False)
 
     # ---- GPS: the reference's own gps.py + Base.py (PyG glue stubbed: BatchNorm wrapper, to_dense_batch, resolvers) ----
     gps = install_gps_stubs()
@@ -401,7 +397,7 @@ def main():
                                           "state_after": {k: v.clone() for k, v in m.state_dict().items() if "running" in k},
                                           "grads": {n: (g.detach() if g is not None else None)
                                                     for (n, _), g in zip(m.named_parameters(), grads)}}
-    torch.save(gmodels, HERE + "/models_gps.pt")
+    save(gmodels, HERE + "/models_gps.pt")
 
     # ---- RadiusGraphPBC numpy post-processing ---------------------------------------------
     glb = {"np": np}
@@ -415,8 +411,8 @@ def main():
     S = rng.integers(-1, 2, (E, 3))
     a = glb["_remove_true_self_loops"](None, src, dst, length, S)
     lim = glb["_limit_neighbors"](None, *a, 6)
-    torch.save({"in": [torch.from_numpy(np.asarray(t)) for t in (src, dst, length, S)],
-                "k": 6, "out": [torch.from_numpy(np.asarray(t)) for t in lim]}, HERE + "/pbc_limit.pt")
+    save({"in": [torch.from_numpy(np.asarray(t)) for t in (src, dst, length, S)],
+          "k": 6, "out": [torch.from_numpy(np.asarray(t)) for t in lim]}, HERE + "/pbc_limit.pt")
     # ---- node heads of type 'mlp_per_node' and 'conv' (Base.py:508-588, 648-680, 800-810, 912-979) -------------------
     # own generator so that the files above stay byte-identical; PyG BatchNorm naming (a module holding `.module`)
     from oracle.gps import PyGBatchNorm
@@ -446,7 +442,7 @@ def main():
         grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
         hmodels[name] = {"state": state, "inputs": t2d(b), "pred": [p.detach() for p in pred], "loss": loss.detach(),
                          "grads": {n: (g.detach() if g is not None else None) for (n, _), g in zip(m.named_parameters(), grads)}}
-    torch.save(hmodels, HERE + "/models_heads.pt")
+    save(hmodels, HERE + "/models_heads.pt")
 
     # ---- MACE through the reference's own MACEStack / blocks / symmetric_contraction / cg / irreps_tools (e3nn restated) ----
     mace = install_mace_stubs()
@@ -477,8 +473,7 @@ def main():
         mmodels[name] = {"state": state, "inputs": inp, "pred": [p.detach() for p in pred], "dobj_dpos": forces.detach(),
                          "grads": {n: (g.detach() if g is not None else None) for (n, _), g in zip(m.named_parameters(), grads)},
                          "cfg": dict(max_ell=max_ell, node_max_ell=node_max_ell, correlation=corr, num_conv_layers=layers, hidden_dim=hidden)}
-    torch.save(mmodels, HERE + "/models_mace.pt")
-    print("golden vectors written to", HERE)
+    save(mmodels, HERE + "/models_mace.pt")
 
 
 if __name__ == "__main__":

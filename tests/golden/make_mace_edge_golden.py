@@ -1,6 +1,6 @@
 """Generate tests/golden/models_mace_edge.pt by running the REFERENCE's own MACEStack with edge attributes (edge_dim > 0),
 on the same stubs as make_golden.py (e3nn restated by oracle/e3.py, opt_einsum_fx the identity, torch_scatter.scatter
-index_add_).  Run in the build container only; /root/reference does not exist on the GPU box.
+index_add_).  Run where the reference checkout is (record.REF); the tests never read it.
 
     python tests/golden/make_mace_edge_golden.py       # writes tests/golden/models_mace_edge.pt, nothing else
 
@@ -8,15 +8,10 @@ With edge_dim = D the reference's edge irreps are (Dx0e + sh).simplify() and the
 (MACEStack.py:198-203, 459-461).  edge_dim 1 takes the edge lengths, as the reference's own CI does
 (tests/test_graphs.py: pytest_train_mace_model_lengths); edge_dim 3 takes random features.
 """
-import os
-import sys
-
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-
-import make_golden as mg  # noqa: E402
+import make_golden as mg
+from record import HERE, save, t2d
 
 CONFIGS = {   # name: (edge_dim, max_ell, node_max_ell, correlation, num_conv_layers, hidden_dim)
     "mace_edge_d1_one_layer": (1, 2, 1, 2, 1, 8),
@@ -48,7 +43,7 @@ def main():
                            num_conv_layers=layers, num_nodes=9, graph_pooling="mean")
         m.eval()
         state = {k: v.clone() for k, v in m.state_dict().items()}
-        inp = mg.t2d(b)
+        inp = t2d(b)
         pos0 = b.pos.clone().requires_grad_(True)
         b.pos = pos0
         pred = m(b)
@@ -59,8 +54,7 @@ def main():
                      "grads": {n: (g.detach() if g is not None else None) for (n, _), g in zip(m.named_parameters(), grads)},
                      "cfg": dict(edge_dim=edge_dim, max_ell=max_ell, node_max_ell=node_max_ell, correlation=corr,
                                  num_conv_layers=layers, hidden_dim=hidden)}
-    torch.save(out, os.path.join(HERE, "models_mace_edge.pt"))
-    print("written", os.path.join(HERE, "models_mace_edge.pt"))
+    save(out, HERE + "/models_mace_edge.pt")
 
 
 if __name__ == "__main__":

@@ -13,17 +13,15 @@ oracle/schnet.py and in this file [3P-memory].
 Each case of models_schnet.pt stores the state dict, the inputs, the eval-mode predictions, and one train-mode step (dropout
 off): predictions, the reference's own loss and every parameter gradient, plus the radius graph of every in-layer conv.
 """
-import os
 import sys
 
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
-sys.path.insert(0, os.path.dirname(HERE))
+import make_golden as mg
+from record import HERE, REF, add_edge_and_pe, record_case, record_dropin, reference_create, save
 
-import make_golden as mg  # noqa: E402
-
+# record.HEAD_GRAPH's value, defined here: the pickled goldens hold one "branch-0" string object per module that spells it, and
+# models_schnet.pt was first written with these two heads sharing one
 HEAD_GRAPH = {"graph": [{"type": "branch-0", "architecture": {"num_sharedlayers": 2, "dim_sharedlayers": 5, "num_headlayers": 2,
                                                                "dim_headlayers": [10, 7]}}]}
 HEAD_CONV = {"node": [{"type": "branch-0", "architecture": {"num_headlayers": 2, "dim_headlayers": [10, 6], "type": "conv"}}]}
@@ -82,9 +80,8 @@ def install_schnet_stubs():
     mg._mod("hydragnn.preprocess")
     mg._mod("hydragnn.preprocess.graph_samples_checks_and_updates", RadiusInteractionGraphCPU=RadiusInteractionGraph)
     sys.modules["hydragnn.models.Base"].BatchNorm = PyGBatchNorm
-    gps = mg.install_gps_stubs()
-    scf = mg._load("hydragnn.models.SCFStack", mg.REF + "/hydragnn/models/SCFStack.py")
-    return scf, gps
+    mg.install_gps_stubs()
+    return mg._load("hydragnn.models.SCFStack", REF + "/hydragnn/models/SCFStack.py")
 
 
 def schnet_batch(gen, sizes, input_dim, box):
@@ -105,18 +102,11 @@ def schnet_batch(gen, sizes, input_dim, box):
     return Batch.from_data_list(samples)
 
 
-def make_models(scf, gps):
+def make_models(scf):
     gen = torch.Generator().manual_seed(24681357)
     out = {}
     for name, (input_dim, hidden, layers, nf, ng, rad, k, head, edge_dim, ekind, pool, use_gps, equiv) in CASES.items():
-        b = schnet_batch(gen, [7, 5, 9, 6], input_dim, 4.0)
-        if ekind == "length":
-            b.edge_attr = (b.pos[b.edge_index[1]] - b.pos[b.edge_index[0]]).norm(dim=1, keepdim=True)
-        elif ekind == "random":
-            b.edge_attr = torch.randn(b.edge_index.shape[1], edge_dim, generator=gen)
-        if use_gps:
-            b.pe = torch.randn(b.x.shape[0], 4, generator=gen)
-            b.rel_pe = (b.pe[b.edge_index[0]] - b.pe[b.edge_index[1]]).abs()
+        b = add_edge_and_pe(schnet_batch(gen, [7, 5, 9, 6], input_dim, 4.0), gen, ekind, edge_dim, use_gps)
         heads = HEAD_GRAPH if head == "graph" else HEAD_CONV
         otype = ["graph"] if head == "graph" else ["node"]
         odim = [1] if head == "graph" else [2]
@@ -127,30 +117,17 @@ def make_models(scf, gps):
                          input_dim, hidden, odim, 4 if use_gps else 0, "GPS" if use_gps else None, "multihead" if use_gps else None,
                          4 if use_gps else 0, otype, heads, "relu", "mse", equiv, max_neighbours=k, loss_weights=[1.0],
                          freeze_conv=False, initial_bias=None, num_conv_layers=layers, num_nodes=None, graph_pooling=pool)
-        state = {kk: v.clone() for kk, v in m.state_dict().items()}
-        graphs = []
-        hooks = [mod.register_forward_hook(lambda mod_, inp, outp: graphs.append(outp[0].clone()))
-                 for mod in m.modules() if isinstance(mod, sys.modules["torch_geometric.nn.models.schnet"].RadiusInteractionGraph)]
-        m.eval()
-        pred_eval = [p.detach() for p in m(b)]
-        for h in hooks:
-            h.remove()
-        m.train()
+        graphs = []                                    # the radius graph of every in-layer conv in the eval-mode forward
         for mod in m.modules():
-            if isinstance(mod, torch.nn.Dropout):
-                mod.p = 0.0
-            if isinstance(mod, gps.GPSConv):
-                mod.dropout = 0.0
+            if isinstance(mod, RadiusInteractionGraph):
+                mod.register_forward_hook(lambda mod_, inp, outp: None if mod_.training else graphs.append(outp[0].clone()))
         value = b.y.reshape(-1)
-        pred = m(b)
-        loss, _ = m.loss(pred, value, [torch.arange(value.numel())])
-        grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-        out[name] = {"state": state, "inputs": mg.t2d(b), "pred_eval": pred_eval, "pred_train": [p.detach() for p in pred],
-                     "value": value, "loss": loss.detach(), "graphs_eval": graphs,
-                     "grads": {n: (g.detach() if g is not None else None) for (n, _), g in zip(m.named_parameters(), grads)},
-                     "cfg": dict(input_dim=input_dim, hidden_dim=hidden, num_conv_layers=layers, num_filters=nf, num_gaussians=ng,
-                                 radius=rad, max_neighbours=k, output_type=otype, output_dim=odim, output_heads=heads,
-                                 edge_dim=edge_dim, graph_pooling=pool, gps=use_gps, equivariance=equiv)}
+        rec = record_case(m, b, value, [torch.arange(value.numel())],
+                          cfg=dict(input_dim=input_dim, hidden_dim=hidden, num_conv_layers=layers, num_filters=nf, num_gaussians=ng,
+                                   radius=rad, max_neighbours=k, output_type=otype, output_dim=odim, output_heads=heads,
+                                   edge_dim=edge_dim, graph_pooling=pool, gps=use_gps, equivariance=equiv))
+        rec["graphs_eval"] = graphs
+        out[name] = {k: rec[k] for k in ("state", "inputs", "pred_eval", "pred_train", "value", "loss", "graphs_eval", "grads", "cfg")}
     return out
 
 
@@ -171,46 +148,15 @@ DROPIN_CASES = {"SchNet-gps-graph": (True, False), "SchNet-equivariant-mlip": (F
 
 
 def make_dropin():
-    import make_dropin_golden as md
-    import hydragnn_b200 as hb
-    create_model_config, _ = md._reference_create()
-    scf, _ = install_schnet_stubs()
-    create_model_config.__globals__["SCFStack"] = scf.SCFStack
-    out = {}
-    for key, (use_gps, mlip) in DROPIN_CASES.items():
-        cfg = _schnet_config(use_gps, mlip)
-        os.environ.pop("HYDRAGNN_ENGINE", None)
-        ref = create_model_config(cfg, verbosity=0, use_gpu=False)
-        assert not type(ref).__module__.startswith("hydragnn_b200")
-        seen = {}
-        real = hb.create_model
-
-        class Spy:
-            __code__ = real.__code__
-
-            def __call__(self, **kw):
-                seen.update(kw)
-                return real(**kw)
-
-        hb.create_model = Spy()
-        os.environ["HYDRAGNN_ENGINE"] = "b200"
-        try:
-            eng = create_model_config(cfg, verbosity=0, use_gpu=False)
-        finally:
-            hb.create_model = real
-            os.environ.pop("HYDRAGNN_ENGINE", None)
-        assert seen and type(eng).__module__.startswith("hydragnn_b200")
-        inner = ref.model if mlip else ref
-        out[key] = {"config": cfg, "kwargs": seen, "state_dict": {k: v.clone() for k, v in ref.state_dict().items()},
-                    "attrs": {a: getattr(ref, a) for a in md.ATTRS}, "repr": str(inner)}
-    return out
+    create_model_config, _ = reference_create()
+    create_model_config.__globals__["SCFStack"] = install_schnet_stubs().SCFStack
+    return {key: record_dropin(create_model_config, _schnet_config(use_gps, mlip))[0] for key, (use_gps, mlip) in DROPIN_CASES.items()}
 
 
 def main():
-    scf, gps = install_schnet_stubs()
-    torch.save(make_models(scf, gps), os.path.join(HERE, "models_schnet.pt"))
-    torch.save(make_dropin(), os.path.join(HERE, "dropin_schnet.pt"))
-    print("written", os.path.join(HERE, "models_schnet.pt"), os.path.join(HERE, "dropin_schnet.pt"))
+    # written as they are: inputs["y"] and "value" are two views of one storage
+    save(make_models(install_schnet_stubs()), HERE + "/models_schnet.pt", compact=False)
+    save(make_dropin(), HERE + "/dropin_schnet.pt", compact=False)
 
 
 if __name__ == "__main__":

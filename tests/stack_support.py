@@ -1,11 +1,14 @@
 """What the test modules share: the model configurations of the reference goldens, the engine model of a golden case, the
-batches the GPU tests build, one training step of an oracle stack and the error summary the benchmark-shape tests bound.
-A plain module on the tests' import path; no test module imports another."""
+checks of a model against a golden case and of the engine against a drop-in golden, the batches the GPU tests build, one
+training step of an oracle stack and the error summary the benchmark-shape tests bound.  A plain module on the tests' import
+path; no test module imports another, and nothing here reads tests/golden/'s makers or the reference checkout they need."""
 import hashlib
+import types
 
 import torch
 
 import hydragnn_b200 as hb
+from hydragnn_b200 import _lib
 from hydragnn_b200.synthetic import ARCH, WORKLOADS, make_samples
 from oracle.radius_graph import radius_graph
 from oracle.workloads import add_edges_cpu
@@ -122,17 +125,128 @@ def seeded_state(case):
     return {k: v.clone() for k, v in sd.items()}
 
 
-def check_grads(case, named_grads, check):
-    """Calls ``check(name, grad, reference)`` for every gradient the case stores.  The conv-head case stores the gradients of its
-    head modules only (its 120-wide stack convs are covered by the other cases); every other case stores all of them."""
-    names = [n for n, _ in named_grads]
+# ---- checks against the reference goldens ---------------------------------------------------------------------------------
+def golden_data(inputs, dtype=torch.float64, device="cpu"):
+    """A golden case's ``inputs`` as attributes on ``device``, the floating-point ones in ``dtype``; ``edge_attr`` is None where
+    the case has none."""
+    d = types.SimpleNamespace(edge_attr=None)
+    for k, v in inputs.items():
+        setattr(d, k, v.to(device, dtype) if v.is_floating_point() else v.to(device))
+    return d
+
+
+def grad_close(rtol, atol):
+    """Element-wise gradient bound: |g - ref| <= atol gmax + rtol |ref|, gmax the largest reference gradient entry of the case."""
+    def check(name, g, ref, gmax):
+        torch.testing.assert_close(g.detach().cpu().double(), ref.double(), rtol=rtol, atol=atol * gmax,
+                                   msg=lambda s: name + ": " + s)
+    return check
+
+
+def grad_norm(rtol, atol):
+    """Norm-wise gradient bound: ||g - ref|| <= rtol ||ref|| + atol."""
+    def check(name, g, ref, gmax):
+        err = float((g.detach().cpu().double() - ref.double()).norm())
+        assert err <= rtol * float(ref.double().norm()) + atol, (name, err)
+    return check
+
+
+def check_grads(case, named, grads):
+    """Every gradient the golden case stores against ``named`` ({parameter name: gradient}): ``grads(name, g, ref, gmax)``
+    checks one (``grad_close`` or ``grad_norm``); where the reference has none, the gradient must be None or zero.  A case whose
+    ``grads_scope`` is not "all" stores the gradients of some parameters only; every other case stores all of them."""
     stored = case["grads"]
-    assert set(stored) <= set(names)
+    assert set(stored) <= set(named)
     if case.get("grads_scope", "all") == "all":
-        assert set(stored) == set(names)
-    for n, g in named_grads:
-        if n in stored:
-            check(n, g, stored[n])
+        assert set(stored) == set(named)
+    gmax = max(float(g.abs().max()) for g in stored.values() if g is not None)
+    for n, ref in stored.items():
+        g = named[n]
+        if ref is None:
+            assert g is None or not g.any(), n
+        else:
+            assert g is not None, n
+            grads(n, g, ref, gmax)
+
+
+def check_golden_case(m, case, data, *, pred, loss, grads, state_after=(1e-5, 1e-7), eval_kernels=()):
+    """``m`` against a golden case: eval-mode predictions, then one train-mode step on the case's targets with every dropout off:
+    predictions, loss, every parameter gradient the case stores and the BatchNorm running statistics afterwards.
+
+    ``data()`` makes ``m``'s input.  Bounds: ``pred`` = (eval, train) rel-L2 of every prediction; ``loss`` = (rtol, atol);
+    ``grads`` as in ``check_grads``; ``state_after`` = (rtol, atol).  ``eval_kernels`` must all run in the eval-mode forward."""
+    m.eval()
+    if eval_kernels:
+        _lib.trace_begin()
+    with torch.no_grad():
+        out = m(data())
+    if eval_kernels:
+        calls = {t[0] for t in _lib.trace_end()}
+        assert set(eval_kernels) <= calls, sorted(calls)
+    assert len(out) == len(case["pred_eval"])
+    for a, b in zip(out, case["pred_eval"]):
+        assert rel_l2(a.cpu(), b) < pred[0]
+    m.train()
+    _zero_dropout(m)
+    m.zero_grad(set_to_none=True)
+    p0 = next(m.parameters())
+    value = case["value"].to(p0.device, p0.dtype)
+    head_index = [i.to(p0.device) for i in case.get("head_index", [torch.arange(value.numel())])]
+    out = m(data())
+    for a, b in zip(out, case["pred_train"]):
+        assert rel_l2(a.detach().cpu(), b) < pred[1]
+    lv, _ = m.loss(out, value, head_index)
+    lv.backward()
+    got, want = float(lv.detach()), float(case["loss"])
+    assert abs(got - want) <= loss[1] + loss[0] * abs(want), (got, want)
+    check_grads(case, {n: p.grad for n, p in m.named_parameters()}, grads)
+    sd = m.state_dict()
+    for k, v in case.get("state_after", {}).items():
+        torch.testing.assert_close(sd[k].cpu().to(v.dtype), v, rtol=state_after[0], atol=state_after[1], msg=lambda s, k=k: k + ": " + s)
+
+
+def engine_case(m, c):
+    """The engine model ``m``'s own record of golden case ``c``, in the case's layout and on the CPU: eval-mode predictions, then
+    one train-mode step (``_train_step``): predictions, loss, gradients (None where a parameter has none) and the BatchNorm
+    statistics after."""
+    m.eval()
+    with torch.no_grad():
+        pred_eval = [p.cpu() for p in m(_batch(c["inputs"]))]
+    pred, loss = _train_step(m, c)
+    return dict(c, pred_eval=pred_eval, pred_train=[p.detach().cpu() for p in pred], loss=loss.detach().cpu(),
+                grads={n: (p.grad.cpu() if p.grad is not None else None) for n, p in m.named_parameters()},
+                state_after={k: v.cpu() for k, v in m.state_dict().items() if "running" in k or "num_batches" in k})
+
+
+def check_seeded_state(eng, state):
+    """The engine's seeded state dict has the names, order, shapes and values of the reference's ``state``, and ``state`` loads
+    into it strictly and comes back out unchanged."""
+    se = eng.state_dict()
+    assert list(se.keys()) == list(state.keys())
+    for k, v in state.items():
+        assert v.shape == se[k].shape and torch.equal(v, se[k]), k
+    eng.load_state_dict(state, strict=True)
+    assert all(torch.equal(v, state[k]) for k, v in eng.state_dict().items())
+
+
+def check_dropin(g, cls, name, batch_norm=True):
+    """The engine model the reference's dispatch builds from the drop-in golden entry ``g`` is interchangeable with the reference's
+    own: a ``cls`` stack (inside the MLIP wrapper where there is one) whose ``str`` is ``name``, as the reference's is, with the
+    reference's seeded state dict, the attributes the training loop reads, and one feature layer per conv layer: PyG's BatchNorm
+    wrapper, or with ``batch_norm`` False an Identity.  Returns the engine model."""
+    mpnn_type = g["kwargs"]["mpnn_type"]
+    assert mpnn_type == g["config"]["Architecture"]["mpnn_type"] and mpnn_type in hb.create.SUPPORTED
+    eng = hb.create_model(**g["kwargs"])
+    inner = getattr(eng, "model", eng)
+    assert type(inner) is cls, type(inner)
+    check_seeded_state(eng, g["state_dict"])
+    for attr, want in g["attrs"].items():
+        assert getattr(eng, attr) == want, attr
+    assert str(inner) == g["repr"] == name
+    kind = torch.nn.BatchNorm1d if batch_norm else torch.nn.Identity
+    assert all(type(f.module if batch_norm else f) is kind for f in inner.feature_layers)
+    assert len(inner.feature_layers) == len(inner.graph_convs) == g["config"]["Architecture"]["num_conv_layers"]
+    return eng
 
 
 # ---- GPU batches -------------------------------------------------------------------------------------------------------------

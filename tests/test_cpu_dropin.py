@@ -12,12 +12,20 @@ the reference's own code, whose ``ValueError`` the generator recorded.
 
 Checked: same parameter names, shapes AND values (both sides seed with ``torch.manual_seed(0)``, create.py:164), and every attribute the
 reference's train / validate / test loop reads through ``model.module`` (train_validate_test.py:225-242,498,731,736,1006-1018).
+The PNA, PNAPlus, CGCNN and GAT configurations of tests/golden/make_{pna,pnaplus,cgcnn,gat}_golden.py are checked the same way,
+with their BatchNorm feature layers (stack_support.check_dropin).
 """
 import os
 import sys
 
 import pytest
 import torch
+
+from hydragnn_b200.cgcnn import CGCNNStack
+from hydragnn_b200.gat import GATStack
+from hydragnn_b200.pna import PNAStack
+from hydragnn_b200.pnaplus import PNAPlusStack
+from stack_support import check_dropin
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -74,3 +82,23 @@ def test_reference_create_model_config_dispatches_to_the_engine(golden_dir, mpnn
     # and the other direction: a strict load into the reference model needs exactly its names and shapes
     assert {k: tuple(v.shape) for k, v in inner.state_dict().items()} == {k: tuple(v.shape) for k, v in ref_inner.items()}
     assert str(inner) == g["repr"]
+
+
+# (golden file, configuration, engine stack, its str): the reference's PNAStack and PNAPlusStack both print "PNAStack"
+STACK_DROPIN = [("dropin_pna.pt", "PNA-edge1-node", PNAStack, "PNAStack"), ("dropin_pna.pt", "PNA-noedge-graph", PNAStack, "PNAStack"),
+                ("dropin_pnaplus.pt", "PNAPlus-edge1-node", PNAPlusStack, "PNAStack"),
+                ("dropin_pnaplus.pt", "PNAPlus-noedge-graph", PNAPlusStack, "PNAStack"),
+                ("dropin_cgcnn.pt", "CGCNN-edge1-node", CGCNNStack, "CGCNNStack"),
+                ("dropin_cgcnn.pt", "CGCNN-edge0-graph", CGCNNStack, "CGCNNStack"),
+                ("dropin_cgcnn.pt", "CGCNN-gps-edge0-graph", CGCNNStack, "CGCNNStack"),
+                ("dropin_gat.pt", "GAT-edge1-node", GATStack, "GATStack"), ("dropin_gat.pt", "GAT-noedge-graph", GATStack, "GATStack"),
+                ("dropin_gat.pt", "GAT-gps-noedge-graph", GATStack, "GATStack")]
+
+
+@pytest.mark.parametrize("golden,key,cls,name", STACK_DROPIN, ids=[k for _, k, _, _ in STACK_DROPIN])
+def test_reference_create_model_config_dispatches_the_stack_to_the_engine(golden_dir, golden, key, cls, name):
+    """PNA (EAM-like: 1-wide edge attribute, node head; no edge attributes, graph head), PNAPlus (the same), CGCNN (after
+    update_config: hidden_dim = input_dim = 1 without GPS, edge_dim 0 or 1; GPS with edge_dim 0) and GAT (edge_dim None without
+    edge features, 1 with the edge length; GPS without edge features): the engine's model is interchangeable with the reference's
+    own stack, whose PyG conv is restated in oracle/."""
+    check_dropin(torch.load(os.path.join(golden_dir, golden))[key], cls, name)

@@ -10,7 +10,7 @@ from hydragnn_b200 import padded
 from hydragnn_b200.sage import MFCStack, SAGEStack
 from oracle.base import oracle_from_case
 from oracle.sage import MFCStackOracle, SAGEStackOracle
-from stack_support import engine_kwargs
+from stack_support import check_dropin, check_seeded_state, engine_kwargs
 
 DROPIN = ["SAGE-graph-bias", "SAGE-node", "SAGE-gps-graph", "MFC-node-bias", "MFC-node", "MFC-gps-graph"]
 STACKS = {"SAGE": SAGEStack, "MFC": MFCStack}
@@ -22,21 +22,8 @@ def _dropin(golden_dir):
 
 @pytest.mark.parametrize("key", DROPIN)
 def test_reference_create_model_config_dispatches_to_the_engine(golden_dir, key):
-    g = _dropin(golden_dir)[key]
-    kind = g["kwargs"]["mpnn_type"]
-    assert kind in hb.create.SUPPORTED
-    eng = hb.create_model(**g["kwargs"])
-    assert type(eng) is STACKS[kind]
-    sr, se = g["state_dict"], eng.state_dict()
-    assert list(sr.keys()) == list(se.keys())
-    for k in sr:
-        assert sr[k].shape == se[k].shape and torch.equal(sr[k], se[k]), k
-    for attr, want in g["attrs"].items():
-        assert getattr(eng, attr) == want, attr
-    eng.load_state_dict(sr, strict=True)
-    assert str(eng) == g["repr"] == kind + "Stack"
-    assert all(isinstance(f.module, torch.nn.BatchNorm1d) for f in eng.feature_layers)
-    assert not padded.supported(eng)
+    kind = key.split("-")[0]
+    assert not padded.supported(check_dropin(_dropin(golden_dir)[key], STACKS[kind], kind + "Stack"))
 
 
 def _cases(golden_dir, kind):
@@ -51,11 +38,7 @@ def test_engine_state_dicts_match_every_golden_case_and_load_both_ways(golden_di
     for name, c in _cases(golden_dir, kind).items():
         eng = hb.create_model(**engine_kwargs(kind, c), use_gpu=False)
         assert type(eng) is STACKS[kind] and str(eng) == c["str"], name
-        sr, se = c["state"], eng.state_dict()
-        assert list(sr.keys()) == list(se.keys()), name
-        for k in sr:
-            assert sr[k].shape == se[k].shape and torch.equal(sr[k], se[k]), (name, k)
-        eng.load_state_dict(sr, strict=True)
+        check_seeded_state(eng, c["state"])
         case = dict(c, cfg={k: v for k, v in c["cfg"].items() if k != "initial_bias"})
         oracle_from_case(oracle, case, state=eng.state_dict())
 

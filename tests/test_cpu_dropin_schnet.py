@@ -7,6 +7,7 @@ import torch
 
 import hydragnn_b200 as hb
 from hydragnn_b200.schnet import SCFStack
+from stack_support import check_dropin
 
 KEYS = ["SchNet-gps-graph", "SchNet-equivariant-mlip"]
 
@@ -17,21 +18,8 @@ def _golden(golden_dir, key):
 
 @pytest.mark.parametrize("key", KEYS)
 def test_reference_create_model_config_dispatches_schnet_to_the_engine(golden_dir, key):
-    g = _golden(golden_dir, key)
-    assert g["kwargs"]["mpnn_type"] == "SchNet" and "SchNet" in hb.create.SUPPORTED
-    eng = hb.create_model(**g["kwargs"])
-    inner = getattr(eng, "model", eng)
-    assert isinstance(inner, SCFStack)
-    sr, se = g["state_dict"], eng.state_dict()
-    assert list(sr.keys()) == list(se.keys())
-    for k in sr:
-        assert sr[k].shape == se[k].shape and torch.equal(sr[k], se[k]), k
-    for attr, want in g["attrs"].items():
-        assert getattr(eng, attr) == want, attr
-    eng.load_state_dict(sr, strict=True)
-    assert all(torch.equal(v, sr[k]) for k, v in eng.state_dict().items())
-    assert str(inner) == g["repr"] == "SCFStack"
-    assert "distance_expansion.offset" in inner.state_dict()
+    eng = check_dropin(_golden(golden_dir, key), SCFStack, "SCFStack", batch_norm=False)
+    assert "distance_expansion.offset" in getattr(eng, "model", eng).state_dict()
 
 
 def test_in_layer_and_edge_index_branches_are_named_like_the_reference(golden_dir):

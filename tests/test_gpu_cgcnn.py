@@ -18,8 +18,8 @@ from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.cgcnn import CGCNNStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
 from conv_reference import cgconv as _ref  # noqa: E402
-from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, _zero_dropout,  # noqa: E402
-                           golden_engine, rel_l2)
+from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _zero_dropout,  # noqa: E402
+                           check_golden_case, engine_case, golden_engine, grad_close, rel_l2)
 
 DEV = "cuda"
 CASES = ["cgcnn_graph_edge0", "cgcnn_node_edge_len", "cgcnn_add_pool_edge3", "cgcnn_multihead", "cgcnn_mlp_per_node", "cgcnn_gps",
@@ -135,49 +135,23 @@ def test_cgconv_raw_abi_errors_and_empty_sizes():
 @pytest.mark.parametrize("name", CASES)
 def test_cgcnn_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_cgcnn.pt")[name]
-    m = golden_engine("CGCNN", c).eval()
-    _lib.trace_begin()
-    with torch.no_grad():
-        pred = m(_batch(c["inputs"]))
-    calls = {t[0] for t in _lib.trace_end()}
-    assert "hgb_cgconv_fwd" in calls
-    for a, b in zip(pred, c["pred_eval"]):
-        assert rel_l2(a.cpu(), b) < 1e-5
-    pred, loss = _train_step(m, c)
-    for a, b in zip(pred, c["pred_train"]):
-        assert rel_l2(a.detach().cpu(), b) < 1e-5
-    torch.testing.assert_close(loss.detach().cpu(), c["loss"], rtol=1e-5, atol=1e-7)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for n, p in m.named_parameters():
-        ref = c["grads"][n]
-        if ref is None:
-            assert p.grad is None or not p.grad.any(), n
-        else:
-            torch.testing.assert_close(p.grad.cpu(), ref, rtol=1e-3, atol=1e-5 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].cpu(), v, rtol=1e-5, atol=1e-7)
+    check_golden_case(golden_engine("CGCNN", c), c, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 1e-7),
+                      grads=grad_close(1e-3, 1e-5), eval_kernels=["hgb_cgconv_fwd"])
 
 
 @pytest.mark.parametrize("name", CASES)
 def test_cgcnn_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_cgcnn.pt")[name]
-    res = []
-    for composed in (False, True):
-        m = golden_engine("CGCNN", c)
-        m.force_higher_order = composed
-        _lib.trace_begin()
-        pred, loss = _train_step(m, c)
-        calls = {t[0] for t in _lib.trace_end()}
-        assert ("hgb_cgconv_bwd" in calls) != composed
-        res.append(([p.detach() for p in pred], {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}))
-    (pf, gf), (pc, gc) = res
-    for a, b in zip(pf, pc):
-        assert rel_l2(a, b) < 1e-5
-    gmax = max(float(g.abs().max()) for g in gc.values())
-    assert set(gf) == set(gc)
-    for n in gc:
-        torch.testing.assert_close(gf[n], gc[n], rtol=1e-3, atol=1e-5 * gmax, msg=lambda s, n=n: n + ": " + s)
+    composed = golden_engine("CGCNN", c)
+    composed.force_higher_order = True
+    _lib.trace_begin()
+    ref = engine_case(composed, c)
+    assert "hgb_cgconv_bwd" not in {t[0] for t in _lib.trace_end()}
+    fused = golden_engine("CGCNN", c)
+    _lib.trace_begin()
+    check_golden_case(fused, ref, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 0), grads=grad_close(1e-3, 1e-5))
+    assert "hgb_cgconv_bwd" in {t[0] for t in _lib.trace_end()}
+    assert {n for n, p in fused.named_parameters() if p.grad is not None} == {n for n, g in ref["grads"].items() if g is not None}
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])

@@ -20,8 +20,8 @@ from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.gat import GATStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
 from conv_reference import gat as _ref  # noqa: E402
-from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, _zero_dropout,  # noqa: E402
-                           check_grads, golden_engine, rel_l2, seeded_state)
+from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, _zero_dropout,  # noqa: E402
+                           check_golden_case, engine_case, golden_engine, grad_close, rel_l2, seeded_state)
 
 DEV = "cuda"
 SLOPE = 0.05
@@ -167,51 +167,23 @@ def test_gat_raw_abi_errors_and_empty_sizes():
 @pytest.mark.parametrize("name", CASES)
 def test_gat_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_gat.pt")[name]
-    m = golden_engine("GAT", c, seeded_state(c)).eval()
-    _lib.trace_begin()
-    with torch.no_grad():
-        pred = m(_batch(c["inputs"]))
-    calls = {t[0] for t in _lib.trace_end()}
-    assert "hgb_gat_fwd" in calls
-    for a, b in zip(pred, c["pred_eval"]):
-        assert float((a.cpu() - b).norm()) <= 1e-5 * max(float(b.norm()), 1e-6)
-    pred, loss = _train_step(m, c)
-    for a, b in zip(pred, c["pred_train"]):
-        assert rel_l2(a.detach().cpu(), b) < 1e-5
-    torch.testing.assert_close(loss.detach().cpu(), c["loss"], rtol=1e-5, atol=1e-7)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-
-    def check(n, g, ref):
-        if ref is None:
-            assert g is None or not g.any(), n
-        else:
-            torch.testing.assert_close(g.cpu(), ref, rtol=1e-3, atol=1e-5 * gmax, msg=lambda s: n + ": " + s)
-
-    check_grads(c, [(n, p.grad) for n, p in m.named_parameters()], check)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].cpu(), v, rtol=1e-5, atol=1e-7)
+    check_golden_case(golden_engine("GAT", c, seeded_state(c)), c, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 1e-7),
+                      grads=grad_close(1e-3, 1e-5), eval_kernels=["hgb_gat_fwd"])
 
 
 @pytest.mark.parametrize("name", CASES)
 def test_gat_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_gat.pt")[name]
-    res = []
-    for composed in (False, True):
-        m = golden_engine("GAT", c, seeded_state(c))
-        m.force_higher_order = composed
-        _lib.trace_begin()
-        pred, loss = _train_step(m, c)
-        calls = {t[0] for t in _lib.trace_end()}
-        assert ("hgb_gat_bwd" in calls) != composed
-        res.append(([p.detach() for p in pred], {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}))
-    (pf, gf), (pc, gc) = res
-    for a, b in zip(pf, pc):
-        assert float((a - b).norm()) <= 1e-5 * max(float(b.norm()), 1e-6)
-    gmax = max(float(g.abs().max()) for g in gc.values())
-    assert set(gf) == set(gc)
-    for n in gc:
-        torch.testing.assert_close(gf[n], gc[n], rtol=1e-3, atol=1e-5 * gmax, msg=lambda s, n=n: n + ": " + s)
+    composed = golden_engine("GAT", c, seeded_state(c))
+    composed.force_higher_order = True
+    _lib.trace_begin()
+    ref = engine_case(composed, c)
+    assert "hgb_gat_bwd" not in {t[0] for t in _lib.trace_end()}
+    fused = golden_engine("GAT", c, seeded_state(c))
+    _lib.trace_begin()
+    check_golden_case(fused, ref, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 0), grads=grad_close(1e-3, 1e-5))
+    assert "hgb_gat_bwd" in {t[0] for t in _lib.trace_end()}
+    assert {n for n, p in fused.named_parameters() if p.grad is not None} == {n for n, g in ref["grads"].items() if g is not None}
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])

@@ -25,7 +25,8 @@ from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.pna import PNAStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
 from conv_reference import pna_bwd as _ref_bwd, pna_fwd as _ref_fwd  # noqa: E402
-from stack_support import _batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, golden_engine, rel_l2  # noqa: E402
+from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, check_golden_case, engine_case, golden_engine,  # noqa: E402
+                           grad_close, rel_l2)
 
 DEV = "cuda"
 CASES = ["pna_graph_noedge", "pna_node_edge_len", "pna_multihead_h5", "pna_gps", "pna_add_pool_edge3"]
@@ -174,44 +175,20 @@ def test_pna_conv_raw_abi_errors_and_empty_sizes():
 @pytest.mark.parametrize("name", CASES)
 def test_pna_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_pna.pt")[name]
-    m = golden_engine("PNA", c).eval()
-    _lib.trace_begin()
-    with torch.no_grad():
-        pred = m(_batch(c["inputs"]))
-    calls = {t[0] for t in _lib.trace_end()}
-    assert "hgb_pna_conv_fwd" in calls                               # the fused conv ran (edge widths here are <= 16)
-    for a, b in zip(pred, c["pred_eval"]):
-        assert rel_l2(a.cpu(), b) < 1e-5
-    pred, loss = _train_step(m, c)
-    for a, b in zip(pred, c["pred_train"]):
-        assert rel_l2(a.detach().cpu(), b) < 1e-5
-    torch.testing.assert_close(loss.detach().cpu(), c["loss"], rtol=1e-5, atol=1e-7)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for n, p in m.named_parameters():
-        ref = c["grads"][n]
-        if ref is not None:
-            torch.testing.assert_close(p.grad.cpu(), ref, rtol=1e-3, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].cpu(), v, rtol=1e-5, atol=1e-7)
+    # the fused conv runs in the eval forward (edge widths here are <= 16)
+    check_golden_case(golden_engine("PNA", c), c, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 1e-7),
+                      grads=grad_close(1e-3, 1e-6), eval_kernels=["hgb_pna_conv_fwd"])
 
 
 @pytest.mark.parametrize("name", CASES)
 def test_pna_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_pna.pt")[name]
-    res = []
-    for composed in (False, True):
-        m = golden_engine("PNA", c)
-        m.force_higher_order = composed
-        pred, loss = _train_step(m, c)
-        res.append(([p.detach() for p in pred], {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}))
-    (pf, gf), (pc, gc) = res
-    for a, b in zip(pf, pc):
-        assert rel_l2(a, b) < 1e-5
-    assert gf.keys() == gc.keys()
-    gmax = max(float(g.abs().max()) for g in gc.values())
-    for n in gf:
-        torch.testing.assert_close(gf[n], gc[n], rtol=1e-3, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
+    composed = golden_engine("PNA", c)
+    composed.force_higher_order = True
+    ref = engine_case(composed, c)
+    fused = golden_engine("PNA", c)
+    check_golden_case(fused, ref, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 0), grads=grad_close(1e-3, 1e-6))
+    assert {n for n, p in fused.named_parameters() if p.grad is not None} == {n for n, g in ref["grads"].items() if g is not None}
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])

@@ -19,7 +19,8 @@ from hydragnn_b200.ops import _p, _stream  # noqa: E402
 from oracle.pnaplus import PNAPlusStackOracle  # noqa: E402
 from oracle.tf32 import tf32_linears  # noqa: E402
 from conv_reference import pnaplus_agg  # noqa: E402
-from stack_support import _batch, _bench_batch, _errors, _graph, _oracle_step, _train_step, golden_engine, rel_l2  # noqa: E402
+from stack_support import (_batch, _bench_batch, _errors, _graph, _oracle_step, check_golden_case, check_grads, engine_case,  # noqa: E402
+                           golden_engine, grad_close, rel_l2)
 
 DEV = "cuda"
 RADIUS, EXPO = 2.0, 5
@@ -120,53 +121,29 @@ def _before_batch_norm(name):
     return name.endswith(("module_0.lin.bias", "module_0.post_nns.0.0.bias"))
 
 
+def _grads(name, g, ref, gmax):
+    if _before_batch_norm(name):
+        assert float(g.abs().max()) <= 1e-3 * gmax and float(ref.abs().max()) <= 1e-3 * gmax, name
+    else:
+        grad_close(1e-3, 1e-6)(name, g, ref, gmax)
+
+
 @pytest.mark.parametrize("name", CASES)
 def test_pnaplus_stack_matches_reference_golden(golden_dir, name):
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
-    m = golden_engine("PNAPlus", c).eval()
-    _lib.trace_begin()
-    with torch.no_grad():
-        pred = m(_batch(c["inputs"]))
-    calls = {t[0] for t in _lib.trace_end()}
-    assert "hgb_pnaplus_conv_fwd" in calls                 # every case is within the fused shapes (GPS: D = hidden = 16)
-    for a, b in zip(pred, c["pred_eval"]):
-        assert rel_l2(a.cpu(), b) < 1e-5
-    pred, loss = _train_step(m, c)
-    for a, b in zip(pred, c["pred_train"]):
-        assert rel_l2(a.detach().cpu(), b) < 1e-5
-    torch.testing.assert_close(loss.detach().cpu(), c["loss"], rtol=1e-5, atol=1e-7)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for n, p in m.named_parameters():
-        ref = c["grads"][n]
-        if ref is None:
-            assert p.grad is None or not p.grad.any(), n
-        elif _before_batch_norm(n):
-            assert float(p.grad.abs().max()) <= 1e-3 * gmax and float(ref.abs().max()) <= 1e-3 * gmax, n
-        else:
-            torch.testing.assert_close(p.grad.cpu(), ref, rtol=1e-3, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].cpu(), v, rtol=1e-5, atol=1e-7)
+    # every case is within the fused shapes (GPS: D = hidden = 16)
+    check_golden_case(golden_engine("PNAPlus", c), c, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 1e-7),
+                      grads=_grads, eval_kernels=["hgb_pnaplus_conv_fwd"])
 
 
 @pytest.mark.parametrize("name", CASES)
 def test_pnaplus_fused_path_equals_composed_path(golden_dir, name):
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
-    res = []
-    for composed in (False, True):
-        m = golden_engine("PNAPlus", c)
-        m.force_higher_order = composed
-        pred, loss = _train_step(m, c)
-        res.append(([p.detach() for p in pred], {n: p.grad.clone() for n, p in m.named_parameters() if p.grad is not None}))
-    (pf, gf), (pc, gc) = res
-    for a, b in zip(pf, pc):
-        assert rel_l2(a, b) < 1e-5
-    gmax = max(float(g.abs().max()) for g in gc.values())
-    for n in gc:
-        if _before_batch_norm(n):
-            assert float(gf[n].abs().max()) <= 1e-3 * gmax and float(gc[n].abs().max()) <= 1e-3 * gmax, n
-            continue
-        torch.testing.assert_close(gf[n], gc[n], rtol=1e-3, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
+    composed = golden_engine("PNAPlus", c)
+    composed.force_higher_order = True
+    ref = engine_case(composed, c)
+    fused = golden_engine("PNAPlus", c)
+    check_golden_case(fused, ref, lambda: _batch(c["inputs"]), pred=(1e-5, 1e-5), loss=(1e-5, 0), grads=_grads)
 
 
 def test_pnaplus_conv_head_with_edge_attributes_raises_before_any_launch(golden_dir):
@@ -194,10 +171,7 @@ def test_pnaplus_mlip_matches_reference_golden_and_forces(golden_dir):
     tot, tasks = m.energy_force_loss(pred, d)
     torch.testing.assert_close(float(tot), float(c["loss"]), rtol=1e-5, atol=0)
     grads = torch.autograd.grad(tot, list(m.model.parameters()), allow_unused=True)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for (n, _), g in zip(m.model.named_parameters(), grads):
-        if c["grads"][n] is not None:
-            torch.testing.assert_close(g.cpu(), c["grads"][n], rtol=1e-3, atol=1e-5 * gmax, msg=lambda s, n=n: n + ": " + s)
+    check_grads(c, {n: g for (n, _), g in zip(m.model.named_parameters(), grads)}, grad_close(1e-3, 1e-5))
     forces = {}
     for composed in (True, False):
         m.model.force_higher_order = composed

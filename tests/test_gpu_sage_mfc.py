@@ -6,7 +6,7 @@ import torch
 
 import hydragnn_b200 as hb
 from hydragnn_b200 import _lib, ops
-from stack_support import engine_kwargs
+from stack_support import check_golden_case, engine_kwargs, golden_data, grad_close
 
 pytestmark = pytest.mark.gpu
 
@@ -146,12 +146,6 @@ def test_no_nodes_and_no_edges():
 
 
 # ---- engine ----------------------------------------------------------------------------------------------------------------------
-class _Data:
-    def __init__(self, d):
-        for k, v in d.items():
-            setattr(self, k, v.cuda().float() if torch.is_tensor(v) and v.is_floating_point() else (v.cuda() if torch.is_tensor(v) else v))
-
-
 def _cases(golden_dir, kind):
     return torch.load(golden_dir + "/models_%s.pt" % kind.lower())
 
@@ -169,28 +163,11 @@ def _engine(kind, c):
 
 @pytest.mark.parametrize("kind", ["SAGE", "MFC"])
 def test_engine_against_every_golden_case(golden_dir, kind):
-    """Eval and train-mode predictions, the loss and every parameter gradient of the reference's own stack (fp32 on the CPU)."""
+    """Eval and train-mode predictions, the loss, every parameter gradient and the BatchNorm running statistics of the
+    reference's own stack (fp32 on the CPU)."""
     for name, c in _cases(golden_dir, kind).items():
-        m = _engine(kind, c)
-        d = _Data(c["inputs"])
-        m.eval()
-        with torch.no_grad():
-            for a, b in zip(m(d), c["pred_eval"]):
-                assert _rel(a, b) < 1e-4, name
-        m.train()
-        pred = m(d)
-        for a, b in zip(pred, c["pred_train"]):
-            assert _rel(a.detach(), b) < 1e-4, name
-        loss, _ = m.loss(pred, c["value"].cuda(), [h.cuda() for h in c["head_index"]])
-        assert abs(float(loss) - float(c["loss"])) <= 1e-4 * abs(float(c["loss"])), name
-        grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-        gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-        for (pn, _), g in zip(m.named_parameters(), grads):
-            want = c["grads"][pn]
-            if want is None:
-                assert g is None or not g.any(), (name, pn)
-                continue
-            torch.testing.assert_close(g.cpu(), want, rtol=2e-3, atol=2e-5 * gmax, msg=lambda s, pn=pn: "%s %s: %s" % (name, pn, s))
+        check_golden_case(_engine(kind, c), c, lambda: golden_data(c["inputs"], torch.float32, "cuda"), pred=(1e-4, 1e-4),
+                          loss=(1e-4, 0), grads=grad_close(2e-3, 2e-5))
 
 
 @pytest.mark.parametrize("workload", ["ogb_sage", "ogb_mfc", "ogb_sage_gps"])

@@ -7,7 +7,7 @@ import torch
 
 from oracle import schnet as so
 from conv_reference import cfconv as _fp64
-from stack_support import _OD, _errors, _oracle, _oracle_step, golden_engine, rel_l2 as _rel
+from stack_support import _OD, _errors, _oracle, _oracle_step, check_golden_case, golden_engine, grad_norm, rel_l2 as _rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -101,31 +101,8 @@ def test_engine_matches_the_reference_stack(golden_dir, name, higher):
     case = torch.load(golden_dir + "/models_schnet.pt")[name]
     m = golden_engine("SchNet", case)
     m.force_higher_order = higher
-    m.eval()
-    with torch.no_grad():
-        pred = m(_batch(case))
-    for p, ref in zip(pred, case["pred_eval"]):
-        assert _rel(p.cpu(), ref) < 1e-5, name
-    m.train()
-    for mod in m.modules():
-        if isinstance(mod, torch.nn.Dropout):
-            mod.p = 0.0
-        if hasattr(mod, "dropout") and isinstance(mod.dropout, float):
-            mod.dropout = 0.0
-    b = _batch(case)
-    pred = m(b)
-    value = case["value"].to(DEV)
-    loss, _ = m.loss(pred, value, [torch.arange(value.numel(), device=DEV)])
-    assert abs(float(loss) - float(case["loss"])) < 1e-5 * max(1.0, abs(float(case["loss"])))
-    grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-    for (n, _), gr in zip(m.named_parameters(), grads):
-        ref = case["grads"][n]
-        if ref is None or float(ref.norm()) == 0:
-            assert gr is None or float(gr.abs().max()) < 1e-6, n
-            continue
-        # a bias followed by BatchNorm has a zero true gradient: both sides hold rounding noise there
-        err = float((gr.cpu().double() - ref.double()).norm())
-        assert err <= 1e-4 * float(ref.double().norm()) + 1e-5, (name, n, err)
+    # norm-wise gradients: a bias followed by BatchNorm has a zero true gradient, both sides hold rounding noise there
+    check_golden_case(m, case, lambda: _batch(case), pred=(1e-5, 1e-5), loss=(1e-5, 0), grads=grad_norm(1e-4, 1e-5))
 
 
 def test_nonzero_edge_shifts_do_not_change_the_result(golden_dir):

@@ -11,18 +11,10 @@ from hydragnn_b200 import padded
 from hydragnn_b200.cgcnn import CGCNNStack
 from oracle.base import oracle_from_case
 from oracle.cgcnn import CGCNNStackOracle, CGConv
-from stack_support import engine_kwargs
+from stack_support import check_golden_case, check_seeded_state, engine_kwargs, golden_data, grad_close
 
 CASES = ["cgcnn_graph_edge0", "cgcnn_node_edge_len", "cgcnn_add_pool_edge3", "cgcnn_multihead", "cgcnn_mlp_per_node", "cgcnn_gps",
          "cgcnn_gps_edge2", "cgcnn_ci_width1"]
-
-
-class _Data:
-    def __init__(self, d, dtype=torch.float64):
-        for k, v in d.items():
-            setattr(self, k, v.to(dtype) if torch.is_tensor(v) and v.is_floating_point() else v)
-        if not hasattr(self, "edge_attr"):
-            self.edge_attr = None
 
 
 def _golden(golden_dir):
@@ -93,27 +85,8 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole CGCNN stack (fp64) against the reference's: eval and train-mode predictions, the loss, every parameter
     gradient and the BatchNorm running statistics."""
     c = _golden(golden_dir)[name]
-    m = oracle_from_case(CGCNNStackOracle, c)
-    d = _Data(c["inputs"])
-    rel = lambda a, b: float((a - b.double()).norm() / b.double().norm())                # noqa: E731
-    m.eval()
-    with torch.no_grad():
-        assert all(rel(a, b) < 1e-6 for a, b in zip(m(d), c["pred_eval"]))
-    m.train()
-    pred = m(d)
-    assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
-    torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
-    grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for (n, _), g in zip(m.named_parameters(), grads):
-        if c["grads"][n] is None:
-            assert g is None or not g.any(), n
-            continue
-        torch.testing.assert_close(g, c["grads"][n].double(), rtol=1e-4, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].to(v.dtype), v, rtol=1e-5, atol=1e-7)
+    check_golden_case(oracle_from_case(CGCNNStackOracle, c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
+                      grads=grad_close(1e-4, 1e-6))
 
 
 def engine_from_case(c, **kw):
@@ -127,11 +100,7 @@ def test_engine_state_dict_and_str_match_the_reference(golden_dir, name):
     c = _golden(golden_dir)[name]
     eng = engine_from_case(c)
     assert isinstance(eng, CGCNNStack) and str(eng) == c["str"] == "CGCNNStack"
-    sr, se = c["state"], eng.state_dict()
-    assert list(sr.keys()) == list(se.keys())
-    for k in sr:
-        assert sr[k].shape == se[k].shape and torch.equal(sr[k], se[k]), k
-    eng.load_state_dict(sr, strict=True)
+    check_seeded_state(eng, c["state"])
     assert all(isinstance(f.module, torch.nn.BatchNorm1d) for f in eng.feature_layers)
 
 
@@ -170,7 +139,7 @@ def test_hidden_dim_other_than_input_dim_without_gps_is_refused_before_any_launc
     eng = engine_from_case(dict(c, cfg=dict(c["cfg"], hidden_dim=5)))
     assert eng.graph_convs[0].module_0.channels == 3 and eng.feature_layers[0].module.num_features == 5
     with pytest.raises(ValueError, match="hidden_dim is 5"):
-        eng(_Data(c["inputs"], torch.float32))
+        eng(golden_data(c["inputs"], torch.float32))
 
 
 def test_padded_step_refuses_cgcnn(golden_dir):

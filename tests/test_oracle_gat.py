@@ -11,18 +11,10 @@ from hydragnn_b200 import ops, padded
 from hydragnn_b200.gat import GATStack
 from oracle.base import oracle_from_case
 from oracle.gat import GATStackOracle, GATv2Conv
-from stack_support import check_grads, engine_kwargs, seeded_state, state_digest
+from stack_support import check_golden_case, engine_kwargs, golden_data, grad_close, seeded_state, state_digest
 
 CASES = ["gat_graph_noedge", "gat_node_edge_len", "gat_multihead", "gat_add_pool_edge3", "gat_one_layer", "gat_input_ne_hidden",
          "gat_conv_head", "gat_gps", "gat_gps_edge2", "gat_loops_dups_isolated"]
-
-
-class _Data:
-    def __init__(self, d, dtype=torch.float64):
-        for k, v in d.items():
-            setattr(self, k, v.to(dtype) if torch.is_tensor(v) and v.is_floating_point() else v)
-        if not hasattr(self, "edge_attr"):
-            self.edge_attr = None
 
 
 def _golden(golden_dir):
@@ -120,32 +112,10 @@ def test_gatv2conv_hand_computed_gradients(concat):
 @pytest.mark.parametrize("name", CASES)
 def test_oracle_stack_matches_reference_golden(golden_dir, name):
     c = _golden(golden_dir)[name]
-    m = oracle_from_case(GATStackOracle, c, seeded_state(c))
-    d = _Data(c["inputs"])
-    rel = lambda a, b: float((a - b.double()).norm() / max(float(b.double().norm()), 1e-12))  # noqa: E731
-    m.eval()
-    with torch.no_grad():
-        assert all(rel(a, b) < 1e-6 for a, b in zip(m(d), c["pred_eval"]))
-    m.train()
-    pred = m(d)
-    assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
-    # the golden is the reference's fp32 arithmetic: the 120-wide head convs of gat_conv_head put its loss 1.2e-6 from fp64
-    torch.testing.assert_close(float(loss), float(c["loss"]), rtol=5e-6, atol=0)
-    grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-
-    def check(n, g, ref):
-        if ref is None:
-            assert g is None or not g.any(), n
-            return
-        # a conv bias in front of a BatchNorm has no gradient in exact arithmetic; the fp32 golden holds up to 1.1e-6 gmax there
-        torch.testing.assert_close(g, ref.double(), rtol=1e-4, atol=2e-6 * gmax, msg=lambda s: n + ": " + s)
-
-    check_grads(c, [(n, g) for (n, _), g in zip(m.named_parameters(), grads)], check)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].to(v.dtype), v, rtol=1e-5, atol=1e-7)
+    # the golden is the reference's fp32 arithmetic: the 120-wide head convs of gat_conv_head put its loss 1.2e-6 from fp64, and a
+    # conv bias in front of a BatchNorm, which has no gradient in exact arithmetic, holds up to 1.1e-6 gmax there
+    check_golden_case(oracle_from_case(GATStackOracle, c, seeded_state(c)), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
+                      loss=(5e-6, 0), grads=grad_close(1e-4, 2e-6))
 
 
 def engine_from_case(c, **kw):
@@ -186,7 +156,7 @@ def test_conv_head_with_edge_features_fails_as_the_reference_does(golden_dir):
                           edge_dim=1, num_conv_layers=2, use_gpu=False)
     c = _golden(golden_dir)["gat_node_edge_len"]
     with pytest.raises(AssertionError):
-        eng(_Data(c["inputs"], torch.float32))
+        eng(golden_data(c["inputs"], torch.float32))
 
 
 def test_existing_refusals_stay():

@@ -12,6 +12,7 @@ import torch
 from hydragnn_b200.pna import AGGREGATORS, SCALERS, PNAStack
 from oracle.base import oracle_from_case
 from oracle.pna import PNAConv, PNAStackOracle
+from stack_support import check_golden_case, check_seeded_state, golden_data, grad_close
 
 # nodes 0..4, x = [1, 2, 4, 8, 16]; edges (source -> target): 1->0, 2->0 (two into 0), 0->3 (one), 2->4 twice (a tie);
 # nodes 1 and 2 receive nothing
@@ -105,18 +106,7 @@ def test_engine_pna_stack_reproduces_the_reference_seeded_state(golden_dir, name
                         pe_dim=4 if cfg["gps"] else 0, global_attn_engine="GPS" if cfg["gps"] else None,
                         global_attn_type="multihead" if cfg["gps"] else None, global_attn_heads=4 if cfg["gps"] else 0, use_gpu=False)
     assert isinstance(m, PNAStack) and str(m) == "PNAStack"
-    sd = m.state_dict()
-    assert list(sd.keys()) == list(c["state"].keys())
-    for k, v in sd.items():
-        assert v.shape == c["state"][k].shape and torch.equal(v, c["state"][k]), k
-
-
-class _Data:
-    def __init__(self, inputs, dtype=torch.float64):
-        for k, v in inputs.items():
-            setattr(self, k, v.to(dtype) if v.is_floating_point() else v)
-        if not hasattr(self, "edge_attr"):
-            self.edge_attr = None
+    check_seeded_state(m, c["state"])
 
 
 @pytest.mark.parametrize("name", ["pna_graph_noedge", "pna_node_edge_len", "pna_multihead_h5", "pna_add_pool_edge3"])
@@ -124,24 +114,8 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole PNA stack (fp64) against the reference's PNAStack.py + Base.py: eval and train-mode predictions, the loss,
     every parameter gradient and the BatchNorm running statistics after the step.  (GPS is the reference's gps.py, not restated.)"""
     c = torch.load(golden_dir + "/models_pna.pt")[name]
-    m = oracle_from_case(PNAStackOracle, c)
-    d = _Data(c["inputs"])
-    rel = lambda a, b: float((a - b.double()).norm() / b.double().norm())                # noqa: E731
-    m.eval()
-    with torch.no_grad():
-        assert all(rel(a, b) < 1e-6 for a, b in zip(m(d), c["pred_eval"]))
-    m.train()
-    pred = m(d)
-    assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
-    torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
-    grads = torch.autograd.grad(loss, list(m.parameters()))
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for (n, _), g in zip(m.named_parameters(), grads):
-        torch.testing.assert_close(g, c["grads"][n].double(), rtol=1e-4, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].to(v.dtype), v, rtol=1e-5, atol=1e-7)
+    check_golden_case(oracle_from_case(PNAStackOracle, c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
+                      grads=grad_close(1e-4, 1e-6))
 
 
 def test_pna_conv_with_edge_dim_refuses_a_missing_edge_attr():

@@ -11,6 +11,7 @@ import torch
 
 from oracle.base import oracle_from_case
 from oracle.pnaplus import BesselBasisLayer, Envelope, PNAPlusStackOracle
+from stack_support import check_golden_case, check_grads, check_seeded_state, golden_data, grad_close
 
 CASES = ["pnaplus_graph_noedge", "pnaplus_node_edge_len", "pnaplus_multihead_h5", "pnaplus_gps", "pnaplus_edge_dim0",
          "pnaplus_add_pool_edge3", "pnaplus_conv_head"]
@@ -88,18 +89,8 @@ def test_engine_pnaplus_stack_reproduces_the_reference_seeded_state(golden_dir, 
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
     m = _create(c)
     assert isinstance(m, PNAPlusStack) and str(m) == c["str"] == "PNAStack"
-    sd = m.state_dict()
-    assert list(sd.keys()) == list(c["state"].keys()) and list(sd.keys())[-1] == "rbf.freq"
-    for k, v in sd.items():
-        assert v.shape == c["state"][k].shape and torch.equal(v, c["state"][k]), k
-
-
-class _Data:
-    def __init__(self, inputs, dtype=torch.float64):
-        for k, v in inputs.items():
-            setattr(self, k, v.to(dtype) if v.is_floating_point() else v)
-        if not hasattr(self, "edge_attr"):
-            self.edge_attr = None
+    assert list(m.state_dict().keys())[-1] == "rbf.freq"
+    check_seeded_state(m, c["state"])
 
 
 @pytest.mark.parametrize("name", ["pnaplus_graph_noedge", "pnaplus_node_edge_len", "pnaplus_multihead_h5", "pnaplus_edge_dim0",
@@ -108,29 +99,11 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole PNAPlus stack (fp64) against the reference's PNAPlusStack.py + Base.py: eval and train-mode predictions,
     the loss, every parameter gradient (None where the reference's is None) and the BatchNorm running statistics."""
     c = torch.load(golden_dir + "/models_pnaplus.pt")[name]
-    m = oracle_from_case(PNAPlusStackOracle, c)
-    d = _Data(c["inputs"])
-    dist = (d.pos[d.edge_index[1]] - d.pos[d.edge_index[0]]).norm(dim=-1)
+    pos, ei = c["inputs"]["pos"], c["inputs"]["edge_index"]
+    dist = (pos[ei[1]] - pos[ei[0]]).norm(dim=-1)
     assert float(dist.max()) > c["cfg"]["radius"] > float(dist.min())                    # edges on both sides of the cutoff
-    rel = lambda a, b: float((a - b.double()).norm() / b.double().norm())                # noqa: E731
-    m.eval()
-    with torch.no_grad():
-        assert all(rel(a, b) < 1e-6 for a, b in zip(m(d), c["pred_eval"]))
-    m.train()
-    pred = m(d)
-    assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
-    torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
-    grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for (n, _), g in zip(m.named_parameters(), grads):
-        if c["grads"][n] is None:
-            assert g is None or not g.any(), n
-            continue
-        torch.testing.assert_close(g, c["grads"][n].double(), rtol=1e-4, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].to(v.dtype), v, rtol=1e-5, atol=1e-7)
+    check_golden_case(oracle_from_case(PNAPlusStackOracle, c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
+                      loss=(1e-6, 0), grads=grad_close(1e-4, 1e-6))
 
 
 def test_edge_dim0_keeps_an_unused_edge_encoder(golden_dir):
@@ -145,7 +118,7 @@ def test_oracle_mlip_matches_reference_golden(golden_dir):
     c = torch.load(golden_dir + "/models_pnaplus.pt")["pnaplus_mlip"]
     m = oracle_from_case(PNAPlusStackOracle, c)
     m.eval()
-    d = _Data(c["inputs"])
+    d = golden_data(c["inputs"])
     d.pos.requires_grad_(True)
     pred = m(d)[0]
     g = int(d.batch.max()) + 1
@@ -159,8 +132,4 @@ def test_oracle_mlip_matches_reference_golden(golden_dir):
     tot = ee + ep + ef
     torch.testing.assert_close(float(tot), float(c["loss"]), rtol=1e-6, atol=0)
     grads = torch.autograd.grad(tot, list(m.parameters()), allow_unused=True)
-    gmax = max(float(x.abs().max()) for x in c["grads"].values() if x is not None)
-    for (n, _), gr in zip(m.named_parameters(), grads):
-        if c["grads"][n] is None:
-            continue
-        torch.testing.assert_close(gr, c["grads"][n].double(), rtol=1e-4, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
+    check_grads(c, {n: gr for (n, _), gr in zip(m.named_parameters(), grads)}, grad_close(1e-4, 1e-6))

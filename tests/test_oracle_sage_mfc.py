@@ -5,17 +5,12 @@ import torch
 
 from oracle.base import oracle_from_case
 from oracle.sage import MFCStackOracle, MFConv, SAGEConv, SAGEStackOracle
+from stack_support import check_golden_case, golden_data, grad_close
 
 SAGE_CASES = ["sage_graph", "sage_node", "sage_multihead", "sage_mlp_per_node", "sage_conv_head", "sage_max_pool_in1", "sage_gps",
               "sage_initial_bias", "sage_initial_bias_node"]
 MFC_CASES = ["mfc_graph_deg5", "mfc_node_deg1", "mfc_multihead_deg100", "mfc_mlp_per_node", "mfc_conv_head", "mfc_max_pool_in1",
              "mfc_gps", "mfc_initial_bias_node"]
-
-
-class _Data:
-    def __init__(self, d, dtype=torch.float64):
-        for k, v in d.items():
-            setattr(self, k, v.to(dtype) if torch.is_tensor(v) and v.is_floating_point() else v)
 
 
 def _set(lin, w, b=None):
@@ -65,26 +60,7 @@ def _golden(golden_dir, kind):
 
 
 def _check(m, c):
-    d = _Data(c["inputs"])
-    rel = lambda a, b: float((a - b.double()).norm() / b.double().norm().clamp(min=1e-30))     # noqa: E731
-    m.eval()
-    with torch.no_grad():
-        assert all(rel(a, b) < 1e-6 for a, b in zip(m(d), c["pred_eval"]))
-    m.train()
-    pred = m(d)
-    assert all(rel(a.detach(), b) < 1e-5 for a, b in zip(pred, c["pred_train"]))
-    loss, _ = m.loss(pred, c["value"].double(), c["head_index"])
-    torch.testing.assert_close(float(loss), float(c["loss"]), rtol=1e-6, atol=0)
-    grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-    gmax = max(float(g.abs().max()) for g in c["grads"].values() if g is not None)
-    for (n, _), g in zip(m.named_parameters(), grads):
-        if c["grads"][n] is None:
-            assert g is None or not g.any(), n
-            continue
-        torch.testing.assert_close(g, c["grads"][n].double(), rtol=1e-4, atol=1e-6 * gmax, msg=lambda s, n=n: n + ": " + s)
-    sd = m.state_dict()
-    for k, v in c["state_after"].items():
-        torch.testing.assert_close(sd[k].to(v.dtype), v, rtol=1e-5, atol=1e-7)
+    check_golden_case(m, c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0), grads=grad_close(1e-4, 1e-6))
 
 
 def _oracle(cls, c):

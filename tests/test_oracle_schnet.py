@@ -8,6 +8,7 @@ import pytest
 
 from oracle import schnet as so
 from oracle.base import oracle_from_case
+from stack_support import check_golden_case, golden_data, grad_norm
 
 
 def test_gaussian_coefficient_and_values():
@@ -60,42 +61,12 @@ def test_coordinate_update_is_a_mean_over_sources():
     assert torch.equal(new[2], pos[2])
 
 
-class _D:
-    def __init__(self, inputs, dtype):
-        for k, v in inputs.items():
-            setattr(self, k, v.to(dtype) if v.is_floating_point() else v)
-        if "edge_attr" not in inputs:
-            self.edge_attr = None
-
-
 @pytest.mark.parametrize("name", ["inlayer_graph", "inlayer_truncated", "equivariant_conv_head", "edge_len", "edge3", "gps",
                                   "gps_edge2", "add_pool"])
 def test_oracle_stack_matches_the_reference(golden_dir, name):
     """The oracle stack at fp64 against the reference's own SCFStack (fp32): eval predictions, the train-mode loss and every
     parameter gradient."""
     case = torch.load(golden_dir + "/models_schnet.pt")[name]
-    m = oracle_from_case(so.SCFStackOracle, case)
-    d = _D(case["inputs"], torch.float64)
-    m.eval()
-    with torch.no_grad():
-        for p, ref in zip(m(d), case["pred_eval"]):
-            assert _rel(p, ref) < 1e-5, name
-    m.train()
-    pred = m(d)
-    for p, ref in zip(pred, case["pred_train"]):
-        assert _rel(p, ref) < 1e-5, name
-    loss, _ = m.loss(pred, case["value"].double(), [torch.arange(case["value"].numel())])
-    assert abs(float(loss) - float(case["loss"])) <= 1e-5 * abs(float(case["loss"]))
-    grads = torch.autograd.grad(loss, list(m.parameters()), allow_unused=True)
-    for (n, _), g in zip(m.named_parameters(), grads):
-        ref = case["grads"][n]
-        if ref is None:
-            assert g is None or float(g.abs().max()) == 0, n
-            continue
-        g = torch.zeros_like(ref, dtype=torch.float64) if g is None else g
-        # a bias followed by BatchNorm has a zero true gradient: the reference's fp32 value there is rounding noise
-        assert float((g - ref.double()).norm()) <= 1e-4 * float(ref.double().norm()) + 1e-6, (name, n)
-
-
-def _rel(a, b):
-    return float((a.double() - b.double()).norm() / b.double().norm())
+    # norm-wise gradients: a bias followed by BatchNorm has a zero true gradient, the reference's fp32 value there is rounding noise
+    check_golden_case(oracle_from_case(so.SCFStackOracle, case), case, lambda: golden_data(case["inputs"]), pred=(1e-5, 1e-5),
+                      loss=(1e-5, 0), grads=grad_norm(1e-4, 1e-6))
