@@ -56,6 +56,8 @@ def create_model_config(config, verbosity=0, use_gpu=True):
         avg_num_neighbors=g("avg_num_neighbors"), conv_checkpointing=training.get("conv_checkpointing", False),
         enable_interatomic_potential=g("enable_interatomic_potential", False), energy_weight=g("energy_weight", 0.0),
         energy_peratom_weight=g("energy_peratom_weight", 0.0), force_weight=g("force_weight", 0.0),
+        use_graph_attr_conditioning=g("use_graph_attr_conditioning", False),
+        graph_attr_conditioning_mode=g("graph_attr_conditioning_mode", "concat_node"),
         graph_pooling=g("graph_pooling", "mean"), verbosity=verbosity, use_gpu=use_gpu)
     prec = str(training.get("precision", "fp32")).lower()
     if prec in ("fp64", "float64", "double"):
@@ -88,7 +90,7 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
     torch.manual_seed(0)
     if global_attn_engine and (global_attn_engine != "GPS" or global_attn_type != "multihead"):
         raise ValueError("b200 engine: only global_attn_engine='GPS' with global_attn_type='multihead' is implemented")
-    if use_graph_attr_conditioning:
+    if use_graph_attr_conditioning and mpnn_type != "MACE":
         raise ValueError("b200 engine: graph_attr conditioning is not implemented yet")
     heads = update_multibranch_heads(output_heads)
     common = dict(input_dim=input_dim, hidden_dim=hidden_dim, output_dim=output_dim, output_type=output_type,
@@ -124,7 +126,8 @@ def create_model(mpnn_type, input_dim, hidden_dim, output_dim, pe_dim=0, global_
         assert node_max_ell >= 1, "MACE requires node_max_ell >= 1."
         from .mace import MACEStack
         model = MACEStack(radius, radial_type, distance_transform, num_radial, edge_dim, max_ell, node_max_ell, avg_num_neighbors,
-                          envelope_exponent, correlation, **common)
+                          envelope_exponent, correlation, use_graph_attr_conditioning=use_graph_attr_conditioning,
+                          graph_attr_conditioning_mode=graph_attr_conditioning_mode, **common)
     elif mpnn_type == "SchNet":
         assert num_gaussians is not None, "SchNet requires num_guassians input."
         assert num_filters is not None, "SchNet requires num_filters input."

@@ -79,6 +79,16 @@ struct LinParams {
   int slots;            // output staging buffers per consumer warpgroup (2 or 4), one [64 x 32] sub-tile each
 };
 
+// hgb_tc_linear_graph_add: a separate parameter type, so the plain layers' kernels keep their parameter block and registers
+struct LinParamsGA : LinParams {
+  const float* gadd;    // [ng, no] (row stride ldg), never with addend: y = a.B^T + bias + gadd[graph(row)], where graph(row) is
+  const int32_t* gptr;  //   the g with gptr[g] <= row < gptr[g + 1] (graph offsets [ng + 1], rows sorted by graph)
+  int ng;
+  int64_t ldg;
+};
+template <bool GA> struct LinParamsOf { using type = LinParams; };
+template <> struct LinParamsOf<true> { using type = LinParamsGA; };
+
 constexpr int TILE_M = 64;                       // rows per tile = one wgmma M
 constexpr uint32_t A_STAGE = TILE_M * 128;       // one pipeline stage = one [64 x 32 fp32] k-block (8 KB)
 constexpr uint32_t SUB_BYTES = TILE_M * 128;     // one output staging buffer = one [64 x 32 fp32] TMA store box (8 KB)
@@ -88,7 +98,7 @@ constexpr int LIN_THREADS = 384;
 enum { EPI_NONE, EPI_RELU, EPI_SILU, EPI_SILU_ZD, EPI_TANH, EPI_OTHER };
 
 // the epilogue of one output: v = accumulator + bias on entry; z receives what the z output stores
-template <int K>
+template <int K, bool GA>
 __device__ __forceinline__ float lin_epilogue1(const LinParams& p, float v, float& z, float a, float g) {
   z = v;
   if (K == EPI_RELU) v = isnan(v) ? v : fmaxf(v, 0.f);     // torch.relu (clamp_min): NaN propagates
@@ -100,7 +110,7 @@ __device__ __forceinline__ float lin_epilogue1(const LinParams& p, float v, floa
   }
   if (K == EPI_TANH) v = tanhf(v);
   if (K == EPI_OTHER) v = hgb_act(v, p.act, p.act_param);
-  if (p.addend) v += a;
+  if (GA || p.addend) v += a;
   if (p.gsrc) {
     if (p.gact == HGB_ACT_RELU_SELECT) v = hgb_relu_select(v, g);
     else v *= p.gact == HGB_ACT_DERIV ? g : hgb_act_grad(g, g, p.gact, p.act_param);   // DERIV: gsrc already holds act'(.)
@@ -110,7 +120,7 @@ __device__ __forceinline__ float lin_epilogue1(const LinParams& p, float v, floa
 
 // Element loop over one [64 x 32] sub-tile of a warpgroup (tid 0..127): 4 float4 per thread, 8 threads per row.  ys holds the
 // accumulators in the TMA SWIZZLE_128B layout and receives y in place; zs receives z.  a / g: this thread's addend / gsrc values.
-template <int K>
+template <int K, bool GA>
 __device__ __forceinline__ void lin_epilogue_sub(const LinParams& p, const float* sb, uint8_t* ys, uint8_t* zs, int tid, const float4* a,
                                                  const float4* g) {
 #pragma unroll
@@ -118,23 +128,38 @@ __device__ __forceinline__ void lin_epilogue_sub(const LinParams& p, const float
     const int idx = j * 128 + tid, r = idx >> 3, q = idx & 7;
     const uint32_t off = (uint32_t)r * 128 + ((q ^ (r & 7)) << 4);
     float4 v = *reinterpret_cast<float4*>(ys + off), z;
-    v.x = lin_epilogue1<K>(p, v.x + sb[4 * q], z.x, a[j].x, g[j].x);
-    v.y = lin_epilogue1<K>(p, v.y + sb[4 * q + 1], z.y, a[j].y, g[j].y);
-    v.z = lin_epilogue1<K>(p, v.z + sb[4 * q + 2], z.z, a[j].z, g[j].z);
-    v.w = lin_epilogue1<K>(p, v.w + sb[4 * q + 3], z.w, a[j].w, g[j].w);
+    v.x = lin_epilogue1<K, GA>(p, v.x + sb[4 * q], z.x, a[j].x, g[j].x);
+    v.y = lin_epilogue1<K, GA>(p, v.y + sb[4 * q + 1], z.y, a[j].y, g[j].y);
+    v.z = lin_epilogue1<K, GA>(p, v.z + sb[4 * q + 2], z.z, a[j].z, g[j].z);
+    v.w = lin_epilogue1<K, GA>(p, v.w + sb[4 * q + 3], z.w, a[j].w, g[j].w);
     *reinterpret_cast<float4*>(ys + off) = v;
     if (zs) *reinterpret_cast<float4*>(zs + off) = z;
   }
 }
 
-// this thread's addend / gsrc values of sub-tile c (columns 32 c ..) of the tile at row0, in lin_epilogue_sub's element order
-__device__ __forceinline__ void lin_load_operands(const LinParams& p, int row0, int c, int tid, float4* a, float4* g) {
+// the graph of row `row` (< m): the last g with gptr[g] <= row, so empty graphs (repeated offsets) are skipped
+__device__ __forceinline__ int lin_graph_of(const LinParamsGA& p, int row) {
+  int lo = 0, hi = p.ng;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(p.gptr + mid) <= row) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// this thread's addend / gsrc values of sub-tile c (columns 32 c ..) of the tile at row0, in lin_epilogue_sub's element order;
+// gid: the graphs of this thread's 4 rows (gadd only)
+template <bool GA>
+__device__ __forceinline__ void lin_load_operands(const typename LinParamsOf<GA>::type& p, int row0, int c, int tid, const int* gid, float4* a, float4* g) {
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int idx = j * 128 + tid, row = row0 + (idx >> 3);
     const int64_t o = (int64_t)row * p.ldy + c * 32 + (idx & 7) * 4;
     const bool in = row < p.m;
     if (p.addend) a[j] = in ? __ldg(reinterpret_cast<const float4*>(p.addend + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (GA)
+      a[j] = in ? __ldg(reinterpret_cast<const float4*>(p.gadd + (int64_t)gid[j] * p.ldg + c * 32 + (idx & 7) * 4))
+                : make_float4(0.f, 0.f, 0.f, 0.f);
     if (p.gsrc) g[j] = in ? __ldg(reinterpret_cast<const float4*>(p.gsrc + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
   }
 }
@@ -146,10 +171,12 @@ __device__ __forceinline__ void lin_load_operands(const LinParams& p, int row0, 
 // Tightest split case, 64 KB of weights per copy: 1 KB + 128 KB B + 32 KB staging leaves 66 KB = 4 A stages of 16 KB.  Four slots
 // per warpgroup (64 KB) are used when at least 4 stages still fit next to them: B <= 128 KB in TF32 mode, <= 48 KB per copy in split
 // mode (every C2 layer has B <= 48 KB).
-template <int NC, bool SPLIT>   // NO = 32 * NC output columns; SPLIT: the fp32-accurate mode
+// GA: the per-graph addend (gadd) of hgb_tc_linear_graph_add; its own instantiations, so the plain layers keep their registers
+template <int NC, bool SPLIT, bool GA>   // NO = 32 * NC output columns; SPLIT: the fp32-accurate mode
 __global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                                    const __grid_constant__ CUtensorMap tmap_y,
-                                                                   const __grid_constant__ CUtensorMap tmap_z, const LinParams p) {
+                                                                   const __grid_constant__ CUtensorMap tmap_z,
+                                                                   const typename LinParamsOf<GA>::type p) {
   constexpr int NO = NC * 32;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -272,18 +299,26 @@ __global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_
                      : p.act == HGB_ACT_SILU ? (p.z && p.z_deriv ? EPI_SILU_ZD : EPI_SILU)
                      : p.act == HGB_ACT_TANH ? EPI_TANH
                                              : EPI_OTHER;
-    const bool operands = p.addend || p.gsrc;
+    const bool operands = GA || p.addend || p.gsrc;
     float acc[NC * 16];
     uint32_t sub = 0;                   // sub-tiles stored so far by this warpgroup
     int li = cw;
     for (int t = blockIdx.x + cw * gridDim.x; t < ntiles; t += 2 * gridDim.x, li += 2) {
       const int row0 = t * TILE_M;
+      int gid[4] = {0, 0, 0, 0};
+      if constexpr (GA) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int row = row0 + ((j * 128 + tid) >> 3);
+          if (row < p.m) gid[j] = lin_graph_of(p, row);
+        }
+      }
       float4 opa[4], opg[4];
 #pragma unroll
       for (int j = 0; j < 4; ++j) opa[j] = opg[j] = make_float4(0.f, 0.f, 0.f, 0.f);
       // the first sub-tile's addend / gsrc are in flight during the MMAs (at NC = 8 these 32 registers would spill: load after them)
       constexpr bool early = NC < 8;
-      if (early && operands) lin_load_operands(p, row0, 0, tid, opa, opg);
+      if (early && operands) lin_load_operands<GA>(p, row0, 0, tid, gid, opa, opg);
 #pragma unroll
       for (int j = 0; j < NC * 16; ++j) acc[j] = 0.f;
       const uint32_t n0 = (uint32_t)(li >> 1) * KB;             // first item of this tile within ring cw
@@ -314,7 +349,7 @@ __global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_
       wgmma_wait<0>();
       fence_regs<NC * 16>(acc);
       if (lane == 0) mbar_arrive(empty + cw * SR + (n0 + KB - 1) % SR);
-      if (!early && operands) lin_load_operands(p, row0, 0, tid, opa, opg);
+      if (!early && operands) lin_load_operands<GA>(p, row0, 0, tid, gid, opa, opg);
       // ===== epilogue, one [64 x 32] sub-tile at a time: accumulators -> swizzled staging buffer -> element loop in place -> TMA
       // store (rows >= m are clipped by the tensor map) =====
 #pragma unroll 1
@@ -340,14 +375,14 @@ __global__ void __launch_bounds__(LIN_THREADS, 1) tc_linear_kernel(const __grid_
         named_bar_sync(2 + cw, 128);
         const float* sb = sbias + c * 32;
         switch (kind) {
-          case EPI_NONE: lin_epilogue_sub<EPI_NONE>(p, sb, ys, zs, tid, opa, opg); break;
-          case EPI_RELU: lin_epilogue_sub<EPI_RELU>(p, sb, ys, zs, tid, opa, opg); break;
-          case EPI_SILU: lin_epilogue_sub<EPI_SILU>(p, sb, ys, zs, tid, opa, opg); break;
-          case EPI_SILU_ZD: lin_epilogue_sub<EPI_SILU_ZD>(p, sb, ys, zs, tid, opa, opg); break;
-          case EPI_TANH: lin_epilogue_sub<EPI_TANH>(p, sb, ys, zs, tid, opa, opg); break;
-          default: lin_epilogue_sub<EPI_OTHER>(p, sb, ys, zs, tid, opa, opg);
+          case EPI_NONE: lin_epilogue_sub<EPI_NONE, GA>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_RELU: lin_epilogue_sub<EPI_RELU, GA>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_SILU: lin_epilogue_sub<EPI_SILU, GA>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_SILU_ZD: lin_epilogue_sub<EPI_SILU_ZD, GA>(p, sb, ys, zs, tid, opa, opg); break;
+          case EPI_TANH: lin_epilogue_sub<EPI_TANH, GA>(p, sb, ys, zs, tid, opa, opg); break;
+          default: lin_epilogue_sub<EPI_OTHER, GA>(p, sb, ys, zs, tid, opa, opg);
         }
-        if (operands && c + 1 < NC) lin_load_operands(p, row0, c + 1, tid, opa, opg);
+        if (operands && c + 1 < NC) lin_load_operands<GA>(p, row0, c + 1, tid, gid, opa, opg);
         fence_proxy_async();            // the staged results are visible to the TMA
         named_bar_sync(2 + cw, 128);
         if (tid == 0) {
@@ -589,18 +624,23 @@ __global__ void tc_wgrad_reduce_kernel(const float* __restrict__ part, int npart
 // ------------------------------------------------------------------------------------------------
 bool shape_ok(int kr, int no) { return kr >= 32 && kr <= 256 && kr % 32 == 0 && no >= 32 && no <= 256 && no % 32 == 0; }
 
-template <int NC, bool SPLIT>
-void launch_linear_t(int grid, size_t smem, cudaStream_t st, const CUtensorMap* tm, const LinParams& p) {
+template <int NC, bool SPLIT, bool GA>
+void launch_linear_t(int grid, size_t smem, cudaStream_t st, const CUtensorMap* tm, const typename LinParamsOf<GA>::type& p) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaFuncSetAttribute(tc_linear_kernel<NC, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX);
+    cudaFuncSetAttribute(tc_linear_kernel<NC, SPLIT, GA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_MAX);
     attr_set = true;
   }
-  tc_linear_kernel<NC, SPLIT><<<grid, LIN_THREADS, smem, st>>>(tm[0], tm[1], tm[2], p);
+  tc_linear_kernel<NC, SPLIT, GA><<<grid, LIN_THREADS, smem, st>>>(tm[0], tm[1], tm[2], p);
 }
 template <int NC>
-void launch_linear(int grid, size_t smem, cudaStream_t st, const CUtensorMap* tm, const LinParams& p) {  // tm: a, y, z
-  if (p.split) launch_linear_t<NC, true>(grid, smem, st, tm, p); else launch_linear_t<NC, false>(grid, smem, st, tm, p);
+void launch_linear(int grid, size_t smem, cudaStream_t st, const CUtensorMap* tm, const LinParamsGA& p) {  // tm: a, y, z
+  if (p.gadd) {
+    if (p.split) launch_linear_t<NC, true, true>(grid, smem, st, tm, p); else launch_linear_t<NC, false, true>(grid, smem, st, tm, p);
+  } else {
+    const LinParams& q = p;
+    if (q.split) launch_linear_t<NC, true, false>(grid, smem, st, tm, q); else launch_linear_t<NC, false, false>(grid, smem, st, tm, q);
+  }
 }
 
 template <int Q, bool SPLIT>
@@ -627,17 +667,20 @@ extern "C" int hgb_tc_linear_supported(int32_t m, int32_t n_out, int32_t k_red) 
 // one (<= 256) x (<= 256) piece: y[m, no] = act(a[m, kr] . B^T + bias) + addend, y / z / addend with row stride ldy
 static int tc_linear_piece(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t trans_b, const float* bias, int32_t m,
                            int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z, const float* addend,
-                           const float* gsrc, int32_t gact, int64_t ldy, int32_t exact, hgb_stream_t stream) {
+                           const float* gsrc, int32_t gact, int64_t ldy, int32_t exact, const float* gadd, int64_t ldg,
+                           const int32_t* gptr, int32_t ng, hgb_stream_t stream) {
   HGB_REQUIRE(a && w && y && m >= 128 && shape_ok(k_red, n_out), "tc_linear: unsupported shape m=%d n=%d k=%d", m, n_out, k_red);
   HGB_REQUIRE(lda % 4 == 0 && ldy % 4 == 0 && ((uintptr_t)a % 16 == 0) && ((uintptr_t)y % 16 == 0) && (!z || (uintptr_t)z % 16 == 0) &&
-                  (!addend || (uintptr_t)addend % 16 == 0) && (!gsrc || (uintptr_t)gsrc % 16 == 0),
+                  (!addend || (uintptr_t)addend % 16 == 0) && (!gsrc || (uintptr_t)gsrc % 16 == 0) &&
+                  (!gadd || ((uintptr_t)gadd % 16 == 0 && ldg % 4 == 0)),
               "tc_linear: operands must be 16-byte aligned with a row stride that is a multiple of 4");
   CUtensorMap tm[3];                               // A loads; y and z stores: [64 x 32] boxes, rows >= m clipped
   int rc = make_tmap(&tm[0], a, m, k_red, lda, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
-  LinParams p;
+  LinParamsGA p;
   p.m = m; p.kr = k_red; p.no = n_out; p.w = w; p.ldw = ldw; p.trans_b = trans_b; p.bias = bias; p.act = act; p.act_param = act_param;
   p.y = y; p.z = z; p.addend = addend; p.ldy = ldy; p.gsrc = gsrc; p.gact = gact; p.z_deriv = (!gsrc && gact == HGB_ACT_DERIV) ? 1 : 0;
+  p.gadd = gadd; p.gptr = gptr; p.ng = ng; p.ldg = ldg;
   rc = make_tmap(&tm[1], y, m, n_out, ldy, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   rc = make_tmap(&tm[2], z ? z : y, m, n_out, ldy, TILE_M, CU_TENSOR_MAP_SWIZZLE_128B);
@@ -679,9 +722,11 @@ static int tc_linear_piece(const float* a, int64_t lda, const float* w, int64_t 
 // y[m, no] = act(a[m, kr] . B^T + bias) + addend;  B(r, c) = w[r, c] (trans_b = 0) or w[c, r] (trans_b = 1).
 // no > 256: independent column pieces.  kr > 256: the pieces of the reduction accumulate through `addend` (linear layers
 // only: an activation or a saved pre-activation needs the whole sum first).
-extern "C" int hgb_tc_linear(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t trans_b, const float* bias, int32_t m,
-                             int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z, const float* addend,
-                             const float* gsrc, int32_t gact, int32_t exact, hgb_stream_t stream) {
+// gadd (with gptr / ng / ldg) replaces addend for the first reduction piece: the per-graph row of hgb_tc_linear_graph_add
+static int tc_linear_pieces(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t trans_b, const float* bias, int32_t m,
+                            int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z, const float* addend,
+                            const float* gsrc, int32_t gact, int32_t exact, const float* gadd, int64_t ldg, const int32_t* gptr, int32_t ng,
+                            hgb_stream_t stream) {
   HGB_REQUIRE(a && w && y && hgb_tc_linear_supported(m, n_out, k_red), "tc_linear: unsupported shape m=%d n=%d k=%d", m, n_out, k_red);
   HGB_REQUIRE(k_red <= 256 || (act == HGB_ACT_NONE && !z && !gsrc), "tc_linear: reduction length %d > 256 needs a plain linear layer", k_red);
   // piece sizes: the B piece (kc x nc fp32) stays resident in shared memory next to >= 2 A stages per consumer ring
@@ -696,11 +741,30 @@ extern "C" int hgb_tc_linear(const float* a, int64_t lda, const float* w, int64_
       const float* wp = trans_b ? w + (int64_t)k0 * ldw + c0 : w + (int64_t)c0 * ldw + k0;
       const float* add = k0 == 0 ? (addend ? addend + c0 : nullptr) : y + c0;
       int rc = tc_linear_piece(a + k0, lda, wp, ldw, trans_b, (bias && k0 == 0) ? bias + c0 : nullptr, m, nc, kc, act, act_param, y + c0,
-                               z ? z + c0 : nullptr, add, gsrc ? gsrc + c0 : nullptr, gact, n_out, exact, stream);
+                               z ? z + c0 : nullptr, add, gsrc ? gsrc + c0 : nullptr, gact, n_out, exact,
+                               (gadd && k0 == 0) ? gadd + c0 : nullptr, ldg, gptr, ng, stream);
       if (rc) return rc;
     }
   }
   return HGB_OK;
+}
+
+extern "C" int hgb_tc_linear(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t trans_b, const float* bias, int32_t m,
+                             int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z, const float* addend,
+                             const float* gsrc, int32_t gact, int32_t exact, hgb_stream_t stream) {
+  return tc_linear_pieces(a, lda, w, ldw, trans_b, bias, m, n_out, k_red, act, act_param, y, z, addend, gsrc, gact, exact, nullptr, 0,
+                          nullptr, 0, stream);
+}
+
+// y[m, no] = a[m, kr] . w^T + gadd[graph(row)]: the concat_node projector Linear(H + G, H) on [h | graph_attr[batch]] with the
+// graph-attribute columns folded into the per-graph row gadd = graph_attr . W_g^T + b [ng, no] (row stride ldg)
+extern "C" int hgb_tc_linear_graph_add(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t m, int32_t n_out, int32_t k_red,
+                                       const float* gadd, int64_t ldg, const int32_t* gptr, int32_t ng, float* y, int32_t exact,
+                                       hgb_stream_t stream) {
+  HGB_REQUIRE(a && w && y && gadd && gptr && ng >= 1 && hgb_tc_linear_supported(m, n_out, k_red),
+              "tc_linear_graph_add: unsupported shape m=%d n=%d k=%d graphs=%d", m, n_out, k_red, ng);
+  return tc_linear_pieces(a, lda, w, ldw, 0, nullptr, m, n_out, k_red, HGB_ACT_NONE, 0.f, y, nullptr, nullptr, nullptr, 0, exact, gadd, ldg,
+                          gptr, ng, stream);
 }
 
 extern "C" int64_t hgb_tc_wgrad_workspace_bytes(int32_t n_out, int32_t k_out) { return (int64_t)HGB_NUM_SMS * n_out * (k_out + 1) * 4; }

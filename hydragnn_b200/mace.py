@@ -329,12 +329,22 @@ class MultiheadDecoder(nn.Module):
         return outs
 
 
+CONDITIONING_MODES = ("film", "concat_node", "fuse_pool")
+
+
 class MACEStack(Base):
-    """hydragnn/models/MACEStack.py:70-498 (no GPS wrapping, no graph-attr conditioning).  With edge_dim = D > 0 every
-    convolution reads ``data.edge_attr`` [E, D] as D extra 0e edge irreps in front of the spherical harmonics."""
+    """hydragnn/models/MACEStack.py:70-498 (no GPS wrapping).  With edge_dim = D > 0 every convolution reads ``data.edge_attr``
+    [E, D] as D extra 0e edge irreps in front of the spherical harmonics.
+
+    Graph-attribute conditioning (``use_graph_attr_conditioning``; hydragnn/models/Base.py:97-106, 217-223, 249-391) changes the
+    scalar block once after the embedding and after every convolution but the last, after that layer's readout -- the reference
+    also conditions the last layer's output, which nothing reads.  Its modules (``graph_conditioner`` for "film",
+    ``graph_concat_projector`` for "concat_node") are created at the first forward on the CPU generator and then moved, as the
+    reference does; "fuse_pool" checks ``graph_attr`` and changes nothing, because MACEStack.forward never pools with it."""
 
     def __init__(self, r_max, radial_type, distance_transform, num_bessel, edge_dim, max_ell, node_max_ell, avg_num_neighbors,
-                 num_polynomial_cutoff, correlation, *args, **kwargs):
+                 num_polynomial_cutoff, correlation, *args, use_graph_attr_conditioning=False, graph_attr_conditioning_mode="fuse_pool",
+                 **kwargs):
         # refused before Base.__init__, which would build the GPS embeddings first
         if kwargs.get("global_attn_engine"):
             raise ValueError("b200 engine: MACE inside GPS is not implemented")
@@ -359,6 +369,13 @@ class MACEStack(Base):
         if self.radial_type not in ("bessel", "gaussian", "chebyshev"):
             raise ValueError("unknown radial_type " + str(radial_type))
         self.num_bessel, self.radius, self.p_cut = num_bessel, float(r_max), float(p_cut)
+        self.use_graph_attr_conditioning = bool(use_graph_attr_conditioning)
+        self.graph_attr_conditioning_mode = graph_attr_conditioning_mode.lower()
+        if self.graph_attr_conditioning_mode not in CONDITIONING_MODES:
+            raise ValueError("graph_attr_conditioning_mode must be one of: 'film', 'concat_node', 'fuse_pool'.")
+        self.graph_conditioner = None
+        self.graph_concat_projector = None
+        self.graph_concat_projector_in_dim = None
         super().__init__(*args, **kwargs)
         # ---- post inheritance (:154-187)
         self.register_buffer("atomic_numbers", torch.arange(1, NUM_ELEMENTS + 1, dtype=torch.int64))
@@ -379,6 +396,85 @@ class MACEStack(Base):
         self.radial_embedding.cutoff_fn.register_buffer("r_max", torch.tensor(float(r_max)))
         self.node_embedding = nn.Module()
         self.node_embedding.linear = E3Linear([(NUM_ELEMENTS, 0, 1)], [(self.hidden_dim, 0, 1)])
+
+    @property
+    def device(self):
+        """Where the parameters live: the device ``load_existing_model`` creates missing conditioning modules on."""
+        return next(self.parameters()).device
+
+    # ---- graph-attribute conditioning (Base.py:249-391) -------------------------------------------------------------------
+    def _new_module_outside_capture(self):
+        if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("MACE graph-attribute conditioning creates its modules at the first forward; run one forward (or "
+                               "load the checkpoint) before capturing a step")
+
+    def _ensure_graph_conditioner(self, graph_attr_dim, device):
+        """FiLM's ``Sequential(Linear(G, max(H, G)), act, Linear(max(H, G), 2H))``, created on the CPU, moved to ``device``."""
+        if self.graph_conditioner is None:
+            self._new_module_outside_capture()
+            hidden = max(self.hidden_dim, graph_attr_dim)
+            self.graph_conditioner = nn.Sequential(nn.Linear(graph_attr_dim, hidden), self.activation_function,
+                                                   nn.Linear(hidden, 2 * self.hidden_dim))
+        if self.graph_conditioner[0].weight.device != device:
+            self.graph_conditioner = self.graph_conditioner.to(device)
+
+    def _ensure_graph_concat_projector(self, graph_attr_dim, channel_dim, device, dtype=None):
+        """concat_node's ``Linear(channel_dim + G, channel_dim)``, created on the CPU, moved to ``device`` / ``dtype``."""
+        in_dim = channel_dim + graph_attr_dim
+        if self.graph_concat_projector is None or self.graph_concat_projector_in_dim != in_dim:
+            self._new_module_outside_capture()
+            self.graph_concat_projector = nn.Linear(in_dim, channel_dim)
+            self.graph_concat_projector_in_dim = in_dim
+        w = self.graph_concat_projector.weight
+        if w.device != device or (dtype is not None and w.dtype != dtype):
+            self.graph_concat_projector = self.graph_concat_projector.to(device=device, dtype=dtype)
+
+    def graph_attr_modules_missing(self):
+        """True while a conditioned model has not created its conditioning modules (no forward, no checkpoint load yet)."""
+        if not self.use_graph_attr_conditioning:
+            return False
+        mode = self.graph_attr_conditioning_mode
+        return ((mode == "film" and self.graph_conditioner is None) or
+                (mode == "concat_node" and self.graph_concat_projector is None))
+
+    def _graph_attr(self, data, num_graphs, like):
+        """``data.graph_attr`` as [num_graphs, G] with ``like``'s device and dtype; the reference's checks and messages."""
+        ga = getattr(data, "graph_attr", None)
+        if ga is None:
+            raise ValueError("use_graph_attr_conditioning=True but data.graph_attr is missing.")
+        ga = ga.to(device=like.device, dtype=like.dtype)
+        if ga.dim() == 1:
+            if ga.numel() % num_graphs == 0:
+                return ga.view(num_graphs, ga.numel() // num_graphs)
+            raise ValueError(f"One-dimensional graph_attr with numel={ga.numel()} is not divisible by num_graphs={num_graphs}.")
+        if ga.dim() == 2:
+            if ga.size(0) != num_graphs:
+                raise ValueError(f"graph_attr first dim {ga.size(0)} does not match num_graphs={num_graphs}.")
+            return ga
+        raise ValueError(f"Unsupported graph_attr ndim={ga.dim()}; expected 1/2.")
+
+    def _conditioning(self, ga, gcsr, higher):
+        """The map h [N, H] -> conditioned h for this batch (None for fuse_pool); the per-graph terms are computed once."""
+        mode, hd = self.graph_attr_conditioning_mode, self.hidden_dim
+        gather = ops.GatherRows.apply
+        if mode == "film":
+            self._ensure_graph_conditioner(ga.shape[1], ga.device)
+            st = run_mlp(self.graph_conditioner, ga, higher)                              # [B, 2H] = [s | t]
+            if higher:
+                scale = 1 + torch.tanh(gather(st[:, :hd].contiguous(), gcsr))
+                shift = gather(st[:, hd:].contiguous(), gcsr)
+                return lambda h: h * scale + shift
+            return lambda h: ops.FilmFn.apply(h, st, gcsr)
+        if mode == "concat_node":
+            self._ensure_graph_concat_projector(graph_attr_dim=ga.shape[1], channel_dim=hd, device=ga.device, dtype=ga.dtype)
+            proj = self.graph_concat_projector
+            w_h, w_g = proj.weight[:, :hd], proj.weight[:, hd:]
+            if higher:
+                c = gather(ops.linear_any_order(ga, w_g, proj.bias), gcsr)
+                return lambda h: ops.linear_any_order(h, w_h) + c
+            c = ops.linear_act(ga, w_g.contiguous(), proj.bias)                           # [B, H] = graph_attr W_g^T + b
+            return lambda h: ops.GraphAddLinearFn.apply(h, w_h, c, gcsr)
+        return None
 
     def _init_conv(self):
         """Decoders and convolutions interleaved, in the order MACEStack._init_conv creates them (:190-275)."""
@@ -422,6 +518,13 @@ class MACEStack(Base):
     def _forward(self, data, higher):
         """MACEStack.forward (:375-421): a readout before the convolutions and after each, outputs summed."""
         assert data.pos is not None, "MACE requires node positions (data.pos) to be set."
+        ga = None
+        if self.use_graph_attr_conditioning:      # checked before any kernel; the graph count is kept for graph_index
+            num_graphs = cached(data, "_num_graphs")
+            if num_graphs is None:
+                num_graphs = 1 if data.batch is None else int(data.batch.max()) + 1
+                remember(data, "_num_graphs", num_graphs)
+            ga = self._graph_attr(data, num_graphs, data.pos)
         plan = self.plan_for(data)
         batch, num_graphs, gcsr = self.graph_index(data)
         pos, n = data.pos, data.pos.shape[0]
@@ -450,14 +553,19 @@ class MACEStack(Base):
         emb = self.node_embedding.linear
         table = emb.weight.reshape(NUM_ELEMENTS, self.hidden_dim) * emb.alpha[0]      # one-hot @ W == row gather
         xs = [ops.GatherRows.apply(table, zcsr)[:, None, :]]
+        cond = None if ga is None else self._conditioning(ga, gcsr, higher)
+        if cond is not None:
+            xs = [cond(xs[0].reshape(n, -1))[:, None, :]]
         ds = getattr(data, "dataset_name", None)
         onehot = torch.nn.functional.one_hot(z, NUM_ELEMENTS).to(pos.dtype)
         outputs = self.multihead_decoders[0](onehot, self.pool(onehot, gcsr, higher), batch, num_graphs, ds, higher)
-        for conv, readout in zip(self.graph_convs, self.multihead_decoders[1:]):
+        for i, (conv, readout) in enumerate(zip(self.graph_convs, self.multihead_decoders[1:])):
             xs = conv(xs, sh, radial, plan, zcsr, higher, eattr)
             scalars = xs[0][:, 0, :]
             out = readout(scalars, self.pool(scalars, gcsr, higher), batch, num_graphs, ds, higher)
             outputs = [a + b for a, b in zip(outputs, out)]
+            if cond is not None and i + 1 < len(self.graph_convs):     # the readout above saw the unconditioned scalars
+                xs = [cond(xs[0].reshape(n, -1))[:, None, :]] + xs[1:]
         return outputs
 
     def _edge_attr(self, data, num_edges):

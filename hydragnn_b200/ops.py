@@ -2302,6 +2302,87 @@ class MaceEdgeEmbedFn(torch.autograd.Function):
         return _edge_vec_scatter(gvec, plan), None, None, None, None, None, None
 
 
+# =====================================================================================================
+# graph-attribute conditioning (hydragnn/models/Base.py _apply_graph_conditioning): rows sorted by graph, gcsr = graph offsets
+# =====================================================================================================
+def raw_tc_linear_graph_add(h2, w, c, gcsr):
+    """y = h2 w^T + c[graph(row)] on the tensor-core kernel (the caller checked ``graph_add_tc_ok``)."""
+    m, k = h2.shape
+    n = w.shape[0]
+    y = torch.empty(m, n, dtype=h2.dtype, device=h2.device)
+    _lib.call("hgb_tc_linear_graph_add", _p(h2), h2.stride(0), _p(w), w.stride(0), m, n, k, _p(c), c.stride(0), _p(gcsr.rowptr), gcsr.n,
+              _p(y), 0 if _TC["enabled"] else 1, _stream())
+    return y
+
+
+def graph_add_tc_ok(h2, w, c):
+    return tc_ok(h2.shape[0], w.shape[0], h2.shape[1], h2, c) and c.stride(1) == 1
+
+
+class GraphAddLinearFn(torch.autograd.Function):
+    """``h W_h^T + c[graph]``: concat_node's Linear(H + G, H) on [h | graph_attr[batch]] with the graph-attribute columns and the
+    bias folded into the per-graph term c = graph_attr W_g^T + b [num_graphs, H].  Forward: one tensor-core pass whose epilogue
+    adds each row's graph row of c.  Backward: dh (tensor-core dgrad), dW_h (weight-gradient kernel) and dc = graph_sum(dy);
+    the parameter parts are skipped under ``only_data_grads``."""
+
+    @staticmethod
+    def forward(ctx, h, w, c, gcsr):
+        h2 = _chk(h)
+        w2 = w if w.stride(1) == 1 else w.contiguous()
+        c2 = _chk(c)
+        if graph_add_tc_ok(h2, w2, c2):
+            y = raw_tc_linear_graph_add(h2, w2, c2, gcsr)
+        else:     # shapes the tensor-core kernel does not take: the same sum from the Linear and gather kernels
+            y = linear_fwd_dispatch(h2, w2, None)[0] + raw_gather(c2, gcsr.idx)
+        ctx.save_for_backward(h2, w2)
+        ctx.gcsr, ctx.tc = gcsr, _TC["enabled"]
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        h2, w2 = ctx.saved_tensors
+        gy = _chk(gy)
+        params = not _DATA_ONLY["on"]
+        need_w = ctx.needs_input_grad[1] and params
+        with tensor_cores(ctx.tc):
+            gh, gw, _ = linear_bwd_dispatch(gy, h2, w2, ctx.needs_input_grad[0], need_w, False)
+        gc = raw_segment_sum(gy, ctx.gcsr.rowptr, None, ctx.gcsr.n) if (ctx.needs_input_grad[2] and params) else None
+        return gh, gw, gc, None
+
+
+class FilmFn(torch.autograd.Function):
+    """FiLM ``h * (1 + tanh s)[graph] + t[graph]`` with st = [s | t] [num_graphs, 2H] (hgb_film_fwd / hgb_film_bwd): dh in the
+    backward pass, plus the per-graph [ds | dt] as fixed-order segmented sums unless ``only_data_grads``."""
+
+    @staticmethod
+    def forward(ctx, h, st, gcsr):
+        h, st = _chk(h), _chk(st)
+        n, c = h.shape
+        y = torch.empty_like(h)
+        _lib.call("hgb_film_fwd", _p(h), n, c, _p(st), st.stride(0), _p(gcsr.rowptr), gcsr.n, _p(y), _stream())
+        ctx.save_for_backward(h, st)
+        ctx.gcsr = gcsr
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        h, st = ctx.saved_tensors
+        gy = _chk(gy)
+        n, c = h.shape
+        gh = torch.empty_like(h) if ctx.needs_input_grad[0] else None
+        gst = None
+        ws, nbytes = None, 0
+        if ctx.needs_input_grad[1] and not _DATA_ONLY["on"]:
+            gst = torch.empty(ctx.gcsr.n, 2 * c, dtype=h.dtype, device=h.device)
+            nbytes = _lib.query("hgb_film_bwd_workspace_bytes", n, c)
+            ws = _ws(nbytes, h.device)
+        _lib.call("hgb_film_bwd", _p(gy), _p(h), n, c, _p(st), st.stride(0), _p(ctx.gcsr.rowptr), ctx.gcsr.n, _p(gh), _p(gst), _p(ws),
+                  nbytes, _stream())
+        return gh, gst, None
+
+
 def adamw_step(p, g, m, v, step_dev, lr, beta1, beta2, eps, weight_decay, grad_scale=1.0, hyper_dev=None):
     _lib.call("hgb_adamw_step", _p(p), _p(g), _p(m), _p(v), p.numel(), float(lr), float(beta1), float(beta2), float(eps),
               float(weight_decay), float(grad_scale), _p(step_dev), _p(hyper_dev), _stream())

@@ -88,6 +88,10 @@ class PaddedGraphStep:
         self._widths = {k: (tuple(v.shape[1:]), v.dtype) for k, v in first_batch.items()
                         if torch.is_tensor(v) and (k in ("x", "pos", "y", "energy", "forces", "edge_shifts")
                                                    or k == "edge_attr" and reads_edge_attr)}
+        if getattr(inner, "use_graph_attr_conditioning", False):
+            # carried as [graphs, G] (1-D per-graph attributes reshaped), zero rows for the filler graphs
+            ga = first_batch.graph_attr
+            self._widths["graph_attr"] = ((ga.numel() // g,), ga.dtype)
         self._capture(node_cap or n, edge_cap or e, graph_cap or g)
         self.recaptures = 0
 
@@ -105,7 +109,7 @@ class PaddedGraphStep:
         hosts = [{}, {}]                                   # two pinned staging sets: the host fills one while the other's copy is in flight
         for key, (tail, dt) in self._widths.items():
             rows = {"x": self.n_cap, "pos": self.n_cap, "forces": self.n_cap, "y": self.g_cap, "energy": self.g_cap,
-                    "edge_shifts": self.e_cap, "edge_attr": self.e_cap}[key]
+                    "edge_shifts": self.e_cap, "edge_attr": self.e_cap, "graph_attr": self.g_cap}[key]
             if key == "edge_shifts" and self.nb:
                 continue
             for h in hosts:
@@ -216,6 +220,8 @@ class PaddedGraphStep:
                 continue
             src = batch[key].to("cpu")
             buf = h[key]
+            if key == "graph_attr":
+                src = src.reshape(g, -1)
             rows = src.shape[0]
             buf[:rows] = src.reshape((rows,) + tuple(buf.shape[1:]))
             if key == "pos":

@@ -51,6 +51,9 @@ WORKLOADS = {
     "mp_cgcnn": dict(sizes=list(range(8, 65)), rho=0.06, species=list(range(1, 84)), radius=8.0, max_neighbours=12, pbc_box=True),
     "mp_cgcnn_gps": dict(sizes=list(range(8, 65)), rho=0.06, species=list(range(1, 84)), radius=8.0, max_neighbours=12,
                          pbc_box=True, pe_dim=6),
+    # examples/multidataset_hpo_sc26/gfm_mlip.json: MACE force training conditioned on graph attributes (concat_node), periodic
+    # cells of 60 to 100 atoms of any species, r = 5 A, k = 20; graph_attr (two per graph) is attached by the caller
+    "gfm_mace": dict(sizes=list(range(60, 101)), rho=0.05, species=list(range(1, 84)), radius=5.0, max_neighbours=20, pbc_box=True),
 }
 
 ARCH = {
@@ -135,6 +138,14 @@ ARCH["ci_schnet"] = dict(mpnn_type="SchNet", input_dim=1, hidden_dim=64, num_con
                                                  "dim_headlayers": [10, 10]}},
                          activation_function="relu", loss_function_type="mse", graph_pooling="mean")
 ARCH["oc20_mace_80"] = ARCH["oc20_mace"]
+ARCH["gfm_mace"] = dict(mpnn_type="MACE", input_dim=1, hidden_dim=128, num_conv_layers=4, num_radial=6, radius=5.0, max_neighbours=20,
+                        max_ell=1, node_max_ell=1, envelope_exponent=5, radial_type="bessel", avg_num_neighbors=13.735293601560318,
+                        edge_dim=1, output_dim=[1], output_type=["graph"], task_weights=[1.0],
+                        output_heads={"graph": {"num_sharedlayers": 2, "dim_sharedlayers": 50, "num_headlayers": 3,
+                                                "dim_headlayers": [128, 128, 128]}},
+                        activation_function="relu", loss_function_type="mae", graph_pooling="add",
+                        enable_interatomic_potential=True, energy_weight=0.0, energy_peratom_weight=1.0, force_weight=10.0,
+                        use_graph_attr_conditioning=True, graph_attr_conditioning_mode="concat_node")
 ARCH["gfm_pnaeq_mini"] = dict(ARCH["gfm_pnaeq"], output_dim=[1], output_type=["graph"], task_weights=[1.0], loss_function_type="mse",
                               output_heads={"graph": ARCH["gfm_pnaeq"]["output_heads"]["graph"]})
 # CGCNN (CGCNNStack.py): the edge length as the one edge feature, and input_dim = hidden_dim = 1 as update_config makes them

@@ -73,6 +73,10 @@ class FlatAdamW(torch.optim.Optimizer):
     ``param_groups[0]["lr"]`` changed -- a CUDA-graph-captured step therefore follows a scheduler."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2):
+        if isinstance(model, torch.nn.Module) and any(getattr(m, "graph_attr_modules_missing", lambda: False)() for m in model.modules()):
+            # the buffer holds the parameters that exist now: a conditioning module created later would never be trained
+            raise ValueError("FlatAdamW: this model's graph-attribute conditioning modules are created at its first forward; run "
+                             "one forward (or load the checkpoint) before building the optimizer")
         params = [p for p in (model.parameters() if isinstance(model, torch.nn.Module) else model) if p.requires_grad]
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.params = params

@@ -53,7 +53,7 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 
 /* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd);
  * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient;
- * 109: hgb_nbr_* (SAGEConv / MFConv) */
+ * 109: hgb_nbr_* (SAGEConv / MFConv); 110: hgb_tc_linear_graph_add, hgb_film_* (graph-attribute conditioning) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -235,6 +235,14 @@ int hgb_tc_linear_supported(int32_t m, int32_t n_out, int32_t k_red);
 int hgb_tc_linear(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t trans_b, const float* bias,
                   int32_t m, int32_t n_out, int32_t k_red, int32_t act, float act_param, float* y, float* z,
                   const float* addend, const float* gsrc, int32_t gact, int32_t exact, hgb_stream_t stream);
+/* y[m,n_out] = a[m,k_red] . w^T + gadd[graph(r)] for every row r, graph(r) = the g with gptr[g] <= r < gptr[g + 1]
+ * (rows sorted by graph, gptr [ng + 1]; empty graphs allowed), gadd [ng, n_out] with row stride ldg (multiple of 4, 16-byte
+ * aligned).  The mainloop of hgb_tc_linear (same shapes, same exact flag); the epilogue adds the graph's row.  This is
+ * Linear(H + G, H) on [h | graph_attr[batch]] with the per-graph term gadd = graph_attr . W_g^T + b computed once per graph,
+ * so neither the [m, H + G] concatenation nor a gathered [m, H] addend is materialised.                               */
+int hgb_tc_linear_graph_add(const float* a, int64_t lda, const float* w, int64_t ldw, int32_t m, int32_t n_out, int32_t k_red,
+                            const float* gadd, int64_t ldg, const int32_t* gptr, int32_t ng, float* y, int32_t exact,
+                            hgb_stream_t stream);
 /* dw[n_out,k_out] (row stride lddw) (+)= dz[m,n_out]^T . x[m,k_out] and db[n_out] (+)= column sums of dz
  * (db may be NULL) in one pass: row slabs of both operands arrive by TMA and are transposed to K-major in shared
  * memory, the bias gradient rides along as extra all-ones rows of the B operand.  Deterministic two-stage reduce.
@@ -710,6 +718,20 @@ int hgb_nbr_linear_fwd(const float* x, int32_t n, int32_t k, const int32_t* rowp
 int hgb_nbr_linear_bwd_data(const float* g_out, int32_t n, int32_t n_out, const int32_t* rowptr, int32_t mean,
                             const int32_t* order, const int32_t* grp_ptr, const int32_t* tiles, int32_t groups, const float* wt,
                             int32_t k, float* g_h, float* g_xr, int32_t exact, hgb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * FiLM conditioning (hgb_cond.cu; hydragnn/models/Base.py _apply_graph_conditioning, mode "film") over rows sorted by
+ * graph (gptr [ng + 1], empty graphs allowed).  st [ng, >= 2c] (row stride ldst) holds [s | t] per graph.
+ *   hgb_film_fwd: y[r] = h[r] * (1 + tanh s[g]) + t[g]      (h, y [n, c])
+ *   hgb_film_bwd: dh[r] = dy[r] * (1 + tanh s[g]) (dh may be NULL); dst [ng, 2c] (NULL: skipped) = [ds | dt] with
+ *                 ds[g] = (1 - tanh^2 s[g]) sum_{r in g} dy[r] h[r], dt[g] = sum_{r in g} dy[r], fixed-order segmented sums
+ *                 (bit-identical across runs); ws of hgb_film_bwd_workspace_bytes(n, c) bytes when dst is given.
+ * ------------------------------------------------------------------------------------------ */
+int hgb_film_fwd(const float* h, int32_t n, int32_t c, const float* st, int64_t ldst, const int32_t* gptr, int32_t ng, float* y,
+                 hgb_stream_t stream);
+int64_t hgb_film_bwd_workspace_bytes(int32_t n, int32_t c);
+int hgb_film_bwd(const float* dy, const float* h, int32_t n, int32_t c, const float* st, int64_t ldst, const int32_t* gptr,
+                 int32_t ng, float* dh, float* dst, void* ws, int64_t ws_bytes, hgb_stream_t stream);
 
 #ifdef __cplusplus
 }
