@@ -16,9 +16,9 @@
 //                       the other and every barrier is waited on phase by phase by the one warpgroup that consumes it.
 //   tc_wgrad_kernel   : dW[NO,KO] (+ db[NO]) = dZ[M,NO]^T . X[M,KO], reduction over M split across CTAs, per-CTA partials +
 //                       deterministic final reduce.  TF32 wgmma wants both operands K-major (M contiguous), the tensors are
-//                       row-major: the TMA lands row slabs and the consumer warpgroups transpose them into a K-major buffer
-//                       (splitting into TF32 hi / lo in fp32-accurate mode) while the previous buffer is on the tensor cores.
-//                       The bias gradient rides along as 16 extra "ones" rows of the B operand.
+//                       row-major: warp-specialised, one warp's TMA lands row slabs, seven transposer warps turn them into a ring
+//                       of K-major buffers (splitting into TF32 hi / lo in fp32-accurate mode), and the two MMA warpgroups only
+//                       issue wgmma on them.  The bias gradient rides along as 16 extra "ones" rows of the B operand.
 #include "hgb_tc.cuh"
 
 namespace {
@@ -403,7 +403,7 @@ struct WgParams {
   int m, no, ko;
   int chunks_per_cta;   // number of 32-row chunks each CTA reduces
   int stages;           // TMA ring of raw row slabs
-  int tbufs;            // K-major (transposed) operand buffers: 2 = transposition of chunk c+1 overlaps the MMAs of chunk c
+  int tbufs;            // ring of K-major (transposed) operand buffers between the transposer warps and the MMA warpgroups
   int split;            // 1: fp32-accurate mode -- both operands are split into TF32 hi / lo twins and every k-step runs lo*hi + hi*lo + hi*hi
   int flush;            // > 0: the register accumulators are added into the partial every `flush` chunks and restarted, so each chain
                         //   of tensor-core additions stays short (the fp32-accurate mode)
@@ -411,9 +411,17 @@ struct WgParams {
 };
 
 constexpr int WG_ROWS = 32;                      // rows of dZ / X per chunk = one 128-byte K-major row of the transposed operands
-constexpr int WG_NA = 128;                       // rows of dW per CTA (two consumer warpgroups x 64)
-constexpr int WG_THREADS = 384;                  // 2 consumer warpgroups + 1 producer warpgroup (one warp issues the TMA)
+constexpr int WG_NA = 128;                       // rows of dW per CTA (two MMA warpgroups x 64)
+constexpr int WG_TRANSPOSERS = 7;                // with three, the transposition bounded the n_out = 128 and 192 calls
+constexpr int WG_THREADS = 256 + 32 * (1 + WG_TRANSPOSERS);   // 2 MMA warpgroups + one TMA warp and WG_TRANSPOSERS transposer warps
+constexpr int WG_AUX_REGS = 40, WG_MMA_REGS = 216;   // 256 x 40 + 256 x 216 = 64 K registers
 
+// Warp-specialised pipeline, one chunk (32 rows of dZ and X) per step:
+//   warp 8           TMA: raw row slabs into a ring of `stages` buffers (full / empty mbarriers)
+//   warps 9..15      transpose each raw stage into the next K-major operand buffer of a ring of `tbufs` (tfull / tempty), splitting
+//                    into TF32 hi / lo in fp32-accurate mode, and release the raw stage
+//   warpgroups 0, 1  wait on tfull, issue the chunk's MMAs, and release the buffer once wgmma_wait shows they have read it
+// The arithmetic is fixed by the chunk partition and the MMA sequence of each chunk, not by how the data gets there.
 template <int Q, bool SPLIT>    // KO = 32 * Q; SPLIT: the fp32-accurate mode
 __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_dz,
                                                                  const __grid_constant__ CUtensorMap tmap_x, const WgParams p) {
@@ -425,6 +433,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
   const int n0 = blockIdx.y * WG_NA;
   const int nrows = min(WG_NA, p.no - n0);
   const int nsl = nrows >> 5;
+  const int n_mma_wg = (nrows + 63) >> 6;                 // warpgroups with dW rows in this CTA
   const uint32_t raw_bytes = (uint32_t)(nsl + Q) * SLAB;
   const uint32_t tb_bytes = HI_BYTES * (SPLIT ? 2 : 1);
   const int S = p.stages, T = p.tbufs;
@@ -432,6 +441,8 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
   uint8_t* raw = smem + (size_t)T * tb_bytes;             // S x [nsl dZ slabs | Q X slabs], row-major as loaded
   uint64_t* full = reinterpret_cast<uint64_t*>(raw + (size_t)S * raw_bytes);
   uint64_t* empty = full + S;
+  uint64_t* tfull = empty + S;
+  uint64_t* tempty = tfull + T;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   const int total_chunks = (p.m + WG_ROWS - 1) / WG_ROWS;
@@ -439,111 +450,125 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
   const int nchunks = max(0, min(total_chunks, c_beg + p.chunks_per_cta) - c_beg);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, 8); }
+    for (int s = 0; s < S; ++s) { mbar_init(full + s, 1); mbar_init(empty + s, WG_TRANSPOSERS); }
+    for (int t = 0; t < T; ++t) { mbar_init(tfull + t, WG_TRANSPOSERS); mbar_init(tempty + t, 4 * n_mma_wg); }
     fence_barrier_init();
   }
-  // transposed buffers: A rows >= nrows stay zero, B rows KO.. are the ones rows (lo twins: zero); everything else is rewritten per chunk
-  for (int i = threadIdx.x; i < (int)(T * tb_bytes / 4); i += blockDim.x) {
-    const uint32_t o = (uint32_t)i * 4 % tb_bytes;
-    const bool lo = o >= HI_BYTES;
-    const int row = (int)((lo ? o - HI_BYTES : o) / 128);
-    reinterpret_cast<float*>(tbuf)[i] = (!lo && row >= WG_NA + KO) ? 1.f : 0.f;
+  // rows of the operand buffers that no chunk writes, set once: A rows nrows..127 zero, B rows KO.. the ones rows (lo twins zero)
+  {
+    const int zrows = WG_NA - nrows, frows = zrows + 16;
+    const int words = T * (SPLIT ? 2 : 1) * frows * 32;
+    for (int i = threadIdx.x; i < words; i += blockDim.x) {
+      const int rr = (i >> 5) % frows, half = (i >> 5) / frows;   // half: buffer * (SPLIT ? 2 : 1) + (lo twin)
+      const int row = rr < zrows ? nrows + rr : WG_NA + KO + (rr - zrows);
+      const bool lo = SPLIT && (half & 1);
+      const int t = SPLIT ? half >> 1 : half;
+      reinterpret_cast<float*>(tbuf + (size_t)t * tb_bytes + (lo ? HI_BYTES : 0) + (size_t)row * 128)[i & 31] =
+          (!lo && rr >= zrows) ? 1.f : 0.f;
+    }
   }
   fence_proxy_async();
   __syncthreads();
 
   if (warp >= 8) {
-    // ===== TMA producer: this CTA's dZ columns n0.. and all of X, 32 rows per chunk =====
-    regs_dec<PRODUCER_REGS>();
-    if (warp == 8 && lane == 0) {
-      for (int c = 0; c < nchunks; ++c) {
-        const int s = c % S;
-        mbar_wait(empty + s, ((c / S) & 1) ^ 1);
-        mbar_expect_tx(full + s, raw_bytes);
-        uint8_t* st = raw + (size_t)s * raw_bytes;
-        const int row0 = (c_beg + c) * WG_ROWS;
-        for (int j = 0; j < nsl; ++j) tma_load_2d(st + (size_t)j * SLAB, &tmap_dz, full + s, n0 + j * 32, row0);
-        for (int j = 0; j < Q; ++j) tma_load_2d(st + (size_t)(nsl + j) * SLAB, &tmap_x, full + s, j * 32, row0);
+    regs_dec<WG_AUX_REGS>();
+    if (warp == 8) {
+      // ===== TMA producer: this CTA's dZ columns n0.. and all of X, 32 rows per chunk =====
+      if (lane == 0) {
+        for (int c = 0; c < nchunks; ++c) {
+          const int s = c % S;
+          mbar_wait(empty + s, ((c / S) & 1) ^ 1);
+          mbar_expect_tx(full + s, raw_bytes);
+          uint8_t* st = raw + (size_t)s * raw_bytes;
+          const int row0 = (c_beg + c) * WG_ROWS;
+          for (int j = 0; j < nsl; ++j) tma_load_2d(st + (size_t)j * SLAB, &tmap_dz, full + s, n0 + j * 32, row0);
+          for (int j = 0; j < Q; ++j) tma_load_2d(st + (size_t)(nsl + j) * SLAB, &tmap_x, full + s, j * 32, row0);
+        }
+      }
+      return;
+    }
+    // ===== transposers: operand row r (A: dZ column n0 + r; B: X column r - nrows) gets the 32 values of this chunk as one K-major
+    // 128-byte row.  A unit is 32 consecutive rows (one per lane) x 4 consecutive m: four conflict-free column reads per lane and
+    // one swizzled 16-byte store.  =====
+    const int tw = warp - 9;
+    const int units = (nsl + Q) * 8;
+    for (int c = 0; c < nchunks; ++c) {
+      const int s = c % S, t = c % T;
+      uint8_t* tb = tbuf + (size_t)t * tb_bytes;
+      const uint8_t* st = raw + (size_t)s * raw_bytes;
+      mbar_wait(full + s, (c / S) & 1);
+      mbar_wait(tempty + t, ((c / T) & 1) ^ 1);
+#pragma unroll 4
+      for (int u = tw; u < units; u += WG_TRANSPOSERS) {
+        const int slab = u >> 3, m4 = u & 7;
+        const float* src = reinterpret_cast<const float*>(st + (size_t)slab * SLAB) + lane + m4 * 4 * 32;
+        const float4 v = make_float4(src[0], src[32], src[64], src[96]);
+        const int orow = slab < nsl ? slab * 32 + lane : WG_NA + (slab - nsl) * 32 + lane;
+        const uint32_t off = (uint32_t)orow * 128 + ((m4 ^ (orow & 7)) << 4);
+        if (SPLIT) {
+          float4 h, l;
+          split_f4(v, h, l);
+          *reinterpret_cast<float4*>(tb + off) = h;
+          *reinterpret_cast<float4*>(tb + HI_BYTES + off) = l;
+        } else {
+          *reinterpret_cast<float4*>(tb + off) = v;
+        }
+      }
+      fence_proxy_async();
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(empty + s);                           // the raw slabs are no longer needed
+        mbar_arrive(tfull + t);                           // this warp's share of the K-major chunk is written
       }
     }
     return;
   }
 
-  // ===== consumer warpgroups (threads 0..255): transpose, then wgmma; warpgroup wg owns dW rows n0 + 64 wg .. +63 =====
-  regs_inc<CONSUMER_REGS>();
+  // ===== MMA warpgroups (threads 0..255): warpgroup wg owns dW rows n0 + 64 wg .. +63 =====
+  regs_inc<WG_MMA_REGS>();
   const int wg = warp >> 2, wq = warp & 3;
-  const bool mma_on = wg * 64 < nrows;
-  const int rows_t = nsl * 32 + KO;                       // operand rows to transpose per chunk
+  if (wg >= n_mma_wg) return;
   float acc[Q][16], accb[8];
-#pragma unroll
-  for (int c = 0; c < Q; ++c)
-#pragma unroll
-    for (int j = 0; j < 16; ++j) acc[c][j] = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) accb[j] = 0.f;
-  bool first = true;
   float* part = p.part + (size_t)blockIdx.x * p.no * (p.ko + 1);
 
-  auto flush = [&]() {   // partial (+)= accumulators; accumulators restart at zero
-    if (mma_on) {
-      const int rb = n0 + wg * 64 + wq * 16 + (lane >> 2);
+  auto store = [&](bool first) {   // partial (first: =, then +=) accumulators
+    const int rb = n0 + wg * 64 + wq * 16 + (lane >> 2);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = rb + 8 * h;
-        if (row < n0 + nrows) {
-          float* pr = part + (size_t)row * (KO + 1);
+    for (int h = 0; h < 2; ++h) {
+      const int row = rb + 8 * h;
+      if (row < n0 + nrows) {
+        float* pr = part + (size_t)row * (KO + 1);
 #pragma unroll
-          for (int c = 0; c < Q; ++c)
+        for (int c = 0; c < Q; ++c)
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
+          for (int i = 0; i < 4; ++i)
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int col = c * 32 + i * 8 + 2 * (lane & 3) + e;
-                const float v = acc[c][4 * i + 2 * h + e];
-                pr[col] = first ? v : pr[col] + v;
-              }
-          if ((lane & 3) == 0) pr[KO] = first ? accb[2 * h] : pr[KO] + accb[2 * h];   // ones column KO: the bias gradient
-        }
+            for (int e = 0; e < 2; ++e) {
+              const int col = c * 32 + i * 8 + 2 * (lane & 3) + e;
+              const float v = acc[c][4 * i + 2 * h + e];
+              pr[col] = first ? v : pr[col] + v;
+            }
+        if ((lane & 3) == 0) pr[KO] = first ? accb[2 * h] : pr[KO] + accb[2 * h];   // ones column KO: the bias gradient
       }
     }
-    first = false;
-#pragma unroll
-    for (int c = 0; c < Q; ++c)
-#pragma unroll
-      for (int j = 0; j < 16; ++j) acc[c][j] = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) accb[j] = 0.f;
   };
 
-  for (int c = 0; c < nchunks; ++c) {
-    const int s = c % S;
-    uint8_t* tb = tbuf + (size_t)(c % T) * tb_bytes;
-    const uint8_t* st = raw + (size_t)s * raw_bytes;
-    mbar_wait(full + s, (c / S) & 1);
-    // transpose: operand row r (A: dZ column n0 + r; B: X column r - nrows) gets the 32 values of this chunk as one K-major 128-byte
-    // row; each item is 4 consecutive m of one row (four conflict-free column reads, one swizzled 16-byte store)
-    for (int it = threadIdx.x; it < rows_t * 8; it += 256) {
-      const int r = it % rows_t, m4 = it / rows_t;
-      const int slab = r < nrows ? r >> 5 : nsl + ((r - nrows) >> 5);
-      const float* src = reinterpret_cast<const float*>(st + (size_t)slab * SLAB) + (r & 31) + m4 * 4 * 32;
-      const float4 v = make_float4(src[0], src[32], src[64], src[96]);
-      const int orow = r < nrows ? r : WG_NA + (r - nrows);
-      const uint32_t off = (uint32_t)orow * 128 + ((m4 ^ (orow & 7)) << 4);
-      if (SPLIT) {
-        float4 h, l;
-        split_f4(v, h, l);
-        *reinterpret_cast<float4*>(tb + off) = h;
-        *reinterpret_cast<float4*>(tb + HI_BYTES + off) = l;
-      } else {
-        *reinterpret_cast<float4*>(tb + off) = v;
-      }
-    }
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(empty + s);               // the raw slabs are no longer needed
-    named_bar_sync(1, 256);                              // the transposed chunk is complete
-    if (mma_on) {
-      const uint32_t ta = smem_u32(tb);
+  // fold groups: the accumulators start at zero, take `flush` chunks (all of them when flush = 0) and are added into the partial.
+  // They are zeroed only here, with no MMA in flight: ptxas serialises every wgmma of a loop in which a non-wgmma instruction may write
+  // an accumulator while a group is pending.  A CTA without chunks writes zeros.
+  int c = 0;
+  for (bool first = true;; first = false) {
+#pragma unroll
+    for (int q = 0; q < Q; ++q)
+#pragma unroll
+      for (int j = 0; j < 16; ++j) acc[q][j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) accb[j] = 0.f;
+    const int c_end = p.flush ? min(nchunks, c + p.flush) : nchunks;
+    for (; c < c_end; ++c) {
+      const int t = c % T;
+      const uint32_t ta = smem_u32(tbuf + (size_t)t * tb_bytes);
+      mbar_wait(tfull + t, (c / T) & 1);
       fence_regs<Q * 16>(&acc[0][0]);
       fence_regs<8>(accb);
       wgmma_fence();
@@ -568,21 +593,22 @@ __global__ void __launch_bounds__(WG_THREADS, 1) tc_wgrad_kernel(const __grid_co
       wgmma_commit();
       fence_regs<Q * 16>(&acc[0][0]);
       fence_regs<8>(accb);
+      // release the buffer whose MMAs are known to be complete: the previous chunk's (one group may stay in flight), or with a
+      // single buffer this chunk's
+      if (T >= 2) {
+        wgmma_wait<1>();
+        if (c > 0 && lane == 0) mbar_arrive(tempty + (c - 1) % T);
+      } else {
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(tempty + t);
+      }
     }
-    // the buffer transposed next must no longer be read by either warpgroup's MMAs
-    if (T == 2) wgmma_wait<1>(); else wgmma_wait<0>();
-    if (p.flush && (c + 1) % p.flush == 0 && c + 1 < nchunks) {
-      wgmma_wait<0>();
-      fence_regs<Q * 16>(&acc[0][0]);
-      fence_regs<8>(accb);
-      flush();
-    }
-    named_bar_sync(2, 256);
+    wgmma_wait<0>();
+    fence_regs<Q * 16>(&acc[0][0]);
+    fence_regs<8>(accb);
+    store(first);
+    if (c >= nchunks) break;
   }
-  wgmma_wait<0>();
-  fence_regs<Q * 16>(&acc[0][0]);
-  fence_regs<8>(accb);
-  flush();                                                // (a CTA without chunks writes zeros)
 }
 
 // 32 outputs x 8 partial-walkers per block; fixed summation order
@@ -786,14 +812,13 @@ extern "C" int hgb_tc_wgrad(const float* dz, int64_t lddz, const float* x, int64
   const int nsl_max = (n_out < WG_NA ? n_out : WG_NA) / 32;
   const size_t raw_bytes = (size_t)(nsl_max + Q) * WG_ROWS * 128;
   const size_t tb_bytes = (size_t)(WG_NA + k_out + 16) * 128 * (exact ? 2 : 1);
-  const size_t budget = SMEM_MAX - 1024 - 256;
-  int tbufs = 2;
-  int stages = budget > 2 * tb_bytes ? (int)((budget - 2 * tb_bytes) / raw_bytes) : 0;
-  if (stages < 2) {
-    tbufs = 1;
-    stages = (int)((budget - tb_bytes) / raw_bytes);
-  }
-  if (stages > 4) stages = 4;
+  // shared memory: up to three K-major buffers (each transposed chunk then waits on no MMA still reading the buffer it reuses), as
+  // long as two raw stages fit beside them; every byte left over deepens the TMA ring.  Each buffer and stage has two mbarriers.
+  const size_t budget = SMEM_MAX - 1024;
+  int tbufs = 3;
+  while (tbufs > 1 && (size_t)tbufs * (tb_bytes + 16) + 2 * (raw_bytes + 16) > budget) --tbufs;
+  const size_t left = budget > (size_t)tbufs * (tb_bytes + 16) ? budget - (size_t)tbufs * (tb_bytes + 16) : 0;
+  const int stages = (int)(left / (raw_bytes + 16));
   HGB_REQUIRE(stages >= 2, "tc_wgrad: stage does not fit shared memory");
   p.stages = stages;
   p.tbufs = tbufs;
@@ -809,7 +834,7 @@ extern "C" int hgb_tc_wgrad(const float* dz, int64_t lddz, const float* x, int64
   p.chunks_per_cta = (total_chunks + gx - 1) / gx;
   gx = (total_chunks + p.chunks_per_cta - 1) / p.chunks_per_cta;
   p.part = (float*)workspace;
-  const size_t smem = 1024 + tbufs * tb_bytes + stages * raw_bytes + 2 * stages * 8;
+  const size_t smem = 1024 + tbufs * (tb_bytes + 16) + stages * (raw_bytes + 16);
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(gx, gy);
   switch (Q) {
