@@ -10,8 +10,8 @@ CGConv's two Linears act on z_e = [x_i | x_j | a_e] (i = edge_index[1] the targe
 with W_f = [A_f | B_f | C_f] (and W_s alike) one per-node Linear gives [P_f | P_s | Q_f | Q_s] = x [A_f; A_s; B_f; B_s]^T, and
 ``ops.CgConvFn`` forms f_e = P_f[i] + Q_f[j] + C_f a_e + b_f and s_e in registers, gates them and sums
 sigmoid(f_e) * softplus(s_e) onto the residual x_i.  Under GPS the conv's edge input is linear in the raw r_e = [edge_attr |
-rel_pe] (or rel_pe alone), so the kernel takes Mt = ((C_f; C_s) L)^T with L built from the bias-free embedding weights, as
-``schnet.SCFStack._embedding`` folds it, and the [E, hidden] edge embedding is never formed.  Higher-order passes and shapes
+rel_pe] (or rel_pe alone), so the kernel takes Mt = ((C_f; C_s) L)^T with L built from the bias-free embedding weights
+(``Base._raw_edge_input``), and the [E, hidden] edge embedding is never formed.  Higher-order passes and shapes
 ``ops.cgconv_supported`` refuses run the same math composed from GatherRows, Linear, ATen sigmoid / softplus and SegmentSum.
 """
 import torch
@@ -20,8 +20,8 @@ from torch import nn
 
 from . import ops
 from .ops import GatherRows, SegmentSum
-from .pna import PNAStack
-from .stacks import Base
+from .gps import PyGBatchNorm
+from .stacks import Base, SingleConv
 
 
 class CGConv(nn.Module):
@@ -67,33 +67,22 @@ class CGConv(nn.Module):
         return SegmentSum.apply(m, tgt) + x
 
 
-class CGCNNSequential(nn.Module):
-    """The PyG ``Sequential`` of CGCNNStack.get_conv (:60-80): the conv is ``module_0``, the lambda step that passes
-    ``equiv_node_feat`` through has no parameters."""
-
-    def __init__(self, conv):
-        super().__init__()
-        self.module_0 = conv
-
-    def forward(self, inv_node_feat, equiv_node_feat, plan, edge_raw=None, higher_order=False, **kwargs):
-        return self.module_0(inv_node_feat, plan, edge_raw, higher_order), equiv_node_feat
-
-
 class CGCNNStack(Base):
+    is_edge_model = True
+
     def __init__(self, edge_dim, *args, **kwargs):
         self.edge_dim = edge_dim
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
 
-    # Base._init_conv (Base.py:446-463): one conv per layer, each followed by BatchNorm(hidden_dim), GPS-wrapped when on
-    _init_conv = PNAStack._init_conv
+    def _feature_layer(self, width):
+        return PyGBatchNorm(width)
 
     def get_conv(self, input_dim, output_dim=None, last_layer=False, edge_dim=None):
         # CGConv keeps its width: the reference passes input_dim as the channels and ignores output_dim
         if edge_dim is None:
             raise ValueError("CGCNN needs an integer edge_dim without global attention (update_config sets 0 when there are no "
                              "edge features); PyG's CGConv fails computing sum(channels) + None")
-        return CGCNNSequential(CGConv(input_dim, edge_dim))
+        return SingleConv(CGConv(input_dim, edge_dim))
 
     def _init_node_conv(self):
         """CGCNNStack._init_node_conv (:84-110), statement for statement: conv-type node heads are not built.  It raises the
@@ -126,22 +115,8 @@ class CGCNNStack(Base):
         return super()._forward(data, higher)
 
     def _embedding(self, data, plan, higher):
-        if not self.use_global_attn:
-            r = data.edge_attr if self.use_edge_attr else None
-            return data.x, data.pos, {"edge_raw": None if r is None else (r, None)}
-        # Base.py:477-491 with the edge embedding folded into the conv (see module doc)
-        lin = (lambda w, t: ops.linear_any_order(t, w, None)) if higher else (lambda w, t: ops.linear_act(t, w, None))
-        x = lin(self.pos_emb.weight, data.pe)
-        if self.input_dim:
-            x = lin(self.node_lin.weight, torch.cat((lin(self.node_emb.weight, data.x.float()), x), 1))
-        h = self.hidden_dim
-        emb, r = self.rel_pos_emb.weight, data.rel_pe
-        if self.use_edge_attr:
-            le = self.edge_lin.weight
-            emb = torch.cat([ops.MatMul.apply(le[:, :h], self.edge_emb.weight, False, False),
-                             ops.MatMul.apply(le[:, h:], self.rel_pos_emb.weight, False, False)], dim=1)
-            r = torch.cat([data.edge_attr, data.rel_pe], dim=1)
-        return x, data.pos, {"edge_raw": (r, emb)}
+        x, edge_raw = self._raw_edge_input(data, higher)
+        return x, data.pos, {"edge_raw": edge_raw}
 
     def __str__(self):
         return "CGCNNStack"

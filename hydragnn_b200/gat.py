@@ -11,7 +11,7 @@ order of construction are the reference's, so reference checkpoints load strictl
 j -> i, z = x_r[i] + x_l[j] + lin_edge(a), the scores, the softmax over the in-edges of i and its self-loop, the attention
 dropout and the weighted sum in one pass over the by-target CSR.  Under GPS the conv's edge input is linear in the raw
 r_e = [edge_attr | rel_pe] (or rel_pe alone), so the kernel takes mt = (W_edge L)^T with L built from the bias-free embedding
-weights, as ``cgcnn.CGCNNStack._embedding`` folds it, and the [E, hidden] edge embedding is never formed.  Higher-order passes
+weights (``Base._raw_edge_input``), and the [E, hidden] edge embedding is never formed.  Higher-order passes
 and shapes ``ops.gat_supported`` refuses run the same math composed from GatherRows, SegmentSum, Linear and ATen elementwise
 ops, with the dropout mask of ``hgb_gat_dropout_keep`` under the same seed.
 """
@@ -22,7 +22,6 @@ import torch.nn.functional as F
 from torch import nn
 
 from . import _lib, ops
-from .cgcnn import CGCNNStack
 from .gps import PyGBatchNorm
 from .ops import GatherRows, SegmentSum
 from .stacks import Base
@@ -168,20 +167,14 @@ class GATSequential(nn.Module):
 
 
 class GATStack(Base):
+    is_edge_model = True
+
     def __init__(self, heads, negative_slope, edge_dim, *args, **kwargs):
         # self.heads is GATv2Conv's number of attention heads, not the number of output heads
         self.heads = heads
         self.negative_slope = negative_slope
         self.edge_dim = edge_dim
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
-
-    def _wrap(self, conv):
-        if not self.use_global_attn:
-            return conv
-        from .gps import GPSConv
-        return GPSConv(self.hidden_dim, conv, heads=self.global_attn_heads, dropout=self.global_attn_dropout,
-                       attn_type=self.global_attn_type)
 
     def _init_conv(self):
         """GATStack._init_conv (:39-111): concat convs with head-multiplied widths, a head-averaging last conv."""
@@ -240,8 +233,9 @@ class GATStack(Base):
             raise AssertionError("GAT conv-type node heads have no edge input (edge_dim=None) but the model uses edge features")
         return super()._forward(data, higher)
 
-    # the GPS embedding with the conv's edge embedding folded in, and the raw edge input without GPS, are CGCNN's
-    _embedding = CGCNNStack._embedding
+    def _embedding(self, data, plan, higher):
+        x, edge_raw = self._raw_edge_input(data, higher)
+        return x, data.pos, {"edge_raw": edge_raw}
 
     def __str__(self):
         return "GATStack"

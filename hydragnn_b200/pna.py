@@ -20,7 +20,7 @@ from . import ops
 from .gps import PyGBatchNorm
 from .ops import GatherRows
 from .pnaeq import DegreeScalerAggregation, post_linear_scaled
-from .stacks import Base, run_mlp
+from .stacks import Base, SingleConv, run_mlp
 
 AGGREGATORS = ["mean", "min", "max", "std"]
 SCALERS = ["identity", "amplification", "attenuation", "linear"]          # PNAStack.py:30-36: no inverse_linear
@@ -85,39 +85,20 @@ class PNAConv(nn.Module):
         return (ops.linear_any_order if higher_order else ops.linear_act)(out, self.lin.weight, self.lin.bias)
 
 
-class PNASequential(nn.Module):
-    """The PyG ``Sequential`` of PNAStack.get_conv (PNAStack.py:55-67): the conv is ``module_0``, the lambda step that passes
-    ``equiv_node_feat`` through has no parameters."""
-
-    def __init__(self, conv):
-        super().__init__()
-        self.module_0 = conv
-
-    def forward(self, inv_node_feat, equiv_node_feat, plan, edge_attr=None, higher_order=False, **kwargs):
-        return self.module_0(inv_node_feat, plan, edge_attr, higher_order), equiv_node_feat
-
-
 class PNAStack(Base):
+    is_edge_model = True
+
     def __init__(self, deg, edge_dim, *args, **kwargs):
         self.aggregators, self.scalers = list(AGGREGATORS), list(SCALERS)
         self.deg = torch.Tensor(deg)                   # PNAStack.py:37: taken as given (PNAEq sanitises, PNA does not)
         self.edge_dim = edge_dim
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
 
     def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
-        return PNASequential(PNAConv(input_dim, output_dim, self.aggregators, self.scalers, self.deg, edge_dim=edge_dim))
+        return SingleConv(PNAConv(input_dim, output_dim, self.aggregators, self.scalers, self.deg, edge_dim=edge_dim))
 
-    def _init_conv(self):
-        """Base._init_conv (Base.py:446-463): one conv per layer, each followed by BatchNorm(hidden_dim)."""
-        for i in range(self.num_conv_layers):
-            conv = self.get_conv(self.embed_dim if i == 0 else self.hidden_dim, self.hidden_dim, edge_dim=self.edge_embed_dim)
-            if self.use_global_attn:
-                from .gps import GPSConv
-                conv = GPSConv(self.hidden_dim, conv, heads=self.global_attn_heads, dropout=self.global_attn_dropout,
-                               attn_type=self.global_attn_type)
-            self.graph_convs.append(conv)
-            self.feature_layers.append(PyGBatchNorm(self.hidden_dim))
+    def _feature_layer(self, width):
+        return PyGBatchNorm(width)
 
     def _embedding(self, data, plan, higher):
         eattr = data.edge_attr if self.use_edge_attr else None

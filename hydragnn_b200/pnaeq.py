@@ -4,10 +4,11 @@ Host-side mirror of ``hydragnn/models/PNAEqStack.py`` (class names ``PainnMessag
 ``PNAEqStack`` and attribute names ``aggr_module``, ``F_in``, ``F_out``, ``towers``, ``pre_nns``, ``post_nns`` are
 kept: the reference's equivariance test monkey-patches them, tests/test_forces_equivariant.py:48-78).
 
-Round-1 implementation: gathers, segmented sums / arg-min-max and every Linear run in libhgb kernels; the
-elementwise algebra of the 4 x 5 PNA aggregation is ATen glue (a single-pass fused PNA kernel is the next step,
-SURVEY K5).  All ops used here are any-order differentiable except the fused Linears, which are swapped for the
-closed MatMul primitive in ``higher_order`` mode.
+Gathers, segment sums and every Linear run in libhgb kernels.  First-order passes reduce the scalar messages into
+[mean | min | max | std] in one ``ops.PnaAggregateFn`` pass and fold the five degree scalers into the post Linear
+(``post_linear_scaled``), so the 20 F-wide aggregate is never built; the update block is ``ops.PainnUpdateFn``.
+Higher-order passes (MLIP training) run the same math composed from the closed primitives and
+``DegreeScalerAggregation``, with the Linears on the any-order MatMul.
 """
 import math
 
@@ -16,7 +17,7 @@ from torch import nn
 
 from . import _lib, ops
 from .ops import GatherRows, SegmentSum, _p, _stream
-from .stacks import Base, PainnConv, run_mlp
+from .stacks import Base, PainnConv, edge_geometry, run_mlp
 
 X_AGGREGATORS = ["mean", "min", "max", "std"]
 X_SCALERS = ["identity", "amplification", "attenuation", "linear", "inverse_linear"]
@@ -92,22 +93,8 @@ class DegreeScalerAggregation(nn.Module):
             else:
                 raise ValueError("unsupported aggregator " + str(a))
         out = torch.cat(outs, dim=-1)
-        deg = cnt.clamp(min=1)[:, None]
-        res = []
-        for s in self.scaler:
-            if s == "identity":
-                res.append(out)
-            elif s == "amplification":
-                res.append(out * (torch.log(deg + 1) / self.avg_deg_log))
-            elif s == "attenuation":
-                res.append(out * (self.avg_deg_log / torch.log(deg + 1)))
-            elif s == "linear":
-                res.append(out * (deg / self.avg_deg_lin))
-            elif s == "inverse_linear":
-                res.append(out * (self.avg_deg_lin / deg))
-            else:
-                raise ValueError("unsupported scaler " + str(s))
-        return torch.cat(res, dim=-1)
+        f = self.scaler_factors(csr)
+        return torch.cat([out if s == "identity" else out * f[:, k, None] for k, s in enumerate(self.scaler)], dim=-1)
 
 
 def post_linear_scaled(post, x, agg4, aggr_module, csr):
@@ -203,11 +190,12 @@ def rbf_basis(dist, num_radial, cutoff):
 
 
 class PNAEqStack(Base):
+    is_edge_model = True
+
     def __init__(self, deg, edge_dim, num_radial, radius, *args, **kwargs):
         self.x_aggregators, self.x_scalers = list(X_AGGREGATORS), list(X_SCALERS)
         self.deg = sanitize_degree(deg)
         self.edge_dim, self.num_radial, self.radius = edge_dim, num_radial, radius
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
 
     def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
@@ -222,17 +210,9 @@ class PNAEqStack(Base):
 
     def _embedding(self, data, plan, higher):
         assert data.pos is not None, "PNAEq requires node positions (data.pos) to be set."
-        x, pos, shifts = data.x, data.pos, data.edge_shifts
-        if higher:
-            vec = GatherRows.apply(pos, plan.by_col) - GatherRows.apply(pos, plan.by_row)
-            if shifts is not None:
-                vec = vec + shifts
-            ln = torch.linalg.norm(vec, dim=-1, keepdim=True)
-            unit = vec / (ln + 1e-9)
-        else:
-            _, ln, unit = ops.EdgeGeomFn.apply(pos, shifts, plan, 1e-9)          # PNAEqStack.py:202-204
+        ln, unit = edge_geometry(data.pos, data.edge_shifts, plan, 1e-9, higher)        # PNAEqStack.py:202-204
         geom = {"rbf": rbf_basis(ln.squeeze(-1), self.num_radial, self.radius), "unit": unit}
-        eattr = data.edge_attr if self.use_edge_attr else None
+        x, eattr = data.x, (data.edge_attr if self.use_edge_attr else None)
         if self.use_global_attn:
             x, eattr = self._gps_embed(data, higher)
         v = torch.zeros(x.shape[0], 3, x.shape[1], dtype=x.dtype, device=x.device)

@@ -2,7 +2,7 @@
 
 Host-side mirror of ``hydragnn/models/PNAPlusStack.py``: its own ``PNAConv`` (PyG 2.6.1 PNAConv with a Bessel-gated message;
 towers = pre_layers = post_layers = 1, ``act="relu"``) and PyG 2.6.1 ``BesselBasisLayer`` / ``Envelope``.  Every conv is
-followed by a PyG BatchNorm feature layer (``PNAStack._init_conv``).  Module and parameter names are the reference's
+followed by a PyG BatchNorm feature layer (``PNAStack._feature_layer``).  Module and parameter names are the reference's
 (``graph_convs.<i>.module_0.{aggr_module, pre_nns.0.0, post_nns.0.0, lin, rbf_lin, rbf_emb.0, edge_encoder}``,
 ``feature_layers.<i>.module``, ``rbf.freq`` last), so reference checkpoints load.
 
@@ -23,7 +23,7 @@ from . import ops
 from .ops import GatherRows
 from .pna import AGGREGATORS, SCALERS, PNAStack
 from .pnaeq import DegreeScalerAggregation, post_linear_scaled
-from .stacks import run_mlp
+from .stacks import SingleConv, run_mlp
 
 # Above this width the fused kernel's per-edge F x F product is not measured to beat the composed path (DESIGN.md, a6d).
 FUSED_MAX_F = 64
@@ -141,18 +141,6 @@ class PNAConv(nn.Module):
         return (ops.linear_any_order if higher_order else ops.linear_act)(out, self.lin.weight, self.lin.bias)
 
 
-class PNAPlusSequential(nn.Module):
-    """The PyG ``Sequential`` of PNAPlusStack.get_conv (:77-91): the conv is ``module_0``, the lambda step that passes
-    ``equiv_node_feat`` through has no parameters."""
-
-    def __init__(self, conv):
-        super().__init__()
-        self.module_0 = conv
-
-    def forward(self, inv_node_feat, equiv_node_feat, plan, bessel=None, edge_attr=None, higher_order=False, **kwargs):
-        return self.module_0(inv_node_feat, plan, bessel, edge_attr, higher_order), equiv_node_feat
-
-
 class PNAPlusStack(PNAStack):
     def __init__(self, deg, edge_dim, envelope_exponent, num_radial, radius, *args, **kwargs):
         self.envelope_exponent, self.num_radial, self.radius = envelope_exponent, num_radial, radius
@@ -160,9 +148,9 @@ class PNAPlusStack(PNAStack):
         self.rbf = BesselBasisLayer(self.num_radial, self.radius, self.envelope_exponent)
 
     def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
-        # the reference's get_conv takes no last_layer; Base passes it only to stacks whose get_conv has one
-        return PNAPlusSequential(PNAConv(input_dim, output_dim, self.aggregators, self.scalers, self.deg, edge_dim=edge_dim,
-                                         num_radial=self.num_radial))
+        # the reference's get_conv takes no last_layer; Base._init_conv passes it and it is ignored here
+        return SingleConv(PNAConv(input_dim, output_dim, self.aggregators, self.scalers, self.deg, edge_dim=edge_dim,
+                                  num_radial=self.num_radial))
 
     def _forward(self, data, higher):
         if self.use_edge_attr and any(isinstance(m, nn.ModuleList) for h in self.heads_NN for m in h.values()):

@@ -17,8 +17,8 @@ import torch
 from torch import nn
 
 from . import ops
-from .pna import PNAStack
-from .stacks import DEGREE_PLAN, Base, cached, remember
+from .gps import PyGBatchNorm
+from .stacks import DEGREE_PLAN, Base, SingleConv, cached, remember
 
 
 def _nbr_layer(x, plan, dp, wl, bl, wr, mean, higher_order):
@@ -75,29 +75,12 @@ class MFConv(nn.Module):
         return _nbr_layer(x, plan, degree_plan, wl, bl, wr, False, higher_order)
 
 
-class NbrSequential(nn.Module):
-    """The PyG ``Sequential`` of SAGEStack.get_conv / MFCStack.get_conv: the conv is ``module_0``, the lambda step that passes
-    ``equiv_node_feat`` through has no parameters."""
+class NbrStack(Base):
+    """What SAGE and MFC share: no edge input, a BatchNorm after every conv, and the conv arguments of ``_embedding``."""
+    is_edge_model = False
 
-    def __init__(self, conv):
-        super().__init__()
-        self.module_0 = conv
-
-    def forward(self, inv_node_feat, equiv_node_feat, plan, degree_plan=None, higher_order=False, **kwargs):
-        return self.module_0(inv_node_feat, plan, degree_plan, higher_order), equiv_node_feat
-
-
-class SAGEStack(Base):
-    weight_groups = 1
-
-    def __init__(self, *args, **kwargs):
-        self.is_edge_model = False
-        super().__init__(*args, **kwargs)
-
-    _init_conv = PNAStack._init_conv
-
-    def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
-        return NbrSequential(SAGEConv(input_dim, output_dim))
+    def _feature_layer(self, width):
+        return PyGBatchNorm(width)
 
     def _embedding(self, data, plan, higher):
         """The input features (the GPS node embedding under global attention) and the in-degree grouping of the batch, built
@@ -108,22 +91,25 @@ class SAGEStack(Base):
             hit = remember(data, DEGREE_PLAN, (plan, ops.degree_plan(plan, self.weight_groups)))
         return x, data.pos, {"degree_plan": hit[1]}
 
+
+class SAGEStack(NbrStack):
+    weight_groups = 1
+
+    def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
+        return SingleConv(SAGEConv(input_dim, output_dim))
+
     def __str__(self):
         return "SAGEStack"
 
 
-class MFCStack(Base):
+class MFCStack(NbrStack):
     def __init__(self, max_degree, *args, **kwargs):
         self.max_degree = max_degree
         self.weight_groups = max_degree + 1
-        self.is_edge_model = False
         super().__init__(*args, **kwargs)
 
-    _init_conv = PNAStack._init_conv
-    _embedding = SAGEStack._embedding
-
     def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
-        return NbrSequential(MFConv(input_dim, output_dim, max_degree=self.max_degree))
+        return SingleConv(MFConv(input_dim, output_dim, max_degree=self.max_degree))
 
     def __str__(self):
         return "MFCStack"

@@ -24,7 +24,7 @@ from torch import nn
 
 from . import ops, radius
 from .ops import GatherRows, SegmentSum
-from .stacks import Base, run_mlp
+from .stacks import Base, edge_geometry, run_mlp
 
 
 FUSED_MAX_FILTERS = 64
@@ -124,11 +124,7 @@ class CFConv(nn.Module):
             w = run_mlp(self.nn, inp, higher_order) * c.view(-1, 1)
             agg = SegmentSum.apply(GatherRows.apply(xl, plan.by_row) * w, plan.by_col)     # message x_j * W, aggr "add" at i
         if self.equivariant:                                                                 # coord_model (:252-260)
-            if higher_order:
-                vec = GatherRows.apply(pos, plan.by_col) - GatherRows.apply(pos, plan.by_row)
-                coord_diff = vec / (torch.linalg.norm(vec, dim=-1, keepdim=True) + 1.0)
-            else:
-                _, _, coord_diff = ops.EdgeGeomFn.apply(pos, None, plan, 1.0)
+            _, coord_diff = edge_geometry(pos, None, plan, 1.0, higher_order)
             trans = torch.clamp(coord_diff * run_mlp(self.coord_mlp, w, higher_order), min=-100, max=100)
             cnt = (plan.by_row.rowptr[1:] - plan.by_row.rowptr[:-1]).clamp(min=1).to(trans.dtype)
             pos = pos + SegmentSum.apply(trans, plan.by_row) / cnt[:, None]                  # mean over the source index
@@ -162,10 +158,11 @@ class CFConvGraphSequential(nn.Module):
 
 
 class SCFStack(Base):
+    is_edge_model = True
+
     def __init__(self, num_filters, edge_dim, num_gaussians, radius, *args, max_neighbours=None, **kwargs):
         self.radius, self.max_neighbours = radius, max_neighbours
         self.num_filters, self.edge_dim, self.num_gaussians = num_filters, edge_dim, num_gaussians
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
 
     @property
@@ -200,23 +197,8 @@ class SCFStack(Base):
                 raise ValueError("SchNet builds its radius graph in every layer and needs max_neighbours (got None)")
             gptr, g = radius._graph_ptr(data, data.pos.shape[0], data.pos.device)
             return data.x, data.pos, {"graph_ptr": gptr, "num_graphs": g, "cache": {}}
-        x = data.x
-        r = data.edge_attr if self.use_edge_attr else None
-        emb = None
-        if self.use_global_attn:                                  # SCFStack.py:199-214, the edge embedding folded (see module doc)
-            lin = (lambda w, t: ops.linear_any_order(t, w, None)) if higher else (lambda w, t: ops.linear_act(t, w, None))
-            x = lin(self.pos_emb.weight, data.pe)
-            if self.input_dim:
-                x = lin(self.node_lin.weight, torch.cat((lin(self.node_emb.weight, data.x.float()), x), 1))
-            h = self.hidden_dim
-            emb = self.rel_pos_emb.weight
-            r = data.rel_pe
-            if self.use_edge_attr:
-                le = self.edge_lin.weight
-                emb = torch.cat([ops.MatMul.apply(le[:, :h], self.edge_emb.weight, False, False),
-                                 ops.MatMul.apply(le[:, h:], self.rel_pos_emb.weight, False, False)], dim=1)
-                r = torch.cat([data.edge_attr, data.rel_pe], dim=1)
-        return x, data.pos, {"smearing": self.distance_expansion, "edge_raw": (r, emb) if r is not None else None}
+        x, edge_raw = self._raw_edge_input(data, higher)          # SCFStack.py:199-214, the edge embedding folded (see module doc)
+        return x, data.pos, {"smearing": self.distance_expansion, "edge_raw": edge_raw}
 
     def __str__(self):
         return "SCFStack"

@@ -200,6 +200,19 @@ def run_mlp(seq, x, higher_order=False):
     return x
 
 
+def edge_geometry(pos, shifts, plan, eps, higher_order=False):
+    """(length [E, 1], unit [E, 3]) of every edge: vec = pos[col] - pos[row] (+ ``shifts``), unit = vec / (length + eps).  One
+    ``ops.EdgeGeomFn`` pass, or in any-order mode the same math composed from GatherRows and ATen."""
+    if not higher_order:
+        _, length, unit = ops.EdgeGeomFn.apply(pos, shifts, plan, eps)
+        return length, unit
+    vec = GatherRows.apply(pos, plan.by_col) - GatherRows.apply(pos, plan.by_row)
+    if shifts is not None:
+        vec = vec + shifts
+    length = torch.linalg.norm(vec, dim=-1, keepdim=True)
+    return length, vec / (length + eps)
+
+
 # ------------------------------------------------------------------------------------------------
 # EGNN  (hydragnn/models/EGCLStack.py:180-300)
 # ------------------------------------------------------------------------------------------------
@@ -246,14 +259,7 @@ class E_GCL(nn.Module):
         if self._fused_ok(x, edge_attr):
             return self._forward_fused(x, coord, plan, edge_shifts, higher_order, cache)
         # geometry with eps = 1.0 (quirk Q3, EGCLStack.py:280-282); "radial" is the length
-        if higher_order:
-            vec = GatherRows.apply(coord, plan.by_col) - GatherRows.apply(coord, plan.by_row)
-            if edge_shifts is not None:
-                vec = vec + edge_shifts
-            radial = torch.linalg.norm(vec, dim=-1, keepdim=True)
-            coord_diff = vec / (radial + 1.0)
-        else:
-            _, radial, coord_diff = ops.EdgeGeomFn.apply(coord, edge_shifts, plan, 1.0)
+        radial, coord_diff = edge_geometry(coord, edge_shifts, plan, 1.0, higher_order)
         # edge_mlp (:245-250).  Its first Linear acts on [x_row | x_col | radial | edge_attr]; it is linear in the blocks,
         # so the two node blocks are multiplied per NODE (N rows instead of E) and gathered per edge afterwards.
         lin0, fin = self.edge_mlp[0], x.shape[1]
@@ -409,6 +415,22 @@ class PainnConv(nn.Module):
         return s, ops.linear_act(v_new, lin.weight, lin.bias)
 
 
+class SingleConv(nn.Module):
+    """The PyG ``Sequential`` a stack's get_conv builds around one conv: the conv is ``module_0``, the lambda step that passes
+    ``equiv_node_feat`` through has no parameters.  The conv takes the stack's conv arguments by name.  Used by
+    * PNA (PNAStack.get_conv, PNAStack.py:55-67),
+    * PNAPlus (PNAPlusStack.get_conv, :77-91),
+    * CGCNN (CGCNNStack.get_conv, :60-80),
+    * SAGE and MFC (SAGEStack.get_conv, MFCStack.get_conv)."""
+
+    def __init__(self, conv):
+        super().__init__()
+        self.module_0 = conv
+
+    def forward(self, inv_node_feat, equiv_node_feat, plan, higher_order=False, **conv_args):
+        return self.module_0(inv_node_feat, plan, higher_order=higher_order, **conv_args), equiv_node_feat
+
+
 class MLPNode(nn.Module):
     """Node-level MLP head (hydragnn/models/Base.py:912-979): one shared MLP (``node_type == 'mlp'``) or one MLP per node
     position (``'mlp_per_node'``: graphs of exactly ``num_nodes`` atoms, node i of every graph goes through ``mlp[i]``)."""
@@ -548,12 +570,20 @@ class Base(nn.Module):
         for i in range(self.num_conv_layers):
             last = i == self.num_conv_layers - 1
             conv = self.get_conv(self.embed_dim if i == 0 else self.hidden_dim, self.hidden_dim, last, edge_dim=self.edge_embed_dim)
-            if self.use_global_attn:                                           # Base._apply_global_attn :234-247
-                from .gps import GPSConv
-                conv = GPSConv(self.hidden_dim, conv, heads=self.global_attn_heads, dropout=self.global_attn_dropout,
-                               attn_type=self.global_attn_type)
-            self.graph_convs.append(conv)
-            self.feature_layers.append(nn.Identity())
+            self.graph_convs.append(self._wrap(conv))
+            self.feature_layers.append(self._feature_layer(self.hidden_dim))
+
+    def _wrap(self, conv):
+        """``conv`` inside a GPS layer when global attention is on (Base._apply_global_attn :234-247), else itself."""
+        if not self.use_global_attn:
+            return conv
+        from .gps import GPSConv
+        return GPSConv(self.hidden_dim, conv, heads=self.global_attn_heads, dropout=self.global_attn_dropout,
+                       attn_type=self.global_attn_type)
+
+    def _feature_layer(self, width):
+        """What follows every encoder conv: Identity here, a BatchNorm in the reference's default Base._init_conv (:446-463)."""
+        return nn.Identity()
 
     def _multihead(self):                                                  # Base.py:590-691
         act = self.activation_function
@@ -667,6 +697,27 @@ class Base(nn.Module):
             if self.use_edge_attr:
                 e = lin(self.edge_lin, torch.cat((lin(self.edge_emb, data.edge_attr), e), 1))
         return x, e
+
+    def _raw_edge_input(self, data, higher):
+        """(x, edge_raw) for a conv that takes its edge input raw: ``edge_raw`` = (r, L), the conv's edge input being r L^T (L
+        None: r itself), or None without one.  Under GPS (Base.py:477-491) the edge embedding is linear in r = [edge_attr |
+        rel_pe] (or rel_pe alone), so L is built from the bias-free embedding weights and the conv folds it into its own
+        weights: the [E, hidden] edge embedding is never formed."""
+        if not self.use_global_attn:
+            r = data.edge_attr if self.use_edge_attr else None
+            return data.x, None if r is None else (r, None)
+        lin = (lambda w, t: ops.linear_any_order(t, w, None)) if higher else (lambda w, t: ops.linear_act(t, w, None))
+        x = lin(self.pos_emb.weight, data.pe)
+        if self.input_dim:
+            x = lin(self.node_lin.weight, torch.cat((lin(self.node_emb.weight, data.x.float()), x), 1))
+        h = self.hidden_dim
+        emb, r = self.rel_pos_emb.weight, data.rel_pe
+        if self.use_edge_attr:
+            le = self.edge_lin.weight
+            emb = torch.cat([ops.MatMul.apply(le[:, :h], self.edge_emb.weight, False, False),
+                             ops.MatMul.apply(le[:, h:], self.rel_pos_emb.weight, False, False)], dim=1)
+            r = torch.cat([data.edge_attr, data.rel_pe], dim=1)
+        return x, (r, emb)
 
     def _higher_order(self, data):
         pos = data.pos
@@ -792,9 +843,10 @@ class Base(nn.Module):
 
 
 class EGCLStack(Base):
+    is_edge_model = True
+
     def __init__(self, edge_attr_dim, *args, max_neighbours=None, **kwargs):
         self.edge_dim = 0 if edge_attr_dim is None else edge_attr_dim       # EGCLStack.py:33-35
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
 
     def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
@@ -813,9 +865,10 @@ class EGCLStack(Base):
 
 
 class PAINNStack(Base):
+    is_edge_model = True
+
     def __init__(self, edge_dim, num_radial, radius, *args, **kwargs):
         self.edge_dim, self.num_radial, self.radius = edge_dim, num_radial, radius
-        self.is_edge_model = True
         super().__init__(*args, **kwargs)
 
     def get_conv(self, input_dim, output_dim, last_layer=False, edge_dim=None):
@@ -830,17 +883,12 @@ class PAINNStack(Base):
 
     def _embedding(self, data, plan, higher):
         assert data.pos is not None, "PAINN requires node positions (data.pos) to be set."
-        x, pos, shifts = data.x, data.pos, data.edge_shifts
+        ln, unit = edge_geometry(data.pos, data.edge_shifts, plan, 1e-9, higher)       # PAINNStack.py:157-159
         if higher:
-            vec = GatherRows.apply(pos, plan.by_col) - GatherRows.apply(pos, plan.by_row)
-            if shifts is not None:
-                vec = vec + shifts
-            ln = torch.linalg.norm(vec, dim=-1, keepdim=True)
-            geom = {"unit": vec / (ln + 1e-9), "len": ln}
+            geom = {"unit": unit, "len": ln}
         else:
-            _, ln, unit = ops.EdgeGeomFn.apply(pos, shifts, plan, 1e-9)      # PAINNStack.py:157-159
             geom = {"epack": ops.PainnEdgeEmbedFn.apply(unit, ln, self.num_radial, self.radius)}
-        eattr = data.edge_attr if self.use_edge_attr else None
+        x, eattr = data.x, (data.edge_attr if self.use_edge_attr else None)
         if self.use_global_attn:
             x, eattr = self._gps_embed(data, higher)
         v = torch.zeros(x.shape[0], 3, x.shape[1], dtype=x.dtype, device=x.device)   # PAINNStack.py:190
