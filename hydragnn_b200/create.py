@@ -163,6 +163,9 @@ class EnhancedModelWrapper(nn.Module):
     F = -dE/dpos (hydragnn/models/create.py:590-738)."""
 
     def __init__(self, original_model, energy_weight, energy_peratom_weight, force_weight):
+        if getattr(original_model, "var_output", 0):
+            # the reference's energy_force_loss reads pred[0] as the energy tensor, which a (outputs, outputs_var) pair is not
+            raise ValueError("b200 engine: interatomic potentials have no mean-and-variance heads; GaussianNLLLoss is not supported")
         super().__init__()
         self.model = original_model
         self.energy_weight, self.energy_peratom_weight, self.force_weight = energy_weight, energy_peratom_weight, force_weight

@@ -201,6 +201,10 @@ class GATStack(Base):
             return
         if self.use_global_attn or len(cfgs) > 1:
             raise ValueError("b200 engine: conv-type node heads are implemented for one branch and without global attention")
+        if self.var_output:
+            # GATStack._init_node_conv keeps the output convs at head_dim, so the reference's variance is [N, 0] and its
+            # GaussianNLLLoss raises
+            raise ValueError("b200 engine: GAT conv-type node heads have no variance outputs; GaussianNLLLoss is not supported")
         k = self.heads
         for br in cfgs:
             a = br["architecture"]

@@ -352,6 +352,9 @@ class MACEStack(Base):
             raise ValueError("b200 engine: MACE distance transforms need ase covalent radii and are not implemented")
         if max_ell > 3:
             raise ValueError("b200 engine: MACE max_ell <= 3")
+        if kwargs.get("loss_function_type") == "GaussianNLLLoss":
+            # the reference's MACE decoders keep their width and Base.loss then unpacks the output list as (pred, var)
+            raise ValueError("b200 engine: MACE has no mean-and-variance heads; GaussianNLLLoss is not supported")
         # ---- prior to inheritance (:111-150): Base.__init__ calls _init_conv, which reads these
         num_conv_layers = kwargs["num_conv_layers"]
         self.edge_dim = int(edge_dim or 0)

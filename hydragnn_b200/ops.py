@@ -1225,6 +1225,46 @@ class LossFn(torch.autograd.Function):
         return gpred * g, None, None, None, None
 
 
+GNLL_EPS = 1e-6          # torch.nn.GaussianNLLLoss's default, the one the reference's loss_function_selection builds
+
+
+class GaussianNLLFn(torch.autograd.Function):
+    """``torch.nn.GaussianNLLLoss()(mean, target, var)`` (full=False, eps=1e-6, mean) with the gradients with respect to mean and
+    var produced in the same pass (``hgb_gnll_fwd_bwd``).  ``valid_rows`` / ``row_width``: mean over the real prefix rows of a
+    capacity-padded batch, as ``LossFn``."""
+
+    @staticmethod
+    def forward(ctx, mean, var, target, valid_rows=None, row_width=1):
+        mean, var, target = _chk(mean), _chk(var), _chk(target)
+        n = mean.numel()
+        if var.numel() != n or target.numel() != n:
+            raise ValueError("GaussianNLLFn: mean, var and target need the same number of elements (%d, %d, %d)"
+                             % (n, var.numel(), target.numel()))
+        loss = torch.empty(1, dtype=mean.dtype, device=mean.device)
+        gmean, gvar = torch.empty_like(mean), torch.empty_like(var)
+        ws = torch.empty(int(_lib.query("hgb_gnll_workspace_bytes", n)), dtype=torch.uint8, device=mean.device)
+        _lib.call("hgb_gnll_fwd_bwd", _p(mean), _p(var), _p(target), n, GNLL_EPS, _p(loss), _p(gmean), _p(gvar), _p(ws),
+                  _p(valid_rows), int(row_width), _stream())
+        ctx.save_for_backward(gmean, gvar)
+        return loss.reshape(())
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        gmean, gvar = ctx.saved_tensors
+        return gmean * g, gvar * g, None, None, None
+
+
+def gaussian_nll_any_order(mean, var, target, mask=None, count=None):
+    """The same loss composed from ATen, differentiable to any order, on any device: ``var`` clamped to ``GNLL_EPS`` in value
+    while its gradient passes through unchanged (torch clamps a copy under no_grad).  With ``mask`` (0/1 per element) the sum
+    of the masked terms is divided by ``count`` instead of taking the mean."""
+    vc = torch.where(var >= GNLL_EPS, var, var - var.detach() + GNLL_EPS)
+    d = mean - target
+    term = 0.5 * (torch.log(vc) + d * d / vc)
+    return term.mean() if mask is None else (term * mask).sum() / count
+
+
 class PnaAggregateFn(torch.autograd.Function):
     """[mean | min | max | std] of every CSR segment in one pass (the four PNA aggregators of PNAEqStack.py:396-400)."""
 

@@ -8,7 +8,8 @@ capacities (``node_cap``, ``edge_cap``, ``graph_cap``) and pads every batch up t
   are masked out of the loss, so they contribute exactly zero to every gradient (0 x finite);
 * the unused tail of the edge list receives dummy edges between consecutive filler atoms (``hgb_pad_edges``);
 * the real counts live on the device (``valid`` = [graphs, nodes, edges]); losses are means over the real prefix
-  (``hgb_loss_fwd_bwd`` with ``valid_rows``; masked ATen means on the any-order MLIP path).
+  (``hgb_loss_fwd_bwd``, or ``hgb_gnll_fwd_bwd`` for mean-and-variance heads, with ``valid_rows``; masked ATen means on the
+  any-order MLIP path).
 
 Nothing in the step reads a size back to the host: neighbour build (optional: edges may also come with the batch, as the
 reference builds them at preprocessing time), CSR plans, forward, loss, backward, flat all-reduce and fused AdamW replay as
@@ -136,12 +137,18 @@ class PaddedGraphStep:
     def _masked_loss(self, pred):
         m, d = self.m, self.data
         inner = getattr(m, "model", m)
+        var = None
+        if inner.var_output:                                 # mean-and-variance heads: the NLL over the real graphs only
+            pred, var = pred
         tot, tasks, off = 0, [], 0
         for ih in range(inner.num_heads):
             w = inner.head_dims[ih]
             tgt = d.y[:, off:off + w] if d.y.dim() == 2 else d.y.reshape(-1, 1)
             off += w
-            li = inner.loss_function.masked(pred[ih], tgt.contiguous(), self.valid[0:1], w)
+            if var is None:
+                li = inner.loss_function.masked(pred[ih], tgt.contiguous(), self.valid[0:1], w)
+            else:
+                li = inner.loss_function.masked(pred[ih], tgt.contiguous(), var[ih], self.valid[0:1], w)
             tot = tot + li * inner.loss_weights[ih]
             tasks.append(li)
         return tot, tasks

@@ -63,7 +63,9 @@ def loss_function_selection(name):
         return _Loss(1, False)
     if name == "rmse":
         return _Loss(0, True)
-    raise ValueError("loss_function_type %r is not supported by the b200 engine (mse / mae / rmse)" % (name,))
+    if name == "GaussianNLLLoss":
+        return _GaussianNLL()
+    raise ValueError("loss_function_type %r is not supported by the b200 engine (mse / mae / rmse / GaussianNLLLoss)" % (name,))
 
 
 class _Loss:
@@ -93,6 +95,25 @@ class _Loss:
         d = (pred - target.to(pred.dtype)) * mask
         val = ((d * d).sum() if self.mode == 0 else d.abs().sum()) / count
         return torch.sqrt(val) if self.sqrt else val
+
+
+class _GaussianNLL:
+    """``torch.nn.GaussianNLLLoss()(pred, target, var)``: the fused value + gradients kernel (``ops.GaussianNLLFn``) when only
+    first derivatives can be asked for, the ATen composition (``ops.gaussian_nll_any_order``) otherwise or off the GPU."""
+
+    def __call__(self, pred, target, var, any_order=False):
+        target = target.to(pred.dtype)
+        if any_order or not pred.is_cuda:
+            return ops.gaussian_nll_any_order(pred, var, target)
+        return ops.GaussianNLLFn.apply(pred.reshape(-1), var.reshape(-1), target.reshape(-1))
+
+    def masked(self, pred, target, var, valid_rows, row_width):
+        """Mean over the first ``valid_rows[0]`` rows only (capacity-padded batches, hydragnn_b200/padded.py)."""
+        return ops.GaussianNLLFn.apply(pred.reshape(-1), var.reshape(-1), target.to(pred.dtype).reshape(-1), valid_rows, row_width)
+
+    def masked_any_order(self, pred, target, var, mask, count):
+        """Any-order differentiable masked mean: ``mask`` is 0/1 per element, ``count`` the (device) number of real elements."""
+        return ops.gaussian_nll_any_order(pred, var, target.to(pred.dtype), mask, count)
 
 
 PAD_MLP_MIN_ROWS = 32768      # below this the chain is launch-bound and the extra pad / slice kernels cost more than the GEMMs save
@@ -476,20 +497,21 @@ def graph_head_mlp(arch, out_dim, act):
     return nn.Sequential(*layers)
 
 
-def decode_branches(kind, head, graph_shared, ids, x, x_graph, batch, hd, num_graphs, higher_order):
+def decode_branches(kind, head, graph_shared, ids, x, x_graph, batch, width, num_graphs, higher_order):
     """One head over several dataset branches (Base.py:770-780, 816-840): the graphs (or their atoms) of branch b go through
-    ``head["branch-b"]``, graph heads after ``graph_shared["branch-b"]`` when the decoder has shared layers."""
+    ``head["branch-b"]``, graph heads after ``graph_shared["branch-b"]`` when the decoder has shared layers.  ``width``: the
+    head's output width (twice its dimension for a mean-and-variance head)."""
     if kind == "graph":
-        out = x_graph.new_zeros(num_graphs, hd)
+        out = x_graph.new_zeros(num_graphs, width)
         for b in ids.unique():
             msk, key = ids == b, "branch-%d" % int(b)
             z = run_mlp(graph_shared[key], x_graph[msk], higher_order) if key in graph_shared else x_graph[msk]
-            out[msk] = run_mlp(head[key], z, higher_order)[:, :hd]
+            out[msk] = run_mlp(head[key], z, higher_order)[:, :width]
     else:
-        out = x.new_zeros(x.shape[0], hd)
+        out = x.new_zeros(x.shape[0], width)
         for b in ids.unique():
             msk = (ids == b)[batch]
-            out[msk] = head["branch-%d" % int(b)](x[msk], higher_order)[:, :hd]
+            out[msk] = head["branch-%d" % int(b)](x[msk], higher_order)[:, :width]
     return out
 
 
@@ -511,9 +533,7 @@ class Base(nn.Module):
         self.config_heads = config_heads
         self.equivariance = bool(equivariance)
         self.activation_function = activation_function_selection(activation_function_type)
-        self.var_output = 0
-        if loss_function_type == "GaussianNLLLoss":
-            raise ValueError("GaussianNLLLoss is not supported by the b200 engine")
+        self.var_output = 1 if loss_function_type == "GaussianNLLLoss" else 0    # Base.py:109-111: mean-and-variance heads
         self.loss_function_type = loss_function_type
         self.loss_function = loss_function_selection(loss_function_type)
         self.ilossweights_hyperp, self.ilossweights_nll = 1, 0
@@ -563,7 +583,7 @@ class Base(nn.Module):
             for head, kind in zip(self.heads_NN, self.head_type):
                 if kind == "graph":
                     for br in head.values():
-                        br[-1].bias.data.fill_(initial_bias)
+                        br[-1].bias.data.fill_(initial_bias)        # all 2 d entries of a mean-and-variance head
 
     # first layer at width input_dim (quirk Q4), last layer flagged (EGCLStack.py:45-70, PAINNStack.py:49-74)
     def _init_conv(self):
@@ -600,7 +620,7 @@ class Base(nn.Module):
             head = nn.ModuleDict()
             if self.head_type[ih] == "graph":
                 for br in self.config_heads["graph"]:
-                    head[br["type"]] = graph_head_mlp(br["architecture"], self.head_dims[ih], act)
+                    head[br["type"]] = graph_head_mlp(br["architecture"], self.head_dims[ih] * (1 + self.var_output), act)
             elif self.head_type[ih] == "node":
                 for br in self.config_heads["node"]:
                     a = br["architecture"]
@@ -608,7 +628,7 @@ class Base(nn.Module):
                         per_node = a["type"] == "mlp_per_node"
                         if per_node:
                             assert self.num_nodes is not None, "num_nodes must be provided for mlp_per_node; use 'mlp' for variable-size graphs"
-                        head[br["type"]] = MLPNode(self.hidden_dim, self.head_dims[ih], a["dim_headlayers"], act,
+                        head[br["type"]] = MLPNode(self.hidden_dim, self.head_dims[ih] * (1 + self.var_output), a["dim_headlayers"], act,
                                                    num_mlp=self.num_nodes if per_node else 1, num_nodes=self.num_nodes if per_node else None)
                     elif a["type"] == "conv":                                            # :665-680, the same modules listed again
                         key, mods = br["type"], nn.ModuleList()
@@ -647,8 +667,8 @@ class Base(nn.Module):
                 ch.append(self.get_conv(hid[k], hid[k + 1], last_layer=False))
                 bh.append(PyGBatchNorm(hid[k + 1]))
             for ih in node_heads:
-                co.append(self.get_conv(hid[-1], self.head_dims[ih], last_layer=True))
-                bo.append(PyGBatchNorm(self.head_dims[ih]))
+                co.append(self.get_conv(hid[-1], self.head_dims[ih] * (1 + self.var_output), last_layer=True))
+                bo.append(PyGBatchNorm(self.head_dims[ih] * (1 + self.var_output)))
             key = br["type"]
             self.convs_node_hidden[key], self.batch_norms_node_hidden[key] = ch, bh
             self.convs_node_output[key], self.batch_norms_node_output[key] = co, bo
@@ -754,28 +774,31 @@ class Base(nn.Module):
         else:
             x_graph = self.pool(x, gcsr, higher)                              # Base.py:733-738
         ds = getattr(data, "dataset_name", None)
-        outputs = []
+        outputs, outputs_var = [], []
         for hd, head, kind in zip(self.head_dims, self.heads_NN, self.head_type):
+            width = hd * (1 + self.var_output)
             if self.num_branches == 1:
                 if kind == "graph":
                     h = run_mlp(self.graph_shared["branch-0"], x_graph, higher)
-                    outputs.append(run_mlp(head["branch-0"], h, higher)[:, :hd])
+                    out = run_mlp(head["branch-0"], h, higher)
                 elif isinstance(head["branch-0"], nn.ModuleList):                 # conv-type node head (Base.py:800-810)
                     a, b = x, equiv
                     mods = head["branch-0"]
                     for conv, bn in zip(mods[0::2], mods[1::2]):
                         a, b = conv(inv_node_feat=a, equiv_node_feat=b, plan=plan, higher_order=higher, **conv_args)
                         a = self.activation_function(bn(a))
-                    outputs.append(a[:, :hd])
+                    out = a
                 else:
-                    outputs.append(head["branch-0"](x, higher)[:, :hd])
-                continue
-            ids = ds[:, 0]                                                   # Base.py:770-780, 816-840
-            out = None if higher else self._grouped_decode(kind, head, ids, x, x_graph, batch, hd, num_graphs)
-            if out is None:
-                out = decode_branches(kind, head, self.graph_shared, ids, x, x_graph, batch, hd, num_graphs, higher)
-            outputs.append(out)
-        return outputs
+                    out = head["branch-0"](x, higher)
+            else:
+                ids = ds[:, 0]                                               # Base.py:770-780, 816-840
+                out = None if higher else self._grouped_decode(kind, head, ids, x, x_graph, batch, width, num_graphs)
+                if out is None:
+                    out = decode_branches(kind, head, self.graph_shared, ids, x, x_graph, batch, width, num_graphs, higher)
+            outputs.append(out[:, :hd])
+            if self.var_output:                                              # Base.py:764-768, 779, 810-811, 838
+                outputs_var.append(out[:, hd:] ** 2)
+        return (outputs, outputs_var) if self.var_output else outputs
 
     def _relu_embed_plan(self, higher):
         """Per conv: hand its s on as a ``ReluEmbed``?  Only where the encoder's step after a PaiNN layer is a plain ReLU
@@ -794,7 +817,7 @@ class Base(nn.Module):
         readout = self.graph_pooling == "mean" and all(k == "graph" for k in self.head_type)
         return [painn(i) and (painn(i + 1) if i + 1 < n else readout) for i in range(n)]
 
-    def _grouped_decode(self, kind, head, ids, x, x_graph, batch, hd, num_graphs):
+    def _grouped_decode(self, kind, head, ids, x, x_graph, batch, width, num_graphs):
         """Branch decoding as grouped GEMMs (SURVEY 8f-4): rows are sorted by dataset branch on the device (CSR over the branch
         ids), each layer of the per-branch MLPs is one ``hgb_grouped_linear`` launch, the result is scattered back -- no
         ``unique()``, no boolean masks, no host synchronisation.  None if the branches differ in architecture."""
@@ -815,7 +838,7 @@ class Base(nn.Module):
         ys = ops.grouped_mlp(seqs, xs, bcsr.rowptr)
         if ys is None:
             return None
-        return SegmentSum.apply(ys, pcsr)[:, :hd]
+        return SegmentSum.apply(ys, pcsr)[:, :width]
 
     def pool(self, x, gcsr, higher_order=False):
         if higher_order and self.graph_pooling != "max":
@@ -827,13 +850,16 @@ class Base(nn.Module):
         return ops.PoolFn.apply(x, gcsr, self.graph_pooling)
 
     def loss(self, pred, value, head_index):
-        """``loss_hpweighted`` (hydragnn/models/Base.py:879-906)."""
+        """``loss_hpweighted`` (hydragnn/models/Base.py:848-906); a mean-and-variance model's ``pred`` is (outputs, outputs_var)."""
+        var = None
+        if self.var_output:
+            pred, var = pred
         tot_loss = 0
         tasks_loss = []
         for ihead in range(self.num_heads):
             head_pre = pred[ihead]
             head_val = value[head_index[ihead]].reshape(head_pre.shape)
-            li = self.loss_function(head_pre, head_val)
+            li = self.loss_function(head_pre, head_val) if var is None else self.loss_function(head_pre, head_val, var[ihead])
             tot_loss = tot_loss + li * self.loss_weights[ihead]
             tasks_loss.append(li)
         return tot_loss, tasks_loss

@@ -53,7 +53,8 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 
 /* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd);
  * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient;
- * 109: hgb_nbr_* (SAGEConv / MFConv); 110: hgb_tc_linear_graph_add, hgb_film_* (graph-attribute conditioning) */
+ * 109: hgb_nbr_* (SAGEConv / MFConv); 110: hgb_tc_linear_graph_add, hgb_film_* (graph-attribute conditioning);
+ * 111: hgb_gnll_fwd_bwd (GaussianNLLLoss) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -506,6 +507,17 @@ int hgb_edge_vec_scatter(const float* gvec, const int32_t* col_rowptr, const int
  * *valid_rows <= 0 no row is real: loss[0] = 0 and gpred is zero everywhere.                          */
 int hgb_loss_fwd_bwd(const float* pred, const float* target, int64_t count, int32_t mode, float gscale,
                      float* loss, float* gpred, const int32_t* valid_rows, int32_t row_width,
+                     hgb_stream_t stream);
+/* Gaussian negative log-likelihood of torch.nn.GaussianNLLLoss (full=False, reduction="mean";
+ * hydragnn/models/Base.py:879-906 with loss_function_type "GaussianNLLLoss"), value and both gradients in one launch:
+ *   loss[0] = mean(0.5 (log v_c + (mean - target)^2 / v_c)),  v_c = max(var, eps),
+ *   gmean = (mean - target) / v_c / count,  gvar = 0.5 (1 / v_c - (mean - target)^2 / v_c^2) / count
+ * (the clamp passes the gradient through unchanged, as torch's clamp of a detached copy does).  mean, var, target, gmean,
+ * gvar [count].  valid_rows / row_width as in hgb_loss_fwd_bwd.  Multi-CTA with a fixed-order fp64 reduction: bit-identical
+ * on repeats.  workspace: hgb_gnll_workspace_bytes(count) bytes, no initial contents needed.                             */
+int64_t hgb_gnll_workspace_bytes(int64_t count);
+int hgb_gnll_fwd_bwd(const float* mean, const float* var, const float* target, int64_t count, float eps, float* loss,
+                     float* gmean, float* gvar, void* workspace, const int32_t* valid_rows, int32_t row_width,
                      hgb_stream_t stream);
 /* Fused AdamW over one flat parameter buffer: p, g, m, v [count]; `grad_scale` multiplies g first
  * (1/world_size after the flat all-reduce); step is 1-based and read from device (`step_dev`, fp32,
