@@ -62,6 +62,14 @@ __device__ __forceinline__ float hgb_act(float x, int act, float p) {
   }
 }
 
+// The activation of a Linear epilogue: hgb_act's runtime code (PR = false), or PReLU (PR = true) with the slope `a` the kernel
+// read from device memory.  A kernel instantiated with PR = true is a separate instance; the runtime-code instances are unchanged.
+template <bool PR>
+__device__ __forceinline__ float hgb_epi_act(float x, int act, float p, float a) {
+  if (PR) return x > 0.f ? x : a * x;      // torch.prelu: z = 0 and NaN take the slope branch
+  return hgb_act(x, act, p);
+}
+
 // gradient g through a ReLU with output y, bit for bit ATen's threshold_backward: +0 where y <= 0, g elsewhere (NaN y included)
 __device__ __forceinline__ float hgb_relu_select(float g, float y) { return y <= 0.f ? 0.f : g; }
 

@@ -14,12 +14,12 @@
 
 // C[m,n] (+)= sum_k A(m,k) B(k,n), A(m,k) = a[m*lda + k] or a[k*lda + m] (TA), same for B.
 // grid.z = split-K slices; with splits > 1 each slice writes its partial to part[z, m, n].
-template <bool TA, bool TB>
-__global__ void __launch_bounds__(256) gemm_kernel(const float* __restrict__ a, const float* __restrict__ b,
-                                                   float* __restrict__ c, int m, int n, int k, int64_t lda, int64_t ldb,
-                                                   int64_t ldc, int beta_one, int k_per_split, float* __restrict__ part,
-                                                   const float* __restrict__ bias, int act, float act_param,
-                                                   float* __restrict__ zout) {
+// PR: PReLU epilogue with the slope at `slope` (gemm_prelu_kernel), else the runtime activation code (gemm_kernel)
+template <bool TA, bool TB, bool PR>
+__device__ __forceinline__ void gemm_body(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ c, int m,
+                                          int n, int k, int64_t lda, int64_t ldb, int64_t ldc, int beta_one, int k_per_split,
+                                          float* __restrict__ part, const float* __restrict__ bias, int act, float act_param,
+                                          float* __restrict__ zout, const float* __restrict__ slope) {
   __shared__ __align__(16) float As[BK][BM + 4];
   __shared__ __align__(16) float Bs[BK][BN + 4];
   const int tid = threadIdx.x;
@@ -82,13 +82,30 @@ __global__ void __launch_bounds__(256) gemm_kernel(const float* __restrict__ a, 
           float v = acc[i][j];
           if (bias) v += bias[gn];
           if (zout) zout[(int64_t)gm * ldc + gn] = v;
-          v = hgb_act(v, act, act_param);
+          v = hgb_epi_act<PR>(v, act, act_param, PR ? __ldg(slope) : 0.f);
           if (beta_one) v += c[(int64_t)gm * ldc + gn];
           c[(int64_t)gm * ldc + gn] = v;
         }
       }
     }
   }
+}
+
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(256) gemm_kernel(const float* __restrict__ a, const float* __restrict__ b,
+                                                   float* __restrict__ c, int m, int n, int k, int64_t lda, int64_t ldb,
+                                                   int64_t ldc, int beta_one, int k_per_split, float* __restrict__ part,
+                                                   const float* __restrict__ bias, int act, float act_param,
+                                                   float* __restrict__ zout) {
+  gemm_body<TA, TB, false>(a, b, c, m, n, k, lda, ldb, ldc, beta_one, k_per_split, part, bias, act, act_param, zout, nullptr);
+}
+
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(256) gemm_prelu_kernel(const float* __restrict__ a, const float* __restrict__ b,
+                                                         float* __restrict__ c, int m, int n, int k, int64_t lda, int64_t ldb,
+                                                         int64_t ldc, const float* __restrict__ bias, float* __restrict__ zout,
+                                                         const float* __restrict__ slope) {
+  gemm_body<TA, TB, true>(a, b, c, m, n, k, lda, ldb, ldc, 0, k, nullptr, bias, HGB_ACT_PRELU, 0.f, zout, slope);
 }
 
 // c[i] (+)= sum over split-K slices of part[s, i].  blockDim = (32, 8): x = output element, y = slice group (slices y, y+8, ...);
@@ -293,6 +310,17 @@ extern "C" int hgb_linear_fwd(const float* x, const float* w, const float* b, in
   return launch_gemm<false, true>(x, w, y, m, n, k, ldx, ldw, n, 0, nullptr, 0, b, act, act_param, z, (cudaStream_t)stream);
 }
 
+extern "C" int hgb_linear_fwd_prelu(const float* x, const float* w, const float* b, int32_t m, int32_t n, int32_t k, int64_t ldx,
+                                    int64_t ldw, const float* slope, float* y, float* z, hgb_stream_t stream) {
+  HGB_REQUIRE(m >= 0 && n > 0 && k > 0 && x && w && y && z && slope && ldx >= k && ldw >= k, "linear_fwd_prelu: bad arguments");
+  if (m == 0) return HGB_OK;
+  const int mtiles = (m + BM - 1) / BM;
+  dim3 grid((n + BN - 1) / BN, mtiles < 65535 ? mtiles : 65535, 1);      // one k slice: the epilogue needs the whole sum
+  gemm_prelu_kernel<false, true><<<grid, 256, 0, (cudaStream_t)stream>>>(x, w, y, m, n, k, ldx, ldw, n, b, z, slope);
+  HGB_LAUNCH_CHECK("linear_fwd_prelu");
+  return HGB_OK;
+}
+
 // ---- activation derivative kernels -----------------------------------------------------------------
 __global__ void act_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ y, const float* __restrict__ z,
                                int64_t count, int act, float p, float* __restrict__ dz) {
@@ -410,9 +438,11 @@ extern "C" int hgb_colsum(const float* x, int32_t m, int32_t n, float* out, void
 #define SK_KMAX 8
 #define SK_NPT 8   // outputs per lane -> n <= 256
 
-__global__ void linear_smallk_fwd_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w, int64_t ldw,
-                                         const float* __restrict__ b, int64_t total, int n, int k, int act, float ap,
-                                         float* __restrict__ y, float* __restrict__ z) {
+template <bool PR>
+__device__ __forceinline__ void linear_smallk_fwd_body(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w,
+                                                       int64_t ldw, const float* __restrict__ b, int64_t total, int n, int k, int act,
+                                                       float ap, float* __restrict__ y, float* __restrict__ z,
+                                                       const float* __restrict__ slope) {
   extern __shared__ float sw[];  // [n][k] + [n]
   for (int i = threadIdx.x; i < n * k; i += blockDim.x) sw[i] = w[(int64_t)(i / k) * ldw + (i % k)];
   for (int i = threadIdx.x; i < n; i += blockDim.x) sw[n * k + i] = b ? b[i] : 0.f;
@@ -423,17 +453,31 @@ __global__ void linear_smallk_fwd_kernel(const float* __restrict__ x, int64_t ld
     float acc = sw[n * k + c];
     for (int q = 0; q < k; ++q) acc = fmaf(__ldg(x + r * ldx + q), sw[c * k + q], acc);
     if (z) z[t] = acc;
-    y[t] = hgb_act(acc, act, ap);
+    y[t] = hgb_epi_act<PR>(acc, act, ap, PR ? __ldg(slope) : 0.f);
   }
+}
+
+__global__ void linear_smallk_fwd_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w, int64_t ldw,
+                                         const float* __restrict__ b, int64_t total, int n, int k, int act, float ap,
+                                         float* __restrict__ y, float* __restrict__ z) {
+  linear_smallk_fwd_body<false>(x, ldx, w, ldw, b, total, n, k, act, ap, y, z, nullptr);
+}
+
+__global__ void linear_smallk_fwd_prelu_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w, int64_t ldw,
+                                               const float* __restrict__ b, int64_t total, int n, int k, float* __restrict__ y,
+                                               float* __restrict__ z, const float* __restrict__ slope) {
+  linear_smallk_fwd_body<true>(x, ldx, w, ldw, b, total, n, k, HGB_ACT_PRELU, 0.f, y, z, slope);
 }
 
 // n % 4 == 0: a thread owns four consecutive output columns of a row (16-byte stores), its weights live in registers, rows are
 // walked with a 2-D block (x: column group, y: row) -- no index division, no shared memory.
-template <int KT>
-__global__ void linear_smallk_fwd_vec4_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w, int64_t ldw,
-                                              const float* __restrict__ b, int m, int n, int k, int act, float ap,
-                                              float* __restrict__ y, float* __restrict__ z) {
+template <int KT, bool PR>
+__device__ __forceinline__ void linear_smallk_fwd_vec4_body(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w,
+                                                            int64_t ldw, const float* __restrict__ b, int m, int n, int k, int act,
+                                                            float ap, float* __restrict__ y, float* __restrict__ z,
+                                                            const float* __restrict__ slope) {
   const int c0 = threadIdx.x * 4;
+  const float sl = PR ? __ldg(slope) : 0.f;
   float wr[4][KT], bias[4];
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -454,8 +498,23 @@ __global__ void linear_smallk_fwd_vec4_kernel(const float* __restrict__ x, int64
     }
     const int64_t o = (int64_t)r * n + c0;
     if (z) *reinterpret_cast<float4*>(z + o) = make_float4(acc[0], acc[1], acc[2], acc[3]);
-    *reinterpret_cast<float4*>(y + o) = make_float4(hgb_act(acc[0], act, ap), hgb_act(acc[1], act, ap), hgb_act(acc[2], act, ap), hgb_act(acc[3], act, ap));
+    *reinterpret_cast<float4*>(y + o) = make_float4(hgb_epi_act<PR>(acc[0], act, ap, sl), hgb_epi_act<PR>(acc[1], act, ap, sl),
+                                                    hgb_epi_act<PR>(acc[2], act, ap, sl), hgb_epi_act<PR>(acc[3], act, ap, sl));
   }
+}
+
+template <int KT>
+__global__ void linear_smallk_fwd_vec4_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w, int64_t ldw,
+                                              const float* __restrict__ b, int m, int n, int k, int act, float ap,
+                                              float* __restrict__ y, float* __restrict__ z) {
+  linear_smallk_fwd_vec4_body<KT, false>(x, ldx, w, ldw, b, m, n, k, act, ap, y, z, nullptr);
+}
+
+template <int KT>
+__global__ void linear_smallk_fwd_vec4_prelu_kernel(const float* __restrict__ x, int64_t ldx, const float* __restrict__ w,
+                                                    int64_t ldw, const float* __restrict__ b, int m, int n, int k,
+                                                    float* __restrict__ y, float* __restrict__ z, const float* __restrict__ slope) {
+  linear_smallk_fwd_vec4_body<KT, true>(x, ldx, w, ldw, b, m, n, k, HGB_ACT_PRELU, 0.f, y, z, slope);
 }
 
 // one pass over (dy, y|z, x): dz = dy * act'(.), dx[m,k] = dz . W, partial dW / db per block.
@@ -651,6 +710,28 @@ extern "C" int hgb_linear_smallk_fwd(const float* x, int64_t ldx, const float* w
   linear_smallk_fwd_kernel<<<hgb_grid_for(total, 256), 256, (size_t)(n * k + n) * 4, (cudaStream_t)stream>>>(x, ldx, w, ldw, b, total, n, k,
                                                                                                        act, act_param, y, z);
   HGB_LAUNCH_CHECK("linear_smallk_fwd");
+  return HGB_OK;
+}
+
+extern "C" int hgb_linear_smallk_fwd_prelu(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* b, int32_t m,
+                                           int32_t n, int32_t k, const float* slope, float* y, float* z, hgb_stream_t stream) {
+  HGB_REQUIRE(x && w && y && z && slope && m >= 0 && hgb_linear_smallk_supported(n, k),
+              "linear_smallk_fwd_prelu: bad arguments or unsupported shape n=%d k=%d", n, k);
+  if (m == 0) return HGB_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (n % 4 == 0 && n >= 16 && ((uintptr_t)y % 16 == 0) && ((uintptr_t)z % 16 == 0)) {
+    const int cg = n / 4;
+    dim3 block(cg, 256 / cg > 0 ? 256 / cg : 1);
+    const int grid = hgb_grid_for(m, block.y, HGB_NUM_SMS * 8);
+#define SKV(KT_) linear_smallk_fwd_vec4_prelu_kernel<KT_><<<grid, block, 0, st>>>(x, ldx, w, ldw, b, m, n, k, y, z, slope)
+    if (k <= 1) SKV(1); else if (k <= 2) SKV(2); else if (k <= 4) SKV(4); else SKV(8);
+#undef SKV
+  } else {
+    const int64_t total = (int64_t)m * n;
+    linear_smallk_fwd_prelu_kernel<<<hgb_grid_for(total, 256), 256, (size_t)(n * k + n) * 4, st>>>(x, ldx, w, ldw, b, total, n, k,
+                                                                                                      y, z, slope);
+  }
+  HGB_LAUNCH_CHECK("linear_smallk_fwd_prelu");
   return HGB_OK;
 }
 

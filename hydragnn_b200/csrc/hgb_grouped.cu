@@ -34,11 +34,11 @@ __device__ __forceinline__ bool locate_tile(const int32_t* __restrict__ rowptr, 
 
 // TB = true : B_g(k, n) = w[g][n][k]  (forward, w [groups, n, k])
 // TB = false: B_g(k, n) = w[g][k][n]  (data gradient: reduction over the layer's outputs, w [groups, k, n])
-template <bool TB>
-__global__ void __launch_bounds__(256) grouped_rows_kernel(const float* __restrict__ a, int64_t lda, const float* __restrict__ w,
-                                                           const float* __restrict__ bias, const int32_t* __restrict__ rowptr,
-                                                           int groups, int tiles, int n, int k, int act, float act_param,
-                                                           float* __restrict__ c, float* __restrict__ z) {
+template <bool TB, bool PR>
+__device__ __forceinline__ void grouped_rows_body(const float* __restrict__ a, int64_t lda, const float* __restrict__ w,
+                                                  const float* __restrict__ bias, const int32_t* __restrict__ rowptr, int groups,
+                                                  int tiles, int n, int k, int act, float act_param, float* __restrict__ c,
+                                                  float* __restrict__ z, const float* __restrict__ slope) {
   __shared__ float As[GBK][GBM + 4];
   __shared__ float Bs[GBK][GBN + 4];
   const int tid = threadIdx.x, n0 = blockIdx.x * GBN;
@@ -93,10 +93,26 @@ __global__ void __launch_bounds__(256) grouped_rows_kernel(const float* __restri
         float v = acc[i][j];
         if (bias) v += bias[(int64_t)g * n + gn];
         if (z) z[(int64_t)(row0 + lm) * n + gn] = v;
-        c[(int64_t)(row0 + lm) * n + gn] = hgb_act(v, act, act_param);
+        c[(int64_t)(row0 + lm) * n + gn] = hgb_epi_act<PR>(v, act, act_param, PR ? __ldg(slope) : 0.f);
       }
     }
   }
+}
+
+template <bool TB>
+__global__ void __launch_bounds__(256) grouped_rows_kernel(const float* __restrict__ a, int64_t lda, const float* __restrict__ w,
+                                                           const float* __restrict__ bias, const int32_t* __restrict__ rowptr,
+                                                           int groups, int tiles, int n, int k, int act, float act_param,
+                                                           float* __restrict__ c, float* __restrict__ z) {
+  grouped_rows_body<TB, false>(a, lda, w, bias, rowptr, groups, tiles, n, k, act, act_param, c, z, nullptr);
+}
+
+// the forward (TB = true) with PReLU in the epilogue, slope read from device memory
+__global__ void __launch_bounds__(256) grouped_rows_prelu_kernel(const float* __restrict__ a, int64_t lda, const float* __restrict__ w,
+                                                                 const float* __restrict__ bias, const int32_t* __restrict__ rowptr,
+                                                                 int groups, int tiles, int n, int k, float* __restrict__ c,
+                                                                 float* __restrict__ z, const float* __restrict__ slope) {
+  grouped_rows_body<true, true>(a, lda, w, bias, rowptr, groups, tiles, n, k, HGB_ACT_PRELU, 0.f, c, z, slope);
 }
 
 // dW_g[nn][kk] = sum_{r in g} dy[r][nn] x[r][kk];  grid = (ceil(k/64), ceil(n/64), groups)
@@ -183,6 +199,19 @@ extern "C" int hgb_grouped_linear(const float* x, int64_t ldx, const float* w, c
   if (trans_w) grouped_rows_kernel<false><<<grid, 256, 0, st>>>(x, ldx, w, bias, rowptr, groups, tiles, n, k, act, act_param, y, z);
   else grouped_rows_kernel<true><<<grid, 256, 0, st>>>(x, ldx, w, bias, rowptr, groups, tiles, n, k, act, act_param, y, z);
   HGB_LAUNCH_CHECK("grouped_linear");
+  return HGB_OK;
+}
+
+extern "C" int hgb_grouped_linear_prelu(const float* x, int64_t ldx, const float* w, const float* bias, const int32_t* rowptr,
+                                        int32_t groups, int32_t m, int32_t n, int32_t k, const float* slope, float* y, float* z,
+                                        hgb_stream_t stream) {
+  HGB_REQUIRE(x && w && rowptr && y && z && slope && groups >= 1 && m >= 0 && n >= 1 && k >= 1 && ldx >= k,
+              "grouped_linear_prelu: bad arguments");
+  if (m == 0) return HGB_OK;
+  const int tiles = (m + GBM - 1) / GBM + groups;
+  dim3 grid((n + GBN - 1) / GBN, tiles < 65535 ? tiles : 65535);
+  grouped_rows_prelu_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, ldx, w, bias, rowptr, groups, tiles, n, k, y, z, slope);
+  HGB_LAUNCH_CHECK("grouped_linear_prelu");
   return HGB_OK;
 }
 

@@ -133,6 +133,82 @@ extern "C" int hgb_gnll_fwd_bwd(const float* mean, const float* var, const float
   return HGB_OK;
 }
 
+// torch.nn.PReLU() with its one learnable slope a, read from device memory on every launch (never by the host: the slope
+// changes every optimiser step and a captured graph replays with whatever value it holds then).  Same arithmetic as ATen's
+// prelu: y = z > 0 ? z : a z, dz = z > 0 ? g : a g (z = 0 and NaN take the slope branch), dL/da = sum over !(z > 0) of z g.
+// The slope gradient is reduced as hgb_gnll_fwd_bwd reduces its loss: a grid that depends on `count` only, each CTA's share
+// summed in a fixed order in fp64, the last CTA to finish adding the partials in index order.
+__global__ void __launch_bounds__(GNLL_THREADS) prelu_fwd_kernel(const float* __restrict__ z, int64_t count,
+                                                                 const float* __restrict__ slope, float* __restrict__ y) {
+  const float a = __ldg(slope);
+  const int64_t stride = (int64_t)gridDim.x * GNLL_THREADS;
+  for (int64_t i = (int64_t)blockIdx.x * GNLL_THREADS + threadIdx.x; i < count; i += stride) {
+    const float v = z[i];
+    y[i] = v > 0.f ? v : a * v;
+  }
+}
+
+template <bool SLOPE>
+__global__ void __launch_bounds__(GNLL_THREADS) prelu_bwd_kernel(
+    const float* __restrict__ g, const float* __restrict__ z, int64_t count, const float* __restrict__ slope,
+    float* __restrict__ dz, float* __restrict__ dslope, double* __restrict__ partial, unsigned int* __restrict__ ticket) {
+  const float a = __ldg(slope);
+  double acc = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * GNLL_THREADS;
+  for (int64_t i = (int64_t)blockIdx.x * GNLL_THREADS + threadIdx.x; i < count; i += stride) {
+    const float v = z[i], gi = g[i];
+    const bool pos = v > 0.f;
+    dz[i] = pos ? gi : a * gi;
+    if (SLOPE && !pos) acc += (double)v * (double)gi;       // exact product of two floats, summed in fp64
+  }
+  if (!SLOPE) return;
+  __shared__ double sm[GNLL_THREADS / 32];
+  __shared__ bool last;
+  const double s = gnll_block_sum(acc, sm);
+  if (threadIdx.x == 0) {
+    partial[blockIdx.x] = s;
+    __threadfence();
+    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double t = 0.0;
+  for (int b = threadIdx.x; b < (int)gridDim.x; b += GNLL_THREADS) t += __ldcg(partial + b);
+  t = gnll_block_sum(t, sm);
+  if (threadIdx.x == 0) {
+    dslope[0] = (float)t;
+    *ticket = 0u;
+  }
+}
+
+extern "C" int hgb_prelu_fwd(const float* z, int64_t count, const float* slope, float* y, hgb_stream_t stream) {
+  HGB_REQUIRE(count > 0 && z && slope && y, "prelu_fwd: bad arguments");
+  prelu_fwd_kernel<<<gnll_blocks(count), GNLL_THREADS, 0, (cudaStream_t)stream>>>(z, count, slope, y);
+  HGB_LAUNCH_CHECK("prelu_fwd");
+  return HGB_OK;
+}
+
+extern "C" int64_t hgb_prelu_workspace_bytes(int64_t count) { return hgb_gnll_workspace_bytes(count); }
+
+extern "C" int hgb_prelu_bwd(const float* g, const float* z, int64_t count, const float* slope, float* dz, float* dslope,
+                             void* workspace, int32_t skip_slope, hgb_stream_t stream) {
+  HGB_REQUIRE(count > 0 && g && z && slope && dz, "prelu_bwd: bad arguments");
+  HGB_REQUIRE(skip_slope || (dslope && workspace), "prelu_bwd: dslope and workspace are needed unless skip_slope");
+  const int blocks = gnll_blocks(count);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (skip_slope) {
+    prelu_bwd_kernel<false><<<blocks, GNLL_THREADS, 0, st>>>(g, z, count, slope, dz, nullptr, nullptr, nullptr);
+  } else {
+    double* partial = (double*)workspace;
+    unsigned int* ticket = (unsigned int*)(partial + blocks);
+    cudaMemsetAsync(ticket, 0, sizeof(unsigned int), st);
+    prelu_bwd_kernel<true><<<blocks, GNLL_THREADS, 0, st>>>(g, z, count, slope, dz, dslope, partial, ticket);
+  }
+  HGB_LAUNCH_CHECK("prelu_bwd");
+  return HGB_OK;
+}
+
 // torch.optim.AdamW semantics (decoupled weight decay, bias correction, eps outside the sqrt):
 //   p *= 1 - lr*wd;  m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;
 //   p -= lr/(1-b1^t) * m / (sqrt(v)/sqrt(1-b2^t) + eps)

@@ -19,8 +19,8 @@ import torch
 from torch import nn
 
 from . import e3, ops
-from .stacks import (ELEMENT_CSR, Base, cached, decode_branches, graph_head_mlp, graph_shared_mlp, graph_sum, remember,
-                     run_mlp)
+from .stacks import (ELEMENT_CSR, Base, apply_act, cached, decode_branches, graph_head_mlp, graph_shared_mlp, graph_sum,
+                     remember, run_mlp)
 
 NUM_ELEMENTS = 118
 
@@ -266,6 +266,8 @@ class _NodeMLP(nn.Module):
 
     def __init__(self, in_scalars, output_dim, hidden, act):
         super().__init__()
+        if isinstance(act, nn.PReLU):
+            self.activation_function = act          # blocks.py: the decoders keep the shared slope under their own name too
         first = E3Linear([(in_scalars, 0, 1)], [(output_dim if hidden is None else hidden[0], 0, 1)])
         layers = [first]
         if hidden is not None:
@@ -280,7 +282,7 @@ class _NodeMLP(nn.Module):
         h = seq[0]([x[:, None, :]], higher)[0][:, 0, :]
         if len(seq) == 1:
             return h
-        h = seq[1](h)
+        h = apply_act(seq[1], h, higher)
         return run_mlp(nn.Sequential(*list(seq)[2:]), h, higher)
 
 
@@ -291,6 +293,8 @@ class MultiheadDecoder(nn.Module):
     def __init__(self, nonlinear, in_scalars, config_heads, head_dims, head_type, act, graph_pooling, num_nodes=None):
         super().__init__()
         self.nonlinear, self.head_dims, self.head_type, self.graph_pooling = nonlinear, head_dims, head_type, graph_pooling
+        if isinstance(act, nn.PReLU):
+            self.activation_function = act
         self.graph_shared = nn.ModuleDict({})
         self.heads_NN = nn.ModuleList()
         if nonlinear and "graph" in config_heads:

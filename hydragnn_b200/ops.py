@@ -664,7 +664,118 @@ class LinearAct(torch.autograd.Function):
 
 
 def linear_act(x, weight, bias=None, act=None, act_param=0.0):
+    """``act(x W^T + b)``; for ``act = "prelu"`` ``act_param`` is the slope tensor (``LinearPReluFn``)."""
+    if act == "prelu":
+        return LinearPReluFn.apply(x, weight, bias, act_param)
     return LinearAct.apply(x, weight, bias, act, act_param)
+
+
+def _prelu_bwd(g, z, slope, need_slope):
+    """(dz, dslope) of y = prelu(z) in one ``hgb_prelu_bwd`` launch; dslope None when not needed or under ``only_data_grads``."""
+    n = z.numel()
+    need = need_slope and not _DATA_ONLY["on"]
+    dz = torch.empty_like(z)
+    if n == 0:
+        return dz, (torch.zeros_like(slope) if need else None)
+    dw = torch.empty_like(slope) if need else None
+    ws = _ws(_lib.query("hgb_prelu_workspace_bytes", n), z.device) if need else None
+    _lib.call("hgb_prelu_bwd", _p(_chk(g)), _p(z), n, _p(slope), _p(dz), _p(dw), _p(ws), 0 if need else 1, _stream())
+    return dz, dw
+
+
+class LinearPReluFn(torch.autograd.Function):
+    """``prelu(x W^T + b)`` with one learnable slope (``nn.PReLU()``), the PReLU in the Linear's forward epilogue: the small-k and
+    exact-fp32 kernels (``hgb_linear_smallk_fwd_prelu``, ``hgb_linear_fwd_prelu``) read the slope from device memory and store z
+    next to y.  Where the tensor-core Linear takes the shape, the layer runs there without an activation and ``hgb_prelu_fwd``
+    follows.  Backward: ``hgb_prelu_bwd`` (dz and the slope gradient, one launch), then the layer's plain backward."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, slope):
+        if slope.numel() != 1:
+            raise ValueError("LinearPReluFn: one shared slope (nn.PReLU()) expected, got %d" % slope.numel())
+        shp = x.shape
+        x2 = _row_major_2d(x)
+        w = weight if weight.stride(1) == 1 else weight.contiguous()
+        sl = _chk(slope)
+        b = _chk(bias)
+        m, k = x2.shape
+        n = w.shape[0]
+        if smallk_ok(n, k):
+            y, z = torch.empty(m, n, dtype=x2.dtype, device=x2.device), torch.empty(m, n, dtype=x2.dtype, device=x2.device)
+            _lib.call("hgb_linear_smallk_fwd_prelu", _p(x2), x2.stride(0), _p(w), w.stride(0), _p(b), m, n, k, _p(sl), _p(y), _p(z),
+                      _stream())
+        elif tc_ok(m, n, k, x2) and k <= 256:
+            z, _ = raw_tc_linear(x2, w, False, b, n, k)
+            y = torch.empty_like(z)
+            if z.numel():
+                _lib.call("hgb_prelu_fwd", _p(z), z.numel(), _p(sl), _p(y), _stream())
+        else:
+            y, z = torch.empty(m, n, dtype=x2.dtype, device=x2.device), torch.empty(m, n, dtype=x2.dtype, device=x2.device)
+            _lib.call("hgb_linear_fwd_prelu", _p(x2), _p(w), _p(b), m, n, k, x2.stride(0), w.stride(0), _p(sl), _p(y), _p(z),
+                      _stream())
+        ctx.save_for_backward(x2, w, z, sl)
+        ctx.shp, ctx.has_bias, ctx.tc = shp, bias is not None, _TC["enabled"]
+        ctx.leaves = [weight] + ([bias] if bias is not None else [])
+        return y.reshape(shp[:-1] + (n,))
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x2, w, z, sl = ctx.saved_tensors
+        m, k = x2.shape
+        n = w.shape[0]
+        dz, dslope = _prelu_bwd(gy.reshape(m, n), z, sl, ctx.needs_input_grad[3])
+        need = ctx.needs_input_grad
+        if smallk_ok(n, k):
+            gx, gw, gb = raw_smallk_bwd(dz, None, None, x2, w, 0, 0.0, need[0], need[1], ctx.has_bias and need[2])
+        else:
+            with tensor_cores(ctx.tc):
+                gx, gw, gb = linear_bwd_dispatch(dz, x2, w, need[0], need[1], ctx.has_bias and need[2], leaves=ctx.leaves)
+        if gx is not None:
+            gx = gx.reshape(ctx.shp)
+        return gx, gw, gb, (dslope.reshape(ctx.saved_tensors[3].shape) if dslope is not None else None)
+
+
+class PReluFn(torch.autograd.Function):
+    """``torch.nn.functional.prelu(x, weight)`` with one learnable slope (``nn.PReLU()``, the reference's "prelu").  The kernels
+    read the slope from device memory (``hgb_prelu_fwd`` / ``hgb_prelu_bwd``), so no host synchronisation, and a captured step
+    follows the optimiser's in-place updates.  The backward writes dx and the slope gradient in one launch, the latter a
+    fixed-order sum (the same bits on every run); under ``only_data_grads`` it is skipped."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        if weight.numel() != 1:
+            raise ValueError("PReluFn: one shared slope (nn.PReLU()) expected, got %d" % weight.numel())
+        x, w = _chk(x), _chk(weight)
+        y = torch.empty_like(x)
+        if x.numel():
+            _lib.call("hgb_prelu_fwd", _p(x), x.numel(), _p(w), _p(y), _stream())
+        ctx.save_for_backward(x, w)
+        ctx.wshape = weight.shape
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        x, w = ctx.saved_tensors
+        n = x.numel()
+        need_w = ctx.needs_input_grad[1] and not _DATA_ONLY["on"]
+        if n == 0:
+            return torch.zeros_like(x), (torch.zeros(ctx.wshape, dtype=w.dtype, device=w.device) if need_w else None)
+        g = _chk(g)
+        dx = torch.empty_like(x)
+        dw = torch.empty(ctx.wshape, dtype=w.dtype, device=w.device) if need_w else None
+        ws = _ws(_lib.query("hgb_prelu_workspace_bytes", n), x.device) if need_w else None
+        _lib.call("hgb_prelu_bwd", _p(g), _p(x), n, _p(w), _p(dx), _p(dw), _p(ws), 0 if need_w else 1, _stream())
+        return dx, dw
+
+
+def prelu(x, weight, higher_order=False):
+    """PReLU on the engine: ``PReluFn`` for first-order CUDA use, ATen's ``F.prelu`` (differentiable to any order) for the
+    force-training path and CPU tensors."""
+    if higher_order or not x.is_cuda:
+        return torch.nn.functional.prelu(x, weight)
+    return PReluFn.apply(x, weight)
 
 
 def _mlp2_fwd(x2, w1, b1, c1, p1, w2, b2, c2, p2):
@@ -1703,6 +1814,41 @@ class GroupedLinearFn(torch.autograd.Function):
         return gx, gw, gb, None, None, None
 
 
+class GroupedLinearPReluFn(torch.autograd.Function):
+    """``GroupedLinearFn`` with PReLU in the epilogue (``hgb_grouped_linear_prelu``: the slope read from device memory, z stored);
+    backward: ``hgb_prelu_bwd``, then the grouped data and weight gradients without an activation."""
+
+    @staticmethod
+    def forward(ctx, x, w, b, rowptr, slope):
+        x, w, sl = _chk(x.contiguous()), _chk(w.contiguous()), _chk(slope)
+        b = _chk(b.contiguous()) if b is not None else None
+        groups, n, k = w.shape
+        m = x.shape[0]
+        y = torch.empty(m, n, dtype=x.dtype, device=x.device)
+        z = torch.empty_like(y)
+        _lib.call("hgb_grouped_linear_prelu", _p(x), k, _p(w), _p(b), _p(rowptr), groups, m, n, k, _p(sl), _p(y), _p(z), _stream())
+        ctx.save_for_backward(x, w, z, rowptr, sl)
+        ctx.has_b = b is not None
+        return y
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, w, z, rowptr, sl = ctx.saved_tensors
+        groups, n, k = w.shape
+        m = x.shape[0]
+        dz, dslope = _prelu_bwd(gy.contiguous(), z, sl, ctx.needs_input_grad[4])
+        gx = gw = gb = None
+        if ctx.needs_input_grad[0]:
+            gx = torch.empty(m, k, dtype=x.dtype, device=x.device)
+            _lib.call("hgb_grouped_linear", _p(dz), n, _p(w), None, _p(rowptr), groups, m, k, n, 1, 0, 0.0, _p(gx), None, _stream())
+        if ctx.needs_input_grad[1] or (ctx.has_b and ctx.needs_input_grad[2]):
+            gw = torch.empty_like(w)
+            gb = torch.empty(groups, n, dtype=x.dtype, device=x.device) if ctx.has_b else None
+            _lib.call("hgb_grouped_wgrad", _p(dz), _p(x), k, _p(rowptr), groups, m, n, k, _p(gw), _p(gb), _stream())
+        return gx, gw, gb, None, dslope
+
+
 def grouped_mlp(seq_by_group, x, rowptr):
     """Run structurally identical ``nn.Sequential`` MLPs (one per group) on rows sorted by group.  Returns None when the
     branches do not share one architecture (the caller then falls back to per-branch launches)."""
@@ -1721,7 +1867,12 @@ def grouped_mlp(seq_by_group, x, rowptr):
             return None
         w = torch.stack([l.weight for l in layer])
         b = torch.stack([l.bias for l in layer]) if layer[0].bias is not None else None
-        x = GroupedLinearFn.apply(x, w, b, rowptr, code[0] if code else None, code[1] if code else 0.0)
+        if code is not None and code[0] == "prelu":
+            if any(m[i + 1] is not mods[0][i + 1] for m in mods):
+                return None                                  # branches with slopes of their own: not the reference's layout
+            x = GroupedLinearPReluFn.apply(x, w, b, rowptr, code[1])
+        else:
+            x = GroupedLinearFn.apply(x, w, b, rowptr, code[0] if code else None, code[1] if code else 0.0)
         i += 2 if code else 1
     return x
 

@@ -29,16 +29,15 @@ from .ops import GatherRows, LinearAct, MatMul, SegmentSum  # noqa: F401
 def activation_function_selection(name):
     table = {"relu": nn.ReLU, "selu": nn.SELU, "elu": nn.ELU, "sigmoid": nn.Sigmoid,
              "lrelu_01": lambda: nn.LeakyReLU(0.1), "lrelu_025": lambda: nn.LeakyReLU(0.25),
-             "lrelu_05": lambda: nn.LeakyReLU(0.5)}
-    if name == "prelu":
-        raise ValueError("activation 'prelu' (a learnable slope) is not supported by the b200 engine")
+             "lrelu_05": lambda: nn.LeakyReLU(0.5), "prelu": nn.PReLU}
     if name not in table:
         raise ValueError("Unknown activation function: " + str(name))
     return table[name]()
 
 
 def _act_code(mod):
-    """(kernel activation name, parameter) of an nn activation module, or None if it is not one."""
+    """(kernel activation name, parameter) of an nn activation module, or None if it is not one.  ``nn.PReLU``'s parameter is its
+    slope tensor, which the kernels read from device memory."""
     if isinstance(mod, nn.ReLU):
         return "relu", 0.0
     if isinstance(mod, nn.SiLU):
@@ -53,7 +52,16 @@ def _act_code(mod):
         return "elu", 0.0
     if isinstance(mod, nn.SELU):
         return "selu", 0.0
+    if isinstance(mod, nn.PReLU):
+        return "prelu", mod.weight
     return None
+
+
+def apply_act(act, x, higher_order=False):
+    """``act(x)`` for an activation module; a PReLU runs on the engine's kernels (``ops.prelu``)."""
+    if isinstance(act, nn.PReLU):
+        return ops.prelu(x, act.weight, higher_order)
+    return act(x)
 
 
 def loss_function_selection(name):
@@ -136,7 +144,7 @@ def _padded_chain(mods, x):
     lins = [m for m in mods if isinstance(m, nn.Linear)]
     if rows < PAD_MLP_MIN_ROWS or not lins or k0 % 32 or not 32 <= k0 <= 1024 or lins[0].in_features != k0:
         return None
-    if any((not isinstance(m, nn.Linear)) and _act_code(m) is None for m in mods):
+    if any((not isinstance(m, nn.Linear)) and _act_code(m) is None for m in mods):      # PReLU too: prelu(0) = 0
         return None
     if all(l.out_features % 32 == 0 for l in lins) or any(l.out_features > 1024 for l in lins):
         return None
@@ -199,10 +207,16 @@ def run_mlp(seq, x, higher_order=False):
         if isinstance(m, nn.Linear):
             code = _act_code(mods[i + 1]) if i + 1 < len(mods) else None
             w, b = wb(m)
+            if not higher_order and code is not None and code[0] == "prelu":
+                x = ops.linear_act(x, w, b, "prelu", code[1])             # the PReLU in the Linear's epilogue
+                i += 2
+                continue
             if (not higher_order and code is not None and i + 2 < len(mods) and isinstance(mods[i + 2], nn.Linear)):
                 # Linear - act - Linear (- act): one autograd node, activation gradient folded into a GEMM epilogue
                 w2, b2 = wb(mods[i + 2])
                 code2 = _act_code(mods[i + 3]) if i + 3 < len(mods) else None
+                if code2 is not None and code2[0] == "prelu":
+                    code2 = None                                          # applied by the next step of the loop
                 x = ops.mlp2(x, w, b, code[0], code[1], w2, b2, code2[0] if code2 else None, code2[1] if code2 else 0.0)
                 i += 4 if code2 is not None else 3
                 continue
@@ -214,7 +228,7 @@ def run_mlp(seq, x, higher_order=False):
             else:
                 x = ops.linear_act(x, w, b)
         else:
-            x = m(x)
+            x = apply_act(m, x, higher_order)
         i += 1
     if padded is not None:
         x = x[..., :[m for m in mods if isinstance(m, nn.Linear)][-1].out_features]
@@ -459,6 +473,8 @@ class MLPNode(nn.Module):
     def __init__(self, input_dim, output_dim, hidden_dim_node, activation, num_mlp=1, num_nodes=None):
         super().__init__()
         self.num_nodes, self.output_dim = num_nodes, output_dim
+        if isinstance(activation, nn.PReLU):
+            self.activation_function = activation       # Base.py:929: the shared slope is listed under the head as well
         self.mlp = nn.ModuleList()
         for _ in range(num_mlp):
             dims = [input_dim] + list(hidden_dim_node)
@@ -532,7 +548,9 @@ class Base(nn.Module):
         self.num_heads = len(self.head_dims)
         self.config_heads = config_heads
         self.equivariance = bool(equivariance)
-        self.activation_function = activation_function_selection(activation_function_type)
+        act = activation_function_selection(activation_function_type)
+        if not isinstance(act, nn.PReLU):
+            self.activation_function = act
         self.var_output = 1 if loss_function_type == "GaussianNLLLoss" else 0    # Base.py:109-111: mean-and-variance heads
         self.loss_function_type = loss_function_type
         self.loss_function = loss_function_selection(loss_function_type)
@@ -555,6 +573,10 @@ class Base(nn.Module):
         self.heads_NN = nn.ModuleList()
         self.convs_node_hidden, self.batch_norms_node_hidden = nn.ModuleDict(), nn.ModuleDict()      # Base.py:88-91
         self.convs_node_output, self.batch_norms_node_output = nn.ModuleDict(), nn.ModuleDict()
+        if isinstance(act, nn.PReLU):
+            # the one learnable slope shared by every site, registered where Base.py:94 registers it, so the state dict lists
+            # its aliases in the reference's order (a parameter-free activation stays where it was)
+            self.activation_function = act
         # global attention: every conv runs at hidden_dim and is wrapped in a GPS layer (Base.py:177-215)
         if self.global_attn_engine:
             if self.global_attn_engine != "GPS":
@@ -762,7 +784,7 @@ class Base(nn.Module):
                 inv, equiv = conv(inv_node_feat=inv, equiv_node_feat=equiv, plan=plan, higher_order=higher, relu_after=True, **conv_args)
                 continue
             inv, equiv = conv(inv_node_feat=inv, equiv_node_feat=equiv, plan=plan, higher_order=higher, **conv_args)
-            inv = self.activation_function(feat(inv))                        # Base.py:726
+            inv = apply_act(self.activation_function, feat(inv), higher)      # Base.py:726
         x = inv
         batch, num_graphs, gcsr = self.graph_index(data)
         if isinstance(x, ReluEmbed):                                          # only graph heads follow: x itself is not needed
@@ -786,7 +808,7 @@ class Base(nn.Module):
                     mods = head["branch-0"]
                     for conv, bn in zip(mods[0::2], mods[1::2]):
                         a, b = conv(inv_node_feat=a, equiv_node_feat=b, plan=plan, higher_order=higher, **conv_args)
-                        a = self.activation_function(bn(a))
+                        a = apply_act(self.activation_function, bn(a), higher)
                     out = a
                 else:
                     out = head["branch-0"](x, higher)

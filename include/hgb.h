@@ -45,6 +45,7 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 #define HGB_ACT_LRELU 5 /* slope in `act_param` */
 #define HGB_ACT_ELU 6
 #define HGB_ACT_SELU 7
+#define HGB_ACT_PRELU 8 /* learnable slope read from device memory: only the *_prelu entry points take it */
 
 /* pooling codes (hydragnn/models/Base.py:147-170) */
 #define HGB_POOL_ADD 0
@@ -54,7 +55,7 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 /* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd);
  * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient;
  * 109: hgb_nbr_* (SAGEConv / MFConv); 110: hgb_tc_linear_graph_add, hgb_film_* (graph-attribute conditioning);
- * 111: hgb_gnll_fwd_bwd (GaussianNLLLoss) */
+ * 111: hgb_gnll_fwd_bwd (GaussianNLLLoss); 112: hgb_prelu_fwd / hgb_prelu_bwd (PReLU with a device-resident slope) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -519,6 +520,28 @@ int64_t hgb_gnll_workspace_bytes(int64_t count);
 int hgb_gnll_fwd_bwd(const float* mean, const float* var, const float* target, int64_t count, float eps, float* loss,
                      float* gmean, float* gvar, void* workspace, const int32_t* valid_rows, int32_t row_width,
                      hgb_stream_t stream);
+/* torch.nn.PReLU() (one learnable slope; hydragnn/utils/model/model.py "prelu"), the slope read from device memory
+ * (`slope`, 1 float) by the kernel, so a captured graph follows in-place updates of it:
+ *   fwd:  y = z > 0 ? z : a z
+ *   bwd:  dz = z > 0 ? g : a g  (z = 0 and NaN take the slope branch, as ATen),  dslope[0] = sum over !(z > 0) of z g.
+ * g, z, y, dz [count].  The slope gradient: products exact in fp64, multi-CTA with a fixed-order fp64 reduction (as
+ * hgb_gnll_fwd_bwd), bit-identical on repeats; workspace: hgb_prelu_workspace_bytes(count) bytes, no initial contents
+ * needed.  skip_slope != 0: dz only, dslope and workspace may be NULL.  One kernel per call.                           */
+int hgb_prelu_fwd(const float* z, int64_t count, const float* slope, float* y, hgb_stream_t stream);
+/* The Linear forward with PReLU in its epilogue (HGB_ACT_PRELU): y = prelu(x W^T + b), the slope read from `slope` (device, 1
+ * float) by the kernel, z (required) receives the pre-activation for hgb_prelu_bwd.  Same shapes and rules as hgb_linear_fwd,
+ * hgb_linear_smallk_fwd and hgb_grouped_linear (trans_w = 0); separate kernel instances, the other activations' kernels are
+ * unchanged.                                                                                                                */
+int hgb_linear_fwd_prelu(const float* x, const float* w, const float* b, int32_t m, int32_t n, int32_t k, int64_t ldx,
+                         int64_t ldw, const float* slope, float* y, float* z, hgb_stream_t stream);
+int hgb_linear_smallk_fwd_prelu(const float* x, int64_t ldx, const float* w, int64_t ldw, const float* b, int32_t m, int32_t n,
+                                int32_t k, const float* slope, float* y, float* z, hgb_stream_t stream);
+int hgb_grouped_linear_prelu(const float* x, int64_t ldx, const float* w, const float* bias, const int32_t* rowptr,
+                             int32_t groups, int32_t m, int32_t n, int32_t k, const float* slope, float* y, float* z,
+                             hgb_stream_t stream);
+int64_t hgb_prelu_workspace_bytes(int64_t count);
+int hgb_prelu_bwd(const float* g, const float* z, int64_t count, const float* slope, float* dz, float* dslope,
+                  void* workspace, int32_t skip_slope, hgb_stream_t stream);
 /* Fused AdamW over one flat parameter buffer: p, g, m, v [count]; `grad_scale` multiplies g first
  * (1/world_size after the flat all-reduce); step is 1-based and read from device (`step_dev`, fp32,
  * incremented by the kernel) so the launch is CUDA-graph capturable.  hyper_dev (optional, device,
