@@ -641,8 +641,9 @@ __global__ void edge_vec_scatter_kernel(const float* __restrict__ gvec, const in
 
 extern "C" int hgb_edge_len_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const float* gd,
                                 int64_t e, float* gvec, hgb_stream_t stream) {
-  HGB_REQUIRE(e >= 0 && pos && row && col && gd && gvec, "edge_len_bwd: bad arguments");
-  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(e >= 0, "edge_len_bwd: bad arguments");
+  if (e == 0) return HGB_OK;   // no edges: no kernel runs (the arrays may then be NULL)
+  HGB_REQUIRE(pos && row && col && gd && gvec, "edge_len_bwd: bad arguments");
   edge_len_bwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, gd, e, gvec);
   HGB_LAUNCH_CHECK("edge_len_bwd");
   return HGB_OK;
@@ -650,8 +651,9 @@ extern "C" int hgb_edge_len_bwd(const float* pos, const int32_t* row, const int3
 
 extern "C" int hgb_edge_len_bwd2(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const float* gd,
                                  const float* ggpos, int64_t e, float* g_gd, float* q, hgb_stream_t stream) {
-  HGB_REQUIRE(e >= 0 && pos && row && col && gd && ggpos && g_gd && q, "edge_len_bwd2: bad arguments");
-  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(e >= 0, "edge_len_bwd2: bad arguments");
+  if (e == 0) return HGB_OK;   // no edges: no kernel runs (the arrays may then be NULL)
+  HGB_REQUIRE(pos && row && col && gd && ggpos && g_gd && q, "edge_len_bwd2: bad arguments");
   edge_len_bwd2_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, gd, ggpos, e, g_gd, q);
   HGB_LAUNCH_CHECK("edge_len_bwd2");
   return HGB_OK;

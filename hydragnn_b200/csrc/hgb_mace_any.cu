@@ -366,9 +366,9 @@ __global__ void mace_edge_embed_bwd_kernel(const float* __restrict__ pos, const 
 extern "C" int hgb_mace_edge_embed_fwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, int64_t e,
                                        int32_t lmax, int32_t num_bessel, float r_max, float p, float* sh, float* radial,
                                        hgb_stream_t stream) {
-  HGB_REQUIRE(pos && row && col && sh && radial && e >= 0 && lmax >= 0 && lmax <= 3 && num_bessel >= 1 && num_bessel <= 64 && r_max > 0.f,
-              "mace_edge_embed_fwd: bad arguments");
-  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(e >= 0 && lmax >= 0 && lmax <= 3 && num_bessel >= 1 && num_bessel <= 64 && r_max > 0.f, "mace_edge_embed_fwd: bad arguments");
+  if (e == 0) return HGB_OK;   // no edges: no kernel runs (the arrays may then be NULL)
+  HGB_REQUIRE(pos && row && col && sh && radial, "mace_edge_embed_fwd: bad arguments");
   mace_edge_embed_fwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, e, lmax, num_bessel, r_max, p, sh, radial);
   HGB_LAUNCH_CHECK("mace_edge_embed_fwd");
   return HGB_OK;
@@ -377,9 +377,9 @@ extern "C" int hgb_mace_edge_embed_fwd(const float* pos, const int32_t* row, con
 extern "C" int hgb_mace_edge_embed_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const float* g_sh,
                                        const float* g_radial, int64_t e, int32_t lmax, int32_t num_bessel, float r_max, float p,
                                        float* g_vec, hgb_stream_t stream) {
-  HGB_REQUIRE(pos && row && col && g_vec && e >= 0 && lmax >= 0 && lmax <= 3 && num_bessel >= 1 && num_bessel <= 64 && r_max > 0.f,
-              "mace_edge_embed_bwd: bad arguments");
+  HGB_REQUIRE(e >= 0 && lmax >= 0 && lmax <= 3 && num_bessel >= 1 && num_bessel <= 64 && r_max > 0.f, "mace_edge_embed_bwd: bad arguments");
   if (e == 0) return HGB_OK;
+  HGB_REQUIRE(pos && row && col && g_vec, "mace_edge_embed_bwd: bad arguments");
   mace_edge_embed_bwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, g_sh, g_radial, e, lmax, num_bessel,
                                                                                     r_max, p, g_vec);
   HGB_LAUNCH_CHECK("mace_edge_embed_bwd");

@@ -2174,6 +2174,8 @@ class EdgeLenFn(torch.autograd.Function):
 
 
 def _edge_vec_scatter(gvec, plan):
+    if plan.num_edges == 0:         # hgb_edge_vec_scatter takes no edge count: it cannot tell no edges from NULL arrays
+        return gvec.new_zeros(plan.num_nodes, 3)
     gpos = torch.empty(plan.num_nodes, 3, dtype=gvec.dtype, device=gvec.device)
     _lib.call("hgb_edge_vec_scatter", _p(gvec), _p(plan.by_col.rowptr), _p(plan.by_col.perm), _p(plan.by_row.rowptr), _p(plan.by_row.perm),
               plan.num_nodes, _p(gpos), _stream())

@@ -427,7 +427,8 @@ int hgb_mace_edge_mix(int32_t mode, const float* src, int64_t ld, const float* e
 /* MACE edge embedding in one pass per edge (SURVEY K2): vec = pos[col] - pos[row] + shift -> real spherical harmonics
  * sh [e, (lmax+1)^2] (component normalisation, e3nn axis convention; MACEStack.py:455-466) and the Bessel basis times the
  * polynomial cutoff radial [e, num_bessel] (mace_utils/modules/radial.py:18-60,110-148; blocks.py:164-177).  lmax <= 3.
- * bwd: g_vec [e, 3] = d L / d vec from g_sh / g_radial (either may be NULL); hgb_edge_vec_scatter turns it into d L / d pos.  */
+ * bwd: g_vec [e, 3] = d L / d vec from g_sh / g_radial (either may be NULL); hgb_edge_vec_scatter turns it into d L / d pos.
+ * With e = 0 nothing runs and every array may be NULL.                                                                       */
 int hgb_mace_edge_embed_fwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, int64_t e, int32_t lmax,
                             int32_t num_bessel, float r_max, float p, float* sh, float* radial, hgb_stream_t stream);
 int hgb_mace_edge_embed_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const float* g_sh,
@@ -487,7 +488,8 @@ int64_t hgb_weighted_colsum_workspace_bytes(int32_t h);
 /* Closed edge-length primitives for d_e = |pos[col] - pos[row] + shift_e| (operations.py:21-36; the length
  * itself is hgb_edge_geom_fwd).  bwd: gvec_e = gd_e vhat_e.  bwd2 (adjoint of bwd + scatter with respect to
  * gd and pos): w_e = ggpos[col] - ggpos[row]; g_gd_e = <vhat_e, w_e>; q_e = gd_e (w_e - vhat <vhat, w_e>) / d_e.
- * scatter: g_pos[i] = sum_{col(e)=i} gvec_e - sum_{row(e)=i} gvec_e (ordered).                           */
+ * scatter: g_pos[i] = sum_{col(e)=i} gvec_e - sum_{row(e)=i} gvec_e (ordered).  With e = 0 bwd and bwd2 run nothing and
+ * every array may be NULL; the scatter takes no edge count, so its arrays must be valid (callers without edges skip it). */
 int hgb_edge_len_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts,
                      const float* gd, int64_t e, float* gvec, hgb_stream_t stream);
 int hgb_edge_len_bwd2(const float* pos, const int32_t* row, const int32_t* col, const float* shifts,
