@@ -27,6 +27,11 @@ Parity pin status (see DESIGN.md "Oracle"):
   produced by the reference's own stack, ``Base.py`` and ``gps.py`` with the PyG convs
   restated here standing in for PyG's; each restated conv is pinned by hand-computed
   cases in ``tests/test_oracle_*.py``.
+* The GaussianNLLLoss mean-and-variance heads and the shared PReLU slope of every
+  stack (``base.StackOracle``), and MACE's edge attributes and graph-attribute
+  conditioning (``mace.MACEOracle``), are PINNED by
+  ``tests/golden/models_{gnll,prelu,mace_edge,mace_cond}.pt``, produced by the
+  reference's own ``Base.py``, stacks and MACE blocks.
 """
 
 from . import geometry, radius_graph, egnn, painn, base, mlip  # noqa: F401

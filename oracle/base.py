@@ -4,10 +4,10 @@ Test infrastructure only.  Restates ``Base`` (hydragnn/models/Base.py:36-982) on
 ``StackOracle``, which every oracle stack subclasses; ``EGCLStack``
 (hydragnn/models/EGCLStack.py:22-152), ``PAINNStack`` (hydragnn/models/PAINNStack.py:27-191)
 and ``PNAEqStack`` as ``OracleModel``; and the ``create_model`` dispatch
-(hydragnn/models/create.py:112-584).  The PNA, PNAPlus, CGCNN, GAT and SchNet stacks are
-in oracle/{pna,pnaplus,cgcnn,gat,schnet}.py.  Parameter names follow the reference (PyG
-``Sequential`` names its children ``module_<i>`` [3P-memory B.5]) so state dicts
-interchange with the engine.
+(hydragnn/models/create.py:112-584) over every stack.  The PNA, PNAPlus, CGCNN, GAT, SchNet,
+SAGE, MFC and MACE stacks are in oracle/{pna,pnaplus,cgcnn,gat,schnet,sage,mace}.py.
+Parameter names follow the reference (PyG ``Sequential`` names its children ``module_<i>``
+[3P-memory B.5]) so state dicts interchange with the engine.
 """
 import torch
 from torch import nn
@@ -38,7 +38,9 @@ def loss_function(name):
         return F.l1_loss
     if name == "rmse":
         return lambda a, b: torch.sqrt(F.mse_loss(a, b))
-    raise ValueError("oracle supports mse / mae / rmse, got " + str(name))
+    if name == "GaussianNLLLoss":
+        return torch.nn.GaussianNLLLoss()
+    raise ValueError("oracle supports mse / mae / rmse / GaussianNLLLoss, got " + str(name))
 
 
 def normalize_heads(output_heads):
@@ -63,8 +65,11 @@ class _Conv(nn.Module):
 class StackOracle(nn.Module):
     """``Base`` (hydragnn/models/Base.py:36-982): loss weights and pooling, the GPS node and edge embeddings, the encoder loop,
     ``graph_shared``, the graph heads, the ``mlp`` / ``mlp_per_node`` / ``conv`` node heads, single- and multi-branch decoding and
-    ``loss_hpweighted``.  A stack sets its own attributes (``edge_dim`` first of all) before calling this constructor and supplies
-    the hooks the reference's stacks override:
+    ``loss_hpweighted``.  Under ``loss_function_type="GaussianNLLLoss"`` every head is a mean-and-variance head: its last layer
+    is ``(1 + var_output) d`` wide, ``forward`` returns (means, variances) and the loss is ``GaussianNLLLoss`` per head; all
+    three follow the ``loss_function_type`` given to this constructor.  Graph-attribute conditioning is refused: only MACE's
+    is restated.  A stack sets its own attributes (``edge_dim`` first of all) before calling this constructor and supplies the
+    hooks the reference's stacks override:
 
     * ``_get_conv(fin, fout, last, edge_dim=None)``: one conv under the reference's child names;
     * ``_feature_layer(width)``: what follows every encoder conv (Identity here, a BatchNorm in ``Base._init_conv``);
@@ -78,8 +83,10 @@ class StackOracle(nn.Module):
     def __init__(self, input_dim, hidden_dim, output_dim, output_type, output_heads, activation_function="relu",
                  loss_function_type="mse", task_weights=None, num_conv_layers=2, num_nodes=None, equivariance=False,
                  graph_pooling="mean", global_attn_engine=None, global_attn_type=None, global_attn_heads=0, pe_dim=0, dropout=0.25,
-                 **_unused):
+                 use_graph_attr_conditioning=False, **_unused):
         super().__init__()
+        if use_graph_attr_conditioning:
+            raise ValueError("oracle restates graph-attribute conditioning for MACE only")
         self.use_global_attn = bool(global_attn_engine)
         if self.use_global_attn and (global_attn_engine != "GPS" or global_attn_type != "multihead"):
             raise ValueError("oracle supports global_attn_engine='GPS' with global_attn_type='multihead'")
@@ -89,6 +96,7 @@ class StackOracle(nn.Module):
         self.num_heads = len(self.head_dims)
         self.config_heads = normalize_heads(output_heads)
         self.activation_function = activation(activation_function)
+        self.loss_function_type = loss_function_type
         self.loss_function = loss_function(loss_function_type)
         w = list(task_weights if task_weights is not None else [1.0] * self.num_heads)
         if len(w) != self.num_heads:
@@ -159,7 +167,7 @@ class StackOracle(nn.Module):
                     layers = []
                     for d0, d1 in zip(dims[:-1], dims[1:]):
                         layers += [nn.Linear(d0, d1), act]
-                    layers.append(nn.Linear(dims[-1], self.head_dims[ih]))
+                    layers.append(nn.Linear(dims[-1], self._out_width(ih)))
                     head[br["type"]] = nn.Sequential(*layers)
             elif self.head_type[ih] == "node":
                 for br in self.config_heads["node"]:
@@ -168,7 +176,7 @@ class StackOracle(nn.Module):
                         per_node = a["type"] == "mlp_per_node"
                         if per_node:
                             assert self.num_nodes is not None, "num_nodes must be provided for mlp_per_node; use 'mlp' for variable-size graphs"
-                        head[br["type"]] = _MLPNode(self.hidden_dim, self.head_dims[ih], a["dim_headlayers"], act,
+                        head[br["type"]] = _MLPNode(self.hidden_dim, self._out_width(ih), a["dim_headlayers"], act,
                                                     num_mlp=self.num_nodes if per_node else 1, num_nodes=self.num_nodes if per_node else None)
                     elif a["type"] == "conv":                                       # Base.py:665-680: the SAME modules, listed again
                         key, mods = br["type"], nn.ModuleList()
@@ -204,11 +212,19 @@ class StackOracle(nn.Module):
                 ch.append(self._get_conv(w(hid[k], False), hid[k + 1], False))
                 bh.append(PyGBatchNorm(w(hid[k + 1], False)))
             for ih in node_heads:
-                co.append(self._get_conv(w(hid[-1], False), self.head_dims[ih], True))
-                bo.append(PyGBatchNorm(w(self.head_dims[ih], True)))
+                co.append(self._get_conv(w(hid[-1], False), self._out_width(ih), True))
+                bo.append(PyGBatchNorm(w(self._out_width(ih), True)))
             key = br["type"]
             self.convs_node_hidden[key], self.batch_norms_node_hidden[key] = ch, bh
             self.convs_node_output[key], self.batch_norms_node_output[key] = co, bo
+
+    def _var_output(self):
+        """``var_output`` (Base.py:109-111): 1 under GaussianNLLLoss, else 0."""
+        return int(self.loss_function_type == "GaussianNLLLoss")
+
+    def _out_width(self, ih):
+        """Width of head ``ih``'s last layer: the mean, then the variance's square root under GaussianNLLLoss."""
+        return self.head_dims[ih] * (1 + self._var_output())
 
     def _conv_width(self, fout, last):
         """Width of what a conv built for ``fout`` outputs."""
@@ -250,44 +266,48 @@ class StackOracle(nn.Module):
         xg = graph_pool(x, batch, G, self.graph_pooling)                     # Base.py:733-738
         ds = getattr(data, "dataset_name", None)
         outs = []
-        for ih, (hd, head, kind) in enumerate(zip(self.head_dims, self.heads_NN, self.head_type)):
+        for ih, (head, kind) in enumerate(zip(self.heads_NN, self.head_type)):
             if self.num_branches == 1:
                 if kind == "graph":
-                    outs.append(head["branch-0"](self.graph_shared["branch-0"](xg))[:, :hd])
+                    outs.append(head["branch-0"](self.graph_shared["branch-0"](xg)))
                 elif isinstance(head["branch-0"], nn.ModuleList):          # conv-type node head (Base.py:800-810)
                     a, b = x, equiv
                     mods = head["branch-0"]
                     for conv, bn in zip(mods[0::2], mods[1::2]):
                         a, b = self._run_conv(conv, a, b, ctx)
                         a = self.activation_function(bn(a))
-                    outs.append(a[:, :hd])
+                    outs.append(a)
                 else:
-                    outs.append(head["branch-0"](x, batch)[:, :hd])
+                    outs.append(head["branch-0"](x, batch))
                 continue
             # multi-branch masking (Base.py:770-780, 816-840)
             ids = ds[:, 0]
             if kind == "graph":
-                out = x.new_zeros(G, hd)
+                out = x.new_zeros(G, self._out_width(ih))
                 for b in ids.unique():
                     m = ids == b
                     key = "branch-%d" % int(b)
-                    out[m] = head[key](self.graph_shared[key](xg[m]))[:, :hd]
+                    out[m] = head[key](self.graph_shared[key](xg[m]))
             else:
-                out = x.new_zeros(x.shape[0], hd)
+                out = x.new_zeros(x.shape[0], self._out_width(ih))
                 for b in ids.unique():
                     m = (ids == b)[batch]
                     if isinstance(head["branch-%d" % int(b)], nn.ModuleList):
                         raise ValueError("oracle: conv-type node heads with several branches are not restated")
-                    out[m] = head["branch-%d" % int(b)](x[m], batch[m])[:, :hd]
+                    out[m] = head["branch-%d" % int(b)](x[m], batch[m])
             outs.append(out)
-        return outs
+        mean = [o[:, :hd] for o, hd in zip(outs, self.head_dims)]          # Base.py:764-846
+        if not self._var_output():
+            return mean
+        return mean, [o[:, hd:] ** 2 for o, hd in zip(outs, self.head_dims)]
 
     def loss(self, pred, value, head_index):
-        """``loss_hpweighted`` (Base.py:879-906)."""
+        """``loss_hpweighted`` (Base.py:848-906); ``pred`` is (means, variances) under GaussianNLLLoss."""
+        pred, var = pred if self._var_output() else (pred, None)
         tot, tasks = 0, []
         for ih in range(self.num_heads):
             tgt = value[head_index[ih]].reshape(pred[ih].shape).to(pred[ih].dtype)
-            li = self.loss_function(pred[ih], tgt)
+            li = self.loss_function(pred[ih], tgt) if var is None else self.loss_function(pred[ih], tgt, var[ih])
             tot = tot + li * self.loss_weights[ih]
             tasks.append(li)
         return tot, tasks
@@ -361,6 +381,7 @@ class _MLPNode(nn.Module):
     def __init__(self, fin, fout, hidden, act, num_mlp=1, num_nodes=None):
         super().__init__()
         self.num_nodes, self.fout = num_nodes, fout
+        self.activation_function = act                    # before mlp, as MLPNode (Base.py:929): a PReLU's slope is listed here
         self.mlp = nn.ModuleList()
         for _ in range(num_mlp):
             dims = [fin] + list(hidden)
@@ -379,16 +400,39 @@ class _MLPNode(nn.Module):
         return outs
 
 
-def oracle_from_case(cls, case, state=None, dtype=torch.float64):
-    """The oracle stack ``cls`` built from a case of tests/golden/models_*.pt, with ``state`` (the case's own by default) loaded
-    strictly, in ``dtype``.  The cases' GPS runs use 4 attention heads and 4-wide encodings, and their train-mode steps were
-    recorded with dropout off."""
+def stack_class(mpnn_type):
+    """The oracle stack class of ``mpnn_type`` (create.py:112-584).  Every one takes ``create_model``'s keyword arguments,
+    ``mpnn_type`` among them: ``OracleModel`` (EGNN, PAINN and PNAEq) reads it and refuses any other name."""
+    from .cgcnn import CGCNNStackOracle
+    from .gat import GATStackOracle
+    from .mace import MACEOracle
+    from .pna import PNAStackOracle
+    from .pnaplus import PNAPlusStackOracle
+    from .sage import MFCStackOracle, SAGEStackOracle
+    from .schnet import SCFStackOracle
+    stacks = {"PNA": PNAStackOracle, "PNAPlus": PNAPlusStackOracle, "CGCNN": CGCNNStackOracle, "GAT": GATStackOracle,
+              "SAGE": SAGEStackOracle, "MFC": MFCStackOracle, "SchNet": SCFStackOracle, "MACE": MACEOracle}
+    return stacks.get(mpnn_type, OracleModel)
+
+
+def case_kwargs(mpnn_type, case):
+    """``create_model`` keyword arguments of a case of tests/golden/models_*.pt: its ``cfg``, the ``deg`` histogram as ``pna_deg``
+    and its ``task_weights`` (1.0 per head by default).  The cases' GPS runs use 4 attention heads and 4-wide encodings."""
     cfg = dict(case["cfg"])
-    if cfg.pop("gps"):
+    if cfg.pop("gps", False):
         cfg.update(global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=4, pe_dim=4)
     if "deg" in case:
         cfg["pna_deg"] = case["deg"]
-    m = cls(**cfg, task_weights=[1.0] * len(cfg["output_type"]), dropout=0.0)
+    return dict(cfg, mpnn_type=mpnn_type, task_weights=case.get("task_weights", [1.0] * len(cfg["output_type"])))
+
+
+def oracle_from_case(stack, case, state=None, dtype=torch.float64):
+    """The oracle stack of a case of tests/golden/models_*.pt, with ``state`` (the case's own by default) loaded strictly, in
+    ``dtype``.  ``stack`` is the case's ``mpnn_type``, or an oracle stack class that needs none.  The cases' train-mode steps
+    were recorded with dropout off."""
+    mpnn_type = stack if isinstance(stack, str) else None
+    cls = stack_class(mpnn_type) if mpnn_type else stack
+    m = cls(**case_kwargs(mpnn_type, case), dropout=0.0)
     m.load_state_dict(case["state"] if state is None else state, strict=True)
     return m.to(dtype)
 
@@ -398,11 +442,7 @@ def create_model(**kw):
     (:164) and wraps the stack for MLIP training when asked (:586-756)."""
     from .mlip import MLIPWrapper
     torch.manual_seed(0)
-    if kw.get("mpnn_type") == "MACE":                      # create.py:542-582 -> MACEStack
-        from .mace import MACEOracle
-        model = MACEOracle(**{k: v for k, v in kw.items() if k != "mpnn_type"})
-    else:
-        model = OracleModel(**kw)
+    model = stack_class(kw.get("mpnn_type"))(**kw)
     if kw.get("enable_interatomic_potential", False):
         model = MLIPWrapper(model, kw.get("energy_weight", 0.0), kw.get("energy_peratom_weight", 0.0),
                             kw.get("force_weight", 0.0))

@@ -15,6 +15,9 @@ Pinning: tests/golden/models_mace.pt was produced by running the reference's OWN
 this restatement reproduces those outputs, forces, parameter gradients, state-dict keys and seeded initial values.  What
 stays unpinned is e3nn itself (oracle/e3.py, see its header), checked through properties (rotation / translation /
 permutation invariance of the energy, equivariance of the forces, identities of the coupling tensors).
+Edge attributes (MACEStack.py:198-203, 459-461) are pinned by tests/golden/models_mace_edge.pt and graph-attribute
+conditioning (Base.py:97-106, 249-391; MACEStack.py:375-421) by tests/golden/models_mace_cond.pt, both made the same way
+(tests/golden/make_mace_{edge,cond}_golden.py).
 Distance transforms (Agnesi / Soft, radial.py:146-248) need ase.data.covalent_radii, which is not in this image:
 they raise NotImplementedError.
 """
@@ -354,15 +357,36 @@ class MultiheadDecoder(nn.Module):
 # the stack
 # ---------------------------------------------------------------------------------------------------------------
 class MACEOracle(nn.Module):
-    """MACEStack (MACEStack.py:70-498) for use_global_attn = False, no graph-attr conditioning, no edge_attr."""
+    """MACEStack (MACEStack.py:70-498) for use_global_attn = False.
+
+    With ``edge_dim`` D > 0 the edge irreps are (D x 0e + sh).simplify() = (D+1)x0e + 1x1o + ... and every interaction reads
+    cat([edge_attr, sh]): the "uvu" tensor product (oracle/e3.py) takes the multiplicity D+1 on its second input, with the path
+    constant sqrt((2 l3 + 1) / (D+1)) on the 0e paths, and the radial MLP's last layer grows to the new weight_numel.
+
+    With ``use_graph_attr_conditioning`` the invariant channels are conditioned on ``data.graph_attr`` after the embedding and
+    after each convolution once that layer's readout has run.  The conditioning modules are created at the first forward (on
+    the CPU generator), so they come after every other state-dict entry.  "fuse_pool" only checks graph_attr: MACEStack never
+    pools with it.
+
+    ``edge_dim``, ``use_graph_attr_conditioning`` and ``graph_attr_conditioning_mode`` come from the arguments or, where these
+    are not given, from a subclass that set them before calling this constructor, as StackOracle's stacks set ``edge_dim``.
+    """
 
     num_elements = 118
 
     def __init__(self, input_dim, hidden_dim, output_dim, output_type, output_heads, activation_function="relu",
                  loss_function_type="mse", task_weights=None, num_conv_layers=2, num_nodes=None, edge_dim=None, num_radial=None,
                  radius=None, radial_type=None, distance_transform=None, max_ell=None, node_max_ell=None, avg_num_neighbors=None,
-                 envelope_exponent=None, correlation=None, graph_pooling="mean", global_attn_engine=None, **_unused):
+                 envelope_exponent=None, correlation=None, graph_pooling="mean", global_attn_engine=None,
+                 use_graph_attr_conditioning=False, graph_attr_conditioning_mode=None, **_unused):
         super().__init__()
+        preset = vars(self)
+        self.edge_dim = int(edge_dim or preset.get("edge_dim") or 0)
+        self.use_graph_attr_conditioning = bool(use_graph_attr_conditioning or preset.get("use_graph_attr_conditioning"))
+        mode = graph_attr_conditioning_mode or preset.get("graph_attr_conditioning_mode") or "concat_node"
+        self.graph_attr_conditioning_mode = mode.lower()                             # Base.py:97-106
+        if self.graph_attr_conditioning_mode not in ("film", "concat_node", "fuse_pool"):
+            raise ValueError("graph_attr_conditioning_mode must be one of: 'film', 'concat_node', 'fuse_pool'.")
         assert radius is not None, "MACE requires radius input."
         assert num_radial is not None, "MACE requires num_radial input."
         assert max_ell is not None, "MACE requires max_ell input."
@@ -371,8 +395,6 @@ class MACEOracle(nn.Module):
         assert node_max_ell >= 1, "MACE requires node_max_ell >= 1."
         if global_attn_engine:
             raise ValueError("oracle MACE: GPS wrapping is not restated")
-        if edge_dim:
-            raise ValueError("oracle MACE: edge_attr is not restated")
         self.mpnn_type, self.hidden_dim, self.input_dim, self.num_nodes = "MACE", hidden_dim, input_dim, num_nodes
         self.max_ell, self.node_max_ell, self.avg_num_neighbors = max_ell, node_max_ell, avg_num_neighbors
         self.head_dims, self.head_type = list(output_dim), list(output_type)
@@ -404,6 +426,10 @@ class MACEOracle(nn.Module):
         self.edge_feats_irreps = e3.Irreps("%dx0e" % num_radial)
         self.node_attr_irreps = e3.Irreps([(self.num_elements, (0, 1))])
         self.sh_irreps = e3.Irreps.spherical_harmonics(max_ell)
+        if self.edge_dim:                                                              # MACEStack.py:198-203
+            self.edge_attrs_irreps = (e3.Irreps("%dx0e" % self.edge_dim) + self.sh_irreps).simplify()
+        else:
+            self.edge_attrs_irreps = self.sh_irreps
         # ---- Base.__init__ -> _init_conv (MACEStack.py:190-275): decoders and convolutions, interleaved
         self.graph_convs = nn.ModuleList()
         self.multihead_decoders = nn.ModuleList()
@@ -424,6 +450,8 @@ class MACEOracle(nn.Module):
         self.radial_embedding = RadialEmbedding(radius, num_radial, p_cut, radial_type, distance_transform)
         self.node_embedding = nn.Module()
         self.node_embedding.linear = e3.Linear(self.node_attr_irreps, e3.create_irreps_string(hidden_dim, 0))
+        self.graph_conditioner = self.graph_concat_projector = self.graph_concat_projector_in_dim = None
+        self.device = torch.device("cpu")          # Base.py:66; read by load_existing_model
 
     def _decoder(self, nonlinear, irreps):
         return MultiheadDecoder(nonlinear, irreps, self.config_heads, self.head_dims, self.head_type, self.activation_function,
@@ -439,7 +467,7 @@ class MACEOracle(nn.Module):
         output_irreps = e3.Irreps(e3.create_irreps_string(output_dim, self.node_max_ell))
         if last_layer:
             hidden_irreps, output_irreps = hidden_irreps[:1], output_irreps[:1]
-        inter = Interaction(node_feats_irreps, self.sh_irreps, self.edge_feats_irreps, interaction_irreps, hidden_irreps,
+        inter = Interaction(node_feats_irreps, self.edge_attrs_irreps, self.edge_feats_irreps, interaction_irreps, hidden_irreps,
                             self.avg_num_neighbors, [mlp_dim] * 3)
         prod = Product(interaction_irreps, hidden_irreps, self.correlation[0], self.num_elements, use_sc=True)
         sizing = e3.Linear(hidden_irreps, output_irreps)
@@ -464,15 +492,63 @@ class MACEOracle(nn.Module):
         attrs = self.node_attributes(data.x).to(dtype)
         feats = self.node_embedding.linear(attrs)
         edge_attrs = e3.spherical_harmonics(self.max_ell, vec, normalize=True, normalization="component")
+        if self.edge_dim:                                                              # MACEStack.py:459-461
+            edge_attrs = torch.cat([data.edge_attr.to(edge_attrs.dtype), edge_attrs], dim=1)
         edge_feats = self.radial_embedding(dist)
         inv, equiv = feats[:, :self.hidden_dim], feats[:, self.hidden_dim:]
+        inv = self.condition(inv, batch, data, num_graphs)
         ds = getattr(data, "dataset_name", None)
         outputs = self.multihead_decoders[0](attrs, batch, num_graphs, ds)
         for conv, readout in zip(self.graph_convs, self.multihead_decoders[1:]):
             inv, equiv = conv(inv, equiv, attrs, edge_attrs, edge_feats, data.edge_index)
             out = readout(torch.cat([inv, equiv], dim=1), batch, num_graphs, ds)
+            inv = self.condition(inv, batch, data, num_graphs)
             outputs = [a + b for a, b in zip(outputs, out)]
         return outputs
+
+    def _ensure_graph_conditioner(self, graph_attr_dim, device):
+        """Base.py:249-259."""
+        if self.graph_conditioner is None:
+            hidden = max(self.hidden_dim, graph_attr_dim)
+            self.graph_conditioner = nn.Sequential(nn.Linear(graph_attr_dim, hidden), self.activation_function,
+                                                   nn.Linear(hidden, 2 * self.hidden_dim))
+        self.graph_conditioner = self.graph_conditioner.to(device=device, dtype=self.node_embedding.linear.weight.dtype)
+
+    def _ensure_graph_concat_projector(self, graph_attr_dim, channel_dim, device, dtype=None):
+        """Base.py:261-276."""
+        in_dim = channel_dim + graph_attr_dim
+        if self.graph_concat_projector is None or self.graph_concat_projector_in_dim != in_dim:
+            self.graph_concat_projector = nn.Linear(in_dim, channel_dim)
+            self.graph_concat_projector_in_dim = in_dim
+        self.graph_concat_projector = self.graph_concat_projector.to(device=device,
+                                                                     dtype=dtype or self.node_embedding.linear.weight.dtype)
+
+    def condition(self, inv, batch, data, num_graphs):
+        """_apply_graph_conditioning (Base.py:299-391) on the invariant channels."""
+        if not self.use_graph_attr_conditioning:
+            return inv
+        ga = getattr(data, "graph_attr", None)
+        if ga is None:
+            raise ValueError("use_graph_attr_conditioning=True but data.graph_attr is missing.")
+        ga = ga.to(device=inv.device, dtype=inv.dtype)
+        if ga.dim() == 1:
+            if ga.numel() % num_graphs:
+                raise ValueError(f"One-dimensional graph_attr with numel={ga.numel()} is not divisible by num_graphs={num_graphs}.")
+            ga = ga.view(num_graphs, ga.numel() // num_graphs)
+        elif ga.dim() == 2:
+            if ga.size(0) != num_graphs:
+                raise ValueError(f"graph_attr first dim {ga.size(0)} does not match num_graphs={num_graphs}.")
+        else:
+            raise ValueError(f"Unsupported graph_attr ndim={ga.dim()}; expected 1/2.")
+        mode = self.graph_attr_conditioning_mode
+        if mode == "film":
+            self._ensure_graph_conditioner(ga.size(-1), inv.device)
+            scale, shift = self.graph_conditioner(ga).split(self.hidden_dim, dim=-1)
+            return inv * (1 + torch.tanh(scale)[batch]) + shift[batch]
+        if mode == "concat_node":
+            self._ensure_graph_concat_projector(ga.size(-1), inv.size(-1), inv.device, inv.dtype)
+            return self.graph_concat_projector(torch.cat([inv, ga[batch]], dim=-1))
+        return inv
 
     def loss(self, pred, value, head_index):
         tot, tasks = 0, []

@@ -1,7 +1,8 @@
-"""What the test modules share: the model configurations of the reference goldens, the engine model of a golden case, the
-checks of a model against a golden case and of the engine against a drop-in golden, the batches the GPU tests build, one
-training step of an oracle stack and the error summary the benchmark-shape tests bound.  A plain module on the tests' import
-path; no test module imports another, and nothing here reads tests/golden/'s makers or the reference checkout they need."""
+"""What the test modules share: the model configurations of the reference goldens, the GaussianNLLLoss and PReLU cases, the
+engine model of a golden case, the checks of a model against a golden case and of the engine against a drop-in golden, the
+batches the GPU tests build, one training step of an oracle stack and the error summary the benchmark-shape tests bound.  A
+plain module on the tests' import path; no test module imports another, and nothing here reads tests/golden/'s makers or the
+reference checkout they need."""
 import hashlib
 import types
 
@@ -10,6 +11,7 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import _lib
 from hydragnn_b200.synthetic import ARCH, WORKLOADS, make_samples
+from oracle.base import case_kwargs
 from oracle.radius_graph import radius_graph
 from oracle.workloads import add_edges_cpu
 
@@ -89,20 +91,59 @@ def mace_batch(gen, sizes=(7, 9), box=4.0, radius=6.0):
     return d
 
 
+# ---- the cases of tests/golden/models_{gnll,prelu}.pt: the reference's own code under GaussianNLLLoss and under "prelu" ----------
+GNLL_CASES = ["pna_ci_multihead", "pna_conv_head", "pna_gps", "egnn_initial_bias", "egnn_two_branches", "egnn_clamped",
+              "painn_mlp_per_node", "cgcnn_graph"]
+PRELU_CASES = ["pna_ci_multihead", "pna_conv_head_slope", "pna_gps", "egnn_graph_node", "egnn_two_branches", "egnn_gnll",
+               "painn_mlp_per_node", "sage_graph_slope"]
+PRELU_MACE_CASES = ["mace", "mace_film"]
+
+
+def case_mpnn_type(name):
+    """The stack of a models_{gnll,prelu}.pt case, named by the first word of the case."""
+    return {"pna": "PNA", "egnn": "EGNN", "painn": "PAINN", "cgcnn": "CGCNN", "sage": "SAGE", "mace": "MACE"}[name.split("_")[0]]
+
+
+def named_case_kwargs(name, c):
+    """create_model keyword arguments of a models_{gnll,prelu}.pt case; a MACE case's cfg holds what differs from MACE_KW."""
+    t = case_mpnn_type(name)
+    if t == "MACE":
+        c = dict(c, cfg=dict(MACE_KW, **c["cfg"]))
+    return case_kwargs(t, c)
+
+
+def prelu_engine(name, c, use_gpu=False):
+    """The engine model of a models_prelu.pt case with the case's slope set."""
+    m = hb.create_model(**named_case_kwargs(name, c), use_gpu=use_gpu)
+    if c.get("slope") is not None:
+        with torch.no_grad():
+            m.activation_function.weight.fill_(c["slope"])
+    return m
+
+
+class Flat:
+    """A mean-and-variance model seen as one returning the list the golden stores: the means of every head, then their
+    variances."""
+
+    def __init__(self, m):
+        self.m = m
+
+    def __getattr__(self, name):
+        return getattr(self.m, name)
+
+    def __call__(self, data):
+        mean, var = self.m(data)
+        return list(mean) + list(var)
+
+    def loss(self, pred, value, head_index):
+        k = len(pred) // 2
+        return self.m.loss((pred[:k], pred[k:]), value, head_index)
+
+
 # ---- the engine model of a case of tests/golden/models_{pna,pnaplus,cgcnn,gat,schnet}.pt ---------------------------------------
-def engine_kwargs(mpnn_type, case):
-    """create_model keyword arguments of a golden case (the reference's create.py fixes GAT's heads = 6, slope = 0.05)."""
-    cfg = dict(case["cfg"])
-    if cfg.pop("gps"):
-        cfg.update(pe_dim=4, global_attn_engine="GPS", global_attn_type="multihead", global_attn_heads=4)
-    if "deg" in case:
-        cfg["pna_deg"] = case["deg"]
-    return dict(mpnn_type=mpnn_type, task_weights=[1.0] * len(cfg["output_type"]), **cfg)
-
-
 def golden_engine(mpnn_type, case, state=None):
     """The engine's model of a golden case on the GPU with ``state`` (the case's own by default) loaded strictly."""
-    m = hb.create_model(**engine_kwargs(mpnn_type, case))
+    m = hb.create_model(**case_kwargs(mpnn_type, case))
     m.load_state_dict(case["state"] if state is None else state, strict=True)
     return m
 
@@ -117,7 +158,7 @@ def state_digest(t):
 def seeded_state(case):
     """The reference's seeded state dict of a models_gat.pt case.  The file holds it as names in order with one SHA-256 per entry;
     the engine's own seeded construction (create_model on the CPU) reproduces it, and is checked against every digest here."""
-    sd = hb.create_model(**engine_kwargs("GAT", case), use_gpu=False).state_dict()
+    sd = hb.create_model(**case_kwargs("GAT", case), use_gpu=False).state_dict()
     want = case["state_sha256"]
     assert list(sd.keys()) == list(want.keys()), "state-dict names or order differ from the reference's"
     bad = [k for k, v in sd.items() if state_digest(v) != want[k]]

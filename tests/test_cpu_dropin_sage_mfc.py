@@ -8,9 +8,8 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import padded
 from hydragnn_b200.sage import MFCStack, SAGEStack
-from oracle.base import oracle_from_case
-from oracle.sage import MFCStackOracle, SAGEStackOracle
-from stack_support import check_dropin, check_seeded_state, engine_kwargs
+from oracle.base import case_kwargs, oracle_from_case
+from stack_support import check_dropin, check_seeded_state
 
 DROPIN = ["SAGE-graph-bias", "SAGE-node", "SAGE-gps-graph", "MFC-node-bias", "MFC-node", "MFC-gps-graph"]
 STACKS = {"SAGE": SAGEStack, "MFC": MFCStack}
@@ -34,13 +33,11 @@ def _cases(golden_dir, kind):
 def test_engine_state_dicts_match_every_golden_case_and_load_both_ways(golden_dir, kind):
     """Seeded construction of every case equals the reference's (names, order, shapes, values; SAGE ignores initial_bias, MFC
     honours it), the reference's checkpoint loads strictly into the engine, and the engine's into the oracle stack."""
-    oracle = SAGEStackOracle if kind == "SAGE" else MFCStackOracle
     for name, c in _cases(golden_dir, kind).items():
-        eng = hb.create_model(**engine_kwargs(kind, c), use_gpu=False)
+        eng = hb.create_model(**case_kwargs(kind, c), use_gpu=False)
         assert type(eng) is STACKS[kind] and str(eng) == c["str"], name
         check_seeded_state(eng, c["state"])
-        case = dict(c, cfg={k: v for k, v in c["cfg"].items() if k != "initial_bias"})
-        oracle_from_case(oracle, case, state=eng.state_dict())
+        oracle_from_case(kind, c, state=eng.state_dict())
 
 
 def test_mfc_requires_max_neighbours(golden_dir):

@@ -11,8 +11,9 @@ import hydragnn_b200 as hb
 from hydragnn_b200 import _lib, ops
 from hydragnn_b200.synthetic import ARCH
 from kernel_harness import Buf, check_bound, launches, stream, twice
-from gnll_oracle import CASES, Flat, case_kwargs, oracle_of
-from stack_support import _batch, _loader, _zero_dropout, check_golden_case, grad_close, rel_l2
+from oracle.base import oracle_from_case
+from stack_support import (GNLL_CASES, Flat, _batch, _loader, _zero_dropout, case_mpnn_type, check_golden_case, golden_data,
+                           grad_close, named_case_kwargs, rel_l2)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -131,12 +132,12 @@ def golden(golden_dir):
 
 
 def _engine(name, c):
-    m = hb.create_model(**case_kwargs(name, c))
+    m = hb.create_model(**named_case_kwargs(name, c))
     m.load_state_dict(c["state"], strict=True)
     return m
 
 
-@pytest.mark.parametrize("name", CASES)
+@pytest.mark.parametrize("name", GNLL_CASES)
 def test_engine_matches_reference_golden(golden, name):
     """Means, variances, the NLL and every gradient of the engine against the reference, at the bounds of the stacks' own golden
     tests; the fused NLL kernel runs in the train step.  The conv head and the clamped case carry (mean - target) / eps terms."""
@@ -148,24 +149,17 @@ def test_engine_matches_reference_golden(golden, name):
     assert "hgb_gnll_fwd_bwd" in {t[0] for t in _lib.trace_end()}
 
 
-class _OD:
-    def __init__(self, inputs, dtype):
-        for k, v in inputs.items():
-            setattr(self, k, v.to(dtype) if v.is_floating_point() else v)
-        self.edge_attr = getattr(self, "edge_attr", None)
-
-
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
-@pytest.mark.parametrize("name", [n for n in CASES if n != "pna_gps"])
+@pytest.mark.parametrize("name", [n for n in GNLL_CASES if n != "pna_gps"])
 def test_engine_training_step_matches_fp64_oracle(golden, name, precision):
     """One train-mode step of the engine, in fp32 and in bf16 (TF32 tensor-core Linears), against the oracle in fp64: rel-L2 of the
     means and variances, the NLL and all gradients together within 1e-4 (fp32) or 2e-2 (bf16)."""
     c = golden[name]
     em = hb.set_precision(_engine(name, c), precision)
-    om = oracle_of(name, c).train()
+    om = oracle_from_case(case_mpnn_type(name), c).train()
     _zero_dropout(om)
     value, hi = c["value"], c["head_index"]
-    opred = om(_OD(c["inputs"], torch.float64))
+    opred = om(golden_data(c["inputs"]))
     oloss, _ = om.loss(opred, value.double(), hi)
     ograds = torch.autograd.grad(oloss, list(om.parameters()))
     em.train()

@@ -1,6 +1,6 @@
 """GPU tests of MACE graph-attribute conditioning: the graph-addend tensor-core Linear (hgb_tc_linear_graph_add) and the FiLM
 kernels (hgb_film_fwd / hgb_film_bwd) one by one against fp64, the engine against the fp64 restatement
-(tests/mace_cond_oracle.py) on first-order and MLIP double-backward passes, and hb.train's padded step carrying graph_attr."""
+(oracle/mace.py) on first-order and MLIP double-backward passes, and hb.train's padded step carrying graph_attr."""
 import copy
 
 import pytest
@@ -11,7 +11,7 @@ pytestmark = pytest.mark.gpu
 import hydragnn_b200 as hb  # noqa: E402
 from hydragnn_b200 import ops  # noqa: E402
 from hydragnn_b200.synthetic import ARCH  # noqa: E402
-from mace_cond_oracle import MACECondOracle  # noqa: E402
+from oracle.mace import MACEOracle  # noqa: E402
 from oracle.mlip import MLIPWrapper  # noqa: E402
 from oracle.workloads import add_edges_cpu  # noqa: E402
 from stack_support import MACE_KW, _gpu_batch, _grad_rel, _loader, mace_batch, random_rotation  # noqa: E402
@@ -111,7 +111,7 @@ def _with_ga(d, gen, g=3, flat=False):
 def _pair(kw, seed=0):
     """Oracle and engine with the same (non-trivial) parameters, the conditioning modules created by a first forward."""
     torch.manual_seed(seed)
-    o = MACECondOracle(**kw)
+    o = MACEOracle(**kw)
     if kw["graph_attr_conditioning_mode"] == "film":
         o._ensure_graph_conditioner(3, torch.device("cpu"))
     elif kw["graph_attr_conditioning_mode"] == "concat_node":
@@ -256,7 +256,7 @@ def test_gfm_mace_shape_mlip_step_with_edge_lengths_matches_oracle():
     torch.manual_seed(0)
     inner = {k: v for k, v in kw.items() if k not in ("mpnn_type", "enable_interatomic_potential", "energy_weight",
                                                        "energy_peratom_weight", "force_weight")}
-    om = MLIPWrapper(MACECondOracle(**inner), 0.0, 1.0, 10.0)
+    om = MLIPWrapper(MACEOracle(**inner), 0.0, 1.0, 10.0)
     em = hb.create_model(**kw)
     torch.manual_seed(7)
     om.model._ensure_graph_concat_projector(2, 128, torch.device("cpu"))

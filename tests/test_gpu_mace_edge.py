@@ -1,6 +1,6 @@
 """GPU tests of MACE with edge attributes (edge_dim = D > 0): the fused first-order kernels (hgb_mace_tp_scatter_{fwd,bwd}
 with edge attributes), the closed mixing primitive of the any-order path (hgb_mace_edge_mix, ops.EdgeMix / EdgeMixT), the
-engine against the fp64 restatement (tests/mace_edge_oracle.py), and hb.train's padded step carrying edge_attr."""
+engine against the fp64 restatement (oracle/mace.py), and hb.train's padded step carrying edge_attr."""
 import copy
 import math
 
@@ -12,7 +12,7 @@ pytestmark = pytest.mark.gpu
 import hydragnn_b200 as hb  # noqa: E402
 from hydragnn_b200 import e3, ops  # noqa: E402
 from hydragnn_b200.synthetic import ARCH, make_samples  # noqa: E402
-from mace_edge_oracle import MACEEdgeOracle  # noqa: E402
+from oracle.mace import MACEOracle  # noqa: E402
 from oracle.mlip import MLIPWrapper  # noqa: E402
 from oracle.workloads import add_edges_cpu, arch_for  # noqa: E402
 from stack_support import MACE_KW, _gpu_batch, _grad_rel, _loader, mace_batch, random_rotation  # noqa: E402
@@ -147,7 +147,7 @@ def test_edge_mix_both_modes_and_derivatives_match_fp64():
 # ---- engine against the fp64 restatement -----------------------------------------------------------------------------
 def _pair(kw, seed=0):
     torch.manual_seed(seed)
-    o = MACEEdgeOracle(**kw)
+    o = MACEOracle(**kw)
     with torch.no_grad():
         for p in o.parameters():
             p.copy_(torch.randn_like(p) * (p.std() if p.numel() > 1 else 1.0))
@@ -258,7 +258,7 @@ def test_oc20_mace_shape_mlip_with_edge_lengths_matches_oracle():
               output_heads={"node": {"num_headlayers": 2, "dim_headlayers": [32, 16], "type": "mlp"}},
               enable_interatomic_potential=True, energy_weight=1.0, energy_peratom_weight=1.0, force_weight=1.0, edge_dim=1)
     torch.manual_seed(0)
-    om = MLIPWrapper(MACEEdgeOracle(**{k: v for k, v in kw.items() if k != "mpnn_type"}), 1.0, 1.0, 1.0)
+    om = MLIPWrapper(MACEOracle(**{k: v for k, v in kw.items() if k != "mpnn_type"}), 1.0, 1.0, 1.0)
     em = hb.create_model(**kw)
     em.model.load_state_dict(om.model.state_dict())
     om.train()

@@ -11,10 +11,10 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import _lib, ops
 from hydragnn_b200.synthetic import ARCH
-from gnll_oracle import Flat
 from kernel_harness import Buf, check_bound, launches, stream, twice
-from prelu_support import MACE_CASES, STACK_CASES, engine, oracle_of
-from stack_support import MODEL_KW, _batch, _loader, _zero_dropout, check_golden_case, golden_data, grad_close, rel_l2
+from oracle.base import oracle_from_case
+from stack_support import (MODEL_KW, PRELU_CASES, PRELU_MACE_CASES, Flat, _batch, _loader, _zero_dropout, case_mpnn_type,
+                           check_golden_case, golden_data, grad_close, prelu_engine, rel_l2)
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -282,12 +282,12 @@ def golden(golden_dir):
 
 
 def _engine(name, c):
-    m = engine(name, c, use_gpu=True)
+    m = prelu_engine(name, c, use_gpu=True)
     m.load_state_dict(c["state"], strict=True)
     return m
 
 
-@pytest.mark.parametrize("name", STACK_CASES)
+@pytest.mark.parametrize("name", PRELU_CASES)
 def test_engine_matches_reference_golden(golden, name):
     """Predictions, loss and every gradient (the slope's summed over every site) of the engine against the reference; the PReLU
     kernels run in the step."""
@@ -310,12 +310,12 @@ def test_engine_matches_reference_golden(golden, name):
         assert "hgb_grouped_linear_prelu" in calls
 
 
-@pytest.mark.parametrize("name", MACE_CASES)
+@pytest.mark.parametrize("name", PRELU_MACE_CASES)
 def test_mace_matches_reference_golden(golden, name):
     """MACE's decoders (and FiLM's conditioner) with the shared PReLU: predictions, the position gradient of the objective and
     every parameter gradient, in eval mode as the MACE goldens are recorded."""
     c = golden[name]
-    m = engine(name, c, use_gpu=True)
+    m = prelu_engine(name, c, use_gpu=True)
     m.eval()
     d = _batch(c["inputs"])
     d.pos.requires_grad_(True)
@@ -338,13 +338,13 @@ def test_mace_matches_reference_golden(golden, name):
 
 
 @pytest.mark.parametrize("precision", ["fp32", "bf16"])
-@pytest.mark.parametrize("name", [n for n in STACK_CASES if n not in ("pna_gps",)])
+@pytest.mark.parametrize("name", [n for n in PRELU_CASES if n not in ("pna_gps",)])
 def test_engine_training_step_matches_fp64_oracle(golden, name, precision):
     """One train-mode step of the engine in fp32 and bf16 (TF32 tensor-core Linears) against the fp64 oracle: predictions, loss
     and all gradients together within 1e-4 (fp32) or 2e-2 (bf16)."""
     c = golden[name]
     em = hb.set_precision(_engine(name, c), precision)
-    om = oracle_of(name, c).train()
+    om = oracle_from_case(case_mpnn_type(name), c).train()
     _zero_dropout(om)
     nll = name == "egnn_gnll"
     if nll:

@@ -6,7 +6,8 @@ import torch
 
 import hydragnn_b200 as hb
 from hydragnn_b200 import _lib, ops
-from stack_support import check_golden_case, engine_kwargs, golden_data, grad_close
+from oracle.base import case_kwargs
+from stack_support import check_golden_case, golden_data, grad_close
 
 pytestmark = pytest.mark.gpu
 
@@ -151,7 +152,7 @@ def _cases(golden_dir, kind):
 
 
 def _engine(kind, c):
-    m = hb.create_model(**engine_kwargs(kind, c))
+    m = hb.create_model(**case_kwargs(kind, c))
     m.load_state_dict(c["state"], strict=True)
     for sub in m.modules():
         if hasattr(sub, "dropout") and isinstance(sub.dropout, float):

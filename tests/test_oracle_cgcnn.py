@@ -9,9 +9,9 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import padded
 from hydragnn_b200.cgcnn import CGCNNStack
-from oracle.base import oracle_from_case
-from oracle.cgcnn import CGCNNStackOracle, CGConv
-from stack_support import check_golden_case, check_seeded_state, engine_kwargs, golden_data, grad_close
+from oracle.base import case_kwargs, oracle_from_case
+from oracle.cgcnn import CGConv
+from stack_support import check_golden_case, check_seeded_state, golden_data, grad_close
 
 CASES = ["cgcnn_graph_edge0", "cgcnn_node_edge_len", "cgcnn_add_pool_edge3", "cgcnn_multihead", "cgcnn_mlp_per_node", "cgcnn_gps",
          "cgcnn_gps_edge2", "cgcnn_ci_width1"]
@@ -85,12 +85,12 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole CGCNN stack (fp64) against the reference's: eval and train-mode predictions, the loss, every parameter
     gradient and the BatchNorm running statistics."""
     c = _golden(golden_dir)[name]
-    check_golden_case(oracle_from_case(CGCNNStackOracle, c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
+    check_golden_case(oracle_from_case("CGCNN", c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
                       grads=grad_close(1e-4, 1e-6))
 
 
 def engine_from_case(c, **kw):
-    return hb.create_model(**engine_kwargs("CGCNN", c), use_gpu=False, **kw)
+    return hb.create_model(**case_kwargs("CGCNN", c), use_gpu=False, **kw)
 
 
 @pytest.mark.parametrize("name", CASES)

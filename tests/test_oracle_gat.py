@@ -9,9 +9,9 @@ import torch
 import hydragnn_b200 as hb
 from hydragnn_b200 import ops, padded
 from hydragnn_b200.gat import GATStack
-from oracle.base import oracle_from_case
-from oracle.gat import GATStackOracle, GATv2Conv
-from stack_support import check_golden_case, engine_kwargs, golden_data, grad_close, seeded_state, state_digest
+from oracle.base import case_kwargs, oracle_from_case
+from oracle.gat import GATv2Conv
+from stack_support import check_golden_case, golden_data, grad_close, seeded_state, state_digest
 
 CASES = ["gat_graph_noedge", "gat_node_edge_len", "gat_multihead", "gat_add_pool_edge3", "gat_one_layer", "gat_input_ne_hidden",
          "gat_conv_head", "gat_gps", "gat_gps_edge2", "gat_loops_dups_isolated"]
@@ -114,12 +114,12 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     c = _golden(golden_dir)[name]
     # the golden is the reference's fp32 arithmetic: the 120-wide head convs of gat_conv_head put its loss 1.2e-6 from fp64, and a
     # conv bias in front of a BatchNorm, which has no gradient in exact arithmetic, holds up to 1.1e-6 gmax there
-    check_golden_case(oracle_from_case(GATStackOracle, c, seeded_state(c)), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
+    check_golden_case(oracle_from_case("GAT", c, seeded_state(c)), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
                       loss=(5e-6, 0), grads=grad_close(1e-4, 2e-6))
 
 
 def engine_from_case(c, **kw):
-    return hb.create_model(**engine_kwargs("GAT", c), use_gpu=False, **kw)
+    return hb.create_model(**case_kwargs("GAT", c), use_gpu=False, **kw)
 
 
 @pytest.mark.parametrize("name", CASES)

@@ -6,8 +6,9 @@ import torch
 
 import hydragnn_b200 as hb
 from hydragnn_b200 import ops
-from gnll_oracle import CASES, Flat, case_kwargs, oracle_of
-from stack_support import check_golden_case, check_seeded_state, golden_data, grad_close
+from oracle.base import oracle_from_case
+from stack_support import (GNLL_CASES, Flat, case_mpnn_type, check_golden_case, check_seeded_state, golden_data, grad_close,
+                           named_case_kwargs)
 
 
 @pytest.fixture(scope="module")
@@ -15,7 +16,7 @@ def golden(golden_dir):
     return torch.load(golden_dir + "/models_gnll.pt")
 
 
-@pytest.mark.parametrize("name", [n for n in CASES if n != "pna_gps"])
+@pytest.mark.parametrize("name", [n for n in GNLL_CASES if n != "pna_gps"])
 def test_oracle_matches_reference_golden(golden, name):
     """The fp64 oracle against the reference: eval and train-mode means and variances, the NLL, every parameter gradient and the
     BatchNorm statistics after the step.  (pna_gps runs the reference's gps.py, which the oracle does not restate.)"""
@@ -23,16 +24,16 @@ def test_oracle_matches_reference_golden(golden, name):
     # the conv head ends in BatchNorm + ReLU, so about half its variances are exactly 0 and clamped to eps: the fp32 reference's
     # gradients then carry terms of (mean - target) / eps, and their rounding sets the bound
     atol = 1e-5 if name == "pna_conv_head" else 1e-6
-    check_golden_case(Flat(oracle_of(name, c)), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
-                      grads=grad_close(1e-4, atol))
+    check_golden_case(Flat(oracle_from_case(case_mpnn_type(name), c)), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
+                      loss=(1e-6, 0), grads=grad_close(1e-4, atol))
 
 
-@pytest.mark.parametrize("name", [n for n in CASES if n != "egnn_clamped"])
+@pytest.mark.parametrize("name", [n for n in GNLL_CASES if n != "egnn_clamped"])
 def test_engine_reproduces_the_reference_seeded_state(golden, name):
     """Head widths doubled at every site (graph heads, mlp / mlp_per_node, conv heads and their BatchNorms), initial_bias over
     all 2 d entries: the engine's seeded state dict equals the reference's key for key and value for value."""
     c = golden[name]
-    m = hb.create_model(**case_kwargs(name, c), use_gpu=False)
+    m = hb.create_model(**named_case_kwargs(name, c), use_gpu=False)
     assert m.var_output == 1 and m.loss_function_type == "GaussianNLLLoss"
     check_seeded_state(m, c["state"])
 

@@ -1,11 +1,11 @@
-"""CPU tests of MACE graph-attribute conditioning: the fp64 restatement (tests/mace_cond_oracle.py) against
+"""CPU tests of MACE graph-attribute conditioning: the fp64 restatement (oracle/mace.py) against
 tests/golden/models_mace_cond.pt, which comes from the reference's own MACEStack (tests/golden/make_mace_cond_golden.py), and
 the engine's lazily created modules, checkpoints and refusals -- all before any kernel runs."""
 import pytest
 import torch
 
 import hydragnn_b200 as hb
-from mace_cond_oracle import MACECondOracle
+from oracle.mace import MACEOracle
 from stack_support import MACE_KW
 
 
@@ -40,7 +40,7 @@ def _ga_dim(c):
 def test_cond_oracle_matches_the_reference_own_code_golden(golden_dir):
     for name, c in _cases(golden_dir):
         torch.manual_seed(0)
-        m = MACECondOracle(**dict(MACE_KW, **c["cfg"]))
+        m = MACEOracle(**dict(MACE_KW, **c["cfg"]))
         m.eval()
         d = _batch(c)
         d.pos.requires_grad_(True)
@@ -111,7 +111,7 @@ def test_conditioned_checkpoints_load_strictly_both_ways(golden_dir):
         fresh = _engine(c["cfg"])
         _ensure_as_load_existing_model(fresh, c["state"])
         fresh.load_state_dict(c["state"], strict=True)
-        o = MACECondOracle(**dict(MACE_KW, **c["cfg"]))
+        o = MACEOracle(**dict(MACE_KW, **c["cfg"]))
         _ensure_as_load_existing_model(o, fresh.state_dict())
         o.load_state_dict(fresh.state_dict(), strict=True)
         for k, v in o.state_dict().items():

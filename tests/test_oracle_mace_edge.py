@@ -1,4 +1,4 @@
-"""CPU tests of MACE with edge attributes (edge_dim > 0): the fp64 restatement (tests/mace_edge_oracle.py) against
+"""CPU tests of MACE with edge attributes (edge_dim > 0): the fp64 restatement (oracle/mace.py) against
 tests/golden/models_mace_edge.pt, which comes from the reference's own MACEStack (tests/golden/make_mace_edge_golden.py),
 and the engine's initialisation against the same golden."""
 import pytest
@@ -6,7 +6,7 @@ import torch
 
 import hydragnn_b200 as hb
 from hydragnn_b200 import padded
-from mace_edge_oracle import MACEEdgeOracle
+from oracle.mace import MACEOracle
 from stack_support import MACE_KW, mace_batch, random_rotation
 
 
@@ -17,7 +17,7 @@ def _golden(golden_dir):
 def test_edge_oracle_matches_the_reference_own_code_golden(golden_dir):
     for name, c in _golden(golden_dir).items():
         torch.manual_seed(0)
-        m = MACEEdgeOracle(**dict(MACE_KW, **c["cfg"]))
+        m = MACEOracle(**dict(MACE_KW, **c["cfg"]))
         sd = m.state_dict()
         assert list(sd.keys()) == list(c["state"].keys()), name
         for k, v in sd.items():
@@ -42,7 +42,7 @@ def test_edge_oracle_matches_the_reference_own_code_golden(golden_dir):
 
 def test_edge_oracle_with_lengths_is_rotation_invariant():
     torch.manual_seed(0)
-    m = MACEEdgeOracle(**dict(MACE_KW, edge_dim=1)).double()
+    m = MACEOracle(**dict(MACE_KW, edge_dim=1)).double()
     gen = torch.Generator().manual_seed(3)
     d = mace_batch(gen)
     d.edge_attr = (d.pos[d.edge_index[1]] - d.pos[d.edge_index[0]]).norm(dim=1, keepdim=True)

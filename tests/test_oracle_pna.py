@@ -11,7 +11,7 @@ import torch
 
 from hydragnn_b200.pna import AGGREGATORS, SCALERS, PNAStack
 from oracle.base import oracle_from_case
-from oracle.pna import PNAConv, PNAStackOracle
+from oracle.pna import PNAConv
 from stack_support import check_golden_case, check_seeded_state, golden_data, grad_close
 
 # nodes 0..4, x = [1, 2, 4, 8, 16]; edges (source -> target): 1->0, 2->0 (two into 0), 0->3 (one), 2->4 twice (a tie);
@@ -114,7 +114,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     """The oracle's whole PNA stack (fp64) against the reference's PNAStack.py + Base.py: eval and train-mode predictions, the loss,
     every parameter gradient and the BatchNorm running statistics after the step.  (GPS is the reference's gps.py, not restated.)"""
     c = torch.load(golden_dir + "/models_pna.pt")[name]
-    check_golden_case(oracle_from_case(PNAStackOracle, c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
+    check_golden_case(oracle_from_case("PNA", c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0),
                       grads=grad_close(1e-4, 1e-6))
 
 

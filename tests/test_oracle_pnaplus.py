@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle.base import oracle_from_case
-from oracle.pnaplus import BesselBasisLayer, Envelope, PNAPlusStackOracle
+from oracle.pnaplus import BesselBasisLayer, Envelope
 from stack_support import check_golden_case, check_grads, check_seeded_state, golden_data, grad_close
 
 CASES = ["pnaplus_graph_noedge", "pnaplus_node_edge_len", "pnaplus_multihead_h5", "pnaplus_gps", "pnaplus_edge_dim0",
@@ -102,7 +102,7 @@ def test_oracle_stack_matches_reference_golden(golden_dir, name):
     pos, ei = c["inputs"]["pos"], c["inputs"]["edge_index"]
     dist = (pos[ei[1]] - pos[ei[0]]).norm(dim=-1)
     assert float(dist.max()) > c["cfg"]["radius"] > float(dist.min())                    # edges on both sides of the cutoff
-    check_golden_case(oracle_from_case(PNAPlusStackOracle, c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
+    check_golden_case(oracle_from_case("PNAPlus", c), c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5),
                       loss=(1e-6, 0), grads=grad_close(1e-4, 1e-6))
 
 
@@ -116,7 +116,7 @@ def test_edge_dim0_keeps_an_unused_edge_encoder(golden_dir):
 def test_oracle_mlip_matches_reference_golden(golden_dir):
     """Energy + per-atom energy + force loss in eval mode: forces and the second-order parameter gradients."""
     c = torch.load(golden_dir + "/models_pnaplus.pt")["pnaplus_mlip"]
-    m = oracle_from_case(PNAPlusStackOracle, c)
+    m = oracle_from_case("PNAPlus", c)
     m.eval()
     d = golden_data(c["inputs"])
     d.pos.requires_grad_(True)

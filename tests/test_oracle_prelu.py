@@ -9,21 +9,21 @@ from torch import nn
 import hydragnn_b200 as hb
 from hydragnn_b200 import ops
 from hydragnn_b200.stacks import activation_function_selection
-from gnll_oracle import Flat
-from prelu_support import MACE_CASES, STACK_CASES, case_kwargs, engine, oracle_of
-from stack_support import check_golden_case, check_seeded_state, golden_data, grad_close
+from oracle.base import oracle_from_case
+from stack_support import (PRELU_CASES, PRELU_MACE_CASES, Flat, case_mpnn_type, check_golden_case, check_seeded_state, golden_data,
+                           grad_close, named_case_kwargs, prelu_engine)
 
 @pytest.fixture(scope="module")
 def golden(golden_dir):
     return torch.load(golden_dir + "/models_prelu.pt")
 
 
-@pytest.mark.parametrize("name", [n for n in STACK_CASES if n != "pna_gps"])
+@pytest.mark.parametrize("name", [n for n in PRELU_CASES if n != "pna_gps"])
 def test_oracle_matches_reference_golden(golden, name):
     """The fp64 oracle against the reference: predictions, loss, every gradient (the shared slope's included, summed over every
     site) and the BatchNorm statistics.  (pna_gps runs the reference's gps.py, which the oracle does not restate.)"""
     c = golden[name]
-    m = oracle_of(name, c)
+    m = oracle_from_case(case_mpnn_type(name), c)
     # the reference names the shared slope where named_parameters first meets it, inside the first head; the oracle registers it
     # on the model first: its gradient is the same sum over every site under another name
     own = dict(m.named_parameters())
@@ -37,12 +37,12 @@ def test_oracle_matches_reference_golden(golden, name):
     check_golden_case(m, c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0), grads=tol)
 
 
-@pytest.mark.parametrize("name", STACK_CASES + ["mace"])
+@pytest.mark.parametrize("name", PRELU_CASES + ["mace"])
 def test_engine_reproduces_the_reference_seeded_state(golden, name):
     """Names, order and values of the engine's seeded state dict equal the reference's, every alias of the one slope included;
     the reference's state loads strictly and comes back unchanged."""
     c = golden[name]
-    m = engine(name, c)
+    m = prelu_engine(name, c)
     assert list(m.state_dict()) == c["keys"]
     if name != "mace":
         check_seeded_state(m, c["state"])
@@ -57,16 +57,16 @@ def test_mace_film_keys_after_the_conditioner_exists(golden):
     """FiLM's graph_conditioner (created at the first forward) holds the shared PReLU: the reference lists it there, after every
     other entry.  The engine builds the same conditioner: its entries come in the same order and hold the same slope tensor."""
     c = golden["mace_film"]
-    m = engine("mace_film", c)
+    m = prelu_engine("mace_film", c)
     m._ensure_graph_conditioner(2, torch.device("cpu"))
     assert list(m.state_dict()) == c["keys"]
     assert m.graph_conditioner[1] is m.activation_function
 
 
-@pytest.mark.parametrize("name", STACK_CASES + MACE_CASES)
+@pytest.mark.parametrize("name", PRELU_CASES + PRELU_MACE_CASES)
 def test_one_slope_tensor_behind_every_alias(golden, name):
     c = golden[name]
-    m = engine(name, c)
+    m = prelu_engine(name, c)
     if name == "mace_film":
         m._ensure_graph_conditioner(2, torch.device("cpu"))
     sd = m.state_dict(keep_vars=True)
@@ -82,15 +82,15 @@ def test_no_reference_refusals(golden):
     assert golden["errors"] == {}
 
 
-@pytest.mark.parametrize("name", STACK_CASES + ["mace"])
+@pytest.mark.parametrize("name", PRELU_CASES + ["mace"])
 def test_str_and_strict_loads_both_ways(golden, name):
     c = golden[name]
-    m = engine(name, c)
-    relu = hb.create_model(**dict(case_kwargs(name, c), activation_function="relu"), use_gpu=False)
+    m = prelu_engine(name, c)
+    relu = hb.create_model(**dict(named_case_kwargs(name, c), activation_function="relu"), use_gpu=False)
     assert str(m) == str(relu)
     m.load_state_dict(c["state"], strict=True)
     sd = m.state_dict()
-    fresh = engine(name, c)
+    fresh = prelu_engine(name, c)
     fresh.load_state_dict(sd, strict=True)
     assert all(torch.equal(v, fresh.state_dict()[k]) for k, v in sd.items())
 

@@ -4,7 +4,7 @@ import pytest
 import torch
 
 from oracle.base import oracle_from_case
-from oracle.sage import MFCStackOracle, MFConv, SAGEConv, SAGEStackOracle
+from oracle.sage import MFConv, SAGEConv
 from stack_support import check_golden_case, golden_data, grad_close
 
 SAGE_CASES = ["sage_graph", "sage_node", "sage_multihead", "sage_mlp_per_node", "sage_conv_head", "sage_max_pool_in1", "sage_gps",
@@ -63,20 +63,15 @@ def _check(m, c):
     check_golden_case(m, c, lambda: golden_data(c["inputs"]), pred=(1e-6, 1e-5), loss=(1e-6, 0), grads=grad_close(1e-4, 1e-6))
 
 
-def _oracle(cls, c):
-    case = dict(c, cfg={k: v for k, v in c["cfg"].items() if k != "initial_bias"})
-    return oracle_from_case(cls, case)
-
-
 @pytest.mark.parametrize("name", SAGE_CASES)
 def test_sage_oracle_stack_matches_reference_golden(golden_dir, name):
-    _check(_oracle(SAGEStackOracle, _golden(golden_dir, "sage")[name]), _golden(golden_dir, "sage")[name])
+    _check(oracle_from_case("SAGE", _golden(golden_dir, "sage")[name]), _golden(golden_dir, "sage")[name])
 
 
 @pytest.mark.parametrize("name", MFC_CASES)
 def test_mfc_oracle_stack_matches_reference_golden(golden_dir, name):
     c = _golden(golden_dir, "mfc")[name]
-    _check(_oracle(MFCStackOracle, c), c)
+    _check(oracle_from_case("MFC", c), c)
 
 
 def test_golden_graphs_cover_the_degree_corner_cases(golden_dir):

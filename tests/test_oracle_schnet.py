@@ -68,5 +68,5 @@ def test_oracle_stack_matches_the_reference(golden_dir, name):
     parameter gradient."""
     case = torch.load(golden_dir + "/models_schnet.pt")[name]
     # norm-wise gradients: a bias followed by BatchNorm has a zero true gradient, the reference's fp32 value there is rounding noise
-    check_golden_case(oracle_from_case(so.SCFStackOracle, case), case, lambda: golden_data(case["inputs"]), pred=(1e-5, 1e-5),
+    check_golden_case(oracle_from_case("SchNet", case), case, lambda: golden_data(case["inputs"]), pred=(1e-5, 1e-5),
                       loss=(1e-5, 0), grads=grad_norm(1e-4, 1e-6))
