@@ -300,9 +300,96 @@ __device__ __forceinline__ void poly_cutoff(float d, float rc, float p, float& e
   denv = (-a * p * xm + b * (p + 1.f) * xp - c * (p + 2.f) * xp * x) / rc;
 }
 
-__global__ void mace_edge_embed_fwd_kernel(const float* __restrict__ pos, const int32_t* __restrict__ row, const int32_t* __restrict__ col,
-                                           const float* __restrict__ shifts, int64_t e, int lmax, int nb, float rc, float p,
-                                           float* __restrict__ sh, float* __restrict__ radial) {
+// ---- distance transforms (mace_utils/modules/radial.py:151-245; blocks.py:141-177) ------------------------------------
+// t = T(d, r0_e) with r0_e from the covalent radii of the edge's two elements.  radii [119] (index = atomic number Z, the
+// element index z + 1) and the parameters are device buffers of the model, read at run time: a loaded state dict or an
+// optimiser-free in-place change reaches a captured step.
+//   Agnesi (c0 = q, c1 = p, c2 = a):  r0 = (R_u + R_v) / 2,  u = d / r0,  T = 1 / (1 + a u^q / (1 + u^(q-p)))
+//   Soft   (c0 = a, c1 = b):          r0 = (R_u + R_v) / 4,  u = d / r0,  T = d + tanh(-u - a u^b) / 2 + 1 / 2
+// dt_eval returns T, T' = dT/dd and (ORDER 2) T'' for one edge.  Agnesi is evaluated as f = a u^q sigma_w with the smaller
+// of u^(q-p) and u^(p-q) in the denominator, so u^(q-p) never overflows: at d -> 0 T -> 1, T' -> 0, T'' -> 0, all finite.
+constexpr int DT_RADII = 119;
+
+__device__ __forceinline__ float dt_radius(const float* sr, const int64_t* __restrict__ z, int node) {
+  const int64_t k = z[node];
+  return sr[1 + (int)(k < 0 ? 0 : (k > DT_RADII - 2 ? DT_RADII - 2 : k))];   // element index 0..117 -> Z 1..118
+}
+
+template <int ORDER>
+__device__ __forceinline__ void dt_eval(int kind, float d, float rsum, float c0, float c1, float c2, float& t, float& t1, float& t2) {
+  if (kind == HGB_DT_AGNESI) {
+    const float q = c0, p = c1, a = c2, r0 = 0.5f * rsum;
+    const float u = d / r0;
+    // sig = 1 / (1 + u^(p-q)) = u^(q-p) / (1 + u^(q-p)) and f / u^k = a u^(q-k) / (1 + u^(q-p)), k = 0, 1, 2
+    float sig, f, fu1, fu2;
+    if ((q - p) * logf(u) > 0.f) {               // u^(q-p) > 1 (small u): divide through by it
+      const float s = powf(u, p - q);
+      sig = 1.f / (1.f + s);
+      f = a * powf(u, p) * sig;
+      fu1 = a * powf(u, p - 1.f) * sig;
+      fu2 = a * powf(u, p - 2.f) * sig;
+    } else {
+      const float w = powf(u, q - p), den = 1.f / (1.f + w);
+      sig = w * den;
+      f = a * powf(u, q) * den;
+      fu1 = a * powf(u, q - 1.f) * den;
+      fu2 = a * powf(u, q - 2.f) * den;
+    }
+    const float tt = 1.f / (1.f + f);
+    const float g = q + (p - q) * sig;            // u f_u / f
+    const float fd = fu1 * g / r0;                // df/dd
+    t = tt;
+    t1 = -tt * tt * fd;
+    if (ORDER >= 2) {
+      const float fdd = fu2 * (g * g - g - (p - q) * (p - q) * sig * (1.f - sig)) / (r0 * r0);
+      t2 = tt * tt * (2.f * tt * fd * fd - fdd);
+    }
+  } else {
+    const float a = c0, b = c1, r0 = 0.25f * rsum;
+    const float u = d / r0;
+    const float v = -u - a * powf(u, b);
+    const float ev = expf(-2.f * fabsf(v));       // tanh and sech^2 from exp(-2|v|): no cancellation in 1 -/+ tanh
+    const float inv1 = 1.f / (1.f + ev);
+    const float th = copysignf((1.f - ev) * inv1, v);
+    const float sech2 = 4.f * ev * inv1 * inv1;
+    t = d + (v < 0.f ? ev * inv1 : inv1);         // d + (1 + tanh v) / 2
+    if (sech2 > 0.f) {                            // else tanh is flat: T' = 1, T'' = 0 (never 0 * inf)
+      const float dv = -(1.f + a * b * powf(u, b - 1.f)) / r0;
+      t1 = fmaf(0.5f * sech2, dv, 1.f);
+      if (ORDER >= 2) t2 = 0.5f * sech2 * (-a * b * (b - 1.f) * powf(u, b - 2.f) / (r0 * r0) - 2.f * th * dv * dv);
+    } else {
+      t1 = 1.f;
+      if (ORDER >= 2) t2 = 0.f;
+    }
+  }
+}
+
+// transform operands of one launch: kind 0 = none (the original kernels), else the radii table staged in shared memory
+struct DtArgs {
+  int kind;
+  const int64_t* z;
+  const float* radii;
+  const float* c0;
+  const float* c1;
+  const float* c2;
+};
+
+__device__ __forceinline__ void dt_stage(const DtArgs& ta, float* sr, float& c0, float& c1, float& c2) {
+  for (int q = threadIdx.x; q < DT_RADII; q += blockDim.x) sr[q] = ta.radii[q];
+  c0 = *ta.c0;
+  c1 = *ta.c1;
+  c2 = ta.kind == HGB_DT_AGNESI ? *ta.c2 : 0.f;
+  __syncthreads();
+}
+
+// Bessel basis (of t = d, or of the transformed length) times the polynomial cutoff of the raw d, blocks.py:172-177
+template <bool DT>
+__device__ __forceinline__ void edge_embed_fwd_body(const float* __restrict__ pos, const int32_t* __restrict__ row,
+                                                    const int32_t* __restrict__ col, const float* __restrict__ shifts, int64_t e,
+                                                    int lmax, int nb, float rc, float p, const DtArgs& ta, float* sr,
+                                                    float* __restrict__ sh, float* __restrict__ radial) {
+  float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+  if (DT) dt_stage(ta, sr, c0, c1, c2);
   const int ns = (lmax + 1) * (lmax + 1);
   const float pref = sqrtf(2.f / rc);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (int64_t)gridDim.x * blockDim.x) {
@@ -315,14 +402,24 @@ __global__ void mace_edge_embed_fwd_kernel(const float* __restrict__ pos, const 
     for (int k = 0; k < ns; ++k) sh[i * ns + k] = s[k];
     float env, denv;
     poly_cutoff(d, rc, p, env, denv);
-    for (int n = 0; n < nb; ++n) radial[i * nb + n] = pref * sinf((float)(n + 1) * HGB_PI_F / rc * d) * inv * env;
+    float t = d, tinv = inv;
+    if (DT) {
+      float t1, t2;
+      dt_eval<1>(ta.kind, d, dt_radius(sr, ta.z, row[i]) + dt_radius(sr, ta.z, col[i]), c0, c1, c2, t, t1, t2);
+      tinv = 1.f / t;
+    }
+    for (int n = 0; n < nb; ++n) radial[i * nb + n] = pref * sinf((float)(n + 1) * HGB_PI_F / rc * t) * tinv * env;
   }
 }
 
-__global__ void mace_edge_embed_bwd_kernel(const float* __restrict__ pos, const int32_t* __restrict__ row, const int32_t* __restrict__ col,
-                                           const float* __restrict__ shifts, const float* __restrict__ g_sh,
-                                           const float* __restrict__ g_radial, int64_t e, int lmax, int nb, float rc, float p,
-                                           float* __restrict__ g_vec) {
+template <bool DT>
+__device__ __forceinline__ void edge_embed_bwd_body(const float* __restrict__ pos, const int32_t* __restrict__ row,
+                                                    const int32_t* __restrict__ col, const float* __restrict__ shifts,
+                                                    const float* __restrict__ g_sh, const float* __restrict__ g_radial, int64_t e,
+                                                    int lmax, int nb, float rc, float p, const DtArgs& ta, float* sr,
+                                                    float* __restrict__ g_vec) {
+  float c0 = 0.f, c1 = 0.f, c2 = 0.f;
+  if (DT) dt_stage(ta, sr, c0, c1, c2);
   const int ns = (lmax + 1) * (lmax + 1);
   const float pref = sqrtf(2.f / rc);
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (int64_t)gridDim.x * blockDim.x) {
@@ -346,18 +443,67 @@ __global__ void mace_edge_embed_bwd_kernel(const float* __restrict__ pos, const 
     if (g_radial) {
       float env, denv;
       poly_cutoff(d, rc, p, env, denv);
+      float t = d, tinv = inv, t1 = 1.f;
+      if (DT) {
+        float t2;
+        dt_eval<1>(ta.kind, d, dt_radius(sr, ta.z, row[i]) + dt_radius(sr, ta.z, col[i]), c0, c1, c2, t, t1, t2);
+        tinv = 1.f / t;
+      }
       float gd = 0.f;
       for (int n = 0; n < nb; ++n) {
         const float w = (float)(n + 1) * HGB_PI_F / rc;
         float sn, cs;
-        sincosf(w * d, &sn, &cs);
-        const float bes = pref * sn * inv;
-        const float dbes = pref * (w * cs * inv - sn * inv * inv);
-        gd = fmaf(g_radial[i * nb + n], dbes * env + bes * denv, gd);
+        sincosf(w * t, &sn, &cs);
+        const float bes = pref * sn * tinv;
+        const float dbes = pref * (w * cs * tinv - sn * tinv * tinv);
+        // chain term basis'(t) T'(d) cutoff(d) (zero where the cutoff is) + basis(t) cutoff'(d)
+        gd = fmaf(g_radial[i * nb + n], (DT ? dbes * t1 : dbes) * env + bes * denv, gd);
       }
       gx = fmaf(gd, ux, gx); gy = fmaf(gd, uy, gy); gz = fmaf(gd, uz, gz);
     }
     g_vec[3 * i] = gx; g_vec[3 * i + 1] = gy; g_vec[3 * i + 2] = gz;
+  }
+}
+
+__global__ void mace_edge_embed_fwd_kernel(const float* __restrict__ pos, const int32_t* __restrict__ row, const int32_t* __restrict__ col,
+                                           const float* __restrict__ shifts, int64_t e, int lmax, int nb, float rc, float p,
+                                           float* __restrict__ sh, float* __restrict__ radial) {
+  edge_embed_fwd_body<false>(pos, row, col, shifts, e, lmax, nb, rc, p, DtArgs{}, nullptr, sh, radial);
+}
+
+__global__ void mace_edge_embed_bwd_kernel(const float* __restrict__ pos, const int32_t* __restrict__ row, const int32_t* __restrict__ col,
+                                           const float* __restrict__ shifts, const float* __restrict__ g_sh,
+                                           const float* __restrict__ g_radial, int64_t e, int lmax, int nb, float rc, float p,
+                                           float* __restrict__ g_vec) {
+  edge_embed_bwd_body<false>(pos, row, col, shifts, g_sh, g_radial, e, lmax, nb, rc, p, DtArgs{}, nullptr, g_vec);
+}
+
+__global__ void mace_edge_embed_dt_fwd_kernel(const float* __restrict__ pos, const int32_t* __restrict__ row, const int32_t* __restrict__ col,
+                                              const float* __restrict__ shifts, int64_t e, int lmax, int nb, float rc, float p, DtArgs ta,
+                                              float* __restrict__ sh, float* __restrict__ radial) {
+  __shared__ float sr[DT_RADII];
+  edge_embed_fwd_body<true>(pos, row, col, shifts, e, lmax, nb, rc, p, ta, sr, sh, radial);
+}
+
+__global__ void mace_edge_embed_dt_bwd_kernel(const float* __restrict__ pos, const int32_t* __restrict__ row, const int32_t* __restrict__ col,
+                                              const float* __restrict__ shifts, const float* __restrict__ g_sh,
+                                              const float* __restrict__ g_radial, int64_t e, int lmax, int nb, float rc, float p, DtArgs ta,
+                                              float* __restrict__ g_vec) {
+  __shared__ float sr[DT_RADII];
+  edge_embed_bwd_body<true>(pos, row, col, shifts, g_sh, g_radial, e, lmax, nb, rc, p, ta, sr, g_vec);
+}
+
+// out[i] = (g ? g[i] : 1) * T^(order)(d[i]) for order 0, 1, 2
+__global__ void mace_dist_transform_kernel(int order, const float* __restrict__ d, const float* __restrict__ g, const int32_t* __restrict__ row,
+                                           const int32_t* __restrict__ col, int64_t e, DtArgs ta, float* __restrict__ out) {
+  __shared__ float sr[DT_RADII];
+  float c0, c1, c2;
+  dt_stage(ta, sr, c0, c1, c2);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < e; i += (int64_t)gridDim.x * blockDim.x) {
+    float t, t1, t2 = 0.f;
+    dt_eval<2>(ta.kind, d[i], dt_radius(sr, ta.z, row[i]) + dt_radius(sr, ta.z, col[i]), c0, c1, c2, t, t1, t2);
+    const float v = order == 0 ? t : (order == 1 ? t1 : t2);
+    out[i] = g ? g[i] * v : v;
   }
 }
 
@@ -383,5 +529,52 @@ extern "C" int hgb_mace_edge_embed_bwd(const float* pos, const int32_t* row, con
   mace_edge_embed_bwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, g_sh, g_radial, e, lmax, num_bessel,
                                                                                     r_max, p, g_vec);
   HGB_LAUNCH_CHECK("mace_edge_embed_bwd");
+  return HGB_OK;
+}
+
+static bool dt_args_ok(int32_t kind, const int64_t* z, const float* radii, const float* c0, const float* c1, const float* c2) {
+  return (kind == HGB_DT_AGNESI || kind == HGB_DT_SOFT) && z && radii && c0 && c1 && (kind != HGB_DT_AGNESI || c2);
+}
+
+extern "C" int hgb_mace_edge_embed_dt_fwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const int64_t* z,
+                                          int64_t e, int32_t lmax, int32_t num_bessel, float r_max, float p, int32_t kind,
+                                          const float* radii, const float* c0, const float* c1, const float* c2, float* sh, float* radial,
+                                          hgb_stream_t stream) {
+  HGB_REQUIRE(e >= 0 && lmax >= 0 && lmax <= 3 && num_bessel >= 1 && num_bessel <= 64 && r_max > 0.f &&
+                  (kind == HGB_DT_AGNESI || kind == HGB_DT_SOFT),
+              "mace_edge_embed_dt_fwd: bad arguments");
+  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(pos && row && col && sh && radial && dt_args_ok(kind, z, radii, c0, c1, c2), "mace_edge_embed_dt_fwd: bad arguments");
+  mace_edge_embed_dt_fwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, e, lmax, num_bessel, r_max, p,
+                                                                                       DtArgs{kind, z, radii, c0, c1, c2}, sh, radial);
+  HGB_LAUNCH_CHECK("mace_edge_embed_dt_fwd");
+  return HGB_OK;
+}
+
+extern "C" int hgb_mace_edge_embed_dt_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const int64_t* z,
+                                          const float* g_sh, const float* g_radial, int64_t e, int32_t lmax, int32_t num_bessel, float r_max,
+                                          float p, int32_t kind, const float* radii, const float* c0, const float* c1, const float* c2,
+                                          float* g_vec, hgb_stream_t stream) {
+  HGB_REQUIRE(e >= 0 && lmax >= 0 && lmax <= 3 && num_bessel >= 1 && num_bessel <= 64 && r_max > 0.f &&
+                  (kind == HGB_DT_AGNESI || kind == HGB_DT_SOFT),
+              "mace_edge_embed_dt_bwd: bad arguments");
+  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(pos && row && col && g_vec && dt_args_ok(kind, z, radii, c0, c1, c2), "mace_edge_embed_dt_bwd: bad arguments");
+  mace_edge_embed_dt_bwd_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(pos, row, col, shifts, g_sh, g_radial, e, lmax,
+                                                                                       num_bessel, r_max, p, DtArgs{kind, z, radii, c0, c1, c2},
+                                                                                       g_vec);
+  HGB_LAUNCH_CHECK("mace_edge_embed_dt_bwd");
+  return HGB_OK;
+}
+
+extern "C" int hgb_mace_dist_transform(int32_t order, int32_t kind, const float* d, const float* g, const int32_t* row, const int32_t* col,
+                                       const int64_t* z, const float* radii, const float* c0, const float* c1, const float* c2, int64_t e,
+                                       float* out, hgb_stream_t stream) {
+  HGB_REQUIRE(e >= 0 && order >= 0 && order <= 2 && (kind == HGB_DT_AGNESI || kind == HGB_DT_SOFT), "mace_dist_transform: bad arguments");
+  if (e == 0) return HGB_OK;
+  HGB_REQUIRE(d && row && col && out && dt_args_ok(kind, z, radii, c0, c1, c2), "mace_dist_transform: bad arguments");
+  mace_dist_transform_kernel<<<hgb_grid_for(e, 256), 256, 0, (cudaStream_t)stream>>>(order, d, g, row, col, e, DtArgs{kind, z, radii, c0, c1, c2},
+                                                                                    out);
+  HGB_LAUNCH_CHECK("mace_dist_transform");
   return HGB_OK;
 }

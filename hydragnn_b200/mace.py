@@ -12,6 +12,10 @@ correlation-2 symmetric contraction are the fused kernels of hgb_mace.cu (``ops.
 spherical harmonics and the radial basis are ATen elementwise glue on [E, 9]-sized tensors.  Any-order path (MLIP double
 backward), correlation 3 and channel counts that are not a multiple of 32: the per-path coupling and the contraction are
 composed from gathers / segment sums / MatMuls plus ATen einsum glue.
+
+Distance transforms (``distance_transform`` "Agnesi" / "Soft", radial.py:151-245): the radial basis reads T(d, r0) of the
+covalent radii of the edge's two elements, the cutoff the raw d.  First order with Bessel radials: inside the fused edge
+embedding (``ops.MaceEdgeEmbedDtFn``); otherwise ``ops.DistTransformFn`` (T, with T' and T'' as its closed derivatives).
 """
 import math
 
@@ -19,6 +23,7 @@ import torch
 from torch import nn
 
 from . import e3, ops
+from .covalent_radii import covalent_radii_tensor
 from .stacks import (ELEMENT_CSR, Base, apply_act, cached, decode_branches, graph_head_mlp, graph_shared_mlp, graph_sum,
                      remember, run_mlp)
 
@@ -352,8 +357,6 @@ class MACEStack(Base):
         # refused before Base.__init__, which would build the GPS embeddings first
         if kwargs.get("global_attn_engine"):
             raise ValueError("b200 engine: MACE inside GPS is not implemented")
-        if distance_transform in ("Agnesi", "Soft"):
-            raise ValueError("b200 engine: MACE distance transforms need ase covalent radii and are not implemented")
         if max_ell > 3:
             raise ValueError("b200 engine: MACE max_ell <= 3")
         if kwargs.get("loss_function_type") == "GaussianNLLLoss":
@@ -389,7 +392,7 @@ class MACEStack(Base):
         self.register_buffer("r_max", torch.tensor(float(r_max)))
         self.register_buffer("num_interactions", torch.tensor(num_conv_layers, dtype=torch.int64))
         self.radial_embedding = nn.Module()
-        self.radial_embedding.bessel_fn, self.radial_embedding.cutoff_fn = nn.Module(), nn.Module()
+        self.radial_embedding.bessel_fn = nn.Module()
         bf = self.radial_embedding.bessel_fn
         if self.radial_type == "bessel":
             bf.register_buffer("bessel_weights", math.pi / r_max * torch.linspace(1.0, num_bessel, num_bessel))
@@ -399,6 +402,22 @@ class MACEStack(Base):
             bf.register_buffer("gaussian_weights", torch.linspace(0.0, r_max, num_bessel))
         else:
             bf.register_buffer("n", torch.arange(1, num_bessel + 1, dtype=torch.get_default_dtype()).unsqueeze(0))
+        # AgnesiTransform / SoftTransform (radial.py:151-245) for the exact strings only, registered between the basis and the
+        # cutoff as RadialEmbeddingBlock does (blocks.py:154-159); any other value means no transform.  Buffers, never trained.
+        self.distance_transform = distance_transform if distance_transform in ops.DIST_TRANSFORMS else None
+        if self.distance_transform is not None:
+            dt, fp = nn.Module(), torch.get_default_dtype()
+            if self.distance_transform == "Agnesi":
+                dt.register_buffer("q", torch.tensor(0.9183, dtype=fp))
+                dt.register_buffer("p", torch.tensor(4.5791, dtype=fp))
+                dt.register_buffer("a", torch.tensor(1.0805, dtype=fp))
+                dt.register_buffer("covalent_radii", covalent_radii_tensor())
+            else:
+                dt.register_buffer("covalent_radii", covalent_radii_tensor())
+                dt.register_buffer("a", torch.tensor(0.2))
+                dt.register_buffer("b", torch.tensor(3.0))
+            self.radial_embedding.distance_transform = dt
+        self.radial_embedding.cutoff_fn = nn.Module()
         self.radial_embedding.cutoff_fn.register_buffer("p", torch.tensor(float(p_cut)))
         self.radial_embedding.cutoff_fn.register_buffer("r_max", torch.tensor(float(r_max)))
         self.node_embedding = nn.Module()
@@ -507,12 +526,14 @@ class MACEStack(Base):
         return MaceConv(inter, prod, E3Linear(hid, hid))
 
     # ---- embeddings (ATen elementwise glue on [E]-sized vectors) ---------------------------------------------------------
-    def _radial(self, d):
-        """RadialEmbeddingBlock (blocks.py:164-177): basis(d) * polynomial cutoff(d), d [E, 1]."""
+    def _radial(self, d, t=None):
+        """RadialEmbeddingBlock (blocks.py:164-177): basis(t) * polynomial cutoff(d), d [E, 1]; t is the transformed length
+        (``DistTransformFn``) under a distance transform, else d itself."""
         p, rc = self.p_cut, self.radius
         x = d / rc
         env = 1.0 - ((p + 1.0) * (p + 2.0) / 2.0) * x.pow(p) + p * (p + 2.0) * x.pow(p + 1) - (p * (p + 1.0) / 2) * x.pow(p + 2)
         cutoff = env * (d < rc)
+        d = d if t is None else t
         bf = self.radial_embedding.bessel_fn
         if self.radial_type == "bessel":
             radial = bf.prefactor * (torch.sin(bf.bessel_weights * d) / d)
@@ -521,6 +542,14 @@ class MACEStack(Base):
         else:
             radial = torch.special.chebyshev_polynomial_t(d.repeat(1, self.num_bessel), bf.n.repeat(len(d), 1))
         return radial * cutoff
+
+    def distance_transform_operands(self, z):
+        """(kind, z, radii, c0, c1, c2) of ``ops.MaceEdgeEmbedDtFn`` / ``ops.DistTransformFn``: the element indices z [N] and the
+        transform's buffers themselves, so the kernels read their current device values (after ``load_state_dict`` too)."""
+        dt = self.radial_embedding.distance_transform
+        if self.distance_transform == "Agnesi":
+            return ops.DIST_TRANSFORMS["Agnesi"], z, dt.covalent_radii, dt.q, dt.p, dt.a
+        return ops.DIST_TRANSFORMS["Soft"], z, dt.covalent_radii, dt.a, dt.b, None
 
     def _forward(self, data, higher):
         """MACEStack.forward (:375-421): a readout before the convolutions and after each, outputs summed."""
@@ -540,20 +569,24 @@ class MACEStack(Base):
         pos = pos - ops.GatherRows.apply(graph_sum(pos, gcsr) / cnt[:, None], gcsr)
         shifts = getattr(data, "edge_shifts", None)
         eattr = self._edge_attr(data, plan.num_edges) if self.use_edge_attr else None
+        # node attributes (process_node_attributes, MACEStack.py:501-535): element index instead of a one-hot matrix
+        z = data.x.squeeze()
+        assert z.dim() == 1, "MACE only supports raw atomic numbers as node_attributes."
+        z = (z.clamp(min=1, max=NUM_ELEMENTS) - 1).long()
+        dt = None if self.distance_transform is None else self.distance_transform_operands(z)
         if not higher and self.radial_type == "bessel":
             # first-order path: geometry, spherical harmonics and Bessel x cutoff of every edge in ONE kernel (SURVEY K2)
-            sh, radial = ops.MaceEdgeEmbedFn.apply(pos, shifts, plan, self.max_ell, self.num_bessel, self.radius, self.p_cut)
+            if dt is None:
+                sh, radial = ops.MaceEdgeEmbedFn.apply(pos, shifts, plan, self.max_ell, self.num_bessel, self.radius, self.p_cut)
+            else:
+                sh, radial = ops.MaceEdgeEmbedDtFn.apply(pos, shifts, plan, dt, self.max_ell, self.num_bessel, self.radius, self.p_cut)
         else:
             vec = ops.GatherRows.apply(pos, plan.by_col) - ops.GatherRows.apply(pos, plan.by_row)
             if shifts is not None:
                 vec = vec + shifts
             dist = vec.pow(2).sum(-1, keepdim=True).sqrt()
             sh = e3.spherical_harmonics_cl(self.max_ell, vec / dist.clamp(min=1e-12))
-            radial = self._radial(dist)
-        # node attributes (process_node_attributes, MACEStack.py:501-535): element index instead of a one-hot matrix
-        z = data.x.squeeze()
-        assert z.dim() == 1, "MACE only supports raw atomic numbers as node_attributes."
-        z = (z.clamp(min=1, max=NUM_ELEMENTS) - 1).long()
+            radial = self._radial(dist, None if dt is None else ops.DistTransformFn.apply(dist, plan, dt))
         zcsr = cached(data, ELEMENT_CSR)
         if zcsr is None or zcsr.idx.numel() != n:
             zcsr = remember(data, ELEMENT_CSR, ops.csr_build(z, NUM_ELEMENTS))

@@ -2495,6 +2495,94 @@ class MaceEdgeEmbedFn(torch.autograd.Function):
         return _edge_vec_scatter(gvec, plan), None, None, None, None, None, None
 
 
+# MACE distance transforms (radial.py:151-245): codes of include/hgb.h.  ``dt`` below is the tuple (kind, z, radii, c0, c1, c2)
+# that MACEStack.distance_transform_operands builds: z [N] int64 element indices and the transform's own buffers, whose device
+# memory the kernels read at run time.
+DIST_TRANSFORMS = {"Agnesi": 1, "Soft": 2}
+
+
+def _dt_ptrs(dt):
+    kind, z, radii, c0, c1, c2 = dt
+    return (int(kind), _p(_chk(z, torch.int64)), _p(_chk(radii)), _p(_chk(c0)), _p(_chk(c1)), _p(_chk(c2)))
+
+
+class MaceEdgeEmbedDtFn(torch.autograd.Function):
+    """MaceEdgeEmbedFn with a distance transform: radial = Bessel(T(d)) x cutoff(d) (blocks.py:164-177) in the same one kernel
+    per edge; the backward adds Bessel'(t) T'(d) cutoff(d).  First-order path only (as MaceEdgeEmbedFn)."""
+
+    @staticmethod
+    def forward(ctx, pos, shifts, plan, dt, lmax, num_bessel, r_max, p):
+        pos, shifts = _chk(pos), _chk(shifts)
+        e = plan.num_edges
+        sh = torch.empty(e, (lmax + 1) ** 2, dtype=pos.dtype, device=pos.device)
+        radial = torch.empty(e, num_bessel, dtype=pos.dtype, device=pos.device)
+        kind, z, radii, c0, c1, c2 = _dt_ptrs(dt)
+        _lib.call("hgb_mace_edge_embed_dt_fwd", _p(pos), _p(plan.row), _p(plan.col), _p(shifts), z, e, int(lmax), int(num_bessel),
+                  float(r_max), float(p), kind, radii, c0, c1, c2, _p(sh), _p(radial), _stream())
+        ctx.save_for_backward(pos, shifts)
+        ctx.plan, ctx.dt, ctx.cfg = plan, dt, (int(lmax), int(num_bessel), float(r_max), float(p))
+        return sh, radial
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g_sh, g_radial):
+        pos, shifts = ctx.saved_tensors
+        plan, (lmax, nb, rc, p) = ctx.plan, ctx.cfg
+        e = plan.num_edges
+        gvec = torch.empty(e, 3, dtype=pos.dtype, device=pos.device)
+        kind, z, radii, c0, c1, c2 = _dt_ptrs(ctx.dt)
+        _lib.call("hgb_mace_edge_embed_dt_bwd", _p(pos), _p(plan.row), _p(plan.col), _p(shifts), z, _p(_chk(g_sh.contiguous())),
+                  _p(_chk(g_radial.contiguous())), e, lmax, nb, rc, p, kind, radii, c0, c1, c2, _p(gvec), _stream())
+        return _edge_vec_scatter(gvec, plan), None, None, None, None, None, None, None
+
+
+def _dist_transform_call(order, d, g, plan, dt):
+    d = _chk(d.contiguous())
+    out = torch.empty_like(d)
+    kind, z, radii, c0, c1, c2 = _dt_ptrs(dt)
+    _lib.call("hgb_mace_dist_transform", int(order), kind, _p(d), _p(None if g is None else _chk(g.contiguous())), _p(plan.row),
+              _p(plan.col), z, radii, c0, c1, c2, plan.num_edges, _p(out), _stream())
+    return out
+
+
+class DistTransformFn(torch.autograd.Function):
+    """t = T(d) per edge (d [E] or [E, 1]); backward g T'(d) = DistTransformGradFn (any-order path: forces and force training)."""
+
+    @staticmethod
+    def forward(ctx, d, plan, dt):
+        ctx.save_for_backward(d)
+        ctx.plan, ctx.dt = plan, dt
+        return _dist_transform_call(0, d, None, plan, dt)
+
+    @staticmethod
+    def backward(ctx, g):
+        d, = ctx.saved_tensors
+        return DistTransformGradFn.apply(g, d, ctx.plan, ctx.dt, 1), None, None
+
+
+class DistTransformGradFn(torch.autograd.Function):
+    """g T^(order)(d), order 1 or 2.  Its backward is g' T^(order)(d) for g and g' g T^(order+1)(d) for d; the distance transform
+    is differentiated at most twice (forces, then the force loss's gradients), a third derivative raises."""
+
+    @staticmethod
+    def forward(ctx, g, d, plan, dt, order):
+        ctx.save_for_backward(g, d)
+        ctx.plan, ctx.dt, ctx.order = plan, dt, order
+        return _dist_transform_call(order, d, g, plan, dt)
+
+    @staticmethod
+    def backward(ctx, gg):
+        g, d = ctx.saved_tensors
+        gd = None
+        if ctx.needs_input_grad[1]:
+            if ctx.order >= 2:
+                raise RuntimeError("MACE distance transform: only the first and second derivatives of T are implemented (no third "
+                                   "derivative of the edge lengths)")
+            gd = DistTransformGradFn.apply(gg * g, d, ctx.plan, ctx.dt, ctx.order + 1)
+        gg_g = DistTransformGradFn.apply(gg, d, ctx.plan, ctx.dt, ctx.order) if ctx.needs_input_grad[0] else None
+        return gg_g, gd, None, None, None
+
+
 # =====================================================================================================
 # graph-attribute conditioning (hydragnn/models/Base.py _apply_graph_conditioning): rows sorted by graph, gcsr = graph offsets
 # =====================================================================================================

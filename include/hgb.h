@@ -55,7 +55,8 @@ typedef void* hgb_stream_t; /* cudaStream_t */
 /* ABI version; 107: hgb_pool_bwd takes relu_y, HGB_ACT_RELU_SELECT (hgb_tc_linear's gact, hgb_act_bwd);
  * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient;
  * 109: hgb_nbr_* (SAGEConv / MFConv); 110: hgb_tc_linear_graph_add, hgb_film_* (graph-attribute conditioning);
- * 111: hgb_gnll_fwd_bwd (GaussianNLLLoss); 112: hgb_prelu_fwd / hgb_prelu_bwd (PReLU with a device-resident slope) */
+ * 111: hgb_gnll_fwd_bwd (GaussianNLLLoss); 112: hgb_prelu_fwd / hgb_prelu_bwd (PReLU with a device-resident slope);
+ * 113: hgb_mace_edge_embed_dt_fwd / _dt_bwd, hgb_mace_dist_transform (MACE's Agnesi and Soft distance transforms) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -434,6 +435,33 @@ int hgb_mace_edge_embed_fwd(const float* pos, const int32_t* row, const int32_t*
 int hgb_mace_edge_embed_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const float* g_sh,
                             const float* g_radial, int64_t e, int32_t lmax, int32_t num_bessel, float r_max, float p, float* g_vec,
                             hgb_stream_t stream);
+
+/* MACE distance transforms (hydragnn/utils/model/mace_utils/modules/radial.py:151-245, applied by RadialEmbeddingBlock in
+ * blocks.py:141-177, wired by MACEStack.py:171-177, 452-466): the Bessel basis reads t = T(d, r0_e) while the polynomial
+ * cutoff keeps the raw length d, radial = basis(t) * cutoff(d).  r0_e comes from the covalent radii of the edge's two elements:
+ *   HGB_DT_AGNESI: c0 = q, c1 = p, c2 = a;  r0 = (R[Z_u] + R[Z_v]) / 2, u = d / r0, T = 1 / (1 + a u^q / (1 + u^(q-p)))
+ *   HGB_DT_SOFT:   c0 = a, c1 = b (c2 unused, may be NULL);  r0 = (R[Z_u] + R[Z_v]) / 4, u = d / r0,
+ *                  T = d + tanh(-u - a u^b) / 2 + 1 / 2
+ * z [n] int64 is the per-node element index Z - 1 (0..117; values outside are clamped), radii [119] the covalent radii by
+ * atomic number and c0..c2 single floats, all in device memory and read by the kernels at run time (a model's buffers: loading
+ * a state dict changes what a captured step computes).  Agnesi is evaluated so that u^(q-p) never overflows: T, T' and T''
+ * are finite for every d >= 0 (T -> 1, T' -> 0 at d -> 0).
+ * edge_embed_dt_fwd / _dt_bwd: hgb_mace_edge_embed_fwd / _bwd with the transform applied to the Bessel argument; the backward
+ * adds basis'(t) T'(d) cutoff(d) to basis(t) cutoff'(d).
+ * dist_transform: out [e] = (g ? g : 1) * T^(order)(d) for order 0 (T), 1 (dT/dd) or 2 (d2T/dd2), d [e] the edge lengths.
+ * With e = 0 nothing runs and every array may be NULL.                                                                       */
+#define HGB_DT_AGNESI 1
+#define HGB_DT_SOFT 2
+int hgb_mace_edge_embed_dt_fwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const int64_t* z,
+                               int64_t e, int32_t lmax, int32_t num_bessel, float r_max, float p, int32_t kind, const float* radii,
+                               const float* c0, const float* c1, const float* c2, float* sh, float* radial, hgb_stream_t stream);
+int hgb_mace_edge_embed_dt_bwd(const float* pos, const int32_t* row, const int32_t* col, const float* shifts, const int64_t* z,
+                               const float* g_sh, const float* g_radial, int64_t e, int32_t lmax, int32_t num_bessel, float r_max,
+                               float p, int32_t kind, const float* radii, const float* c0, const float* c1, const float* c2,
+                               float* g_vec, hgb_stream_t stream);
+int hgb_mace_dist_transform(int32_t order, int32_t kind, const float* d, const float* g, const int32_t* row, const int32_t* col,
+                            const int64_t* z, const float* radii, const float* c0, const float* c1, const float* c2, int64_t e,
+                            float* out, hgb_stream_t stream);
 
 /* Grouped dense layers for multi-branch decoding (hydragnn/models/Base.py:770-780 graph heads, :816-840 node heads,
  * hydragnn/models/MultiTaskModelMP.py): rows sorted by dataset branch, rowptr [groups + 1] on the device, every 64-row tile
