@@ -6,6 +6,7 @@ Public surface (mirrors the slice of ``hydragnn`` that sits on the per-step hot 
     Data, Batch                            -- torch_geometric.data stand-ins
     get_radius_graph[_pbc][_config]        -- hydragnn.preprocess.graph_samples_checks_and_updates
     train, validate, train_step, FlatAdamW, get_distributed_model -- hydragnn.train / hydragnn.utils.distributed
+    select_optimizer, FlatSGD, FlatAdam, FlatAdamax, FlatAdagrad, FlatAdadelta, FlatRMSprop -- hydragnn.utils.optimizer
 
 The CUDA library is loaded lazily on first use; importing the package works on a CPU-only host.
 """
@@ -16,6 +17,8 @@ from .radius import (get_radius_graph, get_radius_graph_config, get_radius_graph
 from .train import (FlatAdamW, GraphedTrainStep, get_distributed_model, get_head_indices, train,  # noqa: F401
                     train_step, validate)
 
+from .optim import (FlatAdadelta, FlatAdagrad, FlatAdam, FlatAdamax, FlatOptimizer, FlatRMSprop, FlatSGD,  # noqa: F401
+                    select_optimizer)
 from .padded import PaddedGraphStep  # noqa: F401
 
 __version__ = "0.2.0"

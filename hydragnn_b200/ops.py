@@ -2667,3 +2667,38 @@ class FilmFn(torch.autograd.Function):
 def adamw_step(p, g, m, v, step_dev, lr, beta1, beta2, eps, weight_decay, grad_scale=1.0, hyper_dev=None):
     _lib.call("hgb_adamw_step", _p(p), _p(g), _p(m), _p(v), p.numel(), float(lr), float(beta1), float(beta2), float(eps),
               float(weight_decay), float(grad_scale), _p(step_dev), _p(hyper_dev), _stream())
+
+
+# ---- the other flat optimizer steps (hgb_optim_flat.cu): torch.optim's single-tensor algorithms over flat buffers ----------
+def sgd_step(p, g, momentum_buffer, step_dev, lr, momentum, dampening, nesterov, weight_decay, grad_scale=1.0, hyper_dev=None):
+    _lib.call("hgb_sgd_step", _p(p), _p(g), _p(momentum_buffer), p.numel(), float(lr), float(momentum), float(dampening),
+              int(bool(nesterov)), float(weight_decay), float(grad_scale), _p(step_dev), _p(hyper_dev), _stream())
+
+
+def adam_step(p, g, exp_avg, exp_avg_sq, max_exp_avg_sq, step_dev, lr, beta1, beta2, eps, weight_decay, amsgrad, grad_scale=1.0,
+              hyper_dev=None):
+    _lib.call("hgb_adam_step", _p(p), _p(g), _p(exp_avg), _p(exp_avg_sq), _p(max_exp_avg_sq), p.numel(), float(lr), float(beta1),
+              float(beta2), float(eps), float(weight_decay), int(bool(amsgrad)), float(grad_scale), _p(step_dev), _p(hyper_dev),
+              _stream())
+
+
+def adamax_step(p, g, exp_avg, exp_inf, step_dev, lr, beta1, beta2, eps, weight_decay, grad_scale=1.0, hyper_dev=None):
+    _lib.call("hgb_adamax_step", _p(p), _p(g), _p(exp_avg), _p(exp_inf), p.numel(), float(lr), float(beta1), float(beta2), float(eps),
+              float(weight_decay), float(grad_scale), _p(step_dev), _p(hyper_dev), _stream())
+
+
+def adagrad_step(p, g, state_sum, step_dev, lr, lr_decay, weight_decay, eps, grad_scale=1.0, hyper_dev=None):
+    _lib.call("hgb_adagrad_step", _p(p), _p(g), _p(state_sum), p.numel(), float(lr), float(lr_decay), float(weight_decay), float(eps),
+              float(grad_scale), _p(step_dev), _p(hyper_dev), _stream())
+
+
+def adadelta_step(p, g, square_avg, acc_delta, step_dev, lr, rho, eps, weight_decay, grad_scale=1.0, hyper_dev=None):
+    _lib.call("hgb_adadelta_step", _p(p), _p(g), _p(square_avg), _p(acc_delta), p.numel(), float(lr), float(rho), float(eps),
+              float(weight_decay), float(grad_scale), _p(step_dev), _p(hyper_dev), _stream())
+
+
+def rmsprop_step(p, g, square_avg, momentum_buffer, grad_avg, step_dev, lr, alpha, eps, weight_decay, momentum, centered,
+                 grad_scale=1.0, hyper_dev=None):
+    _lib.call("hgb_rmsprop_step", _p(p), _p(g), _p(square_avg), _p(momentum_buffer), _p(grad_avg), p.numel(), float(lr), float(alpha),
+              float(eps), float(weight_decay), float(momentum), int(bool(centered)), float(grad_scale), _p(step_dev), _p(hyper_dev),
+              _stream())

@@ -74,6 +74,7 @@ class PaddedGraphStep:
         if not supported(model):
             raise ValueError("PaddedGraphStep: this model (global attention / node heads / branches) needs the eager train_step")
         self.model, self.opt, self.mlip, self.nb = model, opt, bool(compute_grad_energy), neighbour_build
+        self.hyper = None                                   # what the captured optimizer step holds besides lr (_do_capture)
         self.m = model.module
         inner = getattr(self.m, "model", self.m)
         reads_edge_attr = bool(getattr(inner, "use_edge_attr", False))
@@ -180,8 +181,10 @@ class PaddedGraphStep:
 
     def _do_capture(self):
         self.opt.sync_hyper(1.0 / self.ws)
+        self.hyper = self.opt.captured_hyper()
         # warm-up on a side stream WITHOUT touching the parameters' trajectory: run the body, then restore
-        keep = (self.opt.flat_p.clone(), self.opt.m.clone(), self.opt.v.clone(), self.opt.step_dev.clone())
+        state = self.opt.state_tensors()
+        keep = [self.opt.flat_p.clone()] + [t.clone() for t in state]
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
@@ -197,10 +200,8 @@ class PaddedGraphStep:
             self.g_opt = torch.cuda.CUDAGraph()
             with ops.capture_graph(self.g_opt):
                 self.opt.step(1.0 / self.ws)
-        self.opt.flat_p.copy_(keep[0])
-        self.opt.m.copy_(keep[1])
-        self.opt.v.copy_(keep[2])
-        self.opt.step_dev.copy_(keep[3])
+        for dst, src in zip([self.opt.flat_p] + state, keep):
+            dst.copy_(src)
         self._captured = True
 
     # ---- per batch ------------------------------------------------------------------------------------------------------

@@ -4,9 +4,9 @@ Mirror of the hot loop ``train()`` in hydragnn/train/train_validate_test.py:629-
 hydragnn/utils/distributed/distributed.py:396-481, redesigned for one NVSwitch box:
 
 * parameters and gradients live in ONE flat fp32 buffer each (the modules hold views), so the optimizer is a
-  single fused AdamW kernel and the only collective of the step is ONE ``all_reduce`` over the flat gradient
-  (graphs shard by rank with no other communication -- SURVEY 8e); the 1/world_size scaling is folded into
-  the AdamW kernel;
+  single fused kernel (AdamW here; the other types in optim.py) and the only collective of the step is ONE ``all_reduce``
+  over the flat gradient (graphs shard by rank with no other communication -- SURVEY 8e); the 1/world_size scaling is
+  folded into the optimizer kernel;
 * no mpi4py anywhere on the step path (the reference's per-epoch ``MPI.allreduce(nbatch, MIN)``,
   :672, becomes a ``dist.all_reduce(MIN)``);
 * ``GraphedTrainStep`` captures forward + loss + backward + flatten + optimizer of a fixed-shape batch in a CUDA
@@ -16,6 +16,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops
+from .optim import FlatOptimizer
 from .stacks import forget_plans
 
 PRECISION_MAP = {"bf16": torch.float32, "fp32": torch.float32}     # parameters stay fp32 (reference :43-49)
@@ -62,7 +63,7 @@ def get_head_indices(model, data):
     return out
 
 
-class FlatAdamW(torch.optim.Optimizer):
+class FlatAdamW(FlatOptimizer):
     """torch.optim.AdamW semantics over one flat buffer (``hydragnn/utils/optimizer/optimizer.py:12-40`` default).  After
     construction every parameter of ``model`` is a view into ``self.flat_p`` (so checkpoints / ``state_dict`` are unchanged).
 
@@ -73,67 +74,19 @@ class FlatAdamW(torch.optim.Optimizer):
     ``param_groups[0]["lr"]`` changed -- a CUDA-graph-captured step therefore follows a scheduler."""
 
     def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2):
-        if isinstance(model, torch.nn.Module) and any(getattr(m, "graph_attr_modules_missing", lambda: False)() for m in model.modules()):
-            # the buffer holds the parameters that exist now: a conditioning module created later would never be trained
-            raise ValueError("FlatAdamW: this model's graph-attribute conditioning modules are created at its first forward; run "
-                             "one forward (or load the checkpoint) before building the optimizer")
-        params = [p for p in (model.parameters() if isinstance(model, torch.nn.Module) else model) if p.requires_grad]
-        super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
-        self.params = params
+        super().__init__(model, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
         self.betas, self.eps, self.weight_decay = betas, eps, weight_decay
-        dev = self.params[0].device
-        n = sum(p.numel() for p in self.params)
-        self.flat_p = torch.empty(n, dtype=torch.float32, device=dev)
-        self.flat_g = torch.zeros(n, dtype=torch.float32, device=dev)
-        off = 0
-        self.slices = []
-        for p in self.params:
-            k = p.numel()
-            self.flat_p[off:off + k].copy_(p.data.reshape(-1))
-            p.data = self.flat_p[off:off + k].view_as(p.data)
-            self.slices.append((off, k))
-            off += k
         self.m = torch.zeros_like(self.flat_p)
         self.v = torch.zeros_like(self.flat_p)
-        self.step_dev = torch.zeros(1, dtype=torch.float32, device=dev)
-        self.hyper_dev = torch.tensor([lr, 1.0], dtype=torch.float32, device=dev)      # {lr, grad_scale} read by the kernel
-        self._hyper_host = (float(lr), 1.0)
 
-    @property
-    def lr(self):
-        return self.param_groups[0]["lr"]
+    def state_tensors(self):
+        return [self.m, self.v, self.step_dev]
 
-    def zero_grad(self, set_to_none=True):
-        for p in self.params:
-            p.grad = None
-
-    def backward(self, loss):
-        """``loss.backward()`` with the weight-gradient kernels of leaf parameters left running on the side stream until the flat
-        gradient is gathered (ops.deferred_weight_gradients), then ``gather_grads()``."""
-        with ops.deferred_weight_gradients():
-            loss.backward()
-        return self.gather_grads()
-
-    def gather_grads(self):
-        """autograd's per-parameter gradients -> the flat buffer (parameters nobody used contribute zeros)."""
-        ops.join_side_streams()                     # weight-gradient kernels run on a side stream (ops.fork_join)
-        gs = [(p.grad if p.grad is not None else torch.zeros_like(p)).reshape(-1) for p in self.params]
-        torch.cat(gs, out=self.flat_g)
-        return self.flat_g
-
-    def sync_hyper(self, grad_scale=None):
-        """Push lr / grad_scale to the device if they changed (a tiny async H2D copy, outside any captured graph)."""
-        want = (float(self.param_groups[0]["lr"]), self._hyper_host[1] if grad_scale is None else float(grad_scale))
-        if want != self._hyper_host:
-            self.hyper_dev.copy_(torch.tensor(want, dtype=torch.float32), non_blocking=False)
-            self._hyper_host = want
+    def captured_hyper(self):
+        return (tuple(self.betas), self.eps, self.weight_decay)
 
     def step(self, grad_scale=1.0, closure=None):
-        capturing = self.flat_p.is_cuda and torch.cuda.is_current_stream_capturing()
-        if not capturing:
-            self.sync_hyper(grad_scale)
-        elif float(grad_scale) != self._hyper_host[1]:
-            raise RuntimeError("FlatAdamW: call sync_hyper(grad_scale) before capturing a step with a new gradient scale")
+        self._sync_for_step(grad_scale)
         ops.adamw_step(self.flat_p, self.flat_g, self.m, self.v, self.step_dev, self.param_groups[0]["lr"], self.betas[0],
                        self.betas[1], self.eps, self.weight_decay, grad_scale, hyper_dev=self.hyper_dev)
 
@@ -202,7 +155,7 @@ def world():
 
 
 def train_step(model, opt, data, compute_grad_energy=False, head_index=None):
-    """forward -> loss -> backward -> flat all-reduce -> fused AdamW.  Returns (loss, tasks_loss)
+    """forward -> loss -> backward -> flat all-reduce -> fused flat optimizer step.  Returns (loss, tasks_loss)
     (hydragnn/train/train_validate_test.py:702-769 without the tracing scaffolding)."""
     m = model.module
     opt.zero_grad()
@@ -315,7 +268,8 @@ def _train_fast(loader, model, opt, compute_grad_energy, neighbour_build):
     for ibatch, data in enumerate(loader):
         if ibatch >= nbatch:
             break
-        if fast is None or fast.model is not model or fast.mlip != bool(compute_grad_energy) or fast.nb != neighbour_build:
+        if (fast is None or fast.model is not model or fast.mlip != bool(compute_grad_energy) or fast.nb != neighbour_build
+                or fast.hyper != opt.captured_hyper()):             # hyperparameters other than lr are fixed at capture
             fast = opt._hgb_fast = PaddedGraphStep(model, opt, data, compute_grad_energy, neighbour_build)
         g = fast.load(data)
         loss, tasks = fast.run()
@@ -337,7 +291,7 @@ def train(loader, model, opt, verbosity=0, profiler=None, use_deepspeed=False, c
     dev = next(model.parameters()).device
     from . import padded
     if fast is None:
-        fast = dev.type == "cuda" and padded.supported(model) and isinstance(opt, FlatAdamW)
+        fast = dev.type == "cuda" and padded.supported(model) and isinstance(opt, FlatOptimizer)
     if fast:
         model.train()
         train_error, tasks_error = _train_fast(loader, model, opt, compute_grad_energy, neighbour_build)

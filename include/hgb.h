@@ -580,6 +580,35 @@ int hgb_prelu_bwd(const float* g, const float* z, int64_t count, const float* sl
 int hgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t count, float lr, float beta1,
                    float beta2, float eps, float weight_decay, float grad_scale, float* step_dev,
                    const float* hyper_dev, hgb_stream_t stream);
+/* The flat steps of torch.optim.SGD, Adam, Adamax, Adagrad, Adadelta and RMSprop (hydragnn/utils/optimizer/optimizer.py
+ * selects them by name), each torch's single-tensor algorithm (foreach=False) in its operation order, fp32 elementwise.
+ * Shared with hgb_adamw_step: p, g and every state buffer [count] (count >= 0); g is multiplied by grad_scale first;
+ * hyper_dev (optional, device, {lr, grad_scale}) overrides the by-value lr / grad_scale; the 1-based step t is
+ * step_dev[0] + 1 on the device, and step_dev is incremented after the update (a second launch).  Bias corrections and
+ * decayed learning rates are computed from t in fp64 on the device, so a captured step stays right on every replay.
+ * State buffers an option does not use may be NULL, and so may every buffer when count == 0 (only the step advances).
+ *   sgd:      momentum_buffer when momentum != 0; at t == 1 the buffer takes the (decayed) gradient as it is.
+ *             nesterov needs momentum > 0 and dampening 0.
+ *   adam:     L2 weight decay added to g (torch.optim.Adam, not AdamW); max_exp_avg_sq when amsgrad.
+ *   adagrad:  sum starts at initial_accumulator_value (the caller fills it); clr = lr / (1 + (t - 1) lr_decay).
+ *   rmsprop:  momentum_buffer when momentum > 0, grad_avg when centered.                                          */
+int hgb_sgd_step(float* p, const float* g, float* momentum_buffer, int64_t count, float lr, double momentum,
+                 double dampening, int32_t nesterov, double weight_decay, float grad_scale, float* step_dev,
+                 const float* hyper_dev, hgb_stream_t stream);
+int hgb_adam_step(float* p, const float* g, float* exp_avg, float* exp_avg_sq, float* max_exp_avg_sq, int64_t count,
+                  float lr, double beta1, double beta2, double eps, double weight_decay, int32_t amsgrad,
+                  float grad_scale, float* step_dev, const float* hyper_dev, hgb_stream_t stream);
+int hgb_adamax_step(float* p, const float* g, float* exp_avg, float* exp_inf, int64_t count, float lr, double beta1,
+                    double beta2, double eps, double weight_decay, float grad_scale, float* step_dev,
+                    const float* hyper_dev, hgb_stream_t stream);
+int hgb_adagrad_step(float* p, const float* g, float* sum, int64_t count, float lr, double lr_decay, double weight_decay,
+                     double eps, float grad_scale, float* step_dev, const float* hyper_dev, hgb_stream_t stream);
+int hgb_adadelta_step(float* p, const float* g, float* square_avg, float* acc_delta, int64_t count, float lr, double rho,
+                      double eps, double weight_decay, float grad_scale, float* step_dev, const float* hyper_dev,
+                      hgb_stream_t stream);
+int hgb_rmsprop_step(float* p, const float* g, float* square_avg, float* momentum_buffer, float* grad_avg, int64_t count,
+                     float lr, double alpha, double eps, double weight_decay, double momentum, int32_t centered,
+                     float grad_scale, float* step_dev, const float* hyper_dev, hgb_stream_t stream);
 
 /* PaiNN update block at node_size == 1 (the reference's first layer runs at width input_dim, quirk Q4): the whole block
  * (PAINNStack.py:298-328) per node in one kernel.  params16 / gparams16 (device, 16 floats): 0 uw, 1 ub, 2 vw, 3 vb,
