@@ -53,13 +53,13 @@ Grid limits: row tiles were indexed by gridDim.y (at most 65,535), so gemm_kerne
 4,194,240 rows and colsum_stage1 above 33,553,920 rows.  The kernels now stride over row tiles; `test_*_past_65535_row_*`
 run one tile past each limit and check that a row's result does not depend on how many tiles the launch has.
 """
-import math
-
 import numpy as np
 import pytest
 import torch
 
 from hydragnn_b200 import _lib, ops
+from kernel_harness import (ACT, DERIV, LIP, LIP1, LRELU_P, SELU_A, SELU_S, act64, act_eval_err, deriv64, deriv_terms,
+                            grad_from, grad_from_err, l2_bound)
 
 DEV = "cuda"
 GUARD = 3                            # NaN rows after every buffer
@@ -67,16 +67,8 @@ NAN_BITS = 0x7FC00000                # torch.full(nan) fp32
 U = 2.0 ** -24
 NUM_SMS = 132                        # HGB_NUM_SMS
 TNF_ROWS, TNF_THREADS = 64, 128
-SELU_A, SELU_S = 1.6732632423543772848170429916717, 1.0507009873554804934193349852946
-EXP_FLOOR = 2.0 ** -120
-LRELU_P = float(np.float32(0.1))     # the fp32 parameter the kernels receive
 UNDERFLOW = 2.0 ** -126              # the underflow term eta of fl(x) = x (1 + delta) + eta, |eta| <= 2^-150, over < 2^24 roundings
-ACT = dict(none=0, relu=1, silu=2, tanh=3, sigmoid=4, lrelu=5, elu=6, selu=7)
-DERIV = 100
 CODES = list(ACT.values())
-EXP_CODES = (ACT["silu"], ACT["sigmoid"], ACT["elu"], ACT["selu"])
-LIP = {0: 1.0, 1: 1.0, 2: 1.0999, 3: 1.0, 4: 0.25, 5: 1.0, 6: 1.0, 7: 1.7581}        # max |act'|
-LIP1 = {0: 0.0, 1: 0.0, 2: 0.5, 3: 0.77, 4: 0.1, 5: 0.0, 6: 1.0, 7: 1.7581}         # max |act''|
 
 
 def cdiv(a, b):
@@ -324,109 +316,6 @@ def test_workspace_restatement_matches_library():
 
 
 # ---- fp64 references ----------------------------------------------------------------------------------------------------------
-def act64(z, code, p=LRELU_P):
-    if code == ACT["relu"]:
-        return torch.where(z > 0, z, torch.zeros_like(z))
-    if code == ACT["silu"]:
-        return z * torch.sigmoid(z)
-    if code == ACT["tanh"]:
-        return torch.tanh(z)
-    if code == ACT["sigmoid"]:
-        return torch.sigmoid(z)
-    if code == ACT["lrelu"]:
-        return torch.where(z > 0, z, p * z)
-    if code == ACT["elu"]:
-        return torch.where(z > 0, z, torch.expm1(z))
-    if code == ACT["selu"]:
-        return SELU_S * torch.where(z > 0, z, SELU_A * torch.expm1(z))
-    return z
-
-
-def deriv64(x, code, order, p=LRELU_P):
-    """order-th derivative at x; at the kinks x = 0 the kernel's convention: x > 0 takes the right branch, else the left"""
-    if order == 0:
-        return act64(x, code, p)
-    one, zero = torch.ones_like(x), torch.zeros_like(x)
-    pos = x > 0
-    if code == ACT["relu"]:
-        return torch.where(pos, one, zero) if order == 1 else zero
-    if code == ACT["lrelu"]:
-        return torch.where(pos, one, p * one) if order == 1 else zero
-    if code == ACT["silu"]:
-        s = torch.sigmoid(x)
-        return s * (1 + x * (1 - s)) if order == 1 else s * (1 - s) * (2 + x * (1 - 2 * s))
-    if code == ACT["tanh"]:
-        t = torch.tanh(x)
-        return 1 - t * t if order == 1 else -2 * t * (1 - t * t)
-    if code == ACT["sigmoid"]:
-        s = torch.sigmoid(x)
-        return s * (1 - s) if order == 1 else s * (1 - s) * (1 - 2 * s)
-    if code == ACT["elu"]:
-        return torch.where(pos, one if order == 1 else zero, torch.exp(x))
-    if code == ACT["selu"]:
-        return torch.where(pos, SELU_S * one if order == 1 else zero, SELU_S * SELU_A * torch.exp(x))
-    return one if order == 1 else zero
-
-
-def deriv_terms(x, code, order, p=LRELU_P):
-    """magnitude of the terms of the formula the kernel evaluates for the order-th derivative at x"""
-    if order == 0:
-        return act64(x, code, p).abs() + (x.abs() if code in (ACT["silu"], ACT["lrelu"]) else 0)
-    a = x.abs()
-    if code == ACT["silu"]:
-        s = torch.sigmoid(x)
-        return s * (1 + a * (1 + 2 * s)) if order == 1 else s * (1 + s) * (2 + a * (1 + 2 * s))
-    if code == ACT["tanh"]:
-        t = torch.tanh(x).abs()
-        return 1 + t * t if order == 1 else 2 * t * (1 + t * t)
-    if code == ACT["sigmoid"]:
-        s = torch.sigmoid(x)
-        return s * (1 + s) if order == 1 else s * (1 + s) * (1 + 2 * s)
-    return deriv64(x, code, order, p).abs()
-
-
-def act_eval_err(x, code, order=0, p=LRELU_P):
-    """bound on the error of the kernel's fp32 evaluation of the order-th derivative at the fp32 argument x (module docstring)"""
-    if code in (ACT["none"], ACT["relu"]) or (code == ACT["lrelu"] and order > 0):
-        return torch.zeros_like(x)
-    e = (12 + 2.4 * x.abs()) * U * deriv_terms(x, code, order, p)
-    return e + (EXP_FLOOR if code in EXP_CODES else 0.0)
-
-
-def grad_from(y, z, code, p=LRELU_P):
-    """hgb_act_grad: act' from the activation output y (from z for SiLU; z itself for HGB_ACT_DERIV), in fp64"""
-    if code == DERIV:
-        return z
-    if code == ACT["silu"]:
-        return deriv64(z, code, 1)
-    if code == ACT["relu"]:
-        return (y > 0).double()
-    if code == ACT["tanh"]:
-        return 1 - y * y
-    if code == ACT["sigmoid"]:
-        return y * (1 - y)
-    if code == ACT["lrelu"]:
-        return torch.where(y > 0, torch.ones_like(y), p * torch.ones_like(y))
-    if code == ACT["elu"]:
-        return torch.where(y > 0, torch.ones_like(y), y + 1)
-    if code == ACT["selu"]:
-        return torch.where(y > 0, SELU_S * torch.ones_like(y), y + SELU_S * SELU_A)
-    return torch.ones_like(y)
-
-
-def grad_from_err(y, z, code, p=LRELU_P):
-    """bound on the fp32 evaluation error of hgb_act_grad (without the product with dy)"""
-    if code in (ACT["none"], ACT["relu"], ACT["lrelu"]):
-        return torch.zeros_like(y)
-    if code == DERIV:
-        return torch.zeros_like(z)
-    if code == ACT["silu"]:
-        return act_eval_err(z, code, 1)
-    m = {ACT["tanh"]: 1 + y * y, ACT["sigmoid"]: y.abs() * (1 + y.abs()), ACT["elu"]: 1 + y.abs(),
-         ACT["selu"]: y.abs() + SELU_S * SELU_A}[code]
-    return 4 * U * m
-
-
 @pytest.mark.parametrize("code", CODES)
 def test_reference_activations_match_torch(code):
     """act64 against torch.nn.functional in fp64, deriv64 against fp64 autograd of it (orders 1 and 2, away from the kinks)"""
@@ -507,12 +396,6 @@ def check_close(what, name, got, ref, bound, l2=None):
     if l2 is not None:
         assert float(err.norm()) <= l2, "%s: %s: L2 error %.3g exceeds %.3g (||ref|| %.3g)" % (
             what, name, float(err.norm()), l2, float(ref.norm()))
-
-
-def l2_bound(L, mag, extra=None):
-    """3 u sqrt(L) ||mag|| (+ ||extra||): the random-walk model of the module docstring"""
-    b = 3 * U * math.sqrt(max(L, 1)) * float(mag.norm())
-    return b + (float(extra.norm()) if extra is not None else 0.0)
 
 
 def rand(g, *shape, scale=1.0):

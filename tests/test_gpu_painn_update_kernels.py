@@ -43,7 +43,7 @@ contracts products into FMAs, and an FMA only removes a rounding.
    operands (hgb_tc_linear for [uv | vv], the matching hgb_painn_update_* step, and for tc_bwd the dgrad with its addend), as the
    header of hgb_painn_tc.cu states; (ii) against fp64 with v, [U; V] and [guv | gvv] rounded to TF32 (oracle.tf32._round_tf32):
    a K-term product with its bias or addend is within gamma(K + 2) (sum |a b| + |c|) plus TF32_OPERAND sum |a b| for the
-   tensor cores' own operand conversion (see its note), then class R carries the error through the elementwise formulas.  n covers
+   tensor cores' own operand conversion (see its note in kernel_harness.py), then class R carries the error through the elementwise formulas.  n covers
    partial tiles (1, 63, 65, 129), the producer ring wrapping its parity, and more tiles than one persistent wave at one or two
    CTAs per SM (8449, 16897).  At n < 64 the 64-row TMA box is taller than the tensor; the hardware fills the missing rows with
    zeros, the kernels store no row >= n, and the results equal the unfused pieces bit for bit, so the entries accept any n >= 0.
@@ -69,8 +69,7 @@ import pytest
 import torch
 
 from hydragnn_b200 import _lib, ops, pnaeq, stacks
-from kernel_harness import U, Buf, cdiv, check_bound, gamma, grid_for, launches, same_f32, stream, twice, ws_buf
-from oracle.tf32 import _round_tf32
+from kernel_harness import U, Buf, cdiv, check_bound, gamma, grid_for, launches, same_f32, stream, tf32_gemm, twice, ws_buf
 
 DEV = "cuda"
 NUM_SMS = 132
@@ -81,10 +80,6 @@ N_SCALAR = (0, 1, 255, 256, 257, 67585, 135169)
 N_TC = (1, 63, 64, 65, 128, 129, 8449, 16897)
 SCALAR_BWD_BLOCKS = 2 * NUM_SMS               # UPD_SCALAR_BLOCKS
 SCALAR_FWD_BLOCKS = 4 * NUM_SMS
-# The tensor cores take the leading 19 bits of an fp32 operand (truncation, test_gpu_tc.py), within one TF32 ulp (2^-10
-# relative) of _round_tf32's nearest value; over both operands of a product that is 2^-9 (1 + 2^-9) of |product|.  With this term
-# at 0 the worst |error| / bound was 92 on an H100: the conversion, not the accumulation, dominates.
-TF32_OPERAND = 2.0 ** -9 * (1 + 2.0 ** -9)
 # rel-L2 of the fp32-mode modules against fp64, measured once on an H100 (80 GB HBM3, 700 W): worst 3.7e-6 over the outputs and
 # the 10 gradients of every case in section 4; held to 2e-5
 FP32_TOL = 2e-5
@@ -603,19 +598,11 @@ def tc_unfused(x, n, last):
     return out
 
 
-def tf32_gemm(a, w, c, k):
-    """R of a @ w^T + c: fp64 of the TF32-rounded operands, within gamma(k + 2) (sum |a w| + |c|) + TF32_OPERAND sum |a w|"""
-    ta, tw = _round_tf32(a.float()).double(), _round_tf32(w.float()).double()
-    mag = ta.abs() @ tw.abs().t()
-    cc = torch.zeros_like(mag) if c is None else c.double()
-    return R(ta @ tw.t() + cc, gamma(k + 2) * (mag + cc.abs()) + TF32_OPERAND * mag)
-
-
 def tc_refs(x, n, last, g_uv):
     """fp64 references of the four entries (R); g_uv: the kernel's own [guv | gvv], the dgrad's operand"""
     d = lambda t: R(t.double())  # noqa: E731
     na = 2 if last else 3
-    y = tf32_gemm(x["v"].reshape(3 * n, UF), x["wuv"], x["buv"].expand(3 * n, 2 * UF), UF)
+    y = R(*tf32_gemm(x["v"].reshape(3 * n, UF), x["wuv"], x["buv"].expand(3 * n, 2 * UF), UF))
     uv = [R(y.val.reshape(n, 3, 2 * UF)[:, k, :UF], y.err.reshape(n, 3, 2 * UF)[:, k, :UF]) for k in range(3)]
     vv = [R(y.val.reshape(n, 3, 2 * UF)[:, k, UF:], y.err.reshape(n, 3, 2 * UF)[:, k, UF:]) for k in range(3)]
     inner = (uv[0] * vv[0] + uv[1] * vv[1]) + uv[2] * vv[2]
@@ -636,7 +623,7 @@ def tc_refs(x, n, last, g_uv):
     gsv = g * a[na - 2]
     ref["guv"] = [gsv * vv[k] + (0.0 if last else gvo[k] * a[0]) for k in range(3)]
     ref["gvv"] = [gsv * uv[k] + q * vv[k] for k in range(3)]
-    ref["gv"] = tf32_gemm(g_uv, x["wuv"].t(), None if last else x["gv_out"].reshape(3 * n, UF), 2 * UF)
+    ref["gv"] = R(*tf32_gemm(g_uv, x["wuv"].t(), None if last else x["gv_out"].reshape(3 * n, UF), 2 * UF))
     return ref
 
 
