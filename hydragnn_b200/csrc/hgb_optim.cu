@@ -1,4 +1,4 @@
-// libhgb.so -- loss (value + gradient in one pass) and the fused flat AdamW step.
+// libhgb.so -- losses (value + gradient in one pass) and PReLU; the optimizer steps are in hgb_optim_flat.cu.
 #include "hgb_common.cuh"
 
 // single block: deterministic tree reduction; count is small (number of targets in the batch)
@@ -206,47 +206,5 @@ extern "C" int hgb_prelu_bwd(const float* g, const float* z, int64_t count, cons
     prelu_bwd_kernel<true><<<blocks, GNLL_THREADS, 0, st>>>(g, z, count, slope, dz, dslope, partial, ticket);
   }
   HGB_LAUNCH_CHECK("prelu_bwd");
-  return HGB_OK;
-}
-
-// torch.optim.AdamW semantics (decoupled weight decay, bias correction, eps outside the sqrt):
-//   p *= 1 - lr*wd;  m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;
-//   p -= lr/(1-b1^t) * m / (sqrt(v)/sqrt(1-b2^t) + eps)
-__global__ void adamw_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                             int64_t count, float lr, float b1, float b2, float eps, float wd, float gscale,
-                             const float* __restrict__ step_dev, const float* __restrict__ hyper_dev) {
-  if (hyper_dev) {           // learning rate / gradient scale live on the device: a captured step follows the scheduler
-    lr = hyper_dev[0];
-    gscale = hyper_dev[1];
-  }
-  const float t = step_dev[0] + 1.f;
-  const float bc1 = 1.f - powf(b1, t), bc2 = 1.f - powf(b2, t);
-  const float step_size = lr / bc1;
-  const float inv_sqrt_bc2 = rsqrtf(bc2);
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
-    const float gi = g[i] * gscale;
-    float pi = p[i] * (1.f - lr * wd);
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi;
-    v[i] = vi;
-    pi -= step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + eps);
-    p[i] = pi;
-  }
-}
-__global__ void step_inc_kernel(float* step_dev) { step_dev[0] += 1.f; }
-
-extern "C" int hgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t count, float lr, float beta1, float beta2,
-                              float eps, float weight_decay, float grad_scale, float* step_dev, const float* hyper_dev,
-                              hgb_stream_t stream) {
-  HGB_REQUIRE(count >= 0 && p && g && m && v && step_dev, "adamw_step: bad arguments");
-  cudaStream_t st = (cudaStream_t)stream;
-  if (count > 0) {
-    adamw_kernel<<<hgb_grid_for(count, 256), 256, 0, st>>>(p, g, m, v, count, lr, beta1, beta2, eps, weight_decay, grad_scale, step_dev,
-                                                           hyper_dev);
-    HGB_LAUNCH_CHECK("adamw");
-  }
-  step_inc_kernel<<<1, 1, 0, st>>>(step_dev);
-  HGB_LAUNCH_CHECK("adamw_step_inc");
   return HGB_OK;
 }

@@ -1,11 +1,12 @@
-// libhgb.so -- the flat-buffer steps of the other optimizers hydragnn/utils/optimizer/optimizer.py selects: SGD, Adam, Adamax,
-// Adagrad, Adadelta and RMSprop.  Each follows torch.optim's single-tensor algorithm (foreach=False) element by element, in
-// the same operation order, over one flat parameter / gradient / state buffer set.  As in hgb_adamw_step:
+// libhgb.so -- the flat-buffer steps of every optimizer hydragnn/utils/optimizer/optimizer.py selects: SGD, Adam, AdamW,
+// Adamax, Adagrad, Adadelta and RMSprop, one kernel template over one flat parameter / gradient / state buffer set:
 //   * lr and grad_scale come from hyper_dev {lr, grad_scale} when it is given (a captured step follows a scheduler);
 //   * the step count is read from step_dev (1-based inside the update) and incremented by a second launch after it;
 //   * the gradient is multiplied by grad_scale before anything else (1/world after the flat all-reduce).
-// Scalar coefficients (bias corrections, Adagrad's decayed lr) are computed once per thread in fp64 and rounded to fp32, as
-// torch computes them in Python doubles; the elementwise arithmetic is fp32, as ATen's opmath for fp32 tensors.
+// All but AdamW follow torch.optim's single-tensor algorithm (foreach=False) element by element, in the same operation order:
+// scalar coefficients (bias corrections, Adagrad's decayed lr) are computed once per thread in fp64 and rounded to fp32, as
+// torch computes them in Python doubles; the elementwise arithmetic is fp32, as ATen's opmath for fp32 tensors.  AdamW keeps
+// the fp32 hyperparameters and fp32 coefficients of its C entry point.
 #include "hgb_common.cuh"
 
 namespace {
@@ -59,6 +60,25 @@ struct AdamRule {
     }
     const float denom = sqrtf(vv) / bc2_sqrt + eps;
     p = p + neg_step_size * (m / denom);
+  }
+};
+
+// torch.optim.AdamW's update with fp32 hyperparameters and fp32 bias corrections (not Adam's lerp and fp64 coefficients):
+//   p *= 1 - lr wd;  m = b1 m + (1 - b1) g;  v = b2 v + (1 - b2) g^2;  p -= lr / (1 - b1^t) m / (sqrt(v) rsqrt(1 - b2^t) + eps)
+// Every contraction is explicit, so the float4 body and the scalar loop give the same bits.
+struct AdamWRule {
+  float b1, b2, w1, w2, eps, wd;
+  float decay, step_size, inv_sqrt_bc2;
+  __device__ __forceinline__ void coef(float lr, double t) {
+    const float tf = (float)t;
+    decay = __fmaf_rn(-lr, wd, 1.f);
+    step_size = __fdiv_rn(lr, 1.f - powf(b1, tf));
+    inv_sqrt_bc2 = rsqrtf(1.f - powf(b2, tf));
+  }
+  __device__ __forceinline__ void apply(float, float& p, float g, float& m, float& v, float&) const {
+    m = __fmaf_rn(g, w1, __fmul_rn(m, b1));
+    v = __fmaf_rn(g, __fmul_rn(g, w2), __fmul_rn(v, b2));
+    p = __fsub_rn(__fmul_rn(p, decay), __fdiv_rn(__fmul_rn(step_size, m), __fmaf_rn(sqrtf(v), inv_sqrt_bc2, eps)));
   }
 };
 
@@ -166,7 +186,7 @@ __global__ void __launch_bounds__(FLAT_THREADS) flat_step_kernel(Rule r, float* 
   }
 }
 
-__global__ void flat_step_inc_kernel(float* step_dev) { step_dev[0] += 1.f; }
+__global__ void flat_step_count_kernel(float* step_dev) { step_dev[0] += 1.f; }
 
 bool aligned16(const void* a) { return a == nullptr || (reinterpret_cast<uintptr_t>(a) & 15u) == 0; }
 
@@ -181,7 +201,7 @@ int launch(const char* name, const Rule& r, float* p, const float* g, float* s0,
                                                                                    step_dev, hyper_dev, vec);
     HGB_LAUNCH_CHECK(name);
   }
-  flat_step_inc_kernel<<<1, 1, 0, st>>>(step_dev);
+  flat_step_count_kernel<<<1, 1, 0, st>>>(step_dev);
   HGB_LAUNCH_CHECK(name);
   return HGB_OK;
 }
@@ -208,6 +228,14 @@ extern "C" int hgb_adam_step(float* p, const float* g, float* exp_avg, float* ex
                    amsgrad != 0, 0.f, 0.f};
   return launch("adam_step", r, p, g, exp_avg, exp_avg_sq, amsgrad ? max_exp_avg_sq : nullptr, count, lr, grad_scale, step_dev,
                 hyper_dev, stream);
+}
+
+extern "C" int hgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t count, float lr, float beta1, float beta2,
+                              float eps, float weight_decay, float grad_scale, float* step_dev, const float* hyper_dev,
+                              hgb_stream_t stream) {
+  HGB_REQUIRE(count >= 0 && step_dev && (count == 0 || (p && g && m && v)), "adamw_step: bad arguments");
+  const AdamWRule r{beta1, beta2, 1.f - beta1, 1.f - beta2, eps, weight_decay, 0.f, 0.f, 0.f};
+  return launch("adamw_step", r, p, g, m, v, nullptr, count, lr, grad_scale, step_dev, hyper_dev, stream);
 }
 
 extern "C" int hgb_adamax_step(float* p, const float* g, float* exp_avg, float* exp_inf, int64_t count, float lr, double beta1,

@@ -327,7 +327,7 @@ def linear_fwd_dispatch_ex(x2, w, b, code=0, param=0.0, want_z=False, z_deriv=Fa
 # The weight gradient and the data gradient of a layer read the same dZ and are independent of each other.  ``fork_join`` launches
 # the weight-gradient kernels on a SIDE stream forked from the current one, lets the caller launch the data gradient on the main
 # stream, and joins before either result is handed to autograd -- in a captured step the two become parallel branches of the CUDA
-# graph.  Inside ``deferred_weight_gradients()`` (the engine's own step: FlatAdamW.backward) the join of a LEAF parameter that has
+# graph.  Inside ``deferred_weight_gradients()`` (the engine's step: FlatOptimizer.backward) the join of a LEAF parameter that has
 # not received a gradient in this backward pass moves to the end of the pass (an autograd-engine callback): nothing reads such a
 # gradient on the main stream before the optimizer (AccumulateGrad takes the tensor over without a kernel), so the weight-gradient
 # kernels overlap everything that follows.  The inputs of the deferred kernels are kept referenced until the join, which stops
@@ -380,7 +380,7 @@ HOLD_LIMIT = 8 << 30          # bytes of deferred-kernel inputs kept alive befor
 
 
 class deferred_weight_gradients:
-    """Context manager around ``loss.backward()`` of a step whose gradients are first read by ``FlatAdamW.gather_grads``."""
+    """Context manager around ``loss.backward()`` of a step whose gradients are first read by ``FlatOptimizer.gather_grads``."""
 
     def __enter__(self):
         self.prev = _DEFER["on"]
@@ -393,7 +393,7 @@ class deferred_weight_gradients:
 
 
 def join_side_streams():
-    """Join every side stream with deferred weight-gradient work (end of a backward pass; also called by FlatAdamW.gather_grads)."""
+    """Join every side stream with deferred weight-gradient work (end of a backward pass; also called by FlatOptimizer.gather_grads)."""
     for key in list(_PENDING["keys"]):
         torch.cuda.current_stream(key).wait_stream(_SIDE[key])
     _PENDING["keys"].clear()

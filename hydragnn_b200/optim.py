@@ -6,26 +6,24 @@ CUDA-graph-captured step follows a learning-rate scheduler and the 1/world gradi
 the update.  ``train_step``, ``GraphedTrainStep`` and ``PaddedGraphStep`` drive any of them through ``backward``, ``flat_g``,
 ``step(grad_scale)``, ``sync_hyper`` and ``state_tensors``.
 
-``FlatSGD``, ``FlatAdam``, ``FlatAdamax``, ``FlatAdagrad``, ``FlatAdadelta`` and ``FlatRMSprop`` (with ``FlatAdamW`` in train.py)
-are ``torch.optim.Optimizer``s with one param group: the group holds torch's keys with torch's defaults, the kernels follow
-torch's single-tensor algorithms, and ``state_dict()`` / ``load_state_dict()`` speak the matching ``torch.optim`` class's format,
-so optimizer checkpoints move between torch and the engine in both directions.  torch's ``maximize``, ``capturable``,
-``differentiable``, ``foreach`` and ``fused`` flags, sparse gradients and more than one param group are not supported.
+``FlatSGD``, ``FlatAdam``, ``FlatAdamW``, ``FlatAdamax``, ``FlatAdagrad``, ``FlatAdadelta`` and ``FlatRMSprop`` are
+``torch.optim.Optimizer``s with one param group: the group holds torch's keys with torch's defaults, the kernels follow
+torch's single-tensor algorithms (AdamW's in fp32, see ``FlatAdamW``), and ``state_dict()`` / ``load_state_dict()`` speak the
+matching ``torch.optim`` class's format, so optimizer checkpoints move between torch and the engine in both directions.  torch's
+``maximize``, ``capturable``, ``differentiable``, ``foreach`` and ``fused`` flags, sparse gradients and more than one param
+group are not supported.
 """
 import torch
 
 from . import ops
-
-# group flags of torch's optimizers that change the arithmetic and that the flat kernels do not implement
-_UNSUPPORTED_FLAGS = ("maximize", "differentiable", "decoupled_weight_decay")
-
 
 class FlatOptimizer(torch.optim.Optimizer):
     """Flat parameter / gradient buffers and the device hyperparameters shared by the flat optimizers.
 
     A subclass names ``torch_cls`` (the torch optimizer whose semantics and checkpoint format it has), ``hyper`` (the group keys
     it reads), ``buffer_keys()`` (torch's per-parameter state names under the current options, each one flat buffer here) and
-    ``_update(group, state, grad_scale)`` (one kernel launch).  ``FlatAdamW`` keeps its own state and checkpoint code.
+    ``_update(group, state, grad_scale)`` (one kernel launch).  ``fixed`` holds the group values its kernel implements: a
+    checkpoint whose group carries another value of one of these keys is refused, not run as a different algorithm.
 
     Only lr (and the gradient scale) reach a CUDA-graph-captured step through the device; the other hyperparameters are kernel
     arguments, fixed when the step is captured.  ``captured_hyper()`` names them: ``train`` re-captures its padded step when they
@@ -35,6 +33,7 @@ class FlatOptimizer(torch.optim.Optimizer):
     hyper = ("lr",)
     has_step = True              # torch keeps a per-parameter "step" in the state (SGD does not)
     state_at_init = False        # torch creates the state at construction (Adagrad), not at the first step
+    fixed = {"maximize": False, "differentiable": False, "decoupled_weight_decay": False}
 
     def __init__(self, model, defaults):
         name = type(self).__name__
@@ -161,10 +160,10 @@ class FlatOptimizer(torch.optim.Optimizer):
         if len(order) != len(self.params):
             raise ValueError("%s.load_state_dict: %d parameters in the checkpoint, %d in the model" % (name, len(order), len(self.params)))
         g0 = groups[0]
-        for flag in _UNSUPPORTED_FLAGS:
-            if g0.get(flag):
-                raise ValueError("%s.load_state_dict: the checkpoint's optimizer has %s=True, which the flat step does not implement"
-                                 % (name, flag))
+        for key, value in self.fixed.items():
+            if key in g0 and g0[key] != value:
+                raise ValueError("%s.load_state_dict: the checkpoint's optimizer has %s=%s, which the flat step does not implement"
+                                 % (name, key, g0[key]))
         for key in self.hyper:
             if key in g0:
                 self.param_groups[0][key] = tuple(g0[key]) if isinstance(g0[key], list) else g0[key]
@@ -218,6 +217,34 @@ class FlatAdam(FlatOptimizer):
     def _update(self, g, s, grad_scale):
         ops.adam_step(self.flat_p, self.flat_g, s["exp_avg"], s["exp_avg_sq"], s.get("max_exp_avg_sq"), self.step_dev, g["lr"],
                       g["betas"][0], g["betas"][1], g["eps"], g["weight_decay"], g["amsgrad"], grad_scale, hyper_dev=self.hyper_dev)
+
+
+class FlatAdamW(FlatOptimizer):
+    """torch.optim.AdamW over the flat buffers (decoupled weight decay), the default of ``hydragnn/utils/optimizer/optimizer.py``.
+    Its kernel takes fp32 hyperparameters and computes the bias corrections in fp32."""
+    torch_cls = torch.optim.AdamW
+    hyper = ("lr", "betas", "eps", "weight_decay")
+    fixed = {**FlatOptimizer.fixed, "decoupled_weight_decay": True, "amsgrad": False}
+
+    def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2):
+        super().__init__(model, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
+
+    def buffer_keys(self):
+        return ["exp_avg", "exp_avg_sq"]
+
+    @property
+    def m(self):
+        """The flat first moment, ``flat_state["exp_avg"]``."""
+        return self.flat_state["exp_avg"]
+
+    @property
+    def v(self):
+        """The flat second moment, ``flat_state["exp_avg_sq"]``."""
+        return self.flat_state["exp_avg_sq"]
+
+    def _update(self, g, s, grad_scale):
+        ops.adamw_step(self.flat_p, self.flat_g, s["exp_avg"], s["exp_avg_sq"], self.step_dev, g["lr"], g["betas"][0], g["betas"][1],
+                       g["eps"], g["weight_decay"], grad_scale, hyper_dev=self.hyper_dev)
 
 
 class FlatAdamax(FlatOptimizer):
@@ -292,12 +319,6 @@ class FlatRMSprop(FlatOptimizer):
                          hyper_dev=self.hyper_dev)
 
 
-def _flat_classes():
-    from .train import FlatAdamW
-    return {"SGD": FlatSGD, "Adam": FlatAdam, "Adadelta": FlatAdadelta, "Adagrad": FlatAdagrad, "Adamax": FlatAdamax,
-            "AdamW": FlatAdamW, "RMSprop": FlatRMSprop}
-
-
 def select_optimizer(model, config):
     """hydragnn/utils/optimizer/optimizer.py:select_optimizer on the engine: ``config["type"]`` names the optimizer and only
     ``config["learning_rate"]`` is passed, so every other hyperparameter takes torch's default, as in the reference.
@@ -309,7 +330,8 @@ def select_optimizer(model, config):
     if name == "FusedLAMB":
         raise ValueError("select_optimizer: the engine does not implement DeepSpeed's FusedLamb (\"FusedLAMB\"); choose SGD, Adam, "
                          "Adadelta, Adagrad, Adamax, AdamW or RMSprop")
-    cls = _flat_classes().get(name)
+    cls = {"SGD": FlatSGD, "Adam": FlatAdam, "Adadelta": FlatAdadelta, "Adagrad": FlatAdagrad, "Adamax": FlatAdamax,
+           "AdamW": FlatAdamW, "RMSprop": FlatRMSprop}.get(name)
     if cls is None:
         raise NameError("The string used to identify the optimizer is NOT recognized")
     return cls(model, lr=config["learning_rate"])

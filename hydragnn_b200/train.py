@@ -3,10 +3,10 @@
 Mirror of the hot loop ``train()`` in hydragnn/train/train_validate_test.py:629-801 and of the DDP wrap in
 hydragnn/utils/distributed/distributed.py:396-481, redesigned for one NVSwitch box:
 
-* parameters and gradients live in ONE flat fp32 buffer each (the modules hold views), so the optimizer is a
-  single fused kernel (AdamW here; the other types in optim.py) and the only collective of the step is ONE ``all_reduce``
-  over the flat gradient (graphs shard by rank with no other communication -- SURVEY 8e); the 1/world_size scaling is
-  folded into the optimizer kernel;
+* parameters and gradients live in ONE flat fp32 buffer each (the modules hold views), so the optimizer (a
+  ``FlatOptimizer`` of optim.py, AdamW by default) is a single fused kernel and the only collective of the step is ONE
+  ``all_reduce`` over the flat gradient (graphs shard by rank with no other communication -- SURVEY 8e); the 1/world_size
+  scaling is folded into the optimizer kernel;
 * no mpi4py anywhere on the step path (the reference's per-epoch ``MPI.allreduce(nbatch, MIN)``,
   :672, becomes a ``dist.all_reduce(MIN)``);
 * ``GraphedTrainStep`` captures forward + loss + backward + flatten + optimizer of a fixed-shape batch in a CUDA
@@ -61,73 +61,6 @@ def get_head_indices(model, data):
         lo, hi = (start + y_loc[:, ih:ih + 1]).flatten().tolist(), (start + y_loc[:, ih + 1:ih + 2]).flatten().tolist()
         out.append(torch.cat([torch.arange(a, b, device=data.y.device) for a, b in zip(lo, hi)]))
     return out
-
-
-class FlatAdamW(FlatOptimizer):
-    """torch.optim.AdamW semantics over one flat buffer (``hydragnn/utils/optimizer/optimizer.py:12-40`` default).  After
-    construction every parameter of ``model`` is a view into ``self.flat_p`` (so checkpoints / ``state_dict`` are unchanged).
-
-    It IS a ``torch.optim.Optimizer`` (one param group), so ``ReduceLROnPlateau`` and the reference's checkpoint helpers accept
-    it; ``state_dict()`` / ``load_state_dict()`` speak torch.optim.AdamW's format (per-parameter ``step`` / ``exp_avg`` /
-    ``exp_avg_sq``), so optimizer checkpoints move between the reference and the engine in both directions.  The learning rate
-    and the 1/world gradient scale are read by the kernel from a DEVICE vector that ``step()`` refreshes whenever
-    ``param_groups[0]["lr"]`` changed -- a CUDA-graph-captured step therefore follows a scheduler."""
-
-    def __init__(self, model, lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2):
-        super().__init__(model, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay))
-        self.betas, self.eps, self.weight_decay = betas, eps, weight_decay
-        self.m = torch.zeros_like(self.flat_p)
-        self.v = torch.zeros_like(self.flat_p)
-
-    def state_tensors(self):
-        return [self.m, self.v, self.step_dev]
-
-    def captured_hyper(self):
-        return (tuple(self.betas), self.eps, self.weight_decay)
-
-    def step(self, grad_scale=1.0, closure=None):
-        self._sync_for_step(grad_scale)
-        ops.adamw_step(self.flat_p, self.flat_g, self.m, self.v, self.step_dev, self.param_groups[0]["lr"], self.betas[0],
-                       self.betas[1], self.eps, self.weight_decay, grad_scale, hyper_dev=self.hyper_dev)
-
-    # ---- torch.optim.AdamW checkpoint format ---------------------------------------------------------------
-    def state_dict(self):
-        state = {}
-        for i, (off, k) in enumerate(self.slices):
-            shp = self.params[i].shape
-            state[i] = {"step": self.step_dev.detach().clone().reshape(()).cpu(), "exp_avg": self.m[off:off + k].view(shp).clone(),
-                        "exp_avg_sq": self.v[off:off + k].view(shp).clone()}
-        g = self.param_groups[0]
-        group = {k: v for k, v in g.items() if k != "params"}
-        group.update(betas=self.betas, eps=self.eps, weight_decay=self.weight_decay, amsgrad=False, maximize=False,
-                     params=list(range(len(self.params))))
-        return {"state": state, "param_groups": [group]}
-
-    def load_state_dict(self, sd):
-        if "state" not in sd:                                       # round-1 flat format {m, v, step, lr}
-            self.m.copy_(sd["m"])
-            self.v.copy_(sd["v"])
-            self.step_dev.copy_(sd["step"])
-            self.param_groups[0]["lr"] = sd["lr"]
-            return
-        groups = sd["param_groups"]
-        order = [i for g in groups for i in g["params"]]
-        if len(order) != len(self.params):
-            raise ValueError("FlatAdamW.load_state_dict: %d parameters in the checkpoint, %d in the model" % (len(order), len(self.params)))
-        step = None
-        for j, (off, k) in zip(order, self.slices):
-            st = sd["state"].get(j, sd["state"].get(str(j)))
-            if st is None:
-                self.m[off:off + k].zero_()
-                self.v[off:off + k].zero_()
-                continue
-            self.m[off:off + k].copy_(st["exp_avg"].reshape(-1))
-            self.v[off:off + k].copy_(st["exp_avg_sq"].reshape(-1))
-            step = float(st["step"]) if step is None else max(step, float(st["step"]))
-        self.step_dev.fill_(0.0 if step is None else step)
-        g0 = groups[0]
-        self.param_groups[0]["lr"] = g0["lr"]
-        self.betas, self.eps, self.weight_decay = tuple(g0.get("betas", self.betas)), g0.get("eps", self.eps), g0.get("weight_decay", self.weight_decay)
 
 
 class DistributedModel(torch.nn.Module):

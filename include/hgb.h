@@ -528,7 +528,7 @@ int hgb_edge_vec_scatter(const float* gvec, const int32_t* col_rowptr, const int
                          hgb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Loss / optimizer (hydragnn/train/train_validate_test.py:736-769, torch.optim.AdamW)
+ * Loss / optimizer (hydragnn/train/train_validate_test.py:736-769, torch.optim)
  * ------------------------------------------------------------------------------------------ */
 
 /* loss[0] = mean((pred - target)^2) (mode 0) or mean(|pred - target|) (mode 1);
@@ -572,26 +572,25 @@ int hgb_grouped_linear_prelu(const float* x, int64_t ldx, const float* w, const 
 int64_t hgb_prelu_workspace_bytes(int64_t count);
 int hgb_prelu_bwd(const float* g, const float* z, int64_t count, const float* slope, float* dz, float* dslope,
                   void* workspace, int32_t skip_slope, hgb_stream_t stream);
-/* Fused AdamW over one flat parameter buffer: p, g, m, v [count]; `grad_scale` multiplies g first
- * (1/world_size after the flat all-reduce); step is 1-based and read from device (`step_dev`, fp32,
- * incremented by the kernel) so the launch is CUDA-graph capturable.  hyper_dev (optional, device,
- * 2 floats {lr, grad_scale}): when given it overrides the by-value lr / grad_scale, so a captured
- * step follows a learning-rate scheduler (train_validate_test.py:452-476 steps ReduceLROnPlateau). */
-int hgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t count, float lr, float beta1,
-                   float beta2, float eps, float weight_decay, float grad_scale, float* step_dev,
-                   const float* hyper_dev, hgb_stream_t stream);
-/* The flat steps of torch.optim.SGD, Adam, Adamax, Adagrad, Adadelta and RMSprop (hydragnn/utils/optimizer/optimizer.py
- * selects them by name), each torch's single-tensor algorithm (foreach=False) in its operation order, fp32 elementwise.
- * Shared with hgb_adamw_step: p, g and every state buffer [count] (count >= 0); g is multiplied by grad_scale first;
- * hyper_dev (optional, device, {lr, grad_scale}) overrides the by-value lr / grad_scale; the 1-based step t is
- * step_dev[0] + 1 on the device, and step_dev is incremented after the update (a second launch).  Bias corrections and
+/* The flat optimizer steps (hgb_optim_flat.cu) of torch.optim.SGD, Adam, AdamW, Adamax, Adagrad, Adadelta and RMSprop
+ * (hydragnn/utils/optimizer/optimizer.py selects them by name), one kernel template, fp32 elementwise.  Common to all:
+ * p, g and every state buffer [count] (count >= 0); g is multiplied by grad_scale first (1/world_size after the flat
+ * all-reduce); hyper_dev (optional, device, 2 floats {lr, grad_scale}) overrides the by-value lr / grad_scale, so a captured
+ * step follows a learning-rate scheduler (train_validate_test.py:452-476 steps ReduceLROnPlateau); the 1-based step t is
+ * step_dev[0] + 1 on the device, and step_dev (fp32) is incremented after the update (a second launch), so the call is
+ * CUDA-graph capturable.  State buffers an option does not use may be NULL, and so may every buffer when count == 0 (only
+ * the step advances).
+ *   adamw:    decoupled weight decay p *= 1 - lr wd, fp32 hyperparameters, bias corrections computed from t in fp32.
+ * The others follow torch's single-tensor algorithm (foreach=False) in its operation order; their bias corrections and
  * decayed learning rates are computed from t in fp64 on the device, so a captured step stays right on every replay.
- * State buffers an option does not use may be NULL, and so may every buffer when count == 0 (only the step advances).
  *   sgd:      momentum_buffer when momentum != 0; at t == 1 the buffer takes the (decayed) gradient as it is.
  *             nesterov needs momentum > 0 and dampening 0.
  *   adam:     L2 weight decay added to g (torch.optim.Adam, not AdamW); max_exp_avg_sq when amsgrad.
  *   adagrad:  sum starts at initial_accumulator_value (the caller fills it); clr = lr / (1 + (t - 1) lr_decay).
  *   rmsprop:  momentum_buffer when momentum > 0, grad_avg when centered.                                          */
+int hgb_adamw_step(float* p, const float* g, float* m, float* v, int64_t count, float lr, float beta1,
+                   float beta2, float eps, float weight_decay, float grad_scale, float* step_dev,
+                   const float* hyper_dev, hgb_stream_t stream);
 int hgb_sgd_step(float* p, const float* g, float* momentum_buffer, int64_t count, float lr, double momentum,
                  double dampening, int32_t nesterov, double weight_decay, float grad_scale, float* step_dev,
                  const float* hyper_dev, hgb_stream_t stream);

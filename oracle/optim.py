@@ -1,5 +1,6 @@
-"""fp64 restatement of the six update rules the flat optimizers implement, written from torch.optim's documented algorithms
-(the single-tensor, ``foreach=False`` form; no maximize / capturable / differentiable).
+"""fp64 restatement of the seven update rules the flat optimizers implement, written from torch.optim's documented algorithms
+(the single-tensor, ``foreach=False`` form; no maximize / capturable / differentiable): SGD, Adam, AdamW, Adamax, Adagrad,
+Adadelta and RMSprop.
 
 ``step(name, p, g, state, t, **hp)`` updates the fp64 tensors ``p`` and ``state`` (a dict of torch's per-parameter state names)
 in place for the 1-based step ``t`` and the hyperparameters ``hp`` (torch's keyword names, ``lr`` included).  ``new_state``
@@ -10,6 +11,7 @@ import torch
 DEFAULTS = {
     "SGD": dict(lr=1e-3, momentum=0.0, dampening=0.0, weight_decay=0.0, nesterov=False),
     "Adam": dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, amsgrad=False),
+    "AdamW": dict(lr=1e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-2),
     "Adamax": dict(lr=2e-3, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0),
     "Adagrad": dict(lr=1e-2, lr_decay=0.0, weight_decay=0.0, initial_accumulator_value=0.0, eps=1e-10),
     "Adadelta": dict(lr=1.0, rho=0.9, eps=1e-6, weight_decay=0.0),
@@ -21,8 +23,8 @@ def state_keys(name, **hp):
     hp = {**DEFAULTS[name], **hp}
     if name == "SGD":
         return ["momentum_buffer"] if hp["momentum"] != 0 else []
-    if name == "Adam":
-        return ["exp_avg", "exp_avg_sq"] + (["max_exp_avg_sq"] if hp["amsgrad"] else [])
+    if name in ("Adam", "AdamW"):
+        return ["exp_avg", "exp_avg_sq"] + (["max_exp_avg_sq"] if hp.get("amsgrad") else [])
     if name == "RMSprop":
         return ["square_avg"] + (["momentum_buffer"] if hp["momentum"] > 0 else []) + (["grad_avg"] if hp["centered"] else [])
     return {"Adamax": ["exp_avg", "exp_inf"], "Adagrad": ["sum"], "Adadelta": ["square_avg", "acc_delta"]}[name]
@@ -37,7 +39,9 @@ def new_state(name, p, **hp):
 def step(name, p, g, state, t, **hp):
     hp = {**DEFAULTS[name], **hp}
     lr, wd = hp["lr"], hp["weight_decay"]
-    if wd != 0:                                   # every one of the six adds L2 decay to the gradient (Adam: not decoupled)
+    if name == "AdamW":                           # decoupled decay of the parameters
+        p.mul_(1 - lr * wd)
+    elif wd != 0:                                 # every other one adds L2 decay to the gradient
         g = g + wd * p
     if name == "SGD":
         mom = hp["momentum"]
@@ -49,12 +53,12 @@ def step(name, p, g, state, t, **hp):
                 buf.mul_(mom).add_((1 - hp["dampening"]) * g)
             g = g + mom * buf if hp["nesterov"] else buf
         p.sub_(lr * g)
-    elif name == "Adam":
+    elif name in ("Adam", "AdamW"):
         b1, b2 = hp["betas"]
         m, v = state["exp_avg"], state["exp_avg_sq"]
         m.mul_(b1).add_((1 - b1) * g)
         v.mul_(b2).add_((1 - b2) * g * g)
-        if hp["amsgrad"]:
+        if hp.get("amsgrad"):
             torch.maximum(state["max_exp_avg_sq"], v, out=state["max_exp_avg_sq"])
             v = state["max_exp_avg_sq"]
         bc1, bc2 = 1 - b1 ** t, 1 - b2 ** t

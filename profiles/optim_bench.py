@@ -3,11 +3,11 @@
     python profiles/optim_bench.py [--steps 20] [--sizes 1000000 10000000 100000000]
 
 Prints one JSON line with the card name and power limit beside every number:
-* for SGD, Adam, Adamax, Adagrad, Adadelta and RMSprop (torch's defaults, Adam also with amsgrad, SGD also with momentum) at
-  1e6, 1e7 and 1e8 parameters: the flat step (one hgb_*_step kernel plus the step-count increment) against torch.optim with
-  foreach=True, and with fused=True where torch has it (SGD, Adam), alternated in the same call (CUDA events, the median of three
-  regions); the bytes one update needs (4 B x (3 + 2 x states): parameter and gradient read, parameter written, every state
-  read and written -- 12 B per element for plain SGD, 28 B for Adam), the flat step's achieved bandwidth and its share of the
+* for SGD, Adam, AdamW, Adamax, Adagrad, Adadelta and RMSprop (torch's defaults, Adam also with amsgrad, SGD also with
+  momentum) at 1e6, 1e7 and 1e8 parameters: the flat step (one hgb_*_step kernel plus the step-count increment) against
+  torch.optim with foreach=True, and with fused=True where torch has it (SGD, Adam, AdamW), alternated in the same call (CUDA
+  events, the median of three regions); the bytes one update needs (4 B x (3 + 2 x states): parameter and gradient read,
+  parameter written, every state read and written -- 12 B per element for plain SGD, 28 B for Adam and AdamW), the flat step's achieved bandwidth and its share of the
   H100 SXM's 3.35 TB/s, and the relative difference of the parameters from torch's after the timed steps;
 * one eager training step (forward, loss, backward, optimizer) of ARCH["ogb_pna"] under FlatAdam and under FlatAdamW, alternated.
 """
@@ -27,10 +27,10 @@ from hydragnn_b200.synthetic import ARCH  # noqa: E402
 from pna_bench import batch, card, timed  # noqa: E402
 
 HBM = 3.35e12
-CASES = [("SGD", {}), ("SGD", {"momentum": 0.9}), ("Adam", {}), ("Adam", {"amsgrad": True}), ("Adamax", {}), ("Adagrad", {}),
-         ("Adadelta", {}), ("RMSprop", {})]
-FLAT = {"SGD": hb.FlatSGD, "Adam": hb.FlatAdam, "Adamax": hb.FlatAdamax, "Adagrad": hb.FlatAdagrad, "Adadelta": hb.FlatAdadelta,
-        "RMSprop": hb.FlatRMSprop}
+CASES = [("SGD", {}), ("SGD", {"momentum": 0.9}), ("Adam", {}), ("Adam", {"amsgrad": True}), ("AdamW", {}), ("Adamax", {}),
+         ("Adagrad", {}), ("Adadelta", {}), ("RMSprop", {})]
+FLAT = {"SGD": hb.FlatSGD, "Adam": hb.FlatAdam, "AdamW": hb.FlatAdamW, "Adamax": hb.FlatAdamax, "Adagrad": hb.FlatAdagrad,
+        "Adadelta": hb.FlatAdadelta, "RMSprop": hb.FlatRMSprop}
 
 
 def alternate(fns, steps):
@@ -54,7 +54,7 @@ def one_size(name, hp, count, steps):
     fns = {"flat": flat.step}
     torch_params = {}
     variants = {"foreach": {"foreach": True}}
-    if name in ("SGD", "Adam"):
+    if name in ("SGD", "Adam", "AdamW"):
         variants["fused"] = {"fused": True}
     for label, extra in variants.items():
         q = torch.nn.Parameter(p0.clone())

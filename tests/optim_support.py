@@ -1,13 +1,14 @@
 """What the optimizer tests share: the option combinations every flat optimizer is checked over (every option of the table in
 hydragnn_b200/optim.py's classes: momentum 0 and > 0, dampening, nesterov, weight decay 0 and > 0, amsgrad, lr_decay, the initial
-accumulator, centered), the torch and flat classes by type name, and the fp64 oracle trajectory."""
+accumulator, centered), the torch and flat classes by type name, the fp64 oracle trajectory and the hyperparameters as a kernel
+receives them."""
 import torch
 
 import hydragnn_b200 as hb
 from oracle import optim as oopt
 
-FLAT = {"SGD": hb.FlatSGD, "Adam": hb.FlatAdam, "Adamax": hb.FlatAdamax, "Adagrad": hb.FlatAdagrad, "Adadelta": hb.FlatAdadelta,
-        "RMSprop": hb.FlatRMSprop}
+FLAT = {"SGD": hb.FlatSGD, "Adam": hb.FlatAdam, "AdamW": hb.FlatAdamW, "Adamax": hb.FlatAdamax, "Adagrad": hb.FlatAdagrad,
+        "Adadelta": hb.FlatAdadelta, "RMSprop": hb.FlatRMSprop}
 TORCH = {n: getattr(torch.optim, n) for n in FLAT}
 
 CASES = [
@@ -20,6 +21,8 @@ CASES = [
     ("Adam", dict(lr=0.01, weight_decay=0.01)),
     ("Adam", dict(lr=0.01, amsgrad=True)),
     ("Adam", dict(lr=0.01, betas=(0.8, 0.99), amsgrad=True, weight_decay=0.01)),
+    ("AdamW", dict(lr=0.01)),
+    ("AdamW", dict(lr=0.01, betas=(0.8, 0.99), weight_decay=0.05)),
     ("Adamax", dict(lr=0.01)),
     ("Adamax", dict(lr=0.01, weight_decay=0.01, betas=(0.3, 0.9))),        # 1 - beta1 >= 0.5: lerp's other branch
     ("Adagrad", dict(lr=0.05)),
@@ -33,6 +36,15 @@ CASES = [
     ("RMSprop", dict(lr=0.01, centered=True, momentum=0.5, weight_decay=0.01)),
 ]
 IDS = ["%s-%s" % (n, "-".join("%s=%s" % kv for kv in sorted(hp.items()) if kv[0] != "lr") or "default") for n, hp in CASES]
+
+
+def kernel_hp(name, hp):
+    """``hp`` as the kernel receives it: hgb_adamw_step takes its betas, eps and weight decay as fp32."""
+    if name != "AdamW":
+        return hp
+    h = {**oopt.DEFAULTS[name], **hp}
+    f32 = lambda x: float(torch.tensor(x, dtype=torch.float32))  # noqa: E731
+    return {**h, "betas": tuple(f32(b) for b in h["betas"]), "eps": f32(h["eps"]), "weight_decay": f32(h["weight_decay"])}
 
 
 def oracle_run(name, hp, p0, grads, lrs=None, grad_scale=1.0):

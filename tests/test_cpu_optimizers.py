@@ -38,8 +38,6 @@ def test_select_optimizer_builds_what_the_reference_builds(golden, name, zero):
     assert len(opt.param_groups) == 1
     group = opt.state_dict()["param_groups"][0]
     for k, v in rec["group"].items():
-        if name == "AdamW" and k not in ("lr", "betas", "eps", "weight_decay", "amsgrad", "maximize"):
-            continue                                    # FlatAdamW keeps its own (older) group keys
         assert group[k] == v, (k, group[k], v)
 
 
@@ -118,6 +116,7 @@ def _oracle_kernels(monkeypatch):
     monkeypatch.setattr(ops, "sgd_step", make("SGD", ["momentum_buffer"], ["lr", "momentum", "dampening", "nesterov", "weight_decay"]))
     monkeypatch.setattr(ops, "adam_step", make("Adam", ["exp_avg", "exp_avg_sq", "max_exp_avg_sq"],
                                                ["lr", "beta1", "beta2", "eps", "weight_decay", "amsgrad"]))
+    monkeypatch.setattr(ops, "adamw_step", make("AdamW", ["exp_avg", "exp_avg_sq"], ["lr", "beta1", "beta2", "eps", "weight_decay"]))
     monkeypatch.setattr(ops, "adamax_step", make("Adamax", ["exp_avg", "exp_inf"], ["lr", "beta1", "beta2", "eps", "weight_decay"]))
     monkeypatch.setattr(ops, "adagrad_step", make("Adagrad", ["sum"], ["lr", "lr_decay", "weight_decay", "eps"]))
     monkeypatch.setattr(ops, "adadelta_step", make("Adadelta", ["square_avg", "acc_delta"], ["lr", "rho", "eps", "weight_decay"]))
@@ -163,6 +162,35 @@ def test_checkpoints_move_between_torch_and_flat_with_the_world_fold(monkeypatch
     torch_steps(c, oc, range(6, 8))
     for p, q in zip(c.parameters(), ref_m.parameters()):
         torch.testing.assert_close(p, q, rtol=1e-5, atol=1e-6)
+
+
+@pytest.mark.parametrize("name", list(FLAT))
+def test_reduce_lr_on_plateau_drives_the_lr_the_kernel_reads(monkeypatch, name):
+    """ReduceLROnPlateau (train_validate_test.py:452-476 steps it) accepts a flat optimizer, and the lr it lowers reaches the
+    device vector {lr, grad_scale} the kernel reads."""
+    _oracle_kernels(monkeypatch)
+    opt = FLAT[name](_model(), lr=1e-2)
+    sched = torch.optim.lr_scheduler.ReduceLROnPlateau(opt, mode="min", factor=0.5, patience=0)
+    for p in opt.params:
+        p.grad = torch.ones_like(p)
+    opt.gather_grads()
+    opt.step()
+    sched.step(1.0)
+    sched.step(2.0)
+    assert opt.lr == 5e-3
+    opt.sync_hyper()
+    assert abs(float(opt.hyper_dev[0]) - 5e-3) < 1e-9
+
+
+@pytest.mark.parametrize("flat,ref,kw,value", [("AdamW", "Adam", {}, "decoupled_weight_decay=False"),
+                                               ("Adam", "AdamW", {}, "decoupled_weight_decay=True"),
+                                               ("AdamW", "AdamW", dict(amsgrad=True), "amsgrad=True")])
+def test_load_state_dict_refuses_a_checkpoint_of_another_algorithm(flat, ref, kw, value):
+    """Adam's L2 decay, AdamW's decoupled decay and amsgrad are group values torch's checkpoints carry: one the flat step does not
+    run is refused, not stepped as a different algorithm."""
+    opt = FLAT[flat](_model())
+    with pytest.raises(ValueError, match="Flat%s.load_state_dict: .* has %s," % (flat, value)):
+        opt.load_state_dict(TORCH[ref](_model().parameters(), **kw).state_dict())
 
 
 @pytest.mark.parametrize("name,key", [("SGD", "momentum"), ("RMSprop", "momentum"), ("RMSprop", "centered"), ("Adam", "amsgrad")])

@@ -148,7 +148,7 @@ SCAN_N = [0, 1, 1023, 1024, 1025, 2 ** 20, 2 ** 20 + 1, 2 ** 21, 3 * 2 ** 20 + 5
 CSR_CASES = [(0, 4), (5, 1), (40, 2), (1000, 37), (1000, 64), (1000, 65), (3000, 1024), (3000, 1025), (200_000, 5000),
              (4000, 1)]                                           # (e, n); the last: one segment holds every edge
 GROUPED_GRAPHS = ["wide", "shared_key_step", "no_edges", "no_nodes", "mixed"]
-ADAMW_COUNTS = [1, 1000, 600_000]
+ADAMW_COUNTS = [1, 1000, 600_000, 2_200_001]
 LOSS_COUNTS = [1, 7, 1024, 1025, 70_000]
 
 
@@ -168,7 +168,7 @@ def all_tags():
     for n in SCAN_N:
         tags |= scan_plan(n)["tags"]
     for count in ADAMW_COUNTS:
-        tags |= flat_plan("adamw", count)
+        tags |= flat_plan("adamw", cdiv(count, 4))           # aligned buffers: the float4 body, the remainder one by one
     for _, n in CSR_CASES:
         bits = csr_key_bits(n)
         if n in (1, 2):

@@ -40,7 +40,7 @@ def golden(golden_dir):
     return torch.load(golden_dir + "/optimizers.pt")
 
 
-@pytest.mark.parametrize("name", ["SGD", "Adam", "Adadelta", "Adagrad", "Adamax", "RMSprop"])
+@pytest.mark.parametrize("name", ["SGD", "Adam", "AdamW", "Adadelta", "Adagrad", "Adamax", "RMSprop"])
 def test_oracle_equals_reference_trajectories(golden, name):
     rec = golden["types"][name]
     hp = {k: rec["group"][k] for k in oopt.DEFAULTS[name]}
