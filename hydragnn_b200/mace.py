@@ -24,8 +24,8 @@ from torch import nn
 
 from . import e3, ops
 from .covalent_radii import covalent_radii_tensor
-from .stacks import (ELEMENT_CSR, Base, apply_act, cached, decode_branches, graph_head_mlp, graph_shared_mlp, graph_sum,
-                     remember, run_mlp)
+from .stacks import (ELEMENT_CSR, Base, _linear_layers, apply_act, branch_plan, cached, decode_branches, graph_head_mlp,
+                     graph_shared_mlp, graph_sum, grouped_decode, remember, run_mlp)
 
 NUM_ELEMENTS = 118
 
@@ -282,6 +282,14 @@ class _NodeMLP(nn.Module):
             layers.append(nn.Linear(hidden[-1], output_dim))
         self.mlp = nn.ModuleList([nn.Sequential(*layers)])
 
+    def grouped_layers(self):
+        """The MLP as ``ops.grouped_mlp`` takes it: the o3.Linear on scalars is a Linear without bias whose weight is
+        ``weight.reshape(mi, mo) * alpha``, transposed."""
+        seq = self.mlp[0]
+        e = seq[0]
+        mi, mo = e.irreps_in[0][0], e.irreps_out[0][0]
+        return [((e.weight.reshape(mi, mo) * e.alpha[0]).t(), None)] + _linear_layers(list(seq)[1:])
+
     def forward(self, x, higher=False):
         seq = self.mlp[0]
         h = seq[0]([x[:, None, :]], higher)[0][:, 0, :]
@@ -324,12 +332,16 @@ class MultiheadDecoder(nn.Module):
                 raise ValueError("Unknown head type" + str(head_type[ih]) + "; currently only support 'graph' or 'node'")
             self.heads_NN.append(head)
 
-    def forward(self, scalars, pooled, batch, num_graphs, dataset_name, higher=False):
-        ids = None if dataset_name is None else dataset_name[:, 0]
+    def forward(self, scalars, pooled, batch, num_graphs, branches, higher=False):
+        """``branches``: the batch's ``BranchPlan`` (None with one branch)."""
         outs = []
         for hd, head, kind in zip(self.head_dims, self.heads_NN, self.head_type):
             if len(head) > 1:
-                outs.append(decode_branches(kind, head, self.graph_shared, ids, scalars, pooled, batch, hd, num_graphs, higher))
+                out = grouped_decode(kind, head, self.graph_shared, branches, scalars, pooled, hd, higher)
+                if out is None:
+                    out = decode_branches(kind, head, self.graph_shared, branches.ds[:, 0], scalars, pooled, batch, hd, num_graphs,
+                                          higher)
+                outs.append(out)
             elif kind == "graph":
                 z = run_mlp(self.graph_shared["branch-0"], pooled, higher) if self.nonlinear else pooled
                 outs.append(run_mlp(head["branch-0"], z, higher)[:, :hd])
@@ -512,6 +524,7 @@ class MACEStack(Base):
 
     def _multihead(self):
         """Nothing (:500): every decoder is one of ``multihead_decoders``."""
+        self.num_branches = max(len(v) for v in self.config_heads.values())
 
     def _decoder(self, nonlinear, in_scalars):
         return MultiheadDecoder(nonlinear, in_scalars, self.config_heads, self.head_dims, self.head_type, self.activation_function,
@@ -596,7 +609,7 @@ class MACEStack(Base):
         cond = None if ga is None else self._conditioning(ga, gcsr, higher)
         if cond is not None:
             xs = [cond(xs[0].reshape(n, -1))[:, None, :]]
-        ds = getattr(data, "dataset_name", None)
+        ds = branch_plan(data, batch, self.num_branches) if self.num_branches > 1 else None
         onehot = torch.nn.functional.one_hot(z, NUM_ELEMENTS).to(pos.dtype)
         outputs = self.multihead_decoders[0](onehot, self.pool(onehot, gcsr, higher), batch, num_graphs, ds, higher)
         for i, (conv, readout) in enumerate(zip(self.graph_convs, self.multihead_decoders[1:])):

@@ -111,10 +111,15 @@ class EdgePlan:
         'col' -> row[by_col.perm]."""
         if which not in self._nbr:
             idx, perm = (self.col, self.by_row.perm) if which == "row" else (self.row, self.by_col.perm)
-            out = torch.empty_like(perm)
-            _lib.call("hgb_gather_i32", _p(idx), _p(perm), perm.numel(), _p(out), _stream())
-            self._nbr[which] = out
+            self._nbr[which] = gather_i32(idx, perm)
         return self._nbr[which]
+
+
+def gather_i32(idx, perm):
+    """``idx[perm]`` of two int32 vectors."""
+    out = torch.empty_like(perm)
+    _lib.call("hgb_gather_i32", _p(idx), _p(perm), perm.numel(), _p(out), _stream())
+    return out
 
 
 def graph_ptr_from_batch(batch, num_graphs):
@@ -1849,31 +1854,126 @@ class GroupedLinearPReluFn(torch.autograd.Function):
         return gx, gw, gb, None, dslope
 
 
-def grouped_mlp(seq_by_group, x, rowptr):
-    """Run structurally identical ``nn.Sequential`` MLPs (one per group) on rows sorted by group.  Returns None when the
-    branches do not share one architecture (the caller then falls back to per-branch launches)."""
+class GroupedMatMul(torch.autograd.Function):
+    """``y[r] = x[r] W_g^T`` (``trans_w`` 0, w [groups, n, k]) or ``y[r] = x[r] W_g`` (``trans_w`` 1, w [groups, k, n]) for rows
+    sorted by group (``rowptr`` [groups + 1] on the device), on ``hgb_grouped_linear``.  The data gradient is the same product
+    with ``trans_w`` flipped and the weight gradient a ``GroupedWgrad``, whose own derivatives are grouped products again: closed
+    under autograd, as ``MatMul`` is.  ``w_is_weight``: ``w`` is built from parameters, so its gradient is skipped under
+    ``only_data_grads``."""
+
+    @staticmethod
+    def forward(ctx, x, w, rowptr, trans_w, w_is_weight=False):
+        x, w = _chk(x.contiguous()), _chk(w.contiguous())
+        groups = w.shape[0]
+        m, k = x.shape
+        n = w.shape[2] if trans_w else w.shape[1]
+        y = torch.empty(m, n, dtype=x.dtype, device=x.device)
+        _lib.call("hgb_grouped_linear", _p(x), k, _p(w), None, _p(rowptr), groups, m, n, k, int(trans_w), 0, 0.0, _p(y), None,
+                  _stream())
+        ctx.save_for_backward(x, w, rowptr)
+        ctx.trans_w, ctx.w_is_weight = int(trans_w), bool(w_is_weight)
+        return y
+
+    @staticmethod
+    def backward(ctx, g):
+        x, w, rowptr = ctx.saved_tensors
+        gx = gw = None
+        if ctx.needs_input_grad[0]:
+            gx = GroupedMatMul.apply(g, w, rowptr, 1 - ctx.trans_w, ctx.w_is_weight)
+        if ctx.needs_input_grad[1] and not (ctx.w_is_weight and _DATA_ONLY["on"]):
+            #  y = x W_g^T: dW_g = g^T x          y = x W_g: dW_g = x^T g
+            gw = GroupedWgrad.apply(x, g, rowptr) if ctx.trans_w else GroupedWgrad.apply(g, x, rowptr)
+        return gx, gw, None, None, None
+
+
+class GroupedWgrad(torch.autograd.Function):
+    """``H_g = sum_{r in g} a[r]^T b[r]``: [groups, n, k] from a [m, n] and b [m, k] (``hgb_grouped_wgrad``; an empty group gives
+    zeros).  d/da = b H^T and d/db = a H, both ``GroupedMatMul``s."""
+
+    @staticmethod
+    def forward(ctx, a, b, rowptr):
+        a, b = _chk(a.contiguous()), _chk(b.contiguous())
+        groups = rowptr.numel() - 1
+        m, n = a.shape
+        k = b.shape[1]
+        h = torch.empty(groups, n, k, dtype=a.dtype, device=a.device)
+        _lib.call("hgb_grouped_wgrad", _p(a), _p(b), k, _p(rowptr), groups, m, n, k, _p(h), None, _stream())
+        ctx.save_for_backward(a, b, rowptr)
+        return h
+
+    @staticmethod
+    def backward(ctx, h):
+        a, b, rowptr = ctx.saved_tensors
+        ga = GroupedMatMul.apply(b, h, rowptr, 0) if ctx.needs_input_grad[0] else None
+        gb = GroupedMatMul.apply(a, h, rowptr, 1) if ctx.needs_input_grad[1] else None
+        return ga, gb, None
+
+
+class GroupedBiasAdd(torch.autograd.Function):
+    """``y[r] + b[group of r]``: ``GatherRows`` of the per-group bias [groups, n] by the group of every row; the bias gradient is
+    its adjoint ``SegmentSum`` (closed), skipped under ``only_data_grads``.  ``rows``: Csr of the group of every (sorted) row."""
+
+    @staticmethod
+    def forward(ctx, y, b, rows):
+        ctx.rows = rows
+        return y + raw_gather(_chk(b.contiguous()), rows.idx)
+
+    @staticmethod
+    def backward(ctx, g):
+        gb = SegmentSum.apply(g, ctx.rows) if (ctx.needs_input_grad[1] and not _DATA_ONLY["on"]) else None
+        return g, gb, None
+
+
+def grouped_mlp_ok(layers_by_group):
+    """Do the per-group MLPs share one architecture, so that ``grouped_mlp`` can run them?  ``layers_by_group``: one list per
+    group of ``(weight [out, in], bias or None)`` pairs for the Linears and activation modules between them."""
     from torch import nn
     from .stacks import _act_code
-    mods = [list(s) for s in seq_by_group]
-    if any(len(m) != len(mods[0]) for m in mods):
-        return None
+    first = layers_by_group[0]
+    if any(len(g) != len(first) for g in layers_by_group):
+        return False
+    for i, a in enumerate(first):
+        layer = [g[i] for g in layers_by_group]
+        if isinstance(a, tuple):
+            if not all(isinstance(l, tuple) for l in layer) or len({tuple(l[0].shape) for l in layer}) != 1:
+                return False
+            if len({l[1] is None for l in layer}) != 1:
+                return False
+            if i + 1 < len(first) and not isinstance(first[i + 1], nn.Module):
+                return False
+        elif (not isinstance(a, nn.Module) or i == 0 or _act_code(a) is None or not isinstance(first[i - 1], tuple)
+              or any(_act_code(l) is None or _act_code(l)[0] != _act_code(a)[0] for l in layer)):
+            return False
+        elif isinstance(a, nn.PReLU) and any(l is not a for l in layer):
+            return False                                     # branches with slopes of their own: not the reference's layout
+    return isinstance(first[-1], tuple) if first else False
+
+
+def grouped_mlp(layers_by_group, x, rowptr, higher_order=False, rows=None):
+    """Run per-group MLPs that ``grouped_mlp_ok`` accepts on rows sorted by group (``rowptr`` [groups + 1] on the device): one
+    launch per Linear.  First order: ``GroupedLinearFn`` / ``GroupedLinearPReluFn`` with the activation in the epilogue.  Any
+    order (``higher_order``): ``GroupedMatMul`` + ``GroupedBiasAdd`` (``rows``: the group of every row) with the activations as
+    ATen glue, as ``linear_any_order`` does."""
+    from .stacks import _act_code, apply_act
+    first = layers_by_group[0]
     i = 0
-    while i < len(mods[0]):
-        layer = [m[i] for m in mods]
-        if not all(isinstance(l, nn.Linear) for l in layer) or len({tuple(l.weight.shape) for l in layer}) != 1:
-            return None
-        code = _act_code(mods[0][i + 1]) if i + 1 < len(mods[0]) else None
-        if i + 1 < len(mods[0]) and code is None:
-            return None
-        w = torch.stack([l.weight for l in layer])
-        b = torch.stack([l.bias for l in layer]) if layer[0].bias is not None else None
-        if code is not None and code[0] == "prelu":
-            if any(m[i + 1] is not mods[0][i + 1] for m in mods):
-                return None                                  # branches with slopes of their own: not the reference's layout
-            x = GroupedLinearPReluFn.apply(x, w, b, rowptr, code[1])
+    while i < len(first):
+        w = torch.stack([g[i][0] for g in layers_by_group])
+        b = torch.stack([g[i][1] for g in layers_by_group]) if first[i][1] is not None else None
+        act = first[i + 1] if i + 1 < len(first) else None
+        if higher_order:
+            x = GroupedMatMul.apply(x, w, rowptr, 0, True)
+            if b is not None:
+                x = GroupedBiasAdd.apply(x, b, rows)
+            if act is not None:
+                x = apply_act(act, x, True)
         else:
-            x = GroupedLinearFn.apply(x, w, b, rowptr, code[0] if code else None, code[1] if code else 0.0)
-        i += 2 if code else 1
+            code = _act_code(act) if act is not None else None
+            if code is not None and code[0] == "prelu":
+                x = GroupedLinearPReluFn.apply(x, w, b, rowptr, code[1])
+            else:
+                x = GroupedLinearFn.apply(x, w, b, rowptr, code[0] if code else None, code[1] if code else 0.0)
+        i += 2 if act is not None else 1
     return x
 
 

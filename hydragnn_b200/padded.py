@@ -18,7 +18,10 @@ one graph.  A batch larger than a capacity re-captures with grown capacities (ho
 
 Supported: EGNN / PaiNN / MACE / PNAEq stacks without BatchNorm-carrying wrappers (GPS mixes every atom of the mini-batch:
 filler atoms would leak into real ones) or BatchNorm feature layers (PNA: the same leak through the batch statistics), heads
-all of graph type, or the MLIP wrapper (energy + forces).
+all of graph type, or the MLIP wrapper (energy + forces).  Any number of dataset branches, as long as the branches of every
+head share one architecture: they are decoded by the grouped kernels, which read no group size back to the host
+(``stacks.grouped_decode``).  ``dataset_name`` then travels with the batch; filler graphs belong to branch 0.  Models whose
+branches differ decode with boolean masks over ``dataset_name.unique()`` and train eagerly.
 """
 import torch
 import torch.distributed as dist
@@ -26,7 +29,7 @@ import torch.distributed as dist
 from . import _lib, ops, radius
 from .data import Batch
 from .ops import _p, _stream
-from .stacks import forget_plans
+from .stacks import branches_grouped, forget_plans
 
 
 def _round_up(x, m):
@@ -60,9 +63,48 @@ def supported(model):
     # BatchNorm feature layers (PNA) take batch statistics over every row: the filler atoms of a padded batch would enter them
     if any(isinstance(f, torch.nn.BatchNorm1d) for layer in getattr(inner, "feature_layers", ()) for f in layer.modules()):
         return False
-    if getattr(m, "model", None) is not None:               # MLIP wrapper: one head
-        return True
-    return all(t == "graph" for t in inner.head_type) and getattr(inner, "num_branches", 1) == 1
+    if getattr(m, "model", None) is None and not all(t == "graph" for t in inner.head_type):     # else the MLIP wrapper: one head
+        return False
+    return getattr(inner, "num_branches", 1) == 1 or _branches_grouped(inner)
+
+
+def _branches_grouped(inner):
+    """Do the branches of every head (of every MACE readout) share one architecture?"""
+    return all(branches_grouped(kind, head, dec.graph_shared, inner.num_branches)
+               for dec in getattr(inner, "multihead_decoders", [inner]) for head, kind in zip(dec.heads_NN, dec.head_type))
+
+
+def batch_fields(inner, first_batch, reads_edge_attr):
+    """The fields a padded batch carries: name -> (shape of one row, dtype), from a representative batch."""
+    g = int(first_batch.num_graphs)
+    fields = {k: (tuple(v.shape[1:]), v.dtype) for k, v in first_batch.items()
+              if torch.is_tensor(v) and (k in ("x", "pos", "y", "energy", "forces", "edge_shifts") or k == "edge_attr" and reads_edge_attr)}
+    if getattr(inner, "num_branches", 1) > 1:
+        # the dataset branch of every graph, [graphs, 1] int64; filler graphs decode with branch 0
+        if getattr(first_batch, "dataset_name", None) is None:
+            raise ValueError("PaddedGraphStep: a model with %d dataset branches needs dataset_name in every batch" % inner.num_branches)
+        fields["dataset_name"] = ((1,), torch.int64)
+    if getattr(inner, "use_graph_attr_conditioning", False):
+        # carried as [graphs, G] (1-D per-graph attributes reshaped), zero rows for the filler graphs
+        ga = first_batch.graph_attr
+        fields["graph_attr"] = ((ga.numel() // g,), ga.dtype)
+    return fields
+
+
+def stage(buf, key, src, g, n, fill):
+    """Copy field ``key`` of a batch with ``g`` graphs and ``n`` atoms into its host buffer ``buf``; the rows after it are the
+    filler graphs' or atoms' (``fill`` filler atoms on a line, species 1), or zero."""
+    if key == "graph_attr":
+        src = src.reshape(g, -1)
+    rows = src.shape[0]
+    buf[:rows] = src.reshape((rows,) + tuple(buf.shape[1:]))
+    if key == "pos":
+        buf[n:] = 0
+        buf[n:, 0] = 1.5 * torch.arange(fill, dtype=buf.dtype)
+    elif key == "x":
+        buf[n:] = 1
+    else:
+        buf[rows:] = 0
 
 
 class PaddedGraphStep:
@@ -72,7 +114,8 @@ class PaddedGraphStep:
         ``neighbour_build`` = (radius, max_neighbours): build the radius graph inside the captured step from ``pos``;
         None: ``edge_index`` (+ ``edge_shifts``) arrive with every batch."""
         if not supported(model):
-            raise ValueError("PaddedGraphStep: this model (global attention / node heads / branches) needs the eager train_step")
+            raise ValueError("PaddedGraphStep: this model (global attention / node heads / branches of differing architectures) "
+                             "needs the eager train_step")
         self.model, self.opt, self.mlip, self.nb = model, opt, bool(compute_grad_energy), neighbour_build
         self.hyper = None                                   # what the captured optimizer step holds besides lr (_do_capture)
         self.m = model.module
@@ -87,13 +130,7 @@ class PaddedGraphStep:
         self.warmup, self.slack = warmup, slack
         n, g = int(first_batch.pos.shape[0]), int(first_batch.num_graphs)
         e = 0 if neighbour_build else int(first_batch.edge_index.shape[1])
-        self._widths = {k: (tuple(v.shape[1:]), v.dtype) for k, v in first_batch.items()
-                        if torch.is_tensor(v) and (k in ("x", "pos", "y", "energy", "forces", "edge_shifts")
-                                                   or k == "edge_attr" and reads_edge_attr)}
-        if getattr(inner, "use_graph_attr_conditioning", False):
-            # carried as [graphs, G] (1-D per-graph attributes reshaped), zero rows for the filler graphs
-            ga = first_batch.graph_attr
-            self._widths["graph_attr"] = ((ga.numel() // g,), ga.dtype)
+        self._widths = batch_fields(inner, first_batch, reads_edge_attr)
         self._capture(node_cap or n, edge_cap or e, graph_cap or g)
         self.recaptures = 0
 
@@ -111,7 +148,8 @@ class PaddedGraphStep:
         hosts = [{}, {}]                                   # two pinned staging sets: the host fills one while the other's copy is in flight
         for key, (tail, dt) in self._widths.items():
             rows = {"x": self.n_cap, "pos": self.n_cap, "forces": self.n_cap, "y": self.g_cap, "energy": self.g_cap,
-                    "edge_shifts": self.e_cap, "edge_attr": self.e_cap, "graph_attr": self.g_cap}[key]
+                    "edge_shifts": self.e_cap, "edge_attr": self.e_cap, "graph_attr": self.g_cap,
+                    "dataset_name": self.g_cap}[key]
             if key == "edge_shifts" and self.nb:
                 continue
             for h in hosts:
@@ -226,19 +264,7 @@ class PaddedGraphStep:
         for key in self._widths:
             if key not in h:
                 continue
-            src = batch[key].to("cpu")
-            buf = h[key]
-            if key == "graph_attr":
-                src = src.reshape(g, -1)
-            rows = src.shape[0]
-            buf[:rows] = src.reshape((rows,) + tuple(buf.shape[1:]))
-            if key == "pos":
-                buf[n:] = 0
-                buf[n:, 0] = 1.5 * torch.arange(fill, dtype=buf.dtype)
-            elif key == "x":
-                buf[n:] = 1
-            else:
-                buf[rows:] = 0
+            stage(h[key], key, batch[key].to("cpu"), g, n, fill)
         if not self.nb:
             h["edge_index"][:, :e] = batch.edge_index.to("cpu")
         for key, buf in h.items():

@@ -161,10 +161,11 @@ def _padded_chain(mods, x):
 
 
 # Per-batch index plans, cached on the batch object: the CSR views of edge_index (ops.EdgePlan), the graph offsets, MACE's
-# element CSR, the (edge_index, rowptr, graph_ptr) hint a radius build leaves, and the in-degree groupings of the SAGE / MFC
-# layers (ops.DegreePlan).  A step that copies a new batch into the same tensors must forget them (``forget_plans``).
-PLAN_KEYS = EDGE_PLAN, GRAPH_CSR, ELEMENT_CSR, COL_SORTED, DEGREE_PLAN = ("_hgb_plan", "_hgb_gcsr", "_hgb_zcsr", "_hgb_col_sorted",
-                                                                         "_hgb_degplan")
+# element CSR, the (edge_index, rowptr, graph_ptr) hint a radius build leaves, the in-degree groupings of the SAGE / MFC
+# layers (ops.DegreePlan) and the dataset-branch groupings of multi-branch heads (BranchPlan).  A step that copies a new batch
+# into the same tensors must forget them (``forget_plans``).
+PLAN_KEYS = EDGE_PLAN, GRAPH_CSR, ELEMENT_CSR, COL_SORTED, DEGREE_PLAN, BRANCH_PLAN = (
+    "_hgb_plan", "_hgb_gcsr", "_hgb_zcsr", "_hgb_col_sorted", "_hgb_degplan", "_hgb_branches")
 
 
 def cached(data, key):
@@ -531,6 +532,91 @@ def decode_branches(kind, head, graph_shared, ids, x, x_graph, batch, width, num
     return out
 
 
+class BranchGroups(NamedTuple):
+    """Rows (graphs or atoms) grouped by dataset branch on the device: ``rowptr`` [branches + 1] of the sorted rows, ``order`` the
+    sorting permutation as a Csr (``GatherRows`` sorts, its adjoint ``SegmentSum`` scatters back) and ``rows`` the branch of
+    every sorted row (the per-branch bias of ``ops.GroupedBiasAdd``)."""
+    rowptr: torch.Tensor
+    order: ops.Csr
+    rows: ops.Csr
+
+
+def branch_groups(ids, num_branches):
+    bcsr = ops.csr_build(ids.to(torch.int64).contiguous(), num_branches)             # stable: rows keep their order in a branch
+    order = ops.csr_build(bcsr.perm.to(torch.int64), ids.numel())
+    return BranchGroups(bcsr.rowptr, order, ops.Csr(ops.gather_i32(bcsr.idx, bcsr.perm), bcsr.rowptr, None, num_branches))
+
+
+class BranchPlan:
+    """The dataset-branch groupings of one batch (``dataset_name[:, 0]``), built once and shared by every multi-branch head of
+    every readout: the graphs' grouping, and the atoms' once a node head asks for it."""
+
+    def __init__(self, ds, batch, num_branches):
+        self.ds, self.batch, self.num_branches = ds, batch, num_branches
+        self._groups = {}
+
+    def groups(self, kind):
+        if kind not in self._groups:
+            ids = self.ds[:, 0]
+            self._groups[kind] = branch_groups(ids if kind == "graph" else ids[self.batch], self.num_branches)
+        return self._groups[kind]
+
+
+def branch_plan(data, batch, num_branches):
+    """The ``BranchPlan`` of ``data`` (cached under BRANCH_PLAN)."""
+    ds = data.dataset_name
+    plan = cached(data, BRANCH_PLAN)
+    if plan is None or plan.ds is not ds or plan.batch is not batch or plan.num_branches != num_branches:
+        plan = remember(data, BRANCH_PLAN, BranchPlan(ds, batch, num_branches))
+    return plan
+
+
+def _linear_layers(mods):
+    """The layers of ``mods`` as ``ops.grouped_mlp`` takes them: (weight, bias) for a Linear, activation modules as they are."""
+    return [(m.weight, m.bias) if isinstance(m, nn.Linear) else m for m in mods]
+
+
+def branch_layers(kind, head, graph_shared, num_branches):
+    """One layer list per branch of ``head`` for ``ops.grouped_mlp``: a graph head with its branch's shared layers in front, an
+    ``mlp`` node head, or a head that states its own (``grouped_layers``).  None if a branch has another form."""
+    keys = ["branch-%d" % b for b in range(num_branches)]
+    if any(k not in head for k in keys):
+        return None
+    if kind == "graph":
+        return [(_linear_layers(graph_shared[k]) if k in graph_shared else []) + _linear_layers(head[k]) for k in keys]
+    out = []
+    for k in keys:
+        h = head[k]
+        if isinstance(h, MLPNode) and h.num_nodes is None:
+            out.append(_linear_layers(h.mlp[0]))
+        elif hasattr(h, "grouped_layers"):
+            out.append(h.grouped_layers())
+        else:
+            return None
+    return out
+
+
+def branches_grouped(kind, head, graph_shared, num_branches):
+    """Can ``grouped_decode`` decode this head: do its branches share one architecture?"""
+    layers = branch_layers(kind, head, graph_shared, num_branches)
+    return layers is not None and ops.grouped_mlp_ok(layers)
+
+
+def grouped_decode(kind, head, graph_shared, branches, x, x_graph, width, higher_order):
+    """One head over several dataset branches as grouped GEMMs (SURVEY 8f-4): the rows (graphs, or atoms for a node head) are
+    sorted by branch on the device (``branches``: the batch's ``BranchPlan``), each layer of the per-branch MLPs is one grouped
+    launch, the result is scattered back -- no ``unique()``, no boolean masks, no host synchronisation, so a captured step can
+    run it.  Any order of differentiation (``higher_order``: the closed grouped ops).  None if the branches differ in
+    architecture (the caller then runs ``decode_branches``)."""
+    layers = branch_layers(kind, head, graph_shared, branches.num_branches)
+    if layers is None or not ops.grouped_mlp_ok(layers):
+        return None
+    g = branches.groups(kind)
+    xs = GatherRows.apply(x_graph if kind == "graph" else x, g.order)
+    ys = ops.grouped_mlp(layers, xs, g.rowptr, higher_order, g.rows)
+    return SegmentSum.apply(ys, g.order)[:, :width]
+
+
 # ------------------------------------------------------------------------------------------------
 # Base: encoder loop + pooling + multi-head decoder
 # ------------------------------------------------------------------------------------------------
@@ -795,7 +881,7 @@ class Base(nn.Module):
                 x_graph = self.pool(x.materialize(), gcsr, higher)
         else:
             x_graph = self.pool(x, gcsr, higher)                              # Base.py:733-738
-        ds = getattr(data, "dataset_name", None)
+        branches = branch_plan(data, batch, self.num_branches) if self.num_branches > 1 else None
         outputs, outputs_var = [], []
         for hd, head, kind in zip(self.head_dims, self.heads_NN, self.head_type):
             width = hd * (1 + self.var_output)
@@ -813,10 +899,10 @@ class Base(nn.Module):
                 else:
                     out = head["branch-0"](x, higher)
             else:
-                ids = ds[:, 0]                                               # Base.py:770-780, 816-840
-                out = None if higher else self._grouped_decode(kind, head, ids, x, x_graph, batch, width, num_graphs)
+                out = grouped_decode(kind, head, self.graph_shared, branches, x, x_graph, width, higher)     # Base.py:770-780, 816-840
                 if out is None:
-                    out = decode_branches(kind, head, self.graph_shared, ids, x, x_graph, batch, width, num_graphs, higher)
+                    out = decode_branches(kind, head, self.graph_shared, data.dataset_name[:, 0], x, x_graph, batch, width,
+                                          num_graphs, higher)
             outputs.append(out[:, :hd])
             if self.var_output:                                              # Base.py:764-768, 779, 810-811, 838
                 outputs_var.append(out[:, hd:] ** 2)
@@ -838,29 +924,6 @@ class Base(nn.Module):
 
         readout = self.graph_pooling == "mean" and all(k == "graph" for k in self.head_type)
         return [painn(i) and (painn(i + 1) if i + 1 < n else readout) for i in range(n)]
-
-    def _grouped_decode(self, kind, head, ids, x, x_graph, batch, width, num_graphs):
-        """Branch decoding as grouped GEMMs (SURVEY 8f-4): rows are sorted by dataset branch on the device (CSR over the branch
-        ids), each layer of the per-branch MLPs is one ``hgb_grouped_linear`` launch, the result is scattered back -- no
-        ``unique()``, no boolean masks, no host synchronisation.  None if the branches differ in architecture."""
-        keys = ["branch-%d" % b for b in range(self.num_branches)]
-        if any(k not in head for k in keys):
-            return None
-        if kind == "graph":
-            rows_ids, feats = ids, x_graph
-            seqs = [nn.Sequential(*list(self.graph_shared[k]), *list(head[k])) for k in keys]
-        else:
-            if not all(isinstance(head[k], MLPNode) and head[k].num_nodes is None for k in keys):
-                return None
-            rows_ids, feats = ids[batch], x
-            seqs = [head[k].mlp[0] for k in keys]
-        bcsr = ops.csr_build(rows_ids.to(torch.int64).contiguous(), self.num_branches)     # rows grouped by branch (stable)
-        pcsr = ops.csr_build(bcsr.perm.to(torch.int64), feats.shape[0])                     # the permutation as a gather / scatter pair
-        xs = GatherRows.apply(feats, pcsr)
-        ys = ops.grouped_mlp(seqs, xs, bcsr.rowptr)
-        if ys is None:
-            return None
-        return SegmentSum.apply(ys, pcsr)[:, :width]
 
     def pool(self, x, gcsr, higher_order=False):
         if higher_order and self.graph_pooling != "max":
