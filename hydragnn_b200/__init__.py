@@ -7,6 +7,7 @@ Public surface (mirrors the slice of ``hydragnn`` that sits on the per-step hot 
     get_radius_graph[_pbc][_config]        -- hydragnn.preprocess.graph_samples_checks_and_updates
     train, validate, train_step, get_distributed_model -- hydragnn.train / hydragnn.utils.distributed
     select_optimizer, FlatSGD, FlatAdam, FlatAdamW, FlatAdamax, FlatAdagrad, FlatAdadelta, FlatRMSprop -- hydragnn.utils.optimizer
+    branch_weighted_energy_forces, PaddedPredictStep -- examples/multidataset_hpo_sc26/inference_fused.py's weighted prediction
 
 The CUDA library is loaded lazily on first use; importing the package works on a CPU-only host.
 """
@@ -19,5 +20,6 @@ from .train import GraphedTrainStep, get_distributed_model, get_head_indices, tr
 from .optim import (FlatAdadelta, FlatAdagrad, FlatAdam, FlatAdamax, FlatAdamW, FlatOptimizer, FlatRMSprop,  # noqa: F401
                     FlatSGD, select_optimizer)
 from .padded import PaddedGraphStep  # noqa: F401
+from .predict import PaddedPredictStep, branch_weighted_energy_forces  # noqa: F401
 
 __version__ = "0.2.0"

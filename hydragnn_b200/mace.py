@@ -24,7 +24,7 @@ from torch import nn
 
 from . import e3, ops
 from .covalent_radii import covalent_radii_tensor
-from .stacks import (ELEMENT_CSR, Base, _linear_layers, apply_act, branch_plan, cached, decode_branches, graph_head_mlp,
+from .stacks import (ELEMENT_CSR, Base, _linear_layers, apply_act, cached, decode_branches, decode_plan, graph_head_mlp,
                      graph_shared_mlp, graph_sum, grouped_decode, remember, run_mlp)
 
 NUM_ELEMENTS = 118
@@ -609,7 +609,7 @@ class MACEStack(Base):
         cond = None if ga is None else self._conditioning(ga, gcsr, higher)
         if cond is not None:
             xs = [cond(xs[0].reshape(n, -1))[:, None, :]]
-        ds = branch_plan(data, batch, self.num_branches) if self.num_branches > 1 else None
+        ds = decode_plan(data, batch, num_graphs, self.num_branches)
         onehot = torch.nn.functional.one_hot(z, NUM_ELEMENTS).to(pos.dtype)
         outputs = self.multihead_decoders[0](onehot, self.pool(onehot, gcsr, higher), batch, num_graphs, ds, higher)
         for i, (conv, readout) in enumerate(zip(self.graph_convs, self.multihead_decoders[1:])):

@@ -1977,6 +1977,45 @@ def grouped_mlp(layers_by_group, x, rowptr, higher_order=False, rows=None):
     return x
 
 
+class BranchMixFn(torch.autograd.Function):
+    """E [G] = sum_b w[g, b] E_gb from every branch's output e [R, B] (``hgb_branch_mix_fwd``): E_gb is e itself for a graph
+    head (``gcsr`` None, R = G) or the sum of e over the atoms of graph g for a node head (``gcsr``: the graph CSR), written to
+    ``eb`` [G, B].  The backward seeds the heads with w[g(r), b] dE_g (``hgb_branch_mix_bwd``).  ``w`` is data: no gradient."""
+
+    @staticmethod
+    def forward(ctx, e, w, gcsr, eb):
+        e, w = _chk(e.contiguous()), _chk(w.contiguous())
+        r, b = e.shape
+        g = w.shape[0]
+        gptr = None if gcsr is None else gcsr.rowptr
+        out = torch.empty(g, dtype=e.dtype, device=e.device)
+        _lib.call("hgb_branch_mix_fwd", _p(e), _p(gptr), _p(w), g, r, b, _p(eb), _p(out), _stream())
+        ctx.save_for_backward(w)
+        ctx.gptr, ctx.r = gptr, r
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        w, = ctx.saved_tensors
+        g, b = w.shape
+        seeds = torch.empty(ctx.r, b, dtype=w.dtype, device=w.device)
+        _lib.call("hgb_branch_mix_bwd", _p(_chk(dout.contiguous())), _p(ctx.gptr), _p(w), g, ctx.r, b, _p(seeds), _stream())
+        return seeds, None, None, None
+
+
+def branch_mix(e, w, gcsr=None):
+    """(E [G], E_gb [G, B]) of ``BranchMixFn``; E_gb is ``e`` itself (detached) for a graph head."""
+    if e.dim() != 2 or w.dim() != 2 or e.shape[1] != w.shape[1]:
+        raise ValueError("branch_mix: e [R, B] and w [G, B] must have the same B, got %s and %s" % (tuple(e.shape), tuple(w.shape)))
+    graphs = e.shape[0] if gcsr is None else gcsr.n
+    if graphs != w.shape[0]:
+        raise ValueError("branch_mix: %d graphs but %d weight rows" % (graphs, w.shape[0]))
+    if gcsr is None:
+        return BranchMixFn.apply(e, w, None, None), e.detach()
+    eb = torch.empty(w.shape, dtype=e.dtype, device=e.device)
+    return BranchMixFn.apply(e, w, gcsr, eb), eb
+
+
 # =====================================================================================================
 # SAGEConv / MFConv: neighbour aggregation gathered into a degree-grouped wgmma Linear (hgb_nbr.cu)
 # =====================================================================================================

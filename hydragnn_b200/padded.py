@@ -74,12 +74,14 @@ def _branches_grouped(inner):
                for dec in getattr(inner, "multihead_decoders", [inner]) for head, kind in zip(dec.heads_NN, dec.head_type))
 
 
-def batch_fields(inner, first_batch, reads_edge_attr):
-    """The fields a padded batch carries: name -> (shape of one row, dtype), from a representative batch."""
+def batch_fields(inner, first_batch, reads_edge_attr, targets=True):
+    """The fields a padded batch carries: name -> (shape of one row, dtype), from a representative batch.  ``targets``: the
+    loss's targets and the dataset branch of every graph too (a prediction of every branch reads neither)."""
     g = int(first_batch.num_graphs)
+    keys = ("x", "pos", "y", "energy", "forces", "edge_shifts") if targets else ("x", "pos", "edge_shifts")
     fields = {k: (tuple(v.shape[1:]), v.dtype) for k, v in first_batch.items()
-              if torch.is_tensor(v) and (k in ("x", "pos", "y", "energy", "forces", "edge_shifts") or k == "edge_attr" and reads_edge_attr)}
-    if getattr(inner, "num_branches", 1) > 1:
+              if torch.is_tensor(v) and (k in keys or k == "edge_attr" and reads_edge_attr)}
+    if targets and getattr(inner, "num_branches", 1) > 1:
         # the dataset branch of every graph, [graphs, 1] int64; filler graphs decode with branch 0
         if getattr(first_batch, "dataset_name", None) is None:
             raise ValueError("PaddedGraphStep: a model with %d dataset branches needs dataset_name in every batch" % inner.num_branches)
@@ -107,30 +109,31 @@ def stage(buf, key, src, g, n, fill):
         buf[rows:] = 0
 
 
-class PaddedGraphStep:
-    def __init__(self, model, opt, first_batch, compute_grad_energy=False, neighbour_build=None, node_cap=None, edge_cap=None,
-                 graph_cap=None, slack=1.12, warmup=2, capture_allreduce=True):
+class PaddedBatch:
+    """The static device buffers of a capacity-padded batch, their pinned staging and the recapture on growth, shared by the
+    captured training step (``PaddedGraphStep``) and the captured prediction (``predict.PaddedPredictStep``).  A subclass
+    provides ``_do_capture`` (warm-up and capture of its body, which starts with ``_prologue``)."""
+
+    def __init__(self, model, first_batch, neighbour_build, node_cap, edge_cap, graph_cap, slack, warmup, targets=True,
+                 extra=None):
         """``first_batch``: a representative (CPU or CUDA) batch -- sizes capacities, field widths and dtypes.
         ``neighbour_build`` = (radius, max_neighbours): build the radius graph inside the captured step from ``pos``;
-        None: ``edge_index`` (+ ``edge_shifts``) arrive with every batch."""
-        if not supported(model):
-            raise ValueError("PaddedGraphStep: this model (global attention / node heads / branches of differing architectures) "
-                             "needs the eager train_step")
-        self.model, self.opt, self.mlip, self.nb = model, opt, bool(compute_grad_energy), neighbour_build
-        self.hyper = None                                   # what the captured optimizer step holds besides lr (_do_capture)
-        self.m = model.module
+        None: ``edge_index`` (+ ``edge_shifts``) arrive with every batch.  ``extra``: per-graph fields that ``load`` takes
+        besides the batch, name -> (shape of one row, dtype); filler graphs get zero rows."""
+        self.model, self.nb = model, neighbour_build
+        self.m = getattr(model, "module", model)
         inner = getattr(self.m, "model", self.m)
         reads_edge_attr = bool(getattr(inner, "use_edge_attr", False))
         if neighbour_build and reads_edge_attr:
-            raise ValueError("PaddedGraphStep: neighbour_build makes edges without features, but this model reads edge_attr "
-                             "(edge_dim > 0); pass edge_index and edge_attr with every batch instead")
+            raise ValueError("%s: neighbour_build makes edges without features, but this model reads edge_attr "
+                             "(edge_dim > 0); pass edge_index and edge_attr with every batch instead" % type(self).__name__)
         self.dev = next(model.parameters()).device
-        self.ws = dist.get_world_size() if dist.is_initialized() else 1
-        self.capture_allreduce = capture_allreduce
         self.warmup, self.slack = warmup, slack
         n, g = int(first_batch.pos.shape[0]), int(first_batch.num_graphs)
         e = 0 if neighbour_build else int(first_batch.edge_index.shape[1])
-        self._widths = batch_fields(inner, first_batch, reads_edge_attr)
+        self._widths = batch_fields(inner, first_batch, reads_edge_attr, targets)
+        self._extra = dict(extra or {})
+        self._widths.update(self._extra)
         self._capture(node_cap or n, edge_cap or e, graph_cap or g)
         self.recaptures = 0
 
@@ -147,9 +150,9 @@ class PaddedGraphStep:
         d = Batch()
         hosts = [{}, {}]                                   # two pinned staging sets: the host fills one while the other's copy is in flight
         for key, (tail, dt) in self._widths.items():
-            rows = {"x": self.n_cap, "pos": self.n_cap, "forces": self.n_cap, "y": self.g_cap, "energy": self.g_cap,
-                    "edge_shifts": self.e_cap, "edge_attr": self.e_cap, "graph_attr": self.g_cap,
-                    "dataset_name": self.g_cap}[key]
+            rows = self.g_cap if key in self._extra else {
+                "x": self.n_cap, "pos": self.n_cap, "forces": self.n_cap, "y": self.g_cap, "energy": self.g_cap,
+                "edge_shifts": self.e_cap, "edge_attr": self.e_cap, "graph_attr": self.g_cap, "dataset_name": self.g_cap}[key]
             if key == "edge_shifts" and self.nb:
                 continue
             for h in hosts:
@@ -170,8 +173,82 @@ class PaddedGraphStep:
         d._hgb_valid = self.valid
         self.data, self.hosts, self._turn = d, hosts, 0
         self._copied = [None, None]
-        self.g_fb = self.g_opt = None
         self._captured = False
+
+    def _prologue(self):
+        """The first part of every captured body: the edges of the batch (built from ``pos``, or the loaded ones padded with
+        the filler edges) and the index plans rebuilt in the captured region."""
+        d = self.data
+        if self.nb:
+            r, k = self.nb
+            ei, rowptr = radius.radius_graph(d.pos.detach(), float(r), d.ptr, self.g_cap, False, int(k), capacity=self.e_cap)
+            d.edge_index = ei
+            e_real = rowptr[-1:]
+        else:
+            e_real = self.valid[2:3]
+        _lib.call("hgb_pad_edges", _p(e_real), _p(self.valid[1:2]), self.n_cap, self.e_cap, _p(d.edge_index), _p(ops.guard_flag(self.dev)),
+                  _stream())
+        forget_plans(d)                     # index plans are part of the step: every batch brings new edges and elements
+
+    # ---- per batch ------------------------------------------------------------------------------------------------------
+    def load(self, batch, **extra):
+        """Pad ``batch`` (CPU or CUDA tensors) and the per-graph ``extra`` fields into the static buffers.  Re-captures with
+        grown capacities when it does not fit."""
+        n, g = int(batch.pos.shape[0]), int(batch.num_graphs)
+        e = 0 if self.nb else int(batch.edge_index.shape[1])
+        unused = self.g_cap - g
+        if unused < 1 or self.n_cap - n < 2 * unused or (not self.nb and e > self.e_cap):
+            self._capture(max(n, int(self.n_cap / self.slack)), max(e, 0 if self.nb else int(self.e_cap / self.slack)), max(g, self.g_cap - 1))
+            self.recaptures += 1
+            unused = self.g_cap - g
+        self._turn ^= 1
+        h, d = self.hosts[self._turn], self.data
+        if self._copied[self._turn] is not None:
+            self._copied[self._turn].synchronize()          # the copy that last read this staging set has finished (two steps ago)
+        # filler atoms: two per unused slot, the rest in the last slot; on a line 1.5 A apart
+        ptr, bfull, fill = filler_layout(batch.batch.to("cpu", torch.int64), g, self.n_cap, self.g_cap)
+        h["ptr"].copy_(ptr)
+        h["batch"].copy_(bfull)
+        h["valid"][0], h["valid"][1], h["valid"][2] = g, n, e
+        for key in self._widths:
+            if key not in h:
+                continue
+            stage(h[key], key, (extra[key] if key in self._extra else batch[key]).to("cpu"), g, n, fill)
+        if not self.nb:
+            h["edge_index"][:, :e] = batch.edge_index.to("cpu")
+        for key, buf in h.items():
+            dst = self.valid if key == "valid" else d[key]
+            dst.detach().copy_(buf, non_blocking=True)
+        ev = torch.cuda.Event()
+        ev.record()
+        self._copied[self._turn] = ev
+        self.real = g, n
+        if not self._captured:
+            self._do_capture()
+        return g
+
+    def check(self):
+        ops.check_guard(self.dev)
+
+
+class PaddedGraphStep(PaddedBatch):
+    def __init__(self, model, opt, first_batch, compute_grad_energy=False, neighbour_build=None, node_cap=None, edge_cap=None,
+                 graph_cap=None, slack=1.12, warmup=2, capture_allreduce=True):
+        """``first_batch``: a representative (CPU or CUDA) batch -- sizes capacities, field widths and dtypes.
+        ``neighbour_build`` = (radius, max_neighbours): build the radius graph inside the captured step from ``pos``;
+        None: ``edge_index`` (+ ``edge_shifts``) arrive with every batch."""
+        if not supported(model):
+            raise ValueError("PaddedGraphStep: this model (global attention / node heads / branches of differing architectures) "
+                             "needs the eager train_step")
+        self.opt, self.mlip = opt, bool(compute_grad_energy)
+        self.hyper = None                                   # what the captured optimizer step holds besides lr (_do_capture)
+        self.ws = dist.get_world_size() if dist.is_initialized() else 1
+        self.capture_allreduce = capture_allreduce
+        super().__init__(model, first_batch, neighbour_build, node_cap, edge_cap, graph_cap, slack, warmup)
+
+    def _capture(self, n_need, e_need, g_need):
+        super()._capture(n_need, e_need, g_need)
+        self.g_fb = self.g_opt = None
 
     def _masked_loss(self, pred):
         m, d = self.m, self.data
@@ -194,16 +271,7 @@ class PaddedGraphStep:
 
     def _step_body(self, with_opt):
         d, m = self.data, self.m
-        if self.nb:
-            r, k = self.nb
-            ei, rowptr = radius.radius_graph(d.pos.detach(), float(r), d.ptr, self.g_cap, False, int(k), capacity=self.e_cap)
-            d.edge_index = ei
-            e_real = rowptr[-1:]
-        else:
-            e_real = self.valid[2:3]
-        _lib.call("hgb_pad_edges", _p(e_real), _p(self.valid[1:2]), self.n_cap, self.e_cap, _p(d.edge_index), _p(ops.guard_flag(self.dev)),
-                  _stream())
-        forget_plans(d)                     # index plans are part of the step: every batch brings new edges and elements
+        self._prologue()
         self.opt.zero_grad()
         if self.mlip:
             d.pos.requires_grad_(True)
@@ -242,41 +310,6 @@ class PaddedGraphStep:
             dst.copy_(src)
         self._captured = True
 
-    # ---- per batch ------------------------------------------------------------------------------------------------------
-    def load(self, batch):
-        """Pad ``batch`` (CPU or CUDA tensors) into the static buffers.  Re-captures with grown capacities when it does not fit."""
-        n, g = int(batch.pos.shape[0]), int(batch.num_graphs)
-        e = 0 if self.nb else int(batch.edge_index.shape[1])
-        unused = self.g_cap - g
-        if unused < 1 or self.n_cap - n < 2 * unused or (not self.nb and e > self.e_cap):
-            self._capture(max(n, int(self.n_cap / self.slack)), max(e, 0 if self.nb else int(self.e_cap / self.slack)), max(g, self.g_cap - 1))
-            self.recaptures += 1
-            unused = self.g_cap - g
-        self._turn ^= 1
-        h, d = self.hosts[self._turn], self.data
-        if self._copied[self._turn] is not None:
-            self._copied[self._turn].synchronize()          # the copy that last read this staging set has finished (two steps ago)
-        # filler atoms: two per unused slot, the rest in the last slot; on a line 1.5 A apart
-        ptr, bfull, fill = filler_layout(batch.batch.to("cpu", torch.int64), g, self.n_cap, self.g_cap)
-        h["ptr"].copy_(ptr)
-        h["batch"].copy_(bfull)
-        h["valid"][0], h["valid"][1], h["valid"][2] = g, n, e
-        for key in self._widths:
-            if key not in h:
-                continue
-            stage(h[key], key, batch[key].to("cpu"), g, n, fill)
-        if not self.nb:
-            h["edge_index"][:, :e] = batch.edge_index.to("cpu")
-        for key, buf in h.items():
-            dst = self.valid if key == "valid" else d[key]
-            dst.detach().copy_(buf, non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._copied[self._turn] = ev
-        if not self._captured:
-            self._do_capture()
-        return g
-
     def run(self):
         self.opt.sync_hyper()
         self.g_fb.replay()
@@ -284,6 +317,3 @@ class PaddedGraphStep:
             dist.all_reduce(self.opt.flat_g)
             self.g_opt.replay()
         return self.loss, self.tasks
-
-    def check(self):
-        ops.check_guard(self.dev)

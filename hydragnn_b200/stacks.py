@@ -550,6 +550,7 @@ def branch_groups(ids, num_branches):
 class BranchPlan:
     """The dataset-branch groupings of one batch (``dataset_name[:, 0]``), built once and shared by every multi-branch head of
     every readout: the graphs' grouping, and the atoms' once a node head asks for it."""
+    all = False
 
     def __init__(self, ds, batch, num_branches):
         self.ds, self.batch, self.num_branches = ds, batch, num_branches
@@ -560,6 +561,58 @@ class BranchPlan:
             ids = self.ds[:, 0]
             self._groups[kind] = branch_groups(ids if kind == "graph" else ids[self.batch], self.num_branches)
         return self._groups[kind]
+
+
+def all_branch_groups(rows, num_branches, device):
+    """``BranchGroups`` that send every one of ``rows`` rows through every branch: sorted row j = b * rows + r is row r in
+    branch b, so ``rowptr`` = b * rows, ``order`` replicates each row into every branch's group (its adjoint sums the copies)
+    and ``rows`` gives branch j // rows."""
+    j, r1 = torch.arange(rows * num_branches, device=device), max(rows, 1)
+    rowptr = (torch.arange(num_branches + 1, device=device) * rows).to(torch.int32)
+    copies = (torch.arange(rows, device=device)[:, None] + torch.arange(num_branches, device=device)[None, :] * rows).reshape(-1)
+    order = ops.Csr((j % r1).to(torch.int32), (torch.arange(rows + 1, device=device) * num_branches).to(torch.int32),
+                    copies.to(torch.int32), rows)
+    return BranchGroups(rowptr, order, ops.Csr((j // r1).to(torch.int32), rowptr, None, num_branches))
+
+
+class AllBranchPlan:
+    """``BranchPlan``'s counterpart under ``all_branches()``: every graph (or atom) is decoded by every branch."""
+    all = True
+
+    def __init__(self, num_graphs, num_atoms, num_branches, device):
+        self.rows, self.num_branches, self.device = {"graph": num_graphs, "node": num_atoms}, num_branches, device
+        self._groups = {}
+
+    def groups(self, kind):
+        if kind not in self._groups:
+            self._groups[kind] = all_branch_groups(self.rows[kind], self.num_branches, self.device)
+        return self._groups[kind]
+
+
+_ALL_BRANCHES = {"on": False}
+
+
+class all_branches:
+    """Context manager: multi-branch heads decode every row through every branch and return the per-branch columns
+    [rows, branches * width] (``grouped_decode``) instead of each row's own branch; ``dataset_name`` is not read.  Used by
+    ``predict`` to evaluate every branch of a potential in one pass.  Branches of differing architecture raise ValueError."""
+
+    def __enter__(self):
+        self.prev = _ALL_BRANCHES["on"]
+        _ALL_BRANCHES["on"] = True
+        return self
+
+    def __exit__(self, *exc):
+        _ALL_BRANCHES["on"] = self.prev
+        return False
+
+
+def decode_plan(data, batch, num_graphs, num_branches):
+    """The branch plan of a forward pass: ``AllBranchPlan`` under ``all_branches()``, else the batch's ``BranchPlan`` (None
+    with one branch)."""
+    if _ALL_BRANCHES["on"]:
+        return AllBranchPlan(num_graphs, batch.numel(), num_branches, batch.device) if num_branches > 1 else None
+    return branch_plan(data, batch, num_branches) if num_branches > 1 else None
 
 
 def branch_plan(data, batch, num_branches):
@@ -607,13 +660,19 @@ def grouped_decode(kind, head, graph_shared, branches, x, x_graph, width, higher
     sorted by branch on the device (``branches``: the batch's ``BranchPlan``), each layer of the per-branch MLPs is one grouped
     launch, the result is scattered back -- no ``unique()``, no boolean masks, no host synchronisation, so a captured step can
     run it.  Any order of differentiation (``higher_order``: the closed grouped ops).  None if the branches differ in
-    architecture (the caller then runs ``decode_branches``)."""
+    architecture (the caller then runs ``decode_branches``).  With an ``AllBranchPlan`` every row goes through every branch
+    and the result is [rows, branches * width], branch b in columns b * width .. (b + 1) * width - 1."""
     layers = branch_layers(kind, head, graph_shared, branches.num_branches)
     if layers is None or not ops.grouped_mlp_ok(layers):
+        if branches.all:
+            raise ValueError("all-branch decoding needs branches that share one architecture")
         return None
     g = branches.groups(kind)
     xs = GatherRows.apply(x_graph if kind == "graph" else x, g.order)
     ys = ops.grouped_mlp(layers, xs, g.rowptr, higher_order, g.rows)
+    if branches.all:
+        rows = g.order.n
+        return ys[:, :width].reshape(branches.num_branches, rows, width).transpose(0, 1).reshape(rows, -1)
     return SegmentSum.apply(ys, g.order)[:, :width]
 
 
@@ -881,7 +940,9 @@ class Base(nn.Module):
                 x_graph = self.pool(x.materialize(), gcsr, higher)
         else:
             x_graph = self.pool(x, gcsr, higher)                              # Base.py:733-738
-        branches = branch_plan(data, batch, self.num_branches) if self.num_branches > 1 else None
+        branches = decode_plan(data, batch, num_graphs, self.num_branches)
+        if _ALL_BRANCHES["on"] and self.var_output:
+            raise ValueError("all-branch decoding does not take mean-and-variance heads")
         outputs, outputs_var = [], []
         for hd, head, kind in zip(self.head_dims, self.heads_NN, self.head_type):
             width = hd * (1 + self.var_output)
@@ -903,7 +964,7 @@ class Base(nn.Module):
                 if out is None:
                     out = decode_branches(kind, head, self.graph_shared, data.dataset_name[:, 0], x, x_graph, batch, width,
                                           num_graphs, higher)
-            outputs.append(out[:, :hd])
+            outputs.append(out if branches is not None and branches.all else out[:, :hd])
             if self.var_output:                                              # Base.py:764-768, 779, 810-811, 838
                 outputs_var.append(out[:, hd:] ** 2)
         return (outputs, outputs_var) if self.var_output else outputs

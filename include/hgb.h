@@ -475,6 +475,20 @@ int hgb_grouped_linear(const float* x, int64_t ldx, const float* w, const float*
 int hgb_grouped_wgrad(const float* dy, const float* x, int64_t ldx, const int32_t* rowptr, int32_t groups, int32_t m, int32_t n,
                       int32_t k, float* dw, float* db, hgb_stream_t stream);
 
+/* Branch-weighted energy of a multi-branch interatomic potential (hgb_branch_mix.cu), replacing the weighted sums of
+ * examples/multidataset_hpo_sc26/inference_fused.py: _weighted_average :547-563 and _fused_energy_forces :508-544.
+ * e [r, b] holds every branch's output per row; w [g, b] the per-graph branch weights.
+ *   gptr NULL (graph head): r == g, E_gb = e[g, b].
+ *   gptr [g + 1] (node head, device, gptr[g] == r): E_gb = sum of e[i, b] over the atoms of graph g, ascending, written to
+ *   eb [g, b].
+ * out [g] = sum_b w[g, b] E_gb, ascending b.  No atomics: the same bits on every run.  g == 0 launches nothing; r == 0 with
+ * g > 0 (every graph empty) writes zeros without a kernel.
+ * hgb_branch_mix_bwd: seeds [r, b] = w[g(r), b] dout[g(r)]; g == 0 or r == 0 launches nothing.                          */
+int hgb_branch_mix_fwd(const float* e, const int32_t* gptr, const float* w, int32_t g, int32_t r, int32_t b, float* eb, float* out,
+                       hgb_stream_t stream);
+int hgb_branch_mix_bwd(const float* dout, const int32_t* gptr, const float* w, int32_t g, int32_t r, int32_t b, float* seeds,
+                       hgb_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Fused EGNN edge block (hydragnn/models/EGCLStack.py:245-258 edge_model, :256-263 the scatter of
  * node_model, :278-291 forward; unsorted_segment_sum :294-300).  The first Linear of edge_mlp is
