@@ -8,6 +8,7 @@ Public surface (mirrors the slice of ``hydragnn`` that sits on the per-step hot 
     train, validate, train_step, get_distributed_model -- hydragnn.train / hydragnn.utils.distributed
     select_optimizer, FlatSGD, FlatAdam, FlatAdamW, FlatAdamax, FlatAdagrad, FlatAdadelta, FlatRMSprop -- hydragnn.utils.optimizer
     branch_weighted_energy_forces, PaddedPredictStep -- examples/multidataset_hpo_sc26/inference_fused.py's weighted prediction
+    PaddedRelaxStep                        -- examples/multidataset_hpo_sc26/structure_optimization_ASE.py's FIRE relaxation
 
 The CUDA library is loaded lazily on first use; importing the package works on a CPU-only host.
 """
@@ -21,5 +22,6 @@ from .optim import (FlatAdadelta, FlatAdagrad, FlatAdam, FlatAdamax, FlatAdamW, 
                     FlatSGD, select_optimizer)
 from .padded import PaddedGraphStep  # noqa: F401
 from .predict import PaddedPredictStep, branch_weighted_energy_forces  # noqa: F401
+from .relax import PaddedRelaxStep  # noqa: F401
 
 __version__ = "0.2.0"

@@ -19,7 +19,7 @@ void hgb_set_error(const char* fmt, ...) {
 }
 void hgb_count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
-extern "C" int hgb_version(void) { return 113; }
+extern "C" int hgb_version(void) { return 114; }
 extern "C" const char* hgb_last_error(void) { return g_err; }
 extern "C" int64_t hgb_launch_count(void) { return g_launches.load(); }
 

@@ -296,6 +296,49 @@ extern "C" int hgb_radius_pbc_emit(const int32_t* graph_ptr, const double* cell,
   return HGB_OK;
 }
 
+// Degrees of a capacity-sized periodic build: deg[j] = min(count[j], k, cand_cap - candptr[j]) (at least 0), so that
+// hgb_radius_pbc_emit reads no candidate past the cand_cap that hgb_radius_pbc_fill wrote; guard bit 1 when the candidates
+// overflowed (some target's list is then cut short even if the edges fit).
+__global__ void pbc_cap_degree_kernel(const int32_t* __restrict__ count, const int32_t* __restrict__ candptr, int n, int32_t k,
+                                      int64_t cand_cap, int32_t* __restrict__ deg, int32_t* __restrict__ flag) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && candptr[n] > cand_cap) atomicOr(flag, 1);
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const int64_t room = cand_cap - candptr[j];
+    int d = count[j] < k ? count[j] : k;
+    if (room < d) d = room > 0 ? (int)room : 0;
+    deg[j] = d;
+  }
+}
+extern "C" int hgb_radius_pbc_cap_degree(const int32_t* cand_count, const int32_t* candptr, int32_t n, int32_t max_neighbors,
+                                         int64_t cand_capacity, int32_t* deg, int32_t* flag, hgb_stream_t stream) {
+  HGB_REQUIRE(n >= 0 && max_neighbors >= 0 && cand_capacity >= 0 && candptr && flag && (n == 0 || (cand_count && deg)),
+              "radius_pbc_cap_degree: bad arguments");
+  pbc_cap_degree_kernel<<<hgb_grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(cand_count, candptr, n, max_neighbors,
+                                                                                 cand_capacity, deg, flag);
+  HGB_LAUNCH_CHECK("radius_pbc_cap_degree");
+  return HGB_OK;
+}
+
+// zero rows [min(*e_real, e_cap), e_cap) of cell_shift [e_cap, 3] int32 and edge_shifts [e_cap, 3] (the dummy edges' shifts);
+// guard bit 1 when the edges overflowed
+__global__ void pbc_zero_tail_kernel(const int32_t* __restrict__ e_real, int64_t e_cap, int32_t* __restrict__ cell_shift,
+                                     void* __restrict__ edge_shifts, int sh64, int32_t* __restrict__ flag) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && e_real[0] > e_cap) atomicOr(flag, 1);
+  const int64_t lo = 3 * min((int64_t)e_real[0], e_cap);
+  for (int64_t i = lo + (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < 3 * e_cap; i += (int64_t)gridDim.x * blockDim.x) {
+    cell_shift[i] = 0;
+    if (sh64) ((double*)edge_shifts)[i] = 0.0; else ((float*)edge_shifts)[i] = 0.f;
+  }
+}
+extern "C" int hgb_radius_pbc_zero_tail(const int32_t* e_real, int64_t e_cap, int32_t* cell_shift, void* edge_shifts,
+                                        int32_t shifts_is_f64, int32_t* flag, hgb_stream_t stream) {
+  HGB_REQUIRE(e_real && flag && e_cap >= 0 && (e_cap == 0 || (cell_shift && edge_shifts)), "radius_pbc_zero_tail: bad arguments");
+  pbc_zero_tail_kernel<<<hgb_grid_for(3 * e_cap, 256), 256, 0, (cudaStream_t)stream>>>(e_real, e_cap, cell_shift, edge_shifts,
+                                                                                       shifts_is_f64, flag);
+  HGB_LAUNCH_CHECK("radius_pbc_zero_tail");
+  return HGB_OK;
+}
+
 // out[i] = min(in[i], cap)   (degree after the nearest-k truncation)
 __global__ void clamp_i32_kernel(const int32_t* __restrict__ in, int32_t cap, int64_t n, int32_t* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)

@@ -105,6 +105,8 @@ def stage(buf, key, src, g, n, fill):
         buf[n:, 0] = 1.5 * torch.arange(fill, dtype=buf.dtype)
     elif key == "x":
         buf[n:] = 1
+    elif key == "cell":
+        buf[rows:] = torch.eye(3, dtype=buf.dtype)           # filler graphs: open boundaries, but every cell is inverted
     else:
         buf[rows:] = 0
 
@@ -115,12 +117,15 @@ class PaddedBatch:
     provides ``_do_capture`` (warm-up and capture of its body, which starts with ``_prologue``)."""
 
     def __init__(self, model, first_batch, neighbour_build, node_cap, edge_cap, graph_cap, slack, warmup, targets=True,
-                 extra=None):
+                 extra=None, periodic=False):
         """``first_batch``: a representative (CPU or CUDA) batch -- sizes capacities, field widths and dtypes.
         ``neighbour_build`` = (radius, max_neighbours): build the radius graph inside the captured step from ``pos``;
         None: ``edge_index`` (+ ``edge_shifts``) arrive with every batch.  ``extra``: per-graph fields that ``load`` takes
-        besides the batch, name -> (shape of one row, dtype); filler graphs get zero rows."""
-        self.model, self.nb = model, neighbour_build
+        besides the batch, name -> (shape of one row, dtype); filler graphs get zero rows.  ``periodic``: the neighbour build
+        is ``radius.radius_graph_pbc`` on the per-graph ``cell`` [3, 3] fp64 and ``pbc`` [3] int32 that ``extra`` carries
+        (filler graphs: the identity cell, open boundaries), with capacities (``cand_cap``, ``e_cap``) that the subclass sets
+        in its ``_capture``."""
+        self.model, self.nb, self.periodic = model, neighbour_build, periodic
         self.m = getattr(model, "module", model)
         inner = getattr(self.m, "model", self.m)
         reads_edge_attr = bool(getattr(inner, "use_edge_attr", False))
@@ -171,6 +176,8 @@ class PaddedBatch:
         if not self.nb:
             d.edge_index = torch.zeros(2, self.e_cap, dtype=torch.int64, device=dev)
         d._hgb_valid = self.valid
+        if self.periodic:
+            self.cutoff = torch.full((self.g_cap,), float(self.nb[0]), dtype=torch.float64, device=dev)
         self.data, self.hosts, self._turn = d, hosts, 0
         self._copied = [None, None]
         self._captured = False
@@ -179,7 +186,12 @@ class PaddedBatch:
         """The first part of every captured body: the edges of the batch (built from ``pos``, or the loaded ones padded with
         the filler edges) and the index plans rebuilt in the captured region."""
         d = self.data
-        if self.nb:
+        if self.periodic:
+            ei, _, d.edge_shifts, _, outptr, _ = radius.radius_graph_pbc(d.pos.detach(), d.cell, d.pbc, self.cutoff, d.ptr, self.g_cap,
+                                                                         int(self.nb[1]), capacity=(self.cand_cap, self.e_cap))
+            d.edge_index = ei
+            e_real = outptr[-1:]
+        elif self.nb:
             r, k = self.nb
             ei, rowptr = radius.radius_graph(d.pos.detach(), float(r), d.ptr, self.g_cap, False, int(k), capacity=self.e_cap)
             d.edge_index = ei

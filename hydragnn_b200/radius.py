@@ -48,11 +48,16 @@ def radius_graph(pos, r, graph_ptr, num_graphs, loop=False, max_num_neighbors=32
     return ei, rowptr
 
 
-def radius_graph_pbc(pos, cell, pbc, cutoff, graph_ptr, num_graphs, max_num_neighbors=32, known=None):
+def radius_graph_pbc(pos, cell, pbc, cutoff, graph_ptr, num_graphs, max_num_neighbors=32, known=None, capacity=None):
     """Batched periodic neighbour list with nearest-k truncation.  ``cutoff`` is a per-graph fp64 tensor.
-    Returns (edge_index [2,E], cell_shift [E,3] int32, edge_shifts [E,3] pos.dtype, in_degree [N] int32).
+    Returns (edge_index [2,E], cell_shift [E,3] int32, edge_shifts [E,3] pos.dtype, in_degree [N] int32, outptr [N+1] int32,
+    candidate count).
     ``known`` = (candidate count, edge count) from an earlier run on the same positions: no host read of either count, so the
-    build can be captured in a CUDA graph; both are verified on the device (``ops.check_guard``)."""
+    build can be captured in a CUDA graph; both are verified on the device (``ops.check_guard``).
+    ``capacity`` = (candidate capacity, edge capacity): the buffers are sized by them and filled at the head, so the build can
+    be captured while the atoms move.  The true edge count stays on the device as ``outptr[-1]``; the tail of ``cell_shift`` and
+    ``edge_shifts`` is zero (``hydragnn_b200.padded`` fills the tail of ``edge_index`` with dummy edges).  A count over its
+    capacity sets the guard (``ops.check_guard``) and nothing is written or read past a buffer."""
     assert pos.dtype in (torch.float32, torch.float64)
     if not pos.is_cuda:
         raise RuntimeError("hydragnn_b200 radius_graph_pbc needs CUDA tensors (move the sample to the device first)")
@@ -69,7 +74,9 @@ def radius_graph_pbc(pos, cell, pbc, cutoff, graph_ptr, num_graphs, max_num_neig
     cnt = torch.empty(n, dtype=torch.int32, device=dev)
     _lib.call("hgb_radius_pbc_count", _p(pos), is64, _p(graph_ptr), _p(cell), _p(nimg), _p(cutoff), n, g, _p(cnt), st)
     candptr = ops.exclusive_scan(cnt)
-    if known is None:
+    if capacity is not None:
+        c = int(capacity[0])
+    elif known is None:
         c = int(candptr[-1])
     else:
         c = int(known[0])
@@ -81,9 +88,14 @@ def radius_graph_pbc(pos, cell, pbc, cutoff, graph_ptr, num_graphs, max_num_neig
               _p(csrc), _p(cshift), _p(clen), st)
     k = int(min(max_num_neighbors, _NO_CAP))
     deg = torch.empty(n, dtype=torch.int32, device=dev)
-    _lib.call("hgb_clamp_i32", _p(cnt), k, n, _p(deg), st)
+    if capacity is not None:
+        _lib.call("hgb_radius_pbc_cap_degree", _p(cnt), _p(candptr), n, k, c, _p(deg), _p(ops.guard_flag(dev)), st)
+    else:
+        _lib.call("hgb_clamp_i32", _p(cnt), k, n, _p(deg), st)
     outptr = ops.exclusive_scan(deg)
-    if known is None:
+    if capacity is not None:
+        e = int(capacity[1])
+    elif known is None:
         e = int(outptr[-1])
     else:
         e = int(known[1])
@@ -93,6 +105,8 @@ def radius_graph_pbc(pos, cell, pbc, cutoff, graph_ptr, num_graphs, max_num_neig
     shifts = torch.empty(e, 3, dtype=pos.dtype, device=dev)
     _lib.call("hgb_radius_pbc_emit", _p(graph_ptr), _p(cell), n, g, _p(candptr), _p(csrc), _p(cshift), k, _p(outptr), e, _p(ei),
               _p(cell_shift), _p(shifts), is64, st)
+    if capacity is not None:
+        _lib.call("hgb_radius_pbc_zero_tail", _p(outptr[-1:]), e, _p(cell_shift), _p(shifts), is64, _p(ops.guard_flag(dev)), st)
     return ei, cell_shift, shifts, deg, outptr, c
 
 

@@ -56,7 +56,8 @@ typedef void* hgb_stream_t; /* cudaStream_t */
  * 108: hgb_pool_bwd zeroes the rows outside every graph, hgb_loss_fwd_bwd with *valid_rows <= 0 is 0 with a zero gradient;
  * 109: hgb_nbr_* (SAGEConv / MFConv); 110: hgb_tc_linear_graph_add, hgb_film_* (graph-attribute conditioning);
  * 111: hgb_gnll_fwd_bwd (GaussianNLLLoss); 112: hgb_prelu_fwd / hgb_prelu_bwd (PReLU with a device-resident slope);
- * 113: hgb_mace_edge_embed_dt_fwd / _dt_bwd, hgb_mace_dist_transform (MACE's Agnesi and Soft distance transforms) */
+ * 113: hgb_mace_edge_embed_dt_fwd / _dt_bwd, hgb_mace_dist_transform (MACE's Agnesi and Soft distance transforms);
+ * 114: hgb_fire_step (batched FIRE relaxation), hgb_radius_pbc_cap_degree / _zero_tail (capacity-sized periodic builds) */
 int hgb_version(void);
 const char* hgb_last_error(void);
 /* number of kernels this library has launched from the calling process (bench.py gpu_launches) */
@@ -108,6 +109,18 @@ int hgb_radius_pbc_emit(const int32_t* graph_ptr, const double* cell, int32_t n,
                         int32_t max_neighbors, const int32_t* outptr, int64_t e, int64_t* edge_index,
                         int32_t* cell_shift, void* edge_shifts, int32_t shifts_is_f64,
                         hgb_stream_t stream);
+/* Capacity-sized periodic build (radius_graph_pbc(..., capacity=(cand_cap, edge_cap)), which a CUDA graph can hold while the
+ * atoms move): hgb_radius_pbc_fill with cand_capacity = cand_cap writes the candidates that fit, then
+ * deg [n] = max(0, min(cand_count[j], max_neighbors, cand_cap - candptr[j])), so that hgb_radius_pbc_emit (e = edge_cap)
+ * reads no candidate that was not written.  Sets guard bit 1 in *flag when candptr[n] > cand_cap: a candidate overflow cuts
+ * some target's list short even when the edges fit.                                                                     */
+int hgb_radius_pbc_cap_degree(const int32_t* cand_count, const int32_t* candptr, int32_t n, int32_t max_neighbors,
+                              int64_t cand_capacity, int32_t* deg, int32_t* flag, hgb_stream_t stream);
+/* Zeroes rows [min(*e_real, e_cap), e_cap) of cell_shift [e_cap, 3] int32 and edge_shifts [e_cap, 3] (fp32, or fp64 when
+ * shifts_is_f64): the shifts of the dummy edges that hgb_pad_edges puts in the tail.  Sets guard bit 1 in *flag when
+ * *e_real > e_cap (the edges hgb_radius_pbc_emit could not write).                                                      */
+int hgb_radius_pbc_zero_tail(const int32_t* e_real, int64_t e_cap, int32_t* cell_shift, void* edge_shifts,
+                             int32_t shifts_is_f64, int32_t* flag, hgb_stream_t stream);
 /* out[i] = min(in[i], cap) */
 int hgb_clamp_i32(const int32_t* in, int32_t cap, int64_t n, int32_t* out, hgb_stream_t stream);
 /* Capacity padding of a captured neighbour build (hydragnn_b200/padded.py): edge_index [2, e_cap] holds *e_real real
@@ -488,6 +501,24 @@ int hgb_branch_mix_fwd(const float* e, const int32_t* gptr, const float* w, int3
                        hgb_stream_t stream);
 int hgb_branch_mix_bwd(const float* dout, const int32_t* gptr, const float* w, int32_t g, int32_t r, int32_t b, float* seeds,
                        hgb_stream_t stream);
+
+/* One iteration of a batched structure relaxation (hgb_relax.cu): the loop of
+ * examples/multidataset_hpo_sc26/structure_optimization_ASE.py :385-439 around ase.optimize.FIRE (ASE 3.26, fire.py
+ * FIRE.step; dt0 = 0.1, dtmax = 1, Nmin = 5, finc = 1.1, fdec = 0.5, astart = 0.1, fa = 0.99, one |dr| over the structure
+ * clamped to maxstep).  One CTA per structure g < valid[0]; filler graphs are never touched.
+ *   energy [g_cap], forces [n_cap, 3] fp32: the model's E_k and F_k at x_k; gptr [g_cap + 1] atoms of every structure.
+ *   x, v, x_prev [n_cap, 3] fp64; fire [g_cap, 3] fp64 = (dt, a, m_{k-1}); istate [g_cap, 3] int32 = (status, k, FIRE's n),
+ *   status 0 running, 1 converged, 2 reverted, 3 max steps; k = the evaluations made after x_0.
+ *   e_hist / f_hist [>= max_steps + 1, hist_stride] fp64: row k receives E_k and m_k = sqrt(max_i |F_i|^2).
+ * For a running structure: revert when revert != 0, k >= 2, m_{k-1} > 0 and (m_k - m_{k-1}) / m_{k-1} > threshold
+ * (x = x_prev); else converged when k >= 1 and m_k < ftol (the script's fmax); else max steps when k == max_steps; else
+ * the FIRE move to x_{k+1} (x_prev = x_k).  e_out [g_cap] / f_out [n_cap, 3] receive E_k / F_k unless the structure reverted (they then hold
+ * E_{k-1} / F_{k-1}); pos [n_cap, 3] fp32 receives fp32(x).  live [2] is zeroed, then live[0] = structures still running
+ * and live[1] = *guard as it stood when the kernel ran.  Sums are fp64 in a fixed order: the same bits on every run.      */
+int hgb_fire_step(const int32_t* valid, const int32_t* gptr, int32_t g_cap, const float* energy, const float* forces, double* x,
+                  double* v, double* x_prev, double* fire, int32_t* istate, double* e_hist, double* f_hist, int64_t hist_stride,
+                  float* e_out, float* f_out, float* pos, double ftol, double maxstep, int32_t max_steps, int32_t revert,
+                  double threshold, const int32_t* guard, int32_t* live, hgb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Fused EGNN edge block (hydragnn/models/EGCLStack.py:245-258 edge_model, :256-263 the scatter of
